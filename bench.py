@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the hot path (BASELINE.json: 512x512 images/sec @ 20 DDIM steps).
+"""bench.py — headline benchmark of the hot path (512x512 images/sec @ 20 DDIM steps).
 
   python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (one process per GPU)
   python bench.py --impl reference --steps K --warmup W    # reference arm: CPU port (oracle/) on the host cores
+  python bench.py --steps K --dump-outputs DIR             # also write what the last timed step returned to DIR/*.npy
 
 A "step" is one pass of the hot path over one batch: StableDiffusion::sample_image for `--batch` images
-(20 DDIM steps x (cond+uncond UNet) + VAE decode + u8 pack). Default workload = BASELINE configs[1]
-(batch 1, 512x512, 20 steps, cfg 7.5) on every rank (weak scaling: per-GPU work is fixed).
+(20 DDIM steps x (cond+uncond UNet) + VAE decode + u8 pack). Default workload: batch 1, 512x512, 20 steps, cfg 7.5 on every rank (weak scaling: per-GPU work is fixed).
 Prints ONE JSON line on rank 0.
 """
 import argparse
@@ -27,34 +27,40 @@ FLOP_PER_IMAGE = 34_695e9  # algorithmic, SURVEY §8d: 40 x 804.4 + 2518.4 GFLOP
 
 
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            p = json.load(f)
-        return dict(tflops=float(p["bf16_tflops_sustained"]), tflops_burst=float(p["bf16_tflops"]), hbm=float(p["hbm_gbs"]), src="measured")
-    except Exception:
-        return dict(tflops=1400.0, tflops_burst=1590.0, hbm=6650.0, src="fallback")
+    """Dense fp16 tensor rate and HBM3 bandwidth of the H100 SXM data sheet (a card allowed 700 W; a lower power limit lowers the
+    clocks the tensor rate assumes). The roofline's `frac` is a share of this figure, not of a measured peak."""
+    return dict(tflops=989.0, hbm=3350.0, src="H100 SXM data sheet, dense fp16")
 
 
-def gemm_traffic_per_launch():
-    """DRAM bytes per gemm_tc launch from the committed ncu capture (profiles/r2_gemm_traffic.json, else round 1's), or None."""
-    for name in ("r2_gemm_traffic.json", "r1_gemm_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                return float(json.load(f)["traffic_bytes_per_launch"])
-        except Exception:
-            continue
-    return None
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(dirname, arrays):
+    """Writes each array as DIR/<name>.npy in float32; an array larger than the 64 MB budget is replaced by a fixed, seeded sample
+    of its flattened elements (the same indices in every run), stored beside them as <name>_index.npy. Returns what was
+    written, for the JSON line."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float32)
+        if a.nbytes > DUMP_LIMIT_BYTES // len(arrays):
+            k = DUMP_LIMIT_BYTES // len(arrays) // 16
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=k, replace=False)).astype(np.float64)
+            np.save(os.path.join(dirname, f"{name}_index.npy"), idx)
+            a = a.reshape(-1)[idx.astype(np.int64)]
+        np.save(os.path.join(dirname, f"{name}.npy"), a)
+    return {"dir": dirname, "arrays": sorted(arrays), "rank": int(os.environ.get("RANK", "0"))}
 
 
 def workload_config(args, n):
     """`config` of the JSON line — identical in both arms (the reference arm runs on this arm's config)."""
     return {"workload": f"SDv1-4 txt2img {args.size}x{args.size}, {args.ddim_steps} steps, cfg=7.5, batch={n} per GPU",
             "context_len": args.context_len, "precision_option": args.precision,
-            "l2": "inputs larger than L2: >1.9 GB of packed weights stream from HBM every UNet step (L2 = 126 MB)"}
+            "l2": "inputs larger than L2: >1.9 GB of packed weights stream from HBM every UNet step (H100 L2 = 50 MB)"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries, one process for the whole run)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -114,7 +120,8 @@ GF_DEC_64, GF_DEC_32 = 2518.4, 631.6
 def cpu_port_times(n_steps=1, latent=64, ddim_steps_total=20):
     """Times the CPU port of the reference path (oracle/, torch fp32 on the host cores): `n_steps` REAL DDIM steps (cond + uncond
     UNet at the full latent size, L = 77 / Lu = 2, the timesteps a `ddim_steps_total`-step schedule starts with) and one REAL
-    decode_latent. Nothing is extrapolated. Returns (seconds per DDIM step [list], seconds per decode, threads, description)."""
+    decode_latent. Nothing is extrapolated. Returns (seconds per DDIM step [list], seconds per decode, threads, description,
+    {"latent": what the last step returned, "decoded": what the decode returned})."""
     import torch
 
     from oracle import sd_oracle as O
@@ -131,13 +138,13 @@ def cpu_port_times(n_steps=1, latent=64, ddim_steps_total=20):
         steps = []
         for i in range(n_steps):
             t0 = time.perf_counter()
-            O.forward_diffuser(P, lat, ts[i % len(ts)], ctx, unc, 7.5)
+            out = O.forward_diffuser(P, lat, ts[i % len(ts)], ctx, unc, 7.5)
             steps.append(time.perf_counter() - t0)
         t0 = time.perf_counter()
-        O.decode_latent(P, lat * (1.0 / 0.18215))
+        img = O.decode_latent(P, lat * (1.0 / 0.18215))
         dec = time.perf_counter() - t0
     what = f"{n_steps} real {latent}x{latent} DDIM step(s) (cond+uncond UNet, L=77/Lu=2) + 1 real decode_latent, timed directly on {threads} threads"
-    return steps, dec, threads, what
+    return steps, dec, threads, what, {"latent": out.numpy(), "decoded": img.numpy()}
 
 
 def gpu_eager_times():
@@ -183,7 +190,8 @@ def run_reference(args):
     if rank != 0:
         return
     total = args.warmup + args.steps
-    step_s, dec, threads, what = cpu_port_times(total, latent=args.size // 8, ddim_steps_total=args.ddim_steps)
+    step_s, dec, threads, what, outs = cpu_port_times(total, latent=args.size // 8, ddim_steps_total=args.ddim_steps)
+    dumped = dump_outputs(args.dump_outputs, outs) if args.dump_outputs else None
     timed = step_s[args.warmup:]
     mean_step = sum(timed) / len(timed)
     img_s = args.ddim_steps * mean_step + dec
@@ -199,6 +207,7 @@ def run_reference(args):
                          "sample": f"{what} ({mean_step:.2f} s/step, decode {dec:.2f} s)"},
         "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
+        "dumped_outputs": dumped,
     }
     if args.ref_cuda:
         try:
@@ -222,6 +231,10 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-profile", action="store_true")
     ap.add_argument("--no-c5", action="store_true", help="multi-GPU runs: skip the BASELINE configs[4] sub-record (8 images per rank)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned as float32 .npy files in DIR: the u8 images "
+                         "(images.npy) of rank 0 only, or with --impl reference the DDIM step's latent and the decoded image "
+                         "(latent.npy, decoded.npy); the inputs are seeded, so two builds can be compared output for output")
     ap.add_argument("--ref-cuda", action="store_true",
                     help="with --impl reference: also time the torch restatement on cuda:0 (labelled secondary comparator)")
     args = ap.parse_args()
@@ -289,10 +302,10 @@ def main():
             # the public host-buffer call: H2D of context/uncond/latent, sampling, D2H of the u8 images — all inside
             ctx.check(ctx.lib.sdb_sample_image(ctx.h, _lib.ptr(p_ctx.numpy()), n, L, _lib.ptr(p_unc.numpy()), Lu, 7.5, args.ddim_steps,
                                                _lib.ptr(p_lat.numpy()), 0, Hl, Hl, p_rgb.numpy().ctypes.data_as(_lib._u8p)))
-        return dev_step, e2e_step, int(h_ctx.nbytes + h_unc.nbytes + h_lat.nbytes), int(p_rgb.numel())
+        return dev_step, e2e_step, int(h_ctx.nbytes + h_unc.nbytes + h_lat.nbytes), int(p_rgb.numel()), d_rgb
 
     n = args.batch
-    step_dev, step_e2e, h2d, d2h = make_steps(n)
+    step_dev, step_e2e, h2d, d2h, out_rgb = make_steps(n)
 
     def barrier():
         torch.cuda.synchronize()
@@ -327,6 +340,9 @@ def main():
     launches = ctx.launch_count() - l0
     clocks = sampler.window(w0, w1) if rank == 0 else None
     value = world * n * args.steps / (ms * 1e-3)
+    dumped = None
+    if args.dump_outputs and rank == 0:
+        dumped = dump_outputs(args.dump_outputs, {"images": out_rgb.cpu().numpy()})
 
     # ---- end to end through the host-buffer C ABI
     step_e2e()
@@ -343,7 +359,7 @@ def main():
     # the same call with 8 images per rank (world * 8 images per step), its own clocks sample; the headline stays configs[1]
     c5 = None
     if world > 1 and args.batch != 8 and not args.no_c5:
-        c5_dev, c5_e2e, c5_h2d, c5_d2h = make_steps(8)
+        c5_dev, c5_e2e, c5_h2d, c5_d2h, _ = make_steps(8)
         for _ in range(2):
             c5_dev()
         k5 = max(2, min(args.steps, 5))
@@ -371,9 +387,9 @@ def main():
         pk = peaks()
         tot_ms = sum(v["ms"] for v in classes.values())
         ach = g["flops"] / (g["ms"] * 1e-3) / 1e12 if g["ms"] > 0 else 0.0
-        roof = {"bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05 implicit GEMM, all conv/linear layers of one sample_image)",
-                "achieved": ach, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": ach / pk["tflops"], "peak_source": pk["src"] + " bf16 cuBLAS sustained (same tensor rate as fp16)",
-                "traffic": gemm_traffic_per_launch(), "algorithmic_bytes_per_launch": g["bytes"] / max(1, g["launches"]),
+        roof = {"bound": "tensor", "kernel": "gemm_tc_kernel (wgmma implicit GEMM, all conv/linear layers of one sample_image)",
+                "achieved": ach, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": ach / pk["tflops"], "peak_source": pk["src"],
+                "algorithmic_bytes_per_launch": g["bytes"] / max(1, g["launches"]),
                 "launches": g["launches"], "avg_launch_us": g["ms"] * 1e3 / max(1, g["launches"]),
                 "algorithmic_tflop_per_step": g["flops"] / 1e12, "issued_tflop_per_step": g["issued_flops"] / 1e12,
                 # share of the REPLAYED step (the timed value), from event-bracketed launches: an upper bound, each bracket
@@ -383,7 +399,7 @@ def main():
 
     cpu = None
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
-        step_s, dec, threads, what = cpu_port_times(1, latent=Hl, ddim_steps_total=args.ddim_steps)
+        step_s, dec, threads, what, _ = cpu_port_times(1, latent=Hl, ddim_steps_total=args.ddim_steps)
         cpu_img_s = args.ddim_steps * step_s[0] + dec
         cpu = {"value": 1.0 / cpu_img_s, "unit": UNIT, "cores": threads, "kind": "port",
                "sample": f"{what}; {step_s[0]:.2f} s/step x {args.ddim_steps} + decode {dec:.2f} s = {cpu_img_s:.1f} s/image"}
@@ -404,6 +420,7 @@ def main():
             "cpu_baseline": cpu,
             "kernel_classes": classes,
             "weights_broadcast_ms": bcast_ms,
+            "dumped_outputs": dumped,
         }
         if c5 is not None:
             line["c5"] = c5

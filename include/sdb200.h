@@ -1,5 +1,5 @@
 /*
- * sdb200.h — C ABI of the B200-native Stable Diffusion v1.4 sampling path.
+ * sdb200.h — C ABI of the H100-native Stable Diffusion v1.4 sampling path.
  *
  * Drop-in boundary for the hot path of Gadersd/stable-diffusion-burn (reference @ 893fb095):
  * these entry points are what a Rust FFI shim binds in place of the Burn tensor graph in
@@ -36,7 +36,7 @@ int sdb_create(int device, sdb_ctx** out);
 int sdb_destroy(sdb_ctx* ctx);
 /* ctx may be NULL: returns the last error of the calling thread (e.g. a failed sdb_create). */
 const char* sdb_last_error(sdb_ctx* ctx);
-/* "sdb200 <version> sm_100a" */
+/* "sdb200 <version> sm_90a" */
 const char* sdb_version(void);
 
 /* ---- weights -------------------------------------------------------------------------- */
@@ -137,7 +137,7 @@ int sdb_sample_image_dev(sdb_ctx* ctx, const float* d_context, int n, int L, con
  * "graphs" = 0|1 (CUDA-graph replay of the UNet step), "splitk" = 0|1. A/B switches of measured design choices (defaults are the
  * measured-faster settings; results do not change beyond rounding, the first two not at all): "emb_hoist" (time-embedding rows of
  * all timesteps once per sample call), "attn_regsplit" (setmaxnreg build of the attention kernel), "attn_split" (fp16 hi + lo
- * q / k on the 3-pass levels), "prefetch_w", "cluster", "pair_bn256", "raw16", "skip_merge", "gn_epilogue", "mlp_passes",
+ * q / k on the 3-pass levels), "prefetch_w", "raw16", "skip_merge", "gn_epilogue", "mlp_passes",
  * "splitk_min_iters", "splitk_chunk", "gn_apply_ctas", "gn_min_pix". Unknown keys are an error. */
 int sdb_set_option(sdb_ctx* ctx, const char* key, int value);
 /* Per-kernel-class timing: when enabled, every launch is bracketed by CUDA events on the
@@ -155,7 +155,7 @@ int64_t sdb_launch_count(sdb_ctx* ctx);
 
 /* ---- unit-test entry points for single kernels (device pointers) ----------------------------- */
 /* C[M,N] (fp32) = A[M,K] (fp32, rounded to the operand format) x B[K,N] (fp32 [in,out]) + bias.
- * Exercises the tcgen05 GEMM exactly as the Linear layers use it. */
+ * Exercises the wgmma GEMM exactly as the Linear layers use it. */
 int sdb_test_linear(sdb_ctx* ctx, const float* a, const float* w, const float* bias, int M, int K, int N,
                     int passes, float* c);
 /* The GEMM's other epilogues and K-loop forms, each reachable in isolation: out = A[M,K] x W[K,N] (+ bias) (+ residual[M,N])

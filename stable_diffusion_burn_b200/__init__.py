@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) Stable Diffusion v1.4 sampling hot path behind the reference's interface.
+"""H100-native (sm_90a) Stable Diffusion v1.4 sampling hot path behind the reference's interface.
 
 Product code lives in csrc/ (CUDA kernels + C ABI, built into libsdb200.so); this package is the
 thin Python host side mirroring the reference's Rust signatures (pipeline.py). The CPU oracle

@@ -92,7 +92,7 @@ void nccl_check(int rc, const char* what) {
 
 extern "C" {
 
-const char* sdb_version(void) { return "sdb200 0.2.0 sm_100a"; }
+const char* sdb_version(void) { return "sdb200 0.2.0 sm_90a"; }
 
 int sdb_create(int device, sdb_ctx** out) {
   if (!out) {
@@ -111,15 +111,14 @@ int sdb_create(int device, sdb_ctx** out) {
     SDB_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     SDB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
+    if (prop.major != 9 || prop.minor != 0)
       throw Error(std::string("device is sm_") + std::to_string(prop.major) + std::to_string(prop.minor) +
-                  "; kernels are built for sm_100a only");
+                  "; kernels are built for sm_90a only");
+    g_num_sms = prop.multiProcessorCount;
     h = new sdb_ctx();
     h->c.device = device;
     h->c.debug_sync = getenv("SDB_DEBUG_SYNC") && atoi(getenv("SDB_DEBUG_SYNC")) != 0;
-    if (getenv("SDB_CLUSTER")) h->c.opt_cluster = atoi(getenv("SDB_CLUSTER"));
     if (getenv("SDB_PDL")) g_pdl_enabled = atoi(getenv("SDB_PDL")) != 0, g_pdl_late = atoi(getenv("SDB_PDL")) == 2;
-    if (getenv("SDB_PAIR_BN256")) h->c.opt_pair_bn256 = atoi(getenv("SDB_PAIR_BN256"));
     SDB_CUDA(cudaStreamCreateWithFlags(&h->c.stream, cudaStreamNonBlocking));
     model_create(h->c);
     *out = h;
@@ -405,10 +404,6 @@ int sdb_set_option(sdb_ctx* ctx, const char* key, int value) {
     c.opt_graphs = value;
   else if (k == "splitk")
     c.opt_splitk = value;
-  else if (k == "cluster")
-    c.opt_cluster = value;
-  else if (k == "pair_bn256")
-    c.opt_pair_bn256 = value;
   else if (k == "raw16")
     c.opt_raw16 = value;
   else if (k == "splitk_min_iters")

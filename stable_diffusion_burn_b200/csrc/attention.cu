@@ -1,17 +1,13 @@
-// attention.cu — fused QK^T . softmax . PV on tcgen05 (flash-style streaming softmax, no N^2 tensor in HBM).
+// attention.cu — fused QK^T . softmax . PV on wgmma (flash-style streaming softmax, no N^2 tensor in HBM).
 //
 // Replaces qkv_attention (reference src/model/attention.rs:5-45 == src/backend.rs:88-128, mask = None):
 //   softmax((q d^-1/4)(k d^-1/4)^T) v  ==  softmax(q k^T d^-1/2) v.
 //
-// One CTA = NG x 128 query rows of one (sample, head); NG = 2 query tiles ping-pong on one K/V stream
-// (while the softmax warps of tile 0 run their exponentials, the tensor pipe works for tile 1, and the K/V
-// tiles are fetched from L2 once for 256 query rows). Warp roles:
-//   warp 0          : TMA producer — Q tiles once, then K tiles [128 keys][d] and V^T tiles [d][128 keys]
-//   warp 1          : TMEM allocator + tcgen05.mma issuer: S_g = Q_g K^T (fp32 in TMEM), O_g += P_g V
-//   warps 2..2+4*NG : softmax groups — one query row per thread: tcgen05.ld S, running max/sum in fp32
-//                     (exp2 with the d^-1/2 scale folded in), lazy O rescale in TMEM, P written as fp16
-//                     into 128B-swizzled smem
-// S_g(j+1) is issued as soon as the group has copied S_g(j) to registers, so QK^T overlaps the exponentials.
+// One CTA = 128 query rows of one (sample, head). Warp roles:
+//   warpgroup 0    : TMA producer (warp 0) — the Q tile once, then K tiles [128 keys][d] and V tiles through an ST-stage ring
+//   warpgroups 1-2 : 64 query rows each. S = Q K^T with wgmma (Q and K from shared memory, S in registers: m64n128), running
+//                    max / sum in fp32 (exp2 with the d^-1/2 scale folded in), P converted in registers to the A fragment of
+//                    O += P V (wgmma with A from registers, O in registers), lazy O rescale, O / l written as fp16 hi(/lo)
 #include "attention.cuh"
 
 #include <type_traits>
@@ -25,7 +21,7 @@ namespace sdb {
 //              the GEMMs): the logits are fp32-class. With single fp16 operands a logit of magnitude ~30 (peaked softmax of a
 //              trained checkpoint) carries an absolute error ~1e-2, i.e. ~1 % on the dominant probabilities — the largest
 //              single error source of a UNet step on realistic-statistics weights (tests/test_realstats_gpu.py).
-template <int DPAD, int NG, bool VMN = false, bool QK3 = false>
+template <int DPAD, bool VMN = false, bool QK3 = false>
 struct AttnCfg {
   static constexpr int DC = (DPAD + 63) / 64;                          // 64-wide chunks of the head dim
   static constexpr int QK_PARTS = QK3 ? 2 : 1;                          // hi (+ lo) copies of the Q and K tiles
@@ -36,23 +32,10 @@ struct AttnCfg {
   static constexpr int V_CHUNK = VMN ? 128 * 128 : ((DPAD * 128 + 1023) / 1024) * 1024;   // VMN: [128 keys][64 ch]; else [DPAD rows][64 keys]
   static constexpr int V_BYTES = (VMN ? DC : 2) * V_CHUNK;
   static constexpr int V_TX = VMN ? DC * 128 * 128 : 2 * DPAD * 128;    // bytes one V stage receives
-  // P (the exponentials, fp16) goes to the PV product either through a swizzled shared-memory tile or — when the tensor memory has
-  // room for 64 more columns per query tile — through TENSOR MEMORY as the A operand of tcgen05.mma: each softmax thread stores
-  // its own row (128 fp16 = 64 columns of its lane) with tcgen05.st, no swizzle, no generic->async proxy fence, and the P tile
-  // (32 KB written + 32 KB read per query tile and key tile) leaves shared memory, whose bandwidth bounded the d = 40 kernel
-  // (QK^T + PV operands + P + TMA = 344 KB per key tile at 128 B/clk; profiles/r2_attention_timeline_after_elect_2stages.log)
-  static constexpr bool PT = NG * (128 + DPAD + 64) <= 512;
-  static constexpr int P_TILE = PT ? 0 : 2 * 128 * 128;                 // [128 rows][128 keys] fp16
-  static constexpr int FIXED = NG * (Q_TILE + P_TILE) + 512 + 1024;
-  // K/V pipeline stages: two when they fit beside the 1 KB of static shared memory (227 KB per CTA = 226 KB dynamic). The split-q/k
-  // d = 40 pair-of-query-tiles variant needs 225.5 KB for two: with ONE stage the MMA warp waited ~690 clk per key tile for K(j+1)
-  // (clock64 timeline, profiles/r2_attention_timeline_before.log)
+  static constexpr int FIXED = Q_TILE + 512 + 1024;
+  // K/V pipeline stages: two when they fit in the 227 KB of shared memory a block may use
   static constexpr int ST = (FIXED + 2 * (K_BYTES + V_BYTES) <= 226 * 1024) ? 2 : 1;
   static constexpr int SMEM = FIXED + ST * (K_BYTES + V_BYTES);
-  static constexpr int TMEM_NEED = NG * (128 + DPAD + (PT ? 64 : 0));
-  static constexpr int P_COL0 = NG * (128 + DPAD);                      // first P column (PT)
-  static constexpr int TMEM_COLS = TMEM_NEED <= 256 ? 256 : 512;
-  static_assert(TMEM_NEED <= 512, "TMEM budget");
   static_assert(SMEM <= 226 * 1024, "smem budget");
 };
 
@@ -61,44 +44,38 @@ __device__ __forceinline__ float ex2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
 
-// RS = true (register split, NG = 2 only): the block is padded to three full warpgroups — warps 0-3 = TMA producer, MMA issuer and
-// two idle warps, warps 4-11 = the two softmax groups — so that setmaxnreg can move registers between them: the first warpgroup
-// drops to 56 registers per thread, the softmax warpgroups rise to 224. With 10 warps ptxas budgets 65536 / 384 = 168 registers
-// per thread (allocation is per 4 warps) and the 128 score registers of a softmax thread left 12 values spilled to local memory,
-// ~20 reloads per key tile inside the exponentials loop (LDL in the SASS; ncu: long-scoreboard the top stall).
-template <int DPAD, int NG, bool VMN, bool QK3, bool RS>
-__global__ void __launch_bounds__((RS ? 128 : 64) + 128 * NG, 1)
+// RS = true (register split): setmaxnreg moves registers from the producer warpgroup (down to 40 per thread) to the two softmax
+// warpgroups (up to 232). Without it ptxas budgets 65536 / 384 = 168 registers per thread for every role.
+template <int DPAD, bool VMN, bool QK3, bool RS>
+__global__ void __launch_bounds__(384, 1)
 attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ CUtensorMap mk,
                  const __grid_constant__ CUtensorMap mv, const __grid_constant__ CUtensorMap mq_lo,
                  const __grid_constant__ CUtensorMap mk_lo, const AttnParams p) {
-  using Cfg = AttnCfg<DPAD, NG, VMN, QK3>;
+  using Cfg = AttnCfg<DPAD, VMN, QK3>;
   constexpr int DC = Cfg::DC, ST = Cfg::ST;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                              // NG tiles
-  uint8_t* sP = sQ + NG * Cfg::Q_TILE;             // NG tiles
-  uint8_t* sK = sP + NG * Cfg::P_TILE;             // ST stages
+  uint8_t* sQ = smem;
+  uint8_t* sK = sQ + Cfg::Q_TILE;                  // ST stages
   uint8_t* sV = sK + ST * Cfg::K_BYTES;            // ST stages
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + ST * Cfg::V_BYTES);
   uint64_t* q_full = bars;             // 1
   uint64_t* k_full = q_full + 1;       // ST
-  uint64_t* k_empty = k_full + ST;     // ST
+  uint64_t* k_empty = k_full + ST;     // ST (one arrival per softmax warp)
   uint64_t* v_full = k_empty + ST;     // ST
-  uint64_t* v_empty = v_full + ST;     // ST
-  uint64_t* s_full = v_empty + ST;     // NG
-  uint64_t* s_free = s_full + NG;      // NG (128 arrivals each)
-  uint64_t* p_full = s_free + NG;      // NG (128 arrivals each)
-  uint64_t* pv_done = p_full + NG;     // NG
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + NG);
+  uint64_t* v_empty = v_full + ST;     // ST (one arrival per softmax warp)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int SW0 = RS ? 4 : 2;  // first softmax warp
   long long* const dbg = (p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) ? p.dbg : nullptr;
   constexpr int DJ0 = 8;  // stamped key tiles: DJ0 .. DJ0+3
   if (dbg && threadIdx.x == 0) dbg[255] = clock64();
   pdl_trigger();
-  const int q0 = blockIdx.x * (128 * NG);
+  const int q0 = blockIdx.x * 128;
   const int h = blockIdx.y;
   const int s = blockIdx.z;
 
@@ -106,15 +83,9 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
     mbar_init(q_full, 1);
     for (int i = 0; i < ST; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
+      mbar_init(&k_empty[i], 8);
       mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
-    }
-    for (int g = 0; g < NG; ++g) {
-      mbar_init(&s_full[g], 1);
-      mbar_init(&s_free[g], 128);
-      mbar_init(&p_full[g], 128);
-      mbar_init(&pv_done[g], 1);
+      mbar_init(&v_empty[i], 8);
     }
     fence_mbar_init();
   }
@@ -123,37 +94,23 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
     tma_prefetch_desc(&mk);
     tma_prefetch_desc(&mv);
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
   // a device-side length of 0 (or beyond Nk) would leave T = 0 and the epilogue waiting forever: clamp to [1, Nk]
   const int kvlen = p.kvlen ? max(1, min(p.kvlen[s], p.Nk)) : p.Nk;
   const int T = (kvlen + 127) / 128;
-  // columns: S_g at g*128 ; O_g at NG*128 + g*DPAD
 
   // (setmaxnreg sits INSIDE the role branches: ptxas budgets the code after a join with the smaller of the two limits)
-  if (warp < SW0) {
-  if (RS) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-  if (warp == 0) {
+  if (warp < 4) {
+    if (RS) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     // ======================================================================= TMA producer
-    if (elect_one()) {
-      mbar_expect_tx(q_full, NG * Cfg::Q_TILE);
+    if (warp == 0 && elect_one()) {
+      mbar_expect_tx(q_full, Cfg::Q_TILE);
 #pragma unroll
-      for (int g = 0; g < NG; ++g)
-#pragma unroll
-        for (int c = 0; c < DC; ++c) {
-          tma_load_2d(sQ + g * Cfg::Q_TILE + c * 16384, &mq, q_full, p.q_col0 + h * DPAD + c * 64,
-                      s * p.q_rows_per_sample + q0 + g * 128);
-          if (QK3)
-            tma_load_2d(sQ + g * Cfg::Q_TILE + Cfg::Q_HALF + c * 16384, &mq_lo, q_full, p.q_col0 + h * DPAD + c * 64,
-                        s * p.q_rows_per_sample + q0 + g * 128);
-        }
+      for (int c = 0; c < DC; ++c) {
+        tma_load_2d(sQ + c * 16384, &mq, q_full, p.q_col0 + h * DPAD + c * 64, s * p.q_rows_per_sample + q0);
+        if (QK3) tma_load_2d(sQ + Cfg::Q_HALF + c * 16384, &mq_lo, q_full, p.q_col0 + h * DPAD + c * 64, s * p.q_rows_per_sample + q0);
+      }
       for (int j = 0; j < T; ++j) {
         const int st = j % ST;
         const uint32_t ph = (j / ST) & 1;
@@ -182,285 +139,211 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // ======================================================================= MMA issuer
-    constexpr uint32_t idesc_s = make_idesc_f16(128, 128);
-    constexpr uint32_t idesc_o = make_idesc_f16(128, DPAD, false, /*b_mn_major=*/VMN);
-    auto mstamp = [&](int j, int g, int k) {
-      if (dbg && lane == 0 && j >= DJ0 && j < DJ0 + 4) dbg[128 + (j - DJ0) * 16 + g * 8 + k] = clock64();
+  } else {
+    if (RS) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // ======================================================================= softmax warpgroups + epilogue
+    // accumulator layout of m64nN (see Wgmma in common.cuh): this thread holds rows rw + 8 hh (hh = 0, 1) of the warpgroup's
+    // 64, columns 8 (i / 4) + 2 (lane % 4) + i % 2 of element i, with hh = (i / 2) % 2
+    const int wg = (warp - 4) >> 2;
+    const int rw = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // row inside the CTA's 128
+    const int cl = 2 * (lane & 3);
+    const float sl2 = p.scale * 1.4426950408889634f;  // d^-1/2 * log2(e)
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    float o[DPAD / 2];
+#pragma unroll
+    for (int i = 0; i < DPAD / 2; ++i) o[i] = 0.f;
+    auto sstamp = [&](int j, int k) {
+      if (dbg && threadIdx.x == 128 && j >= DJ0 && j < DJ0 + 4) dbg[(j - DJ0) * 8 + k] = clock64();
     };
-    auto issue_qk = [&](int g, int j) {
+    const uint32_t qa = smem_u32(sQ) + wg * (64 * 128);
+    // keys per S sub-tile: the 128-key tile in one m64n128 product, or for d = 160 in two m64n64 halves (S, P and O of a 128-key
+    // product do not fit the registers beside an 80-register O: the wgmma would be serialised and the thread would spill)
+    constexpr int KW = DPAD > 128 ? 64 : 128, NSUB = 128 / KW;
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < T; ++j) {
       const int st = j % ST;
-      mstamp(j - 1, g, 0);
-      if (g == 0) mbar_wait(&k_full[st], (j / ST) & 1);
-      mstamp(j - 1, g, 4);
-      if (j > 0) mbar_wait(&s_free[g], (j - 1) & 1);  // group g has copied S_g(j-1) out of TMEM
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t qa = smem_u32(sQ + g * Cfg::Q_TILE), ka = smem_u32(sK + st * Cfg::K_BYTES);
+      const uint32_t ph = (j / ST) & 1;
+      sstamp(j, 0);
+      mbar_wait(&k_full[st], ph);
+      sstamp(j, 1);
+      int valid_tile[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        valid_tile[hh] = min(128, kvlen - j * 128);
+        if (p.causal) valid_tile[hh] = max(1, min(valid_tile[hh], q0 + rw + 8 * hh - j * 128 + 1));  // additive -inf mask above the diagonal
+      }
+#pragma unroll 1
+      for (int sub = 0; sub < NSUB; ++sub) {
+        float sv[KW / 2];
+#pragma unroll
+        for (int i = 0; i < KW / 2; ++i) sv[i] = 0.f;
+        const uint32_t ka = smem_u32(sK + st * Cfg::K_BYTES) + sub * KW * 128;  // key rows [sub KW, sub KW + KW) of the tile
+        wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < DPAD / 16; ++kk) {
           const uint32_t off = (kk / 4) * 16384 + (kk % 4) * 32;
-          umma_f16(tmem_base + g * 128, make_sdesc_sw128(qa + off), make_sdesc_sw128(ka + off), idesc_s, kk > 0 ? 1u : 0u);
+          Wgmma<KW>::template ss<0>(sv, make_sdesc_sw128(qa + off), make_sdesc_sw128(ka + off), 1);
           if (QK3) {  // + q_lo k_hi^T + q_hi k_lo^T
-            umma_f16(tmem_base + g * 128, make_sdesc_sw128(qa + Cfg::Q_HALF + off), make_sdesc_sw128(ka + off), idesc_s, 1u);
-            umma_f16(tmem_base + g * 128, make_sdesc_sw128(qa + off), make_sdesc_sw128(ka + Cfg::K_HALF + off), idesc_s, 1u);
+            Wgmma<KW>::template ss<0>(sv, make_sdesc_sw128(qa + Cfg::Q_HALF + off), make_sdesc_sw128(ka + off), 1);
+            Wgmma<KW>::template ss<0>(sv, make_sdesc_sw128(qa + off), make_sdesc_sw128(ka + Cfg::K_HALF + off), 1);
           }
         }
-        if (g == NG - 1) umma_commit(&k_empty[st]);  // the K stage is free once the last group's QK retires
-        umma_commit(&s_full[g]);
-      }
-      __syncwarp();
-      mstamp(j - 1, g, 1);
-    };
-    mbar_wait(q_full, 0);
-    for (int g = 0; g < NG; ++g) issue_qk(g, 0);
-    for (int j = 0; j < T; ++j) {
-      const int st = j % ST;
-      for (int g = 0; g < NG; ++g) {
-        // S_g(j+1) first: it only needs the group to have copied S_g(j) out of TMEM, so it runs while the group is
-        // still in its exponentials and the next softmax never waits for the tensor pipe
-        if (j + 1 < T) issue_qk(g, j + 1);
-        if (g == 0) mbar_wait(&v_full[st], (j / ST) & 1);
-        mstamp(j, g, 5);
-        mbar_wait(&p_full[g], j & 1);
-        mstamp(j, g, 2);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t pa = smem_u32(sP + g * Cfg::P_TILE), va = smem_u32(sV + st * Cfg::V_BYTES);
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(sv);
+        if (sub == NSUB - 1 && lane == 0) mbar_arrive(&k_empty[st]);
+        if (sub == 0) sstamp(j, 2);
+        int valid[2];  // valid keys of this sub-tile per row (<= 0: none)
 #pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {
-            const uint32_t poff = (kk / 4) * 16384 + (kk % 4) * 32;
-            // K-major V^T: 16 keys = 32 bytes inside a 128-byte row; MN-major V: 16 keys = 16 rows of 128 bytes
-            const uint32_t voff = VMN ? kk * 2048 : (kk / 4) * Cfg::V_CHUNK + (kk % 4) * 32;
-            const uint64_t vdesc = VMN ? make_sdesc_sw128_mn(va + voff, Cfg::V_CHUNK) : make_sdesc_sw128(va + voff);
-            if (Cfg::PT)  // A = P in tensor memory: 16 keys = 8 columns
-              umma_f16_ts(tmem_base + NG * 128 + g * DPAD, tmem_base + Cfg::P_COL0 + g * 64 + kk * 8, vdesc, idesc_o,
-                          (j > 0 || kk > 0) ? 1u : 0u);
-            else
-              umma_f16(tmem_base + NG * 128 + g * DPAD, make_sdesc_sw128(pa + poff), vdesc, idesc_o, (j > 0 || kk > 0) ? 1u : 0u);
-          }
-          if (g == NG - 1) umma_commit(&v_empty[st]);
-          umma_commit(&pv_done[g]);
+        for (int hh = 0; hh < 2; ++hh) valid[hh] = valid_tile[hh] - sub * KW;
+        const bool full = valid[0] >= KW && valid[1] >= KW;
+        // 4 independent max chains per row, then the 4 lanes that share a row
+        float mxa[2][4];
+#pragma unroll
+        for (int a = 0; a < 4; ++a) mxa[0][a] = mxa[1][a] = -INFINITY;
+#pragma unroll
+        for (int i = 0; i < KW / 2; ++i) {
+          const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + cl + (i & 1);
+          if (full || col < valid[hh]) mxa[hh][(i >> 2) & 3] = fmaxf(mxa[hh][(i >> 2) & 3], sv[i]);
         }
-        __syncwarp();
-        mstamp(j, g, 3);
-      }
-    }
-  }
-  } else {
-    if (RS) asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    // ======================================================================= softmax groups + epilogue
-    const int g = (warp - SW0) >> 2;
-    const int qd = warp & 3;
-    const int r = qd * 32 + lane;
-    const uint32_t lane_sel = uint32_t(qd * 32) << 16;
-    const uint32_t tS = tmem_base + g * 128 + lane_sel;
-    const uint32_t tO = tmem_base + NG * 128 + g * DPAD + lane_sel;
-    uint8_t* prow = sP + g * Cfg::P_TILE + r * 128;
-    const uint32_t tP = tmem_base + Cfg::P_COL0 + g * 64 + lane_sel;  // this row's 64 P columns (PT)
-    const float sl2 = p.scale * 1.4426950408889634f;  // d^-1/2 * log2(e)
-    float m_run = -INFINITY, l_run = 0.f;
-    auto sstamp = [&](int j, int k) {
-      if (dbg && qd == 0 && lane == 0 && j >= DJ0 && j < DJ0 + 4) dbg[g * 64 + (j - DJ0) * 8 + k] = clock64();
-    };
-    for (int j = 0; j < T; ++j) {
-      sstamp(j, 0);
-      mbar_wait(&s_full[g], j & 1);
-      sstamp(j, 1);
-      tc_fence_after();
-      uint32_t sv[128];
+        float m_new[2], alpha[2];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) tmem_ld32(tS + c * 32, *reinterpret_cast<uint32_t(*)[32]>(&sv[c * 32]));
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&s_free[g]);
-      sstamp(j, 2);
-      int valid = min(128, kvlen - j * 128);
-      if (p.causal) valid = max(1, min(valid, q0 + g * 128 + r - j * 128 + 1));  // additive -inf mask above the diagonal
-      // 8 independent max chains (a single chain of 128 dependent FMNMX would cost ~500 cycles of pure latency)
-      float mxa[8];
-#pragma unroll
-      for (int a = 0; a < 8; ++a) mxa[a] = -INFINITY;
-      if (valid == 128) {
-#pragma unroll
-        for (int i = 0; i < 128; ++i) mxa[i & 7] = fmaxf(mxa[i & 7], __uint_as_float(sv[i]));
-      } else {
-#pragma unroll
-        for (int i = 0; i < 128; ++i)
-          if (i < valid) mxa[i & 7] = fmaxf(mxa[i & 7], __uint_as_float(sv[i]));
-      }
-      const float mx = fmaxf(fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3])), fmaxf(fmaxf(mxa[4], mxa[5]), fmaxf(mxa[6], mxa[7])));
-      // Lazy rescale with a threshold: the running maximum is only a reference point (softmax is shift invariant), so it is moved —
-      // and O_g / l rescaled — only when a row's maximum grew by more than 2^8; otherwise the tile is exponentiated against the
-      // stale reference and P may reach 256 (exact in fp16, fp32 sums). With a plain `m_new > m_run` test one of the 32 rows of
-      // a warp has a new maximum in ~97 % of the key tiles, i.e. the "lazy" rescale ran (3 x tcgen05.ld/st of O, ~340 clk) on
-      // almost every tile (clock64 timeline, profiles/r2_attention_timeline_p_in_tmem.log).
-      const float m_cand = fmaxf(m_run, mx * sl2);
-      const bool resc = __any_sync(0xffffffffu, m_cand > m_run + 8.0f);  // first tile: m_run = -inf -> true
-      const float m_new = resc ? m_cand : m_run;
-      const float alpha = resc ? ex2(m_run - m_new) : 1.0f;  // 0 on the first tile
-      sstamp(j, 3);
-      if (j > 0) {
-        mbar_wait(&pv_done[g], (j - 1) & 1);  // O_g holds PV(j-1); the P buffer is free again
-        sstamp(j, 4);
-        tc_fence_after();
-        if (resc) {
-#pragma unroll
-          for (int c = 0; c < DPAD; c += 16) {
-            uint32_t o[16];
-            tmem_ld16(tO + c, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(tO + c, o);
-          }
-          tmem_st_wait();
+        for (int hh = 0; hh < 2; ++hh) {
+          float mx = fmaxf(fmaxf(mxa[hh][0], mxa[hh][1]), fmaxf(mxa[hh][2], mxa[hh][3]));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          // Lazy rescale with a threshold: the running maximum is only a reference point (softmax is shift invariant), so it is
+          // moved — and O / l rescaled — only when the row's maximum grew by more than 2^8; otherwise the tile is exponentiated
+          // against the stale reference and P may reach 256 (exact in fp16, fp32 sums).
+          const float m_cand = fmaxf(m_run[hh], mx * sl2);
+          const bool resc = m_cand > m_run[hh] + 8.0f;  // first tile: m_run = -inf -> true
+          m_new[hh] = resc ? m_cand : m_run[hh];
+          alpha[hh] = resc ? ex2(m_run[hh] - m_new[hh]) : 1.0f;  // 0 on the first tile
         }
-      }
-      sstamp(j, 5);
-      float sum4[4] = {0.f, 0.f, 0.f, 0.f};  // independent partial row sums (ILP), folded in fixed order below
-      const uint32_t prow_s = smem_u32(prow);
-      auto emit = [&](auto masked) {
-        uint32_t pw[16];  // PT: 32 keys of this row, stored to tensor memory every fourth unit
-        (void)pw;
+        if (sub == 0) sstamp(j, 3);
+        float sum[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // independent partial row sums (ILP), folded in fixed order below
+        uint32_t pa[KW / 4];                        // P as fp16 pairs: the A fragments of the KW / 16 k-steps of P V
 #pragma unroll
-        for (int u = 0; u < 16; ++u) {  // 16-byte units of 8 keys
-          uint32_t w[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int i0 = u * 8 + 2 * e;
-            float p0 = ex2(fmaf(__uint_as_float(sv[i0]), sl2, -m_new));
-            float p1 = ex2(fmaf(__uint_as_float(sv[i0 + 1]), sl2, -m_new));
-            if (decltype(masked)::value) {
-              p0 = (i0 < valid) ? p0 : 0.f;
-              p1 = (i0 + 1 < valid) ? p1 : 0.f;
-            }
-            sum4[e] += p0 + p1;  // fp32 terms; the fp16 rounding of P is unbiased and averages out over the row
-            const __half2 hp = __floats2half2_rn(p0, p1);
-            w[e] = *reinterpret_cast<const uint32_t*>(&hp);
+        for (int i = 0; i < KW / 2; i += 2) {
+          const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + cl;
+          float p0 = ex2(fmaf(sv[i], sl2, -m_new[hh]));
+          float p1 = ex2(fmaf(sv[i + 1], sl2, -m_new[hh]));
+          if (!full) {
+            p0 = (col < valid[hh]) ? p0 : 0.f;
+            p1 = (col + 1 < valid[hh]) ? p1 : 0.f;
           }
-          if (Cfg::PT) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) pw[(u & 3) * 4 + e] = w[e];
-            if ((u & 3) == 3) tmem_st16(tP + (u >> 2) * 16, pw);
-          } else {
-            const int chunk = u >> 3, uu = u & 7;
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(prow_s + chunk * 16384 + ((uu ^ (r & 7)) << 4)),
-                         "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3])
-                         : "memory");
-          }
+          sum[hh][(i >> 2) & 1] += p0 + p1;  // fp32 terms; the fp16 rounding of P is unbiased and averages out over the row
+          pa[i >> 1] = pack_h2(p0, p1);
         }
-      };
-      if (valid == 128)
-        emit(std::false_type{});
-      else
-        emit(std::true_type{});
-      const float sum = (sum4[0] + sum4[1]) + (sum4[2] + sum4[3]);
-      l_run = l_run * alpha + sum;
-      m_run = m_new;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          float t = sum[hh][0] + sum[hh][1];
+          t += __shfl_xor_sync(0xffffffffu, t, 1);
+          t += __shfl_xor_sync(0xffffffffu, t, 2);
+          l_run[hh] = l_run[hh] * alpha[hh] + t;
+          m_run[hh] = m_new[hh];
+        }
+        if (alpha[0] != 1.0f || alpha[1] != 1.0f) {
+#pragma unroll
+          for (int i = 0; i < DPAD / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+        }
+        if (sub == 0) {
+          sstamp(j, 4);
+          mbar_wait(&v_full[st], ph);
+          sstamp(j, 5);
+        }
+        const uint32_t va = smem_u32(sV + st * Cfg::V_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < KW / 16; ++kk) {
+          const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+          const int kg = sub * (KW / 16) + kk;  // 16-key step inside the 128-key tile
+          // K-major V^T: 16 keys = 32 bytes inside a 128-byte row; MN-major V: 16 keys = 16 rows of 128 bytes
+          if (VMN)
+            Wgmma<DPAD>::template rs<1>(o, a, make_sdesc_sw128_mn(va + kg * 2048, Cfg::V_CHUNK), 1);
+          else
+            Wgmma<DPAD>::template rs<0>(o, a, make_sdesc_sw128(va + (kg / 4) * Cfg::V_CHUNK + (kg % 4) * 32), 1);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(o);
+      }
+      if (lane == 0) mbar_arrive(&v_empty[st]);
       sstamp(j, 6);
-      if (Cfg::PT)
-        tmem_st_wait();       // this thread's P columns are in tensor memory
-      else
-        fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor-core (async) proxy
-      tc_fence_before();
-      mbar_arrive(&p_full[g]);
-      sstamp(j, 7);
     }
     // ---- epilogue: O / l -> fp16 hi(/lo)
-    mbar_wait(&pv_done[g], (T - 1) & 1);
-    tc_fence_after();
-    const float inv_l = 1.0f / l_run;
-    const int qrow = q0 + g * 128 + r;
-    const bool ok = qrow < p.Nq;
-    const size_t orow = (size_t)(s * p.q_rows_per_sample + qrow) * p.ldo + h * p.d;
+    const float inv_l[2] = {1.0f / l_run[0], 1.0f / l_run[1]};
 #pragma unroll
-    for (int c = 0; c < DPAD; c += 16) {
-      uint32_t o[16];
-      tmem_ld16(tO + c, o);
-      tmem_ld_wait();
+    for (int hh = 0; hh < 2; ++hh) {
+      const int qrow = q0 + rw + 8 * hh;
+      if (qrow >= p.Nq) continue;
+      const size_t orow = (size_t)(s * p.q_rows_per_sample + qrow) * p.ldo + h * p.d;
 #pragma unroll
-      for (int gg = 0; gg < 16; gg += 8) {
-        if (ok && c + gg < p.d) {
-          __half2 hh[4], hl[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float f0 = __uint_as_float(o[gg + 2 * e]) * inv_l, f1 = __uint_as_float(o[gg + 2 * e + 1]) * inv_l;
-            hh[e] = __floats2half2_rn(f0, f1);
-            const float2 hf = __half22float2(hh[e]);
-            hl[e] = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
-          }
-          *reinterpret_cast<uint4*>(p.out_hi + orow + c + gg) = *reinterpret_cast<uint4*>(hh);
-          if (p.out_lo) *reinterpret_cast<uint4*>(p.out_lo + orow + c + gg) = *reinterpret_cast<uint4*>(hl);
+      for (int i = 2 * hh; i < DPAD / 2; i += 4) {
+        const int col = 8 * (i >> 2) + cl;
+        if (col < p.d) {
+          const float f0 = o[i] * inv_l[hh], f1 = o[i + 1] * inv_l[hh];
+          const __half2 hi = __floats2half2_rn(f0, f1);
+          const float2 hf = __half22float2(hi);
+          *reinterpret_cast<__half2*>(p.out_hi + orow + col) = hi;
+          if (p.out_lo) *reinterpret_cast<__half2*>(p.out_lo + orow + col) = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
         }
       }
     }
-    tc_fence_before();
   }
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
 }
 
-// option "attn_regsplit": NG = 2 launches use the register-split variant (see attention_kernel). Off by default: it removes every
-// spill (STACK 48 -> 0 bytes, no LDL / STL in the SASS) and is bit-identical, but measured neutral (143.38 ms per image with it,
-// 143.30 ms without, tools/step_time.py): the spill reloads were not what the softmax warps wait for.
+// option "attn_regsplit": launches use the register-split variant (see attention_kernel). Same arithmetic in the same order:
+// bit-identical to the variant without it.
 int g_attn_regsplit = 0;
 
-template <int DPAD, int NG, bool VMN, bool QK3, bool RS>
+template <int DPAD, bool VMN, bool QK3, bool RS>
 static void launch_attn3(const AttnMaps& m, const AttnParams& p, cudaStream_t st) {
-  constexpr int smem = AttnCfg<DPAD, NG, VMN, QK3>::SMEM;
+  constexpr int smem = AttnCfg<DPAD, VMN, QK3>::SMEM;
   static DeviceOnce once;
   if (once.first())
-    SDB_CUDA(cudaFuncSetAttribute(attention_kernel<DPAD, NG, VMN, QK3, RS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid((p.Nq + 128 * NG - 1) / (128 * NG), p.heads, p.nb);
-  launch_k(attention_kernel<DPAD, NG, VMN, QK3, RS>, grid, dim3((RS ? 128 : 64) + 128 * NG), (size_t)smem, st, m.q, m.k, m.v, m.q_lo,
-           m.k_lo, p);
+    SDB_CUDA(cudaFuncSetAttribute(attention_kernel<DPAD, VMN, QK3, RS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  dim3 grid((p.Nq + 127) / 128, p.heads, p.nb);
+  launch_k(attention_kernel<DPAD, VMN, QK3, RS>, grid, dim3(384), (size_t)smem, st, m.q, m.k, m.v, m.q_lo, m.k_lo, p);
 }
-template <int DPAD, int NG, bool VMN, bool QK3>
+template <int DPAD, bool VMN, bool QK3>
 static void launch_attn2(const AttnMaps& m, const AttnParams& p, cudaStream_t st) {
-  if constexpr (NG == 2) {
-    if (g_attn_regsplit) return launch_attn3<DPAD, NG, VMN, QK3, true>(m, p, st);
-  }
-  launch_attn3<DPAD, NG, VMN, QK3, false>(m, p, st);
+  if (g_attn_regsplit) return launch_attn3<DPAD, VMN, QK3, true>(m, p, st);
+  launch_attn3<DPAD, VMN, QK3, false>(m, p, st);
 }
-template <int DPAD, int NG>
+template <int DPAD>
 static void launch_attn(const AttnMaps& m, const AttnParams& p, cudaStream_t st) {
   if (p.v_mn)
-    launch_attn2<DPAD, NG, true, false>(m, p, st);
+    launch_attn2<DPAD, true, false>(m, p, st);
   else
-    launch_attn2<DPAD, NG, false, false>(m, p, st);
+    launch_attn2<DPAD, false, false>(m, p, st);
 }
 
 bool attention_supports_qk3(int dpad) { return dpad == 48 || dpad == 80; }
 
 void attention_launch(const AttnMaps& m, const AttnParams& p, cudaStream_t st) {
-  const bool two = p.Nq > 128;  // two ping-pong query tiles per CTA when there are at least two tiles of rows
   if (p.qk3) {
-    // split q / k operands (levels 0-1 of the UNet: V always MN-major there). Shared memory: d = 40 keeps two query tiles and two
-    // K/V stages (225.5 KB); d = 80 fits one query tile and one stage
+    // split q / k operands (levels 0-1 of the UNet: V always MN-major there)
     SDB_CHECK(p.v_mn && attention_supports_qk3(p.dpad), "split q/k attention: head dim / V layout");
     if (p.dpad == 48)
-      two ? launch_attn2<48, 2, true, true>(m, p, st) : launch_attn2<48, 1, true, true>(m, p, st);
+      launch_attn2<48, true, true>(m, p, st);
     else
-      launch_attn2<80, 1, true, true>(m, p, st);
+      launch_attn2<80, true, true>(m, p, st);
     return;
   }
   switch (p.dpad) {
     case 48:
-      two ? launch_attn<48, 2>(m, p, st) : launch_attn<48, 1>(m, p, st);
+      launch_attn<48>(m, p, st);
       break;
     case 64:
-      launch_attn<64, 1>(m, p, st);
+      launch_attn<64>(m, p, st);
       break;
     case 80:
-      two ? launch_attn<80, 2>(m, p, st) : launch_attn<80, 1>(m, p, st);
+      launch_attn<80>(m, p, st);
       break;
     case 160:
-      launch_attn<160, 1>(m, p, st);
+      launch_attn<160>(m, p, st);
       break;
     default:
       throw Error("attention: unsupported head dim " + std::to_string(p.dpad));

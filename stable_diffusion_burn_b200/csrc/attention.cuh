@@ -27,6 +27,6 @@ struct AttnMaps {
 };
 void attention_launch(const AttnMaps& m, const AttnParams& p, cudaStream_t st);
 bool attention_supports_qk3(int dpad);
-extern int g_attn_regsplit;  // 1: two-query-tile launches run the register-split (setmaxnreg) variant (default 0: measured neutral)
+extern int g_attn_regsplit;  // 1: launches run the register-split (setmaxnreg) variant
 
 }  // namespace sdb

@@ -1,13 +1,14 @@
-// gemm_tc.cu — tcgen05 implicit-GEMM for conv3x3 / conv1x1 / Linear on sm_100a.
+// gemm_tc.cu — wgmma implicit-GEMM for conv3x3 / conv1x1 / Linear on sm_90a.
 //
 // Replaces burn nn::conv::Conv2d / nn::Linear on the reference hot path
 // (call sites: src/model/unet/mod.rs:716,726,729 ResBlock convs; :468,479 proj_in/out;
 //  :645-651 q/k/v/out; :580,553 GEGLU/ff; src/model/autoencoder/mod.rs:513-528, 567-606).
 //
-// One CTA = one 128 x BN output tile (x one K split); with CG = 2 a CTA pair shares one 256 x BN MMA. Warp roles:
-//   warp 0   : TMA producer  (cp.async.bulk.tensor 5-D activation boxes + 2-D weight boxes)
-//   warp 1   : TMEM allocator + single-thread tcgen05.mma issuer (fp16 x fp16 -> fp32 in TMEM)
-//   warps 2-9: epilogue (tcgen05.ld -> smem transpose -> bias / time-embedding row / residual / GEGLU -> global)
+// One CTA = one 128 x BN output tile (x one K split). Warp roles:
+//   warpgroup 0    : TMA producer (warp 0: cp.async.bulk.tensor 5-D activation boxes + 2-D weight boxes; warps 1-3 idle)
+//   warpgroups 1-2 : consumers. Each issues wgmma m64nBNk16 (fp16 x fp16 -> fp32 in registers) for 64 of the 128 rows, then
+//                    both write the accumulator to shared memory as a row-major fp32 image and run the epilogue from it
+//                    (bias / time-embedding row / residual / GEGLU / statistics -> global)
 // Multi-pass products (PASSES = 2, 3) add the low-order fp16 halves of the operands
 // (A_lo*B_hi, A_hi*B_lo) into the same accumulator for fp32-class accuracy.
 #include "gemm_tc.cuh"
@@ -20,16 +21,23 @@ static constexpr int BM = 128;
 static constexpr int BK = 64;  // fp16 elements per k chunk = 128 bytes = one swizzle row
 static constexpr int A_TILE_BYTES = BM * BK * 2;
 
-// CG = 1: one CTA per 128 x BN tile. CG = 2: a CTA pair (cluster of 2 along M) runs ONE tcgen05.mma.cta_group::2
-// of shape 256 x BN per k-step: each CTA stages its own 128 A rows and only HALF of the weight tile, so the operand
-// bytes per FLOP that cross the L2->SM fabric drop by 25-45 % (the bound measured in profiles/r1_gemm_tc_ncu_full.md).
-template <int BN, int PASSES, int CG = 1>
+template <int BN, int PASSES>
 struct StageLayout {
-  static constexpr int B_TILE_BYTES = (BN / CG) * BK * 2;
+  static constexpr int B_TILE_BYTES = BN * BK * 2;
   static constexpr int A_TILES = PASSES >= 2 ? 2 : 1;
   static constexpr int B_TILES = PASSES >= 3 ? 2 : 1;
   static constexpr int BYTES = A_TILES * A_TILE_BYTES + B_TILES * B_TILE_BYTES;
 };
+// The epilogue's view of the accumulator: [128 rows][BN] fp32 in shared memory (over the idle pipeline stages), rows padded by
+// 16 B so that the 128-bit reads of 4 rows x 32 columns per warp instruction are bank-conflict free; after it, 32 KB of scratch
+// for the GroupNorm column sums.
+template <int BN>
+struct AccLayout {
+  static constexpr int PITCH = (BN + 4) * 4;
+  static constexpr int BYTES = BM * PITCH;
+  static constexpr int GN_BYTES = 32 * 1024;
+};
+static constexpr int EW = 8;  // consumer / epilogue warps (two warpgroups)
 
 // Activation + fp32 / fp16(hi,lo) stores of 4 consecutive columns of one output row. Deliberately NOT inlined: the epilogue
 // runs once per CTA, so its cost is dominated by cold instruction fetch (ncu: stall_no_inst); one shared copy of this
@@ -96,29 +104,8 @@ __device__ __forceinline__ void gn_write_partials(const GemmParams& p, const flo
   }
 }
 
-// Variants whose pipeline fits twice in an SM's shared memory are launched two CTAs per SM (<= 102 registers per thread);
-// the others own the SM and may use the whole register file.
-template <int BN, int PASSES, int STAGES, int CG>
-__host__ __device__ constexpr int min_ctas_per_sm() {
-  return STAGES * StageLayout<BN, PASSES, CG>::BYTES <= 108 * 1024 ? 2 : 1;
-}
-
-// Epilogue warps (a multiple of 4: one group per TMEM lane quarter). Measured: 16 warps on the SM-owning variants do not
-// shorten the epilogue (6.4k vs 6.7k cycles for 128 x 160) and lengthen the tail, so those use 8. The variants that share an
-// SM between two CTAs use 4: with 8 they were capped at 96 registers per thread and spilled 140-950 bytes per thread, and with
-// the shared-memory carve-out at its maximum L1 holds nothing, so every spill access is an L2 round trip (ncu on the q|k|v
-// projection: 225 K local loads + 152 K local stores, 48 MB of local traffic for 19 MB of output, long-scoreboard the top stall).
-// 4 warps (192 threads per CTA) leave 170 registers per thread: no spills.
-// The GEGLU epilogue is the exception: it is bound by its own arithmetic (erf-GELU on every output), 16 warps per SM beat 8
-// even at 96 registers (measured on the level-0 GEGLU projection: 8 warps 74 us, 4 warps 90 us), and as a compile-time variant
-// (EPI_GEGLU*) it no longer carries the other epilogues' registers.
-template <int BN, int PASSES, int STAGES, int CG, int EPI>
-__host__ __device__ constexpr int epilogue_warps() {
-  return (min_ctas_per_sm<BN, PASSES, STAGES, CG>() == 2 && EPI < 4) ? 4 : 8;
-}
-
 // EPI selects what the epilogue does beside bias / residual / stores. It is a compile-time choice because the once-per-CTA
-// epilogue is instruction-issue bound: statistics code that is merely skipped at run time still cost ~0.5 us per launch.
+// epilogue is instruction-issue bound: statistics code that is merely skipped at run time still costs issue slots.
 //   EPI_PLAIN  nothing more          EPI_GN   GroupNorm statistics of the output tensor (column sums per channel bucket)
 //   EPI_LNS    LayerNorm row statistics of the output rows (partial sum / sum of squares per N-tile share)
 //   EPI_LNC    the A operand is the RAW input of a LayerNorm whose gamma is folded into the weights: the normalisation is applied
@@ -128,23 +115,26 @@ __host__ __device__ constexpr int epilogue_warps() {
 //              the LayerNorm-consuming correction
 enum : int { EPI_PLAIN = 0, EPI_GN = 1, EPI_LNS = 2, EPI_LNC = 3, EPI_GEGLU = 4, EPI_GEGLU_LNC = 5 };
 
-template <int BN, int PASSES, int STAGES, int CG, int EPI>
-__global__ void __launch_bounds__(64 + 32 * epilogue_warps<BN, PASSES, STAGES, CG, EPI>(), min_ctas_per_sm<BN, PASSES, STAGES, CG>())
+template <int BN, int PASSES, int STAGES>
+__host__ __device__ constexpr int region_bytes() {
+  return STAGES * StageLayout<BN, PASSES>::BYTES > AccLayout<BN>::BYTES + AccLayout<BN>::GN_BYTES
+             ? STAGES * StageLayout<BN, PASSES>::BYTES
+             : AccLayout<BN>::BYTES + AccLayout<BN>::GN_BYTES;
+}
+
+template <int BN, int PASSES, int STAGES, int EPI>
+__global__ void __launch_bounds__(128 + 32 * EW, 1)
 gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   constexpr bool kGN = EPI == EPI_GN, kLNS = EPI == EPI_LNS, kLNC = EPI == EPI_LNC || EPI == EPI_GEGLU_LNC;
   constexpr bool kGEGLU = EPI == EPI_GEGLU || EPI == EPI_GEGLU_LNC;
-  using L = StageLayout<BN, PASSES, CG>;
-  constexpr bool TWO = CG == 2;
-  constexpr int EW = epilogue_warps<BN, PASSES, STAGES, CG, EPI>();  // epilogue warps
-  constexpr int EG = EW / 4;                                    // warps sharing one TMEM lane quarter
+  using L = StageLayout<BN, PASSES>;
+  constexpr int EG = EW / 4;                                    // warps sharing one 32-row quarter of the tile
   constexpr int CSTEP = 32 * EG;                                // column stride between the chunks of one warp
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128B swizzle atoms
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * L::BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + region_bytes<BN, PASSES, STAGES>());
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -172,14 +162,11 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   const int it_begin = kz * per_split;
   const int it_end = min(total_iters, it_begin + per_split);
 
-  const uint32_t crank = TWO ? cluster_ctarank() : 0;
-  const bool leader = crank == 0;  // the CTA that issues the pair's MMAs and owns the "full" barriers
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], EW);  // one arrival per consumer warp
     }
-    mbar_init(accum_bar, 1);
     fence_mbar_init();
   }
   if (warp == 0 && lane == 0) {
@@ -187,30 +174,13 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     tma_prefetch_desc(&maps.b[0]);
     if (p.kc0 < p.kc) tma_prefetch_desc(&maps.a[1][0]);
   }
-  constexpr uint32_t TMEM_COLS = BN <= 64 ? 64 : (BN <= 128 ? 128 : 256);  // power of two >= BN
-  if (warp == 1) {
-    if (TWO) {
-      tmem_alloc2(tmem_slot, TMEM_COLS);
-      tmem_relinquish2();
-    } else {
-      tmem_alloc(tmem_slot, TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if (TWO)
-    cluster_sync_all();  // the peer's barriers must be initialised before anything signals them
-  else
-    __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   if (dbg && threadIdx.x == 0) dbg[1] = clock64();
   // Programmatic dependent launch: everything above overlapped the previous kernel's tail. From here on each role waits for the
   // previous kernel (griddepcontrol.wait) only where it first touches data that kernel may have written:
   //   producer : WEIGHTS are immutable, so the weight tiles of the first STAGES k-chunks (and an L2 prefetch of the rest of this
   //              CTA's weight strip when the launch is weight-bound) are issued BEFORE the wait; activation tiles after it
-  //   MMA warp : consumes shared memory behind the mbarriers only: no wait
-  //   epilogue : waits before its first read of residual / time-embedding rows; all of this kernel's stores follow that wait
+  //   consumers: wait before the epilogue's first read of residual / time-embedding rows; all of this kernel's stores follow it
   if (warp == 0) {
     // ===================================================== TMA producer (one elected lane: see elect_one in common.cuh)
     if (elect_one()) {
@@ -219,15 +189,8 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
         const CUtensorMap* bm = it < main_iters ? maps.b : maps.bx;
         const int bk = (it < main_iters ? it : it - main_iters) * BK;
         uint8_t* sb = smem + s * L::BYTES + L::A_TILES * A_TILE_BYTES;
-        if (!TWO) {
-          tma_load_2d(sb, &bm[0], &full_bar[s], bk, b_row0);
-          if (PASSES >= 3) tma_load_2d(sb + L::B_TILE_BYTES, &bm[1], &full_bar[s], bk, b_row0);
-        } else {
-          // rows [crank*BN/2, +BN/2) of the weight tile into this CTA's smem, bytes reported to the leader's barrier
-          const uint32_t fb = mapa_shared(smem_u32(&full_bar[s]), 0);
-          tma_load_2d_2sm(sb, &bm[0], fb, bk, b_row0 + crank * (BN / 2));
-          if (PASSES >= 3) tma_load_2d_2sm(sb + L::B_TILE_BYTES, &bm[1], fb, bk, b_row0 + crank * (BN / 2));
-        }
+        tma_load_2d(sb, &bm[0], &full_bar[s], bk, b_row0);
+        if (PASSES >= 3) tma_load_2d(sb + L::B_TILE_BYTES, &bm[1], &full_bar[s], bk, b_row0);
       };
       auto load_a = [&](int it, int s) {
         int src, c0, cw, ch, cp;
@@ -244,28 +207,21 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
           cw = w0, ch = h0, cp = 0;
         }
         uint8_t* st = smem + s * L::BYTES;
-        if (!TWO) {
-          tma_load_5d(st, &maps.a[src][0], &full_bar[s], c0, cw, ch, cp, n0);
-          if (PASSES >= 2) tma_load_5d(st + A_TILE_BYTES, &maps.a[src][1], &full_bar[s], c0, cw, ch, cp, n0);
-        } else {
-          const uint32_t fb = mapa_shared(smem_u32(&full_bar[s]), 0);
-          tma_load_5d_2sm(st, &maps.a[src][0], fb, c0, cw, ch, cp, n0);
-          if (PASSES >= 2) tma_load_5d_2sm(st + A_TILE_BYTES, &maps.a[src][1], fb, c0, cw, ch, cp, n0);
-        }
+        tma_load_5d(st, &maps.a[src][0], &full_bar[s], c0, cw, ch, cp, n0);
+        if (PASSES >= 2) tma_load_5d(st + A_TILE_BYTES, &maps.a[src][1], &full_bar[s], c0, cw, ch, cp, n0);
       };
       // ---- before the wait: weights only (the pipeline slots are all free: fresh barriers)
       const int npre = min(STAGES, it_end - it_begin);
       for (int i = 0; i < npre; ++i) {
-        if (leader) mbar_expect_tx(&full_bar[i], L::BYTES * CG);  // A + B bytes of both CTAs report to the leader's barrier
+        mbar_expect_tx(&full_bar[i], L::BYTES);
         load_b(it_begin + i, i);
       }
       if (p.prefetch_w) {
         for (int it = it_begin + npre; it < it_end; ++it) {
           const CUtensorMap* bm = it < main_iters ? maps.b : maps.bx;
           const int bk = (it < main_iters ? it : it - main_iters) * BK;
-          const int row = b_row0 + (TWO ? crank * (BN / 2) : 0);
-          tma_prefetch_l2_2d(&bm[0], bk, row);
-          if (PASSES >= 3) tma_prefetch_l2_2d(&bm[1], bk, row);
+          tma_prefetch_l2_2d(&bm[0], bk, b_row0);
+          if (PASSES >= 3) tma_prefetch_l2_2d(&bm[1], bk, b_row0);
         }
       }
       pdl_wait();
@@ -276,7 +232,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       uint32_t ph = npre == STAGES ? 1 : 0;
       for (int it = it_begin + npre; it < it_end; ++it) {
         mbar_wait(&empty_bar[s], ph ^ 1);
-        if (leader) mbar_expect_tx(&full_bar[s], L::BYTES * CG);
+        mbar_expect_tx(&full_bar[s], L::BYTES);
         load_a(it, s);
         load_b(it, s);
         if (++s == STAGES) {
@@ -285,61 +241,62 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer (pair leader only when CG = 2)
-    constexpr uint32_t idesc = make_idesc_f16(BM * CG, BN);
-    int s = 0;
-    uint32_t ph = 0;
-    for (int it = it_begin; leader && it < it_end; ++it) {
-      mbar_wait(&full_bar[s], ph);
-      tc_fence_after();
-      if (dbg && lane == 0 && it == it_begin) dbg[3] = clock64();
-      if (elect_one()) {
-        const uint32_t a_hi = smem_u32(smem + s * L::BYTES);
+  } else if (warp >= 4) {
+    // ===================================================== consumers: wgmma mainloop, then the epilogue
+    pdl_wait();  // residual / time-embedding rows below may come from the previous kernel; every store of this kernel follows
+    const int wg = (warp - 4) >> 2;  // rows [64 wg, 64 wg + 64) of the tile
+    {
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int s = 0, prev = -1;
+      uint32_t ph = 0;
+      for (int it = it_begin; it < it_end; ++it) {
+        mbar_wait(&full_bar[s], ph);
+        if (dbg && threadIdx.x == 128 && it == it_begin) dbg[3] = clock64();
+        const uint32_t a_hi = smem_u32(smem + s * L::BYTES) + wg * (64 * 128);
         const uint32_t a_lo = a_hi + A_TILE_BYTES;
-        const uint32_t b_hi = a_hi + L::A_TILES * A_TILE_BYTES;
+        const uint32_t b_hi = smem_u32(smem + s * L::BYTES) + L::A_TILES * A_TILE_BYTES;
         const uint32_t b_lo = b_hi + L::B_TILE_BYTES;
+        wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
           const uint32_t koff = k * 32;  // 16 fp16 = 32 bytes inside the 128B swizzle row
           const uint64_t da = make_sdesc_sw128(a_hi + koff);
           const uint64_t db = make_sdesc_sw128(b_hi + koff);
-          const uint32_t acc = (it > it_begin || k > 0) ? 1u : 0u;
-          if (TWO) {
-            umma_f16_2sm(tmem_base, da, db, idesc, acc);
-            if (PASSES >= 2) umma_f16_2sm(tmem_base, make_sdesc_sw128(a_lo + koff), db, idesc, 1u);
-            if (PASSES >= 3) umma_f16_2sm(tmem_base, da, make_sdesc_sw128(b_lo + koff), idesc, 1u);
-          } else {
-            umma_f16(tmem_base, da, db, idesc, acc);
-            if (PASSES >= 2) umma_f16(tmem_base, make_sdesc_sw128(a_lo + koff), db, idesc, 1u);
-            if (PASSES >= 3) umma_f16(tmem_base, da, make_sdesc_sw128(b_lo + koff), idesc, 1u);
-          }
+          Wgmma<BN>::template ss<0>(acc, da, db, 1);
+          if (PASSES >= 2) Wgmma<BN>::template ss<0>(acc, make_sdesc_sw128(a_lo + koff), db, 1);
+          if (PASSES >= 3) Wgmma<BN>::template ss<0>(acc, da, make_sdesc_sw128(b_lo + koff), 1);
         }
-        if (TWO) {
-          umma_commit_2sm(&empty_bar[s], 0x3);                     // release the slot in both CTAs of the pair
-          if (it == it_end - 1) umma_commit_2sm(accum_bar, 0x3);   // both epilogues may start
-        } else {
-          umma_commit(&empty_bar[s]);                    // frees the smem slot when these MMAs retire
-          if (it == it_end - 1) umma_commit(accum_bar);  // accumulator complete
+        wgmma_commit();
+        // one group stays in flight: the products of the previous stage are complete, so its slot goes back to the producer
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = s;
+        if (++s == STAGES) {
+          s = 0;
+          ph ^= 1;
         }
-        if (dbg && it == it_end - 1) dbg[4] = clock64();
       }
-      __syncwarp();
-      if (++s == STAGES) {
-        s = 0;
-        ph ^= 1;
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (dbg && threadIdx.x == 128) dbg[4] = clock64();
+      // every consumer's products are complete before the accumulator image overwrites the stages
+      asm volatile("bar.sync 1, %0;" ::"n"(EW * 32) : "memory");
+      float* img = reinterpret_cast<float*>(smem);
+      const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < BN / 2; j += 2) {
+        const int row = r0 + 8 * ((j >> 1) & 1), col = 8 * (j >> 2) + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(img + row * (AccLayout<BN>::PITCH / 4) + col) = make_float2(acc[j], acc[j + 1]);
       }
+      asm volatile("bar.sync 1, %0;" ::"n"(EW * 32) : "memory");
     }
-  } else {
-    // ===================================================== epilogue (warps 2..9)
-    pdl_wait();  // residual / time-embedding rows below may come from the previous kernel; every store of this kernel follows
-    // Each thread owns one accumulator row in TMEM (warp w may touch lanes 32*(w%4)..+31); the two warps that
-    // share a lane quarter split the 32-column chunks between them. A row-per-thread store pattern would touch 32
-    // cache lines per instruction, so every 32x32 block is transposed through shared memory (the pipeline stages
-    // are idle by now; rows padded to 144 B keep both the 128-bit writes and reads bank-conflict free) and
-    // written/read as 4 rows x 128 contiguous bytes per warp instruction.
-    const int q = warp & 3;             // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;   // which share of the column chunks this warp owns (0..EG-1)
+    // The epilogue reads the accumulator image row-wise: warp w serves the 32-row quarter q = w % 4 and its share `half` of
+    // the 32-column chunks. A row-per-thread store pattern would touch 32 cache lines per instruction, so rows are read and
+    // written as 4 rows x 128 contiguous bytes per warp instruction.
+    const int q = warp & 3;             // 32-row quarter of the tile this warp serves
+    const int half = (warp - 4) >> 2;   // which share of the column chunks this warp owns (0..EG-1)
     const int r = q * 32 + lane;        // accumulator row
     const int pw = w0 + r % p.TW;
     const int phh = h0 + (r / p.TW) % p.TH;
@@ -350,8 +307,8 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
 
     // ---- work that needs no accumulator, done while the main loop runs: the element offsets of the 8 rows this lane
     // serves in every column chunk (rr = 4 i + sub), the bias of each chunk, and the first chunk's addends (residual or
-    // time-embedding row; run_gemm guarantees at most one of them). The epilogue is a chain of L2 round trips
-    // (~650 cycles each, measured with clock64 stamps): everything issued here is off that chain.
+    // time-embedding row; run_gemm guarantees at most one of them). The epilogue is a chain of L2 round trips: everything
+    // issued here is off that chain.
     const int sub = lane >> 3;          // row within a group of 4
     const int cq = (lane & 7) * 4;      // 4-column group inside the 32-column chunk
     constexpr int NCHUNK = (BN + CSTEP - 1) / CSTEP;
@@ -429,22 +386,10 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     const bool pre_issued = plain;
     if (pre_issued) issue_addends(col0 + half * 32 + cq);
 
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
     if (p.pdl_late) pdl_trigger();
-    if (dbg && threadIdx.x == 64) dbg[5] = clock64();
-    const uint32_t trow = tmem_base + (uint32_t(q * 32) << 16);
-    constexpr uint32_t TROW = 144;                                   // padded row pitch of the staging tile (bytes)
-    const uint32_t tile_s = smem_u32(smem) + (warp - 2) * (32 * TROW);  // one 32-row tile per warp (4.6 KB each)
-    const uint32_t tile2_s = tile_s + EW * 32 * TROW;                    // second bank, GEGLU only (x | gate)
-
-    auto stage = [&](uint32_t t, const uint32_t (&v)[32]) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(t + lane * TROW + k * 16), "r"(v[4 * k]),
-                     "r"(v[4 * k + 1]), "r"(v[4 * k + 2]), "r"(v[4 * k + 3])
-                     : "memory");
-    };
+    if (dbg && threadIdx.x == 128) dbg[5] = clock64();
+    constexpr uint32_t TROW = AccLayout<BN>::PITCH;
+    const uint32_t arow = smem_u32(smem) + q * 32 * TROW;  // row 32 q of the accumulator image
     auto unstage = [&](uint32_t t, int rr) {
       float4 f;
       asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
@@ -454,9 +399,8 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       return f;
     };
     // element offsets fit 32 bits (run_gemm checks rows * ld < 2^31): one IMAD per row instead of 64-bit address chains
-    // GroupNorm statistics of the output (p.gn_part): per-quarter column sums, staged in the second transposition bank
-    // (which only the GEGLU epilogue uses; run_gemm never combines the two)
-    float2* const gn_cs = reinterpret_cast<float2*>(smem + EW * 32 * TROW);
+    // GroupNorm statistics of the output (p.gn_part): per-quarter column sums, in the scratch after the accumulator image
+    float2* const gn_cs = reinterpret_cast<float2*>(smem + AccLayout<BN>::BYTES);
     const GnTile gnt = gn_tile_of(p, n0, th, tw);
     auto store_out = [&](float4 f, int mr, int col) {
       epilogue_store(f, (unsigned)(mr * p.ldc + col), (unsigned)(mr * p.ldc16 + col), p.out_f32, p.out_f16, p.out_f16_lo, p.act);
@@ -468,26 +412,20 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       float* wsbase = p.ws + (size_t)kz * Mtot * p.N;
 #pragma unroll 1
       for (int c = half * 32; c < BN; c += CSTEP) {
-        uint32_t v[32];
-        tmem_ld32(trow + c, v);
-        tmem_ld_wait();
-        stage(tile_s, v);
-        __syncwarp();
         const int col = col0 + c + cq;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const int rr = i * 4 + sub;
           const int mr = __shfl_sync(0xffffffffu, m, rr);
-          if (mr >= 0 && col < p.N) __stcg(reinterpret_cast<float4*>(wsbase + (size_t)mr * p.N + col), unstage(tile_s, rr));
+          if (mr >= 0 && col < p.N) __stcg(reinterpret_cast<float4*>(wsbase + (size_t)mr * p.N + col), unstage(arow + c * 4, rr));
         }
-        __syncwarp();
       }
       __threadfence();
       asm volatile("bar.sync 1, %0;" ::"n"(EW * 32) : "memory");  // all epilogue warps have published their part of the tile
       // Tile-level rendezvous of the split_k CTAs (all co-resident: run_gemm keeps ctas*split within one wave), then
       // every CTA folds its own slice of the tile rows in z order (deterministic) and runs the epilogue on it.
       unsigned int* tk = p.tickets + 2 * ((size_t)blockIdx.y * gridDim.x + blockIdx.x);
-      if (warp == 2 && lane == 0) {
+      if (warp == 4 && lane == 0) {
         atomicAdd(tk, 1u);
         const long long t0 = clock64();
         while (atomicAdd(tk, 0u) < (unsigned)p.split_k) {
@@ -503,10 +441,10 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
         constexpr int C4 = BN / 4;
         // thread -> (row lane, fixed 4-column group): a thread's GroupNorm column sums stay in registers across its rows
         constexpr int RL = (EW * 32) / C4;  // row lanes
-        const int te = threadIdx.x - 64;
+        const int te = threadIdx.x - 128;
         const int rlane = te / C4, cg4 = te - rlane * C4;
         const int rpi = BM / gnt.tn;  // rows per image inside the tile
-        float4* const gn_red = reinterpret_cast<float4*>(smem + EW * 32 * TROW);  // [RL][TN][C4][2] float4, <= 32 KB (second bank)
+        float4* const gn_red = reinterpret_cast<float4*>(smem + AccLayout<BN>::BYTES);  // [RL][TN][C4][2] float4, <= 32 KB
 #pragma unroll 1
         for (int k = 0; k < gnt.tn; ++k) {
         float4 gsum = make_float4(0.f, 0.f, 0.f, 0.f), gsq = gsum;
@@ -585,7 +523,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
         }
       }
       asm volatile("bar.sync 1, %0;" ::"n"(EW * 32) : "memory");
-      if (warp == 2 && lane == 0) {
+      if (warp == 4 && lane == 0) {
         // last CTA to finish resets both counters: the buffer is all zero again for the next launch
         if (atomicAdd(tk + 1, 1u) == (unsigned)(p.split_k - 1)) {
           tk[0] = 0u;
@@ -598,14 +536,6 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       const int ocol0 = blockIdx.y * HB;
 #pragma unroll 1
       for (int c = half * 32; c < HB; c += CSTEP) {
-        uint32_t v[32];
-        tmem_ld32(trow + c, v);
-        tmem_ld_wait();
-        stage(tile_s, v);
-        tmem_ld32(trow + HB + c, v);
-        tmem_ld_wait();
-        stage(tile2_s, v);
-        __syncwarp();
         const float4 bx = *reinterpret_cast<const float4*>(p.bias + col0 + c + cq);
         const float4 bg = *reinterpret_cast<const float4*>(p.bias + col0 + HB + c + cq);
         float4 ux = make_float4(0.f, 0.f, 0.f, 0.f), ug = ux;
@@ -620,7 +550,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
           float rmu = 0.f, rrs = 1.f;
           if constexpr (kLNC) rmu = __shfl_sync(0xffffffffu, ln_mu, rr), rrs = __shfl_sync(0xffffffffu, ln_rs, rr);
           if (mr >= 0) {
-            float4 tx = unstage(tile_s, rr), tg = unstage(tile2_s, rr);
+            float4 tx = unstage(arow + c * 4, rr), tg = unstage(arow + (HB + c) * 4, rr);
             if constexpr (kLNC) {
               tx.x = rrs * (tx.x - rmu * ux.x), tx.y = rrs * (tx.y - rmu * ux.y), tx.z = rrs * (tx.z - rmu * ux.z), tx.w = rrs * (tx.w - rmu * ux.w);
               tg.x = rrs * (tg.x - rmu * ug.x), tg.y = rrs * (tg.y - rmu * ug.y), tg.z = rrs * (tg.z - rmu * ug.z), tg.w = rrs * (tg.w - rmu * ug.w);
@@ -633,7 +563,6 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
             epilogue_store(y, 0u, (unsigned)(mr * p.ldc16 + ocol0 + c + cq), nullptr, p.out_f16, p.out_f16_lo, 0);
           }
         }
-        __syncwarp();
       }
     } else {
       constexpr int NCH = NCHUNK;  // column chunks per warp (the warps of a lane quarter interleave them)
@@ -646,16 +575,11 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       for (int j = 0; j < NCH; ++j) {
         const int c = half * 32 + j * CSTEP;
         if (c < BN) {
-          uint32_t v[32];
-          tmem_ld32(trow + c, v);
-          tmem_ld_wait();
-          stage(tile_s, v);
-          __syncwarp();
           const int col = col0 + c + cq;
           float4 gsum = make_float4(0.f, 0.f, 0.f, 0.f), gsq = gsum;
           (void)gsum, (void)gsq;
           if (col < p.N) {
-            const uint32_t tl = tile_s + sub * TROW + cq * 4;
+            const uint32_t tl = arow + c * 4 + sub * TROW + cq * 4;
 #pragma unroll
             for (int b4 = 0; b4 < 2; ++b4) {
               float4 t[4];
@@ -706,7 +630,6 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
               d[2] = make_float2(gsum.z, gsq.z), d[3] = make_float2(gsum.w, gsq.w);
             }
           }
-          __syncwarp();
           // the next chunk's addends travel while its accumulator columns are read and staged
           if (j + 1 < NCH && c + CSTEP < BN) issue_addends(col0 + c + CSTEP + cq);
         }
@@ -736,116 +659,72 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       }
       if constexpr (kGN) {
         asm volatile("bar.sync 1, %0;" ::"n"(EW * 32) : "memory");  // every quarter's column sums are in shared memory
-        gn_write_partials(p, gn_cs, BN, threadIdx.x - 64, EW * 32, gnt, col0, p.up2 ? (int)blockIdx.z * p.gn_phase_slots : 0);
+        gn_write_partials(p, gn_cs, BN, threadIdx.x - 128, EW * 32, gnt, col0, p.up2 ? (int)blockIdx.z * p.gn_phase_slots : 0);
       }
     }
-    tc_fence_before();
-    if (dbg && threadIdx.x == 64) dbg[6] = clock64();
+    if (dbg && threadIdx.x == 128) dbg[6] = clock64();
   }
-
-  if (TWO)
-    cluster_sync_all();  // no CTA may exit while its peer can still signal its barriers / read its smem
-  else
-    __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if (TWO)
-      tmem_dealloc2(tmem_base, TMEM_COLS);
-    else
-      tmem_dealloc(tmem_base, TMEM_COLS);
-  }
+  __syncthreads();
   if (dbg && threadIdx.x == 0) dbg[7] = clock64();
 }
 
 // ------------------------------------------------------------------ launcher
-template <int BN, int PASSES, int CG>
+template <int BN, int PASSES>
 constexpr int pick_stages() {
   // as many stages as fit in ~200 KB, capped at 8
-  constexpr int per = StageLayout<BN, PASSES, CG>::BYTES;
+  constexpr int per = StageLayout<BN, PASSES>::BYTES;
   constexpr int n = (200 * 1024) / per;
   return n > 8 ? 8 : n;
 }
-template <int BN, int PASSES, int CG>
-constexpr int pick_stages_half() {
-  // configuration that lets two CTAs share one SM (<= ~110 KB each)
-  constexpr int per = StageLayout<BN, PASSES, CG>::BYTES;
-  constexpr int n = (104 * 1024) / per;
-  return n > 4 ? 4 : (n < 2 ? 2 : n);
-}
 
-template <int BN, int PASSES, int STAGES, int CG, int EPI>
+template <int BN, int PASSES, int STAGES, int EPI>
 static void launch_epi(const GemmMaps& maps, const GemmParams& p, cudaStream_t stream) {
-  constexpr int smem = STAGES * StageLayout<BN, PASSES, CG>::BYTES + (2 * STAGES + 1) * 8 + 16 + 1024;
-  constexpr int EW = epilogue_warps<BN, PASSES, STAGES, CG, EPI>();
-  static_assert(STAGES * StageLayout<BN, PASSES, CG>::BYTES >= 2 * EW * 32 * 144, "epilogue staging tiles must fit in the stages");
-  static_assert(4 * BN * 8 <= EW * 32 * 144 && ((EW * 32) / (BN / 4)) * 4 * (BN / 4) * 32 <= EW * 32 * 144,
-                "GroupNorm column sums must fit in the second staging bank");
+  constexpr int smem = region_bytes<BN, PASSES, STAGES>() + 2 * STAGES * 8 + 1024;
+  static_assert(smem <= 227 * 1024, "shared memory per block");
+  static_assert(4 * BN * 8 <= AccLayout<BN>::GN_BYTES && 2 * (EW * 32) * 4 * 16 <= AccLayout<BN>::GN_BYTES,
+                "GroupNorm column sums must fit in the scratch after the accumulator image");
   static DeviceOnce once;
   if (once.first())
-    SDB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, PASSES, STAGES, CG, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    SDB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, PASSES, STAGES, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   dim3 grid(p.tiles_n * p.tiles_h * p.tiles_w, (p.N + BN - 1) / BN, p.up2 ? 4 : p.split_k);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid, cfg.blockDim = dim3(64 + 32 * EW), cfg.dynamicSmemBytes = smem, cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = p.cluster, attr[0].val.clusterDim.y = 1, attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr, cfg.numAttrs = g_pdl_enabled ? 2 : 1;
-  SDB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, PASSES, STAGES, CG, EPI>, maps, p));
+  launch_k(gemm_tc_kernel<BN, PASSES, STAGES, EPI>, grid, dim3(128 + 32 * EW), (size_t)smem, stream, maps, p);
 }
-
 // the statistics-producing epilogues exist for the tile widths their tensors use (run_gemm checks with gemm_tc_supports_epi)
-template <int BN, int PASSES, int STAGES, int CG>
+template <int BN, int PASSES, int STAGES>
 static void launch_inst(const GemmMaps& maps, const GemmParams& p, cudaStream_t stream) {
   SDB_CHECK((p.gn_part != nullptr) + (p.ln_out != nullptr) + (p.ln_in != nullptr) <= 1, "one statistics role per launch");
   if constexpr (BN == 128) {
     if (p.geglu) {
       SDB_CHECK(!p.gn_part && !p.ln_out && p.split_k == 1, "GEGLU epilogue: no statistics output, no split-K");
-      return p.ln_in ? launch_epi<BN, PASSES, STAGES, CG, EPI_GEGLU_LNC>(maps, p, stream)
-                     : launch_epi<BN, PASSES, STAGES, CG, EPI_GEGLU>(maps, p, stream);
+      return p.ln_in ? launch_epi<BN, PASSES, STAGES, EPI_GEGLU_LNC>(maps, p, stream)
+                     : launch_epi<BN, PASSES, STAGES, EPI_GEGLU>(maps, p, stream);
     }
   }
   SDB_CHECK(!p.geglu, "the GEGLU epilogue is built for 128-wide tiles");
   if constexpr (BN >= 128) {
-    if (p.gn_part) return launch_epi<BN, PASSES, STAGES, CG, EPI_GN>(maps, p, stream);
+    if (p.gn_part) return launch_epi<BN, PASSES, STAGES, EPI_GN>(maps, p, stream);
   }
   if constexpr (BN == 160) {
-    if (p.ln_out) return launch_epi<BN, PASSES, STAGES, CG, EPI_LNS>(maps, p, stream);
+    if (p.ln_out) return launch_epi<BN, PASSES, STAGES, EPI_LNS>(maps, p, stream);
   }
   if constexpr (BN == 128 || BN == 160) {
-    if (p.ln_in) return launch_epi<BN, PASSES, STAGES, CG, EPI_LNC>(maps, p, stream);
+    if (p.ln_in) return launch_epi<BN, PASSES, STAGES, EPI_LNC>(maps, p, stream);
   }
   SDB_CHECK(!p.gn_part && !p.ln_out && !p.ln_in, "this statistics epilogue is not built for this tile width");
-  launch_epi<BN, PASSES, STAGES, CG, EPI_PLAIN>(maps, p, stream);
+  launch_epi<BN, PASSES, STAGES, EPI_PLAIN>(maps, p, stream);
 }
 bool gemm_tc_supports(int BN, int epi) {
   return epi == EPI_PLAIN || (epi == EPI_GN && BN >= 128) || (epi == EPI_LNS && BN == 160) || (epi == EPI_LNC && (BN == 128 || BN == 160));
 }
 
-template <int BN, int PASSES, int CG>
-static void launch_cg(const GemmMaps& maps, const GemmParams& p, cudaStream_t stream) {
-  const long long ctas = (long long)p.tiles_n * p.tiles_h * p.tiles_w * ((p.N + BN - 1) / BN) * (p.up2 ? 4 : p.split_k);
-  constexpr int SH = pick_stages_half<BN, PASSES, CG>();
-  constexpr bool half_ok = SH * StageLayout<BN, PASSES, CG>::BYTES <= 104 * 1024 && SH * StageLayout<BN, PASSES, CG>::BYTES >= 8 * 32 * 144 * 2;
-  // many short tiles: two co-resident CTAs per SM overlap one tile's epilogue with the other's mainloop
-  if (half_ok && ctas >= 2 * 148)
-    launch_inst<BN, PASSES, half_ok ? SH : pick_stages<BN, PASSES, CG>(), CG>(maps, p, stream);
-  else
-    launch_inst<BN, PASSES, pick_stages<BN, PASSES, CG>(), CG>(maps, p, stream);
-}
 template <int BN, int PASSES>
 static void launch_bn(const GemmMaps& maps, const GemmParams& p, cudaStream_t stream) {
-  if (p.cluster == 2)
-    launch_cg<BN, PASSES, 2>(maps, p, stream);
-  else
-    launch_cg<BN, PASSES, 1>(maps, p, stream);
+  launch_inst<BN, PASSES, pick_stages<BN, PASSES>()>(maps, p, stream);
 }
 
 void gemm_tc_launch(const GemmMaps& maps, const GemmParams& p, int BN, int passes, cudaStream_t stream) {
   SDB_CHECK(p.TN * p.TH * p.TW == BM, "M tile must cover 128 rows");
   SDB_CHECK(p.N % 32 == 0, "N must be a multiple of 32");
-  SDB_CHECK(p.cluster == 1 || (p.cluster == 2 && (p.tiles_n * p.tiles_h * p.tiles_w) % 2 == 0), "CTA pairs need an even M-tile count");
 #define SDB_DISPATCH(bn)                                             \
   case bn:                                                           \
     if (passes == 1) launch_bn<bn, 1>(maps, p, stream);              \

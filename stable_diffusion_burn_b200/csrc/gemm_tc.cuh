@@ -1,4 +1,4 @@
-// gemm_tc.cuh — descriptor of one tcgen05 implicit-GEMM launch (conv3x3 / conv1x1 / Linear).
+// gemm_tc.cuh — descriptor of one wgmma implicit-GEMM launch (conv3x3 / conv1x1 / Linear).
 #pragma once
 #include "common.cuh"
 
@@ -7,13 +7,12 @@ namespace sdb {
 // A operand = fp16 activation tensor viewed as 5-D [n][phase][h][w][c] (c innermost), loaded by TMA
 // boxes {64 c, TW, TH, 1, TN} at tap-shifted coordinates (zero fill outside = conv padding).
 // B operand = packed fp16 weights [N][K] (K-major), K index = tap * Cin_total + c.
-// D (fp32, TMEM) [128 rows = TN*TH*TW output pixels][BN output channels].
+// D (fp32, registers of two consumer warpgroups) [128 rows = TN*TH*TW output pixels][BN output channels].
 struct GemmMaps {
   CUtensorMap a[4][2];  // [source][hi/lo]: 0/1 = channel-concatenated operands of every tap; 2/3 = "extra K" operands read at
                         // the centre tap only, appended after the taps (the ResBlock's 1x1 skip conv folded into conv_out)
   CUtensorMap bx[2];    // weights of the extra-K segment [N][xK]
-  CUtensorMap b[2];     // [hi/lo]  box {64, BN} (cluster = 1) or {64, BN/2} (cluster = 2: each CTA of a pair
-                        //          stages the half of the weight tile that the cta_group::2 MMA reads from it)
+  CUtensorMap b[2];     // [hi/lo]  box {64, BN}
 };
 
 struct GemmParams {
@@ -29,7 +28,6 @@ struct GemmParams {
   int split_k;
   int up2, gn_phase_slots; // up2 = 1: folded nearest-2x upsample conv, grid.z = the 4 output phases (weights packed [4][N][K], taps
                            // / output pixel shifted by the phase); gn_phase_slots = GroupNorm partial slots one phase writes
-  int cluster;             // 1, or 2 = CTA pairs along M issue tcgen05.mma.cta_group::2 (256 x BN)
   // epilogue
   float* out_f32;          // [M][ldc] or null
   __half* out_f16;         // [M][ldc16] or null (hi part)

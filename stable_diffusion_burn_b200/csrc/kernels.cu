@@ -346,7 +346,7 @@ gn_apply_kernel(const GnSrc s0, const GnSrc s1, int bucket, int H, int W, int pi
   const int n = blockIdx.y;
   const int C0 = s0.C, C1 = s1.C, C = C0 + C1, gs = C / 32, HW = H * W;
   const int nb0 = C0 / bucket, nbt = C / bucket;
-  // fold of the producer's partial slots. A serial walk would be a chain of L2 round trips (~0.35 us each): the slots of one
+  // fold of the producer's partial slots. A serial walk would be a chain of L2 round trips: the slots of one
   // (bucket, stat) item are spread over `lanes` threads, four loads in flight each, and the lanes are combined in index order
   // (fixed order everywhere -> every CTA of the image derives bit-identical statistics)
   __shared__ double s_lane[512];
@@ -494,7 +494,7 @@ void gn_sums_from_partials_launch(const float* part, int cap, int slots, int nbk
   SDB_CUDA(cudaGetLastError());
 }
 
-int g_gn_apply_ctas = 592;  // measured (tools/step_time.py, ms per image): 1184 ?, 592 146.1, 296 149.3, 148 155.5
+int g_gn_apply_ctas = 0;  // 0: four CTAs per SM of the device
 void gn_apply_launch(const GnSrc& s0, const GnSrc& s1, int bucket, int n, int H, int W, int silu, const float* gamma,
                      const float* beta, float eps, Half2Ptr out, cudaStream_t st) {
   const int C = s0.C + s1.C, HW = H * W;
@@ -503,7 +503,8 @@ void gn_apply_launch(const GnSrc& s0, const GnSrc& s1, int bucket, int n, int H,
             "GroupNorm apply: channel / bucket geometry");
   // no co-residency constraint any more; every CTA repeats the fold of its image's partials (8-24 KB from L2), so the grid is
   // kept to g_gn_apply_ctas CTAs (4 per SM by default), at least one pixel each
-  int pix = (int)((((long long)HW * n) + g_gn_apply_ctas - 1) / g_gn_apply_ctas);
+  const int ctas = g_gn_apply_ctas > 0 ? g_gn_apply_ctas : 4 * g_num_sms;
+  int pix = (int)((((long long)HW * n) + ctas - 1) / ctas);
   if (pix < 1) pix = 1;
   dim3 grid(ceil_div(HW, pix), n);
   launch_k(gn_apply_kernel, grid, dim3(256), (size_t)2 * C * sizeof(float), st, s0, s1, bucket, H, W, pix, silu, gamma, beta, eps,
@@ -637,7 +638,7 @@ void convert_f16_launch(const float* x, long long count, Half2Ptr out, cudaStrea
   SDB_CHECK(count % 8 == 0, "convert count");
   const long long c8 = count / 8;
   int grid = (int)((c8 + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
   convert_f16_kernel<<<grid, 256, 0, st>>>(x, c8, out.hi, out.lo);
   SDB_CUDA(cudaGetLastError());
 }
@@ -663,14 +664,14 @@ __global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, int C, int HW, 
 void nchw_to_nhwc_launch(const float* x, int n, int C, int H, int W, float* y, cudaStream_t st) {
   const long long total = (long long)n * C * H * W;
   int grid = (int)((total + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
   nchw_to_nhwc_kernel<<<grid, 256, 0, st>>>(x, C, H * W, y, total);
   SDB_CUDA(cudaGetLastError());
 }
 void nhwc_to_nchw_launch(const float* x, int n, int C, int H, int W, float* y, cudaStream_t st) {
   const long long total = (long long)n * C * H * W;
   int grid = (int)((total + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
   nhwc_to_nchw_kernel<<<grid, 256, 0, st>>>(x, C, H * W, y, total);
   SDB_CUDA(cudaGetLastError());
 }
@@ -749,15 +750,14 @@ void conv3x3_cin4_launch(const float* x_nchw, int n, int H, int W, const float* 
 //   CTA = 8 x 32 output pixels, 256 threads, one pixel each; channels in chunks of 16. Per chunk the (8+2) x (32+2) halo tile is
 //   loaded (float4, 64 B contiguous per pixel), GroupNorm + SiLU applied on the way in, and stored channel-quad-major
 //   [4][pixel][4] so that the warp's float4 reads are conflict-free; the chunk's weights sit beside it (broadcast reads).
-// Each x element crosses HBM/L2 1.33 times (halo), against 9 times for the tap-by-tap warp-per-pixel kernel this replaces
-// (512 us -> ~70 us on the VAE's last conv).
+// Each x element crosses HBM/L2 1.33 times (halo), against 9 times for a tap-by-tap warp-per-pixel kernel.
 // TH = rows of the CTA tile (threads = 32 * TH): 8 for large images; 2 for small ones, where an 8-row tile would leave most SMs
-// idle (UNet conv_out at 64x64, batch 2: 32 CTAs with TH = 8 -> 140 us). With so few warps per SM nothing hides the latency of a
+// idle (UNet conv_out at 64x64, batch 2: 32 CTAs with TH = 8). With so few warps per SM nothing hides the latency of a
 // chunk's loads, so the small variant takes 64 channels per round (5 rounds for 320 channels instead of 20).
 // KS = channel-split groups inside the CTA (threads = 32 * TH * KS): group ks takes the channel chunks ks, ks + KS, ... with its own
 // halo tile and weight slice, and the groups' partial sums are added in group order at the end (deterministic). The small-image
 // variant uses it to put 10 warps on an SM instead of 2: at 64x64, batch 2 the 128 two-warp CTAs left every SM with two warps
-// and the kernel latency-bound at 136 us (ncu launch list, profiles/r2_launches_summary.md).
+// and the kernel latency-bound.
 template <int COUT, int TH, int CK, int KS = 1>
 __global__ void __launch_bounds__(32 * TH * KS)
 conv3x3_small_cout_kernel(const float* __restrict__ x, int H, int W, int C, const double* __restrict__ sums,
@@ -846,7 +846,7 @@ void conv3x3_small_cout_launch(const float* x, int n, int H, int W, int C, const
   SDB_CHECK(C % 16 == 0, "conv3x3_small_cout: channels must be a multiple of 16");
   // too few 8-row tiles to fill the machine -> 2-row tiles, 32 channels per round and group, the channel chunks split over
   // KS = 5 or 4 groups of two warps (10 / 8 warps per CTA; 320 = 10 x 32 and 512 = 16 x 32 channels)
-  const bool small = (long long)ceil_div(W, 32) * ceil_div(H, 8) * n < 2 * 148 && C % 32 == 0;
+  const bool small = (long long)ceil_div(W, 32) * ceil_div(H, 8) * n < 2 * g_num_sms && C % 32 == 0;
   const int ksplit = !small ? 1 : ((C / 32) % 5 == 0 ? 5 : ((C / 32) % 4 == 0 ? 4 : 1));
   const int th = small ? 2 : 8, ck = small ? 32 : 16;
   dim3 grid(ceil_div(W, 32), ceil_div(H, th), n), block(32 * th * ksplit);
@@ -946,7 +946,7 @@ void gemv_launch(const float* x, const float* W, const float* b, int K, int N, f
   launch_k(gemv_kernel, dim3(ceil_div(N, 32)), dim3(256), 0, st, x, (const int*)nullptr, W, b, K, N, 0, y);
   SDB_CUDA(cudaGetLastError());
 }
-// emb_silu = silu(lin2(silu(lin1(timestep_embedding(t)))))  — two multi-CTA GEMVs (was one CTA: 140 us)
+// emb_silu = silu(lin2(silu(lin1(timestep_embedding(t)))))  — two multi-CTA GEMVs
 void time_embed_launch(const int* t, const float* w1, const float* b1, const float* w2, const float* b2, float* hidden,
                        float* emb_silu, cudaStream_t st) {
   launch_k(gemv_kernel, dim3(40), dim3(256), 0, st, (const float*)nullptr, t, w1, b1, 320, 1280, 1, hidden);
@@ -1088,7 +1088,7 @@ __global__ void cfg_ddim_kernel(const float* __restrict__ eu, const float* __res
 void cfg_ddim_launch(const float* eps_u, const float* eps_c, float* latent, long long count, float scale,
                      float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st) {
   int grid = (int)((count + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
   launch_k(cfg_ddim_kernel, dim3(grid), dim3(256), 0, st, eps_u, eps_c, latent, count, scale, sqrt_one_minus_at, sqrt_at, sqrt_aprev, dir_coef);
   SDB_CUDA(cudaGetLastError());
 }
@@ -1100,7 +1100,7 @@ __global__ void cfg_combine_kernel(const float* __restrict__ eu, const float* __
 }
 void cfg_combine_launch(const float* eps_u, const float* eps_c, long long count, float scale, float* pred, cudaStream_t st) {
   int grid = (int)((count + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
   cfg_combine_kernel<<<grid, 256, 0, st>>>(eps_u, eps_c, count, scale, pred);
   SDB_CUDA(cudaGetLastError());
 }
@@ -1123,7 +1123,7 @@ __global__ void to_rgb8_kernel(const float* __restrict__ img, int HW, long long 
 void to_rgb8_launch(const float* img_nchw, int n, int H, int W, uint8_t* rgb, cudaStream_t st) {
   const long long total = (long long)n * 3 * H * W;
   int grid = (int)((total + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
   to_rgb8_kernel<<<grid, 256, 0, st>>>(img_nchw, H * W, total, rgb);
   SDB_CUDA(cudaGetLastError());
 }
@@ -1147,7 +1147,7 @@ __global__ void randn_kernel(float* __restrict__ x, long long count, uint32_t k0
 }
 void randn_launch(float* x, long long count, uint64_t seed, cudaStream_t st) {
   int grid = (int)((count + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
   randn_kernel<<<grid, 256, 0, st>>>(x, count, (uint32_t)seed * 2654435761u + 1u, (uint32_t)(seed >> 32) ^ 0x5bd1e995u);
   SDB_CUDA(cudaGetLastError());
 }
@@ -1171,7 +1171,7 @@ __global__ void pack_conv_kernel(const float* __restrict__ w, int Cout, int Cin,
 void pack_conv_launch(const float* w, int Cout, int Cin, int ksize, Half2Ptr out, cudaStream_t st) {
   const long long total = (long long)Cout * ksize * ksize * Cin;
   int grid = (int)((total + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
   pack_conv_kernel<<<grid, 256, 0, st>>>(w, Cout, Cin, ksize * ksize, out.hi, out.lo);
   SDB_CUDA(cudaGetLastError());
 }
@@ -1205,7 +1205,7 @@ __global__ void pack_conv_up2_kernel(const float* __restrict__ w, int Cout, int 
 void pack_conv_up2_launch(const float* w, int Cout, int Cin, Half2Ptr out, cudaStream_t st) {
   const long long total = (long long)16 * Cout * Cin;
   int grid = (int)((total + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
   pack_conv_up2_kernel<<<grid, 256, 0, st>>>(w, Cout, Cin, out.hi, out.lo);
   SDB_CUDA(cudaGetLastError());
 }
@@ -1276,7 +1276,7 @@ void pack_geglu_launch(const float* w, const float* b, int in, int h4, int half_
                        cudaStream_t st, const float* in_scale) {
   const long long total = (long long)2 * h4 * in;
   int grid = (int)((total + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
   pack_geglu_kernel<<<grid, 256, 0, st>>>(w, b, in, h4, half_tile, dst.hi, dst.lo, bias_packed, in_scale);
   SDB_CUDA(cudaGetLastError());
 }
@@ -1360,7 +1360,7 @@ __global__ void synth_fill_kernel(float* __restrict__ dst, long long count, uint
 }
 void synth_fill_launch(float* dst, long long count, uint32_t key, float bound, float offset, cudaStream_t st) {
   int grid = (int)((count + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
   synth_fill_kernel<<<grid, 256, 0, st>>>(dst, count, key, bound, offset);
   SDB_CUDA(cudaGetLastError());
 }
@@ -1387,7 +1387,7 @@ synth_fill_table_kernel(float* __restrict__ base, const SynthDesc* __restrict__ 
   }
 }
 void synth_fill_table_launch(float* base, const SynthDesc* d_desc, int ntensors, long long nchunks, cudaStream_t st) {
-  const int grid = (int)std::min<long long>(nchunks, 148 * 16);
+  const int grid = (int)std::min<long long>(nchunks, g_num_sms * 16);
   synth_fill_table_kernel<<<grid, 256, 0, st>>>(base, d_desc, ntensors, nchunks);
   SDB_CUDA(cudaGetLastError());
 }

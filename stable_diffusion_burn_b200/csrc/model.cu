@@ -729,7 +729,7 @@ static void run_resnet(Fwd& f, ResnetW& r, const Act& x, Act& out) {
 }
 
 // reference autoencoder/mod.rs:562-608: 1 head, d = C = 512, N = H*W tokens. S is materialised per image
-// (64 MB at 64x64) because the op runs once per image; q/k/v/proj are the same tcgen05 GEMMs.
+// (64 MB at 64x64) because the op runs once per image; q/k/v/proj are the same wgmma GEMMs.
 static void run_vae_attention(Fwd& f, VaeAttnW& a, const Act& x, Act& out) {
   Ctx& c = f.c;
   const size_t mark = c.work.off;

@@ -11,12 +11,13 @@
 
 namespace sdb {
 
-// Programmatic dependent launch (measured, tools/step_time.py, one process): off 155.3 ms/image; on with every kernel releasing its
-// dependents at entry 155.3 -> +1 % (early CTAs of the next kernel sit on the SMs while the GEMM still runs); on with the GEMMs
-// releasing them when their epilogue starts and loading their first weight tiles ahead of griddepcontrol.wait: -2.3 %.
+// Programmatic dependent launch: with every kernel releasing its dependents at entry, early CTAs of the next kernel sit on the
+// SMs while the GEMM still runs; the GEMMs therefore release them when their epilogue starts and load their first weight tiles
+// ahead of griddepcontrol.wait.
 // SDB_PDL=0 disables, 1 = release at entry everywhere, 2 (default) = late release in the GEMMs.
 int g_pdl_late = 1;
 bool g_pdl_enabled = true;
+int g_num_sms = 132;
 
 // ------------------------------------------------------------------ arena
 void Arena::init(size_t bytes) {
@@ -226,16 +227,9 @@ void run_attention(Ctx& c, const AttnOp& a) {
     const long long t0 = dbg_buf[255];
     auto rel = [&](int i) { return dbg_buf[i] ? dbg_buf[i] - t0 : -1; };
     fprintf(stderr, "attn_dbg nb=%d d=%d Nq=%d Nk=%d qk3=%d\n", a.nb, a.d, a.Nq, a.Nk, p.qk3);
-    for (int jj = 0; jj < 4; ++jj) {
-      for (int g = 0; g < 2; ++g)
-        fprintf(stderr, "  j=%d softmax g%d: wait_s %lld s_ready %lld loaded %lld max %lld pv_ok %lld rescaled %lld exps %lld p_arrive %lld\n", 8 + jj, g,
-                rel(g * 64 + jj * 8 + 0), rel(g * 64 + jj * 8 + 1), rel(g * 64 + jj * 8 + 2), rel(g * 64 + jj * 8 + 3), rel(g * 64 + jj * 8 + 4),
-                rel(g * 64 + jj * 8 + 5), rel(g * 64 + jj * 8 + 6), rel(g * 64 + jj * 8 + 7));
-      for (int g = 0; g < 2; ++g)
-        fprintf(stderr, "  j=%d mma g%d: qk(j+1) begin %lld k_ok %lld issued %lld | pv: v_ok %lld p_ok %lld issued %lld\n", 8 + jj, g,
-                rel(128 + jj * 16 + g * 8 + 0), rel(128 + jj * 16 + g * 8 + 4), rel(128 + jj * 16 + g * 8 + 1), rel(128 + jj * 16 + g * 8 + 5),
-                rel(128 + jj * 16 + g * 8 + 2), rel(128 + jj * 16 + g * 8 + 3));
-    }
+    for (int jj = 0; jj < 4; ++jj)
+      fprintf(stderr, "  j=%d softmax warpgroup 0: start %lld k_ready %lld s_done %lld max %lld rescaled %lld v_ready %lld pv_done %lld\n",
+              8 + jj, rel(jj * 8 + 0), rel(jj * 8 + 1), rel(jj * 8 + 2), rel(jj * 8 + 3), rel(jj * 8 + 4), rel(jj * 8 + 5), rel(jj * 8 + 6));
   }
 }
 
@@ -335,18 +329,13 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
   p.tiles_n = (a0.n + p.TN - 1) / p.TN;
   const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
 
-  // CTA pairs along M issue one cta_group::2 MMA (256 x BN): each CTA stages only half of the weight tile.
-  // Needs an even number of M tiles and no split-K (decided below).
-  bool pair = c.opt_cluster && (m_tiles % 2 == 0);
-  // N tile (measured per layer in profiles/r1_gemm_layers.md): 160 divides the UNet widths 320/640/1280 evenly
+  // N tile: 160 divides the UNet widths 320/640/1280 evenly
   int BN;
   if (ep.geglu)
     BN = 128;
-  else if (pair && c.opt_pair_bn256 && w.N % 256 == 0 && (long long)m_tiles * (w.N / 256) >= 64)
-    BN = 256;  // pair tile 256 x 256: the fewest operand bytes per FLOP
   else if (w.N % 160 == 0)
     BN = 160;
-  else if (w.N % 256 == 0 && (long long)m_tiles * (w.N / 256) >= 296)
+  else if (w.N % 256 == 0 && (long long)m_tiles * (w.N / 256) >= 2 * g_num_sms)
     BN = 256;
   else if (w.N % 128 == 0)
     BN = 128;
@@ -365,14 +354,13 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
   int split = 1;
   if (c.opt_splitk && kind != G_CONV3_UP2 && !ep.geglu && !ep.ln_out && !ep.ln_in) {
     const int ctas = m_tiles * n_tiles;
-    if (ctas <= 74 && iters >= c.opt_splitk_min_iters) {
-      // floor: ctas*split must stay within ONE wave of the 148 SMs (a 2-wave grid costs 2x, see profiles/r1);
+    if (ctas <= g_num_sms / 2 && iters >= c.opt_splitk_min_iters) {
+      // floor: ctas*split must stay within ONE wave of the SMs (one CTA per SM: a 2-wave grid costs 2x);
       // every split keeps >= 16 k-chunks so the rendezvous + fold stays small against its mainloop
-      split = std::min(std::min(148 / ctas, iters / c.opt_splitk_chunk), 16);
+      split = std::min(std::min(g_num_sms / ctas, iters / c.opt_splitk_chunk), 16);
       if (split < 1) split = 1;
     }
   }
-  p.cluster = pair ? 2 : 1;  // pairs and split-K compose: a cluster spans x only, both CTAs share blockIdx.z
   if (split > 1) {  // no empty K ranges: every split must own at least one iteration
     const int per = (iters + split - 1) / split;
     split = (iters + per - 1) / per;
@@ -381,9 +369,9 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
   static const bool gemm_dbg = getenv("SDB_GEMM_DBG") != nullptr || getenv("SDB_LABEL_LOG") != nullptr;
   if (c.debug_sync || c.profiling || gemm_dbg) {
     char buf[256];
-    snprintf(buf, sizeof(buf), "gemm kind=%d n=%d H=%d W=%d P=%d C0=%d C1=%d N=%d K=%d xk=%d BN=%d split=%d passes=%d geglu=%d epi=%s%s tile=%dx%dx%d cluster=%d",
+    snprintf(buf, sizeof(buf), "gemm kind=%d n=%d H=%d W=%d P=%d C0=%d C1=%d N=%d K=%d xk=%d BN=%d split=%d passes=%d geglu=%d epi=%s%s tile=%dx%dx%d",
              kind, a0.n, a0.H, a0.W, a0.P, a0.C, a1in ? a1.C : 0, w.N, w.K, p.xkc * 64, BN, split, passes, ep.geglu,
-             ep.gn ? "gn" : (ep.ln_out ? "lns" : (ep.ln_in ? "lnc" : "-")), ep.residual16.hi ? "+r16" : (ep.residual ? "+r32" : ""), p.TN, p.TH, p.TW, p.cluster);
+             ep.gn ? "gn" : (ep.ln_out ? "lns" : (ep.ln_in ? "lnc" : "-")), ep.residual16.hi ? "+r16" : (ep.residual ? "+r32" : ""), p.TN, p.TH, p.TW);
     c.dbg_label = buf;
   }
 
@@ -476,7 +464,7 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
     const __half* whi = w.p.hi;
     const __half* wlo = w.p.lo;
     const int wrows = (w.rows ? w.rows : w.N) * phases_out;
-    const int bbox = pair ? BN / 2 : BN;
+    const int bbox = BN;
     maps.b[0] = make_w_map(whi, w.K, wrows, bbox, w.ld);
     maps.b[1] = maps.b[0];
     if (passes >= 3) maps.b[1] = make_w_map(wlo, w.K, wrows, bbox, w.ld);
@@ -498,7 +486,7 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
       const size_t need = (size_t)split * (size_t)Mtot * w.N * sizeof(float);
       p.ws = reinterpret_cast<float*>(c.work.alloc(need));
       SDB_CHECK((long long)m_tiles * n_tiles * 2 <= 65536, "split-K ticket buffer");
-      SDB_CHECK((long long)m_tiles * n_tiles * split <= 148, "split-K CTAs must be co-resident");
+      SDB_CHECK((long long)m_tiles * n_tiles * split <= g_num_sms, "split-K CTAs must be co-resident");
       p.tickets = c.splitk_tickets;
     }
     {

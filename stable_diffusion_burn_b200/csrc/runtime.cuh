@@ -125,7 +125,6 @@ struct Ctx {
   int opt_precision = 0;  // 0 = per-layer policy, 1/2/3 = force
   int opt_graphs = 1;
   int opt_splitk = 1;
-  int opt_pair_bn256 = 0;
   int opt_splitk_min_iters = 32, opt_splitk_chunk = 8;  // split-K: shortest K loop that is split, k-chunks kept per split
   int opt_skip_merge = 1; // ResBlock skip 1x1 conv folded into conv_out's K loop (needs raw16)
   int opt_raw16 = 1;      // epilogues also write the fp16 hi/lo copy a later raw-operand consumer needs (no staging launch)
@@ -133,9 +132,7 @@ struct Ctx {
   int opt_attn_split = 1;   // fused attention on the 3-pass levels takes q / k as fp16 hi + lo pairs (fp32-class logits)
   int opt_emb_hoist = 1;    // sample_latent computes the time-embedding rows of every timestep once per call (not once per step)
   int opt_prefetch_w = 0;   // 1: weight-bound GEMMs (<= 4 M tiles) prefetch their weight strip into L2 ahead of griddepcontrol.wait.
-                            // Measured off (tools/step_time.py, same process): 143.38 ms per image with it, 142.59 ms without
   int opt_gn_epilogue = 1;  // GroupNorm statistics produced by the GEMM epilogue that writes the tensor (no stats pass, no rendezvous)
-  int opt_cluster = 1;    // CTA pairs issue cta_group::2 MMAs (256 x BN) wherever the M-tile count is even and K is not split
   // profiling
   bool profiling = false;
   std::vector<ProfEvent> prof;
@@ -179,7 +176,7 @@ struct ExtraK {
   WeightOp w;  // [N][x0.C + x1.C]
 };
 
-// one tcgen05 GEMM / implicit conv (+ split-K reduction when chosen)
+// one wgmma GEMM / implicit conv (+ split-K reduction when chosen)
 //   a0 (+a1 = channel concat), geometry kind, weights, passes (1..3), epilogue
 void run_gemm(Ctx& c, int kind, const ActOp& a0, const ActOp* a1, const WeightOp& w, int passes, const Epilogue& ep,
               const ExtraK* xk = nullptr);

@@ -6,7 +6,7 @@ Same names, argument meaning and error behaviour as
   Autoencoder::decode_latent                                       src/model/autoencoder/mod.rs:68-71
 Tensors are numpy fp32 arrays with the reference's shapes (NCHW, [n, L, 768]); errors raise
 (the reference panics). No computation happens in Python and there is no fallback path: every call
-goes to libsdb200.so and fails loudly if the CUDA library or a B200 is missing.
+goes to libsdb200.so and fails loudly if the CUDA library or an H100 is missing.
 
 Differences forced by the tier (documented in DESIGN.md): the initial latent is an explicit argument
 (the reference draws it from an unseeded backend RNG) and H/W are parameters (the reference hard-codes 64x64).

@@ -22,7 +22,7 @@ _PATTERN = r"(?i)<\|startoftext\|>|<\|endoftext\|>|'s|'t|'re|'ve|'m|'ll|'d|\p{L}
 
 
 def find_vocab(path: str | None = None) -> str:
-    cands = [path, os.environ.get("SDB_BPE_VOCAB"), VOCAB_FILE, os.path.join("/root/reference", VOCAB_FILE)]
+    cands = [path, os.environ.get("SDB_BPE_VOCAB"), VOCAB_FILE]
     for c in cands:
         if c and os.path.isfile(c):
             return c

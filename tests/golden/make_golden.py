@@ -57,11 +57,9 @@ def enc_golden():
     keep = {}
     with torch.no_grad():
         for name, img in enc_images().items():
-            taps = {}
-            y = O.encode_image(P, torch.from_numpy(img), taps=taps)
+            y = O.encode_image(P, torch.from_numpy(img))
             keep["img:" + name] = img
             keep["lat:" + name] = y.numpy()
-            keep["mid:" + name] = taps["mid"].numpy()
             print("vae_enc", name, tuple(y.shape), "rms", float(y.pow(2).mean().sqrt()), flush=True)
     np.savez_compressed(os.path.join(OUT, "vae_enc.npz"), **keep)
 
@@ -108,13 +106,12 @@ def round2_cases(P):
             lat = O.sample_latent(P, ctx, unc, 7.5, 20, init, taps=taps)
             print("sample_20step latent", time.time() - t1, flush=True)
             imgf = O.latent_to_image_f32(P, lat)
-            keep = {"latent": lat.numpy(), "u8_sub": O.to_u8(imgf)[:, ::2, ::2, :].copy(), "img_f32_sub": imgf[:, ::4, ::4, :].numpy().copy()}
+            keep = {"latent": lat.numpy(), "u8_sub": O.to_u8(imgf)[:, ::2, ::2, :].copy()}
             ts, _ = O.ddim_timesteps(20)
             for i in (0, 9, 19):
                 keep[f"step{i}:t"] = np.int32(ts[i])
-                for k in ("latent_in", "uncond", "cond", "latent"):
+                for k in ("latent_in", "uncond", "cond"):
                     keep[f"step{i}:{k}"] = taps[f"step{i}/{k}"].numpy()
-            keep["latent_rms_per_step"] = np.asarray([float(taps[f"step{i}/latent"].pow(2).mean().sqrt()) for i in range(20)], np.float32)
             np.savez_compressed(os.path.join(OUT, "sample_20step.npz"), **keep)
 
 
@@ -156,13 +153,8 @@ def main():
             if ONLY and name not in ONLY:
                 continue
             t1 = time.time()
-            taps = {}
-            y = O.unet_forward(P, x, t, ctx, taps=taps)
+            y = O.unet_forward(P, x, t, ctx)
             keep = {"out": y.numpy()}
-            for k in ("emb", "input_blocks/conv", "input_blocks/rt1", "input_blocks/d1", "input_blocks/r2", "middle_block",
-                      "output_blocks/ru", "output_blocks/rt7"):
-                v = taps[k].numpy()
-                keep["tap:" + k] = v if v.size <= 70000 else v.reshape(-1)[:: max(1, v.size // 65536)][:65536].copy()
             np.savez_compressed(os.path.join(OUT, f"unet_{name}.npz"), **keep)
             print(name, time.time() - t1, "rms", float(y.pow(2).mean().sqrt()), flush=True)
         if ONLY and "vae" not in ONLY:

@@ -1,5 +1,5 @@
-"""Generates tests/golden/ref_python.npz: outputs of the REFERENCE'S OWN Python model (/root/reference/python/dump.py, run
-unmodified on tests/ref_shim/tinygrad) on this repo's synthetic weights (seed 0). Needs /root/reference (this container only).
+"""Generates tests/golden/ref_python.npz: outputs of the REFERENCE'S OWN Python model (python/dump.py of the reference checkout, run
+unmodified on tests/ref_shim/tinygrad) on this repo's synthetic weights (seed 0). Needs the reference checkout: set SDB_REFERENCE_DIR to it.
 
   python tests/ref_shim/make_ref_golden.py
 

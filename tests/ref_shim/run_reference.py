@@ -1,4 +1,4 @@
-"""Runs the reference's own Python model (/root/reference/python/dump.py, imported unmodified) on the tinygrad stand-in.
+"""Runs the reference's own Python model (python/dump.py of the reference checkout named by SDB_REFERENCE_DIR, imported unmodified) on the tinygrad stand-in.
 
 TEST INFRASTRUCTURE. What is reference-authored here: the model topology and op sequence (python/dump.py:24-350, 352-461),
 the savers that define the dump-dir names, transposes and metadata the Rust loaders read (python/save.py, unet.py,
@@ -14,7 +14,7 @@ import sys
 import numpy as np
 import torch
 
-REF_PY = "/root/reference/python"
+REF_PY = os.path.join(os.environ.get("SDB_REFERENCE_DIR", ""), "python")
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 
@@ -24,7 +24,7 @@ def available() -> bool:
 
 
 def load_dump_module():
-    """import /root/reference/python/dump.py with the stand-in `tinygrad` package ahead of everything else."""
+    """import the reference's python/dump.py with the stand-in `tinygrad` package ahead of everything else."""
     for p in (HERE, REF_PY):
         if p not in sys.path:
             sys.path.insert(0, p)

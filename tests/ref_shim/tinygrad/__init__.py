@@ -1,4 +1,4 @@
-"""Minimal stand-in for tinygrad 0.9.2 (TEST INFRASTRUCTURE, see ../README.md): only what /root/reference/python uses."""
+"""Minimal stand-in for tinygrad 0.9.2 (TEST INFRASTRUCTURE, see ../README.md): only what the reference's python/ directory uses."""
 from .tensor import Tensor  # noqa: F401
 
 

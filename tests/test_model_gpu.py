@@ -63,9 +63,8 @@ def test_attention(ctx, n, Nq, Nk, C, heads):
 
 
 def test_attention_register_split_bit_identical(ctx):
-    """option attn_regsplit = 1: the two-query-tile launches run a register-split variant (setmaxnreg moves registers from the
-    TMA / MMA warpgroup to the softmax warpgroups: no spills; measured neutral, so off by default). Same arithmetic in the same
-    order -> bit-identical to the 10-warp variant."""
+    """option attn_regsplit = 1: the launches run a register-split variant (setmaxnreg moves registers from the TMA producer
+    warpgroup to the softmax warpgroups). Same arithmetic in the same order -> bit-identical to the variant without it."""
     rng = np.random.default_rng(11)
     for n, Nq, Nk, C, heads in [(1, 4096, 4096, 320, 8), (2, 1024, 1024, 640, 8), (2, 256, 77, 320, 8), (1, 200, 300, 640, 8)]:
         q = rng.standard_normal((n, Nq, C)).astype(np.float32)

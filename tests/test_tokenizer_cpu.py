@@ -1,21 +1,27 @@
 """The reference's only test, reproduced (src/tokenizer.rs:205-221): the one golden vector the reference holds."""
+import gzip
 import os
 
 import pytest
 
 from stable_diffusion_burn_b200 import tokenizer as T
 
-try:
-    VOCAB = T.find_vocab()
-except FileNotFoundError:
-    VOCAB = None
-
-pytestmark = pytest.mark.skipif(VOCAB is None, reason="bpe_simple_vocab_16e6.txt (reference data file) not available")
+# the part of the CLIP BPE vocabulary the tokenizer reads: the first 48895 lines of bpe_simple_vocab_16e6.txt (the version header
+# and the 48894 merges), gzipped
+GOLD_VOCAB = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "bpe_simple_vocab_16e6_head.txt.gz")
 
 
 @pytest.fixture(scope="module")
-def tok():
-    return T.SimpleTokenizer(VOCAB)
+def vocab(tmp_path_factory):
+    path = tmp_path_factory.mktemp("vocab") / T.VOCAB_FILE
+    with gzip.open(GOLD_VOCAB, "rb") as f:
+        path.write_bytes(f.read())
+    return str(path)
+
+
+@pytest.fixture(scope="module")
+def tok(vocab):
+    return T.SimpleTokenizer(vocab)
 
 
 def test_reference_kat_encode_decode(tok):
@@ -41,12 +47,12 @@ def test_cleaning_quirks(tok):
     assert tok.decode(tok.encode("café ☕")).strip() == "café ☕"
 
 
-def test_agrees_with_an_independent_clip_tokenizer(tok, tmp_path):
+def test_agrees_with_an_independent_clip_tokenizer(tok, vocab, tmp_path):
     """Second opinion on the mirror: transformers.CLIPTokenizer (independently written from the same published BPE) built from the
     same merges file must produce the same ids on plain prompts (no ftfy-specific cleaning involved)."""
     tr = pytest.importorskip("transformers")
     import json
-    merges = open(VOCAB, encoding="utf-8").read().split("\n")[1:49152 - 256 - 2 + 1]
+    merges = open(vocab, encoding="utf-8").read().split("\n")[1:49152 - 256 - 2 + 1]
     vocab = [u for _, u in T._byte_unicode_table()]
     vocab = vocab + [v + "</w>" for v in vocab] + ["".join(m.split()) for m in merges] + ["<|startoftext|>", "<|endoftext|>"]
     (tmp_path / "vocab.json").write_text(json.dumps({v: i for i, v in enumerate(vocab)}))

@@ -1,6 +1,6 @@
 """Timeline probe of the fused attention kernel. With SDB_ATTN_DBG=1 every launch prints clock64 stamps of CTA (0,0,0) for key
-tiles 8..11: when each softmax group saw S ready / had copied it out / knew its max / saw PV(j-1) done / finished its exponentials,
-and when the MMA warp issued QK(j+1) and PV(j).   SDB_ATTN_DBG=1 python tools/micro_attn.py [regsplit]"""
+tiles 8..11, taken by the first softmax warpgroup: tile start, K ready, S = QK^T done, row maxima, O rescaled, V ready, PV done.
+   SDB_ATTN_DBG=1 python tools/micro_attn.py [regsplit]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

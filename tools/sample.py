@@ -59,7 +59,7 @@ def parse_args(argv):
             except ValueError:
                 dev = 0
         elif d in ("cpu", "mps"):
-            print(f"Device {d}: this library runs on sm_100a GPUs only (no CPU fallback)", file=sys.stderr)
+            print(f"Device {d}: this library runs on sm_90a (H100) GPUs only (no CPU fallback)", file=sys.stderr)
             raise SystemExit(1)
         else:
             print(f"Unknown device: {argv[7]}", file=sys.stderr)
