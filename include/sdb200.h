@@ -186,9 +186,12 @@ int sdb_test_groupnorm(sdb_ctx* ctx, const float* x, const float* gamma, const f
 /* LayerNorm over the last dim, [rows, c]. */
 int sdb_test_layernorm(sdb_ctx* ctx, const float* x, const float* gamma, const float* beta, int rows, int c,
                        float* y);
-/* qkv_attention (src/model/attention.rs:5-45): q [n,Nq,C], k,v [n,Nk,C], heads -> out [n,Nq,C]. */
+/* qkv_attention (src/model/attention.rs:5-45): q [n,Nq,C], k,v [n,Nk,C], heads -> out [n,Nq,C].
+ * kvlen: host array [n], sample s attends to its first kvlen[s] keys (each in [1, Nk], else an error); NULL = Nk for all.
+ * flags: 1 = causal mask (key j visible to query i only if j <= i; Nk <= 128), 2 = V transposed, staged as the CLIP encoder
+ * stages it (q / k as single fp16 values in one matrix, V^T; needs Nq == Nk and C / heads a multiple of 16). */
 int sdb_test_attention(sdb_ctx* ctx, const float* q, const float* k, const float* v, int n, int Nq, int Nk,
-                       int C, int heads, float* out);
+                       int C, int heads, const int32_t* kvlen, int flags, float* out);
 
 #ifdef __cplusplus
 }

@@ -74,7 +74,8 @@ SIGNATURES = [
                                           C.c_int, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int)]),
     ("sdb_test_groupnorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_test_layernorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, _f32p]),
-    ("sdb_test_attention", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
+    ("sdb_test_attention", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                     C.POINTER(C.c_int32), C.c_int, _f32p]),
 ]
 
 _lib = None
@@ -347,9 +348,16 @@ class Context:
         self.check(self.lib.sdb_test_layernorm(self.h, ptr(x), ptr(g), ptr(b), rows, c, ptr(y)))
         return y
 
-    def test_attention(self, q, k, v, heads):
+    def test_attention(self, q, k, v, heads, kvlen=None, causal=False, v_transposed=False):
+        """kvlen: per-sample key counts (None = all Nk keys); causal: key j visible to query i only if j <= i;
+        v_transposed: the CLIP layout (V^T, single fp16 q / k)."""
         q = f32(q); k = f32(k); v = f32(v)
         n, Nq, Cc = q.shape; Nk = k.shape[1]
         out = np.empty_like(q)
-        self.check(self.lib.sdb_test_attention(self.h, ptr(q), ptr(k), ptr(v), n, Nq, Nk, Cc, heads, ptr(out)))
+        lens = None if kvlen is None else np.ascontiguousarray(kvlen, dtype=np.int32)
+        assert lens is None or lens.shape == (n,), "kvlen needs one length per sample"
+        flags = (1 if causal else 0) | (2 if v_transposed else 0)
+        self.check(self.lib.sdb_test_attention(self.h, ptr(q), ptr(k), ptr(v), n, Nq, Nk, Cc, heads,
+                                               None if lens is None else lens.ctypes.data_as(C.POINTER(C.c_int32)), flags,
+                                               ptr(out)))
         return out

@@ -789,10 +789,10 @@ int sdb_test_layernorm(sdb_ctx* ctx, const float* x, const float* gamma, const f
 }
 
 int sdb_test_attention(sdb_ctx* ctx, const float* q, const float* k, const float* v, int n, int Nq, int Nk, int C,
-                       int heads, float* out) {
+                       int heads, const int32_t* kvlen, int flags, float* out) {
   API_BEGIN(ctx)
   c.work.reset();
-  model_test_attention(c, q, k, v, n, Nq, Nk, C, heads, out);
+  model_test_attention(c, q, k, v, n, Nq, Nk, C, heads, kvlen, flags, out);
   API_END
 }
 

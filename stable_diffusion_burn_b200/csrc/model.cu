@@ -1337,8 +1337,67 @@ void model_clip_forward_host(Ctx& c, const int* tokens, int n, int L, float* out
 }
 
 // ================================================================================ attention unit-test entry
+// V transposed (flags & 2): stages q / k / V^T exactly as model_clip_forward_dev does
+static void test_attention_vt(Ctx& c, const float* q, const float* k, const float* v, int n, int L, int C, int heads,
+                              const int* lens, bool causal, float* out) {
+  const int d = C / heads;
+  SDB_CHECK(d % 16 == 0, "test_attention: V transposed needs a head dim that is a multiple of 16");
+  const int Lp = round_up(L, 8), Mr = n * Lp, Mp = round_up(Mr, 32);
+  // q | k in one [n*Lp][2C] matrix (single fp16 values), V^T [C][Mp] with sample s at columns s*Lp; pad rows / columns zero
+  std::vector<__half> hqk((size_t)Mr * 2 * C, __float2half(0.f)), hvT((size_t)C * Mp, __float2half(0.f));
+  for (int s = 0; s < n; ++s)
+    for (int i = 0; i < L; ++i)
+      for (int j = 0; j < C; ++j) {
+        const size_t src = ((size_t)s * L + i) * C + j, row = (size_t)s * Lp + i;
+        hqk[row * 2 * C + j] = __float2half(q[src]);
+        hqk[row * 2 * C + C + j] = __float2half(k[src]);
+        hvT[(size_t)j * Mp + row] = __float2half(v[src]);
+      }
+  __half* dqk = c.work.get<__half>(hqk.size());
+  __half* dvT = c.work.get<__half>(hvT.size());
+  Half2Ptr o16;
+  o16.hi = c.work.get<__half>((size_t)Mr * C);
+  o16.lo = c.work.get<__half>((size_t)Mr * C);
+  int* dlen = lens ? c.work.get<int>(n) : nullptr;
+  SDB_CUDA(cudaMemcpyAsync(dqk, hqk.data(), hqk.size() * 2, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(dvT, hvT.data(), hvT.size() * 2, cudaMemcpyHostToDevice, c.stream));
+  if (lens) SDB_CUDA(cudaMemcpyAsync(dlen, lens, n * 4, cudaMemcpyHostToDevice, c.stream));
+  AttnOp at;
+  at.q = dqk, at.ldq = 2 * C, at.q_col0 = 0, at.q_rows = Lp;
+  at.k = dqk, at.ldk = 2 * C, at.k_col0 = C, at.k_rows = Lp;
+  at.vT = dvT, at.ldv = Mp;
+  at.nb = n, at.heads = heads, at.d = d, at.dpad = d, at.Nq = L, at.Nk = L;
+  at.kvlen = dlen;
+  at.causal = causal ? 1 : 0;
+  at.out = o16, at.ldo = C;
+  run_attention(c, at);
+  std::vector<__half> hi((size_t)Mr * C), lo((size_t)Mr * C);
+  SDB_CUDA(cudaMemcpyAsync(hi.data(), o16.hi, hi.size() * 2, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, lo.size() * 2, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  for (int s = 0; s < n; ++s)
+    for (int i = 0; i < L; ++i)
+      for (int j = 0; j < C; ++j) {
+        const size_t src = ((size_t)s * Lp + i) * C + j;
+        out[((size_t)s * L + i) * C + j] = __half2float(hi[src]) + __half2float(lo[src]);
+      }
+}
+
 void model_test_attention(Ctx& c, const float* q, const float* k, const float* v, int n, int Nq, int Nk, int C, int heads,
-                          float* out) {
+                          const int32_t* kvlen, int flags, float* out) {
+  SDB_CHECK(n >= 1 && Nq >= 1 && Nk >= 1 && heads >= 1 && C % heads == 0, "test_attention: shapes");
+  SDB_CHECK((flags & ~3) == 0, "test_attention: flags are 1 (causal) | 2 (V transposed)");
+  // the kernel clamps a device-side length into [1, Nk] (it cannot report an error); this entry rejects it instead
+  std::vector<int> lens(n, Nk);
+  if (kvlen)
+    for (int s = 0; s < n; ++s) {
+      SDB_CHECK(kvlen[s] >= 1 && kvlen[s] <= Nk, "test_attention: every kvlen must be in [1, Nk]");
+      lens[s] = kvlen[s];
+    }
+  if (flags & 2) {
+    SDB_CHECK(Nq == Nk, "test_attention: V transposed stages q and k in one matrix (CLIP layout): Nq must equal Nk");
+    return test_attention_vt(c, q, k, v, n, Nk, C, heads, kvlen ? lens.data() : nullptr, flags & 1, out);
+  }
   // stages q / k|v exactly as the SpatialTransformer does: head-padded rows, V row-major beside K (consumed MN-major)
   const int d = C / heads, dpad = (d % 16 == 0) ? d : (d + 15) / 16 * 16, hd = heads * dpad;
   const int Nkp = round_up(Nk, 8);
@@ -1369,8 +1428,7 @@ void model_test_attention(Ctx& c, const float* q, const float* k, const float* v
   Half2Ptr o16;
   o16.hi = c.work.get<__half>((size_t)n * Nq * C);
   o16.lo = c.work.get<__half>((size_t)n * Nq * C);
-  int* dlen = c.work.get<int>(n);
-  std::vector<int> lens(n, Nk);
+  int* dlen = c.work.get<int>(n);  // always set: the key matrix is padded to Nkp rows per sample
   SDB_CUDA(cudaMemcpyAsync(dq, hq.data(), hq.size() * 2, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaMemcpyAsync(dkv, hkv.data(), hkv.size() * 2, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaMemcpyAsync(dlen, lens.data(), n * 4, cudaMemcpyHostToDevice, c.stream));
@@ -1381,6 +1439,7 @@ void model_test_attention(Ctx& c, const float* q, const float* k, const float* v
   at.q_lo = dq_lo, at.k_lo = dkv_lo;  // used by the head dims that have the split-product kernel (40, 80) unless attn_split = 0
   at.nb = n, at.heads = heads, at.d = d, at.dpad = dpad, at.Nq = Nq, at.Nk = Nkp;
   at.kvlen = dlen;
+  at.causal = flags & 1;
   at.out = o16, at.ldo = C;
   run_attention(c, at);
   std::vector<__half> hi((size_t)n * Nq * C), lo((size_t)n * Nq * C);

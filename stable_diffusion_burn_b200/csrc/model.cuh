@@ -34,6 +34,6 @@ bool npy_read_f32(const std::string& file, std::vector<float>& out);
 long long dump_tensor_read(const std::string& file, int ndim, int64_t* dims, std::vector<float>& payload);
 void model_load_dump_dir(Ctx& c, const char* root);
 void model_test_attention(Ctx& c, const float* q, const float* k, const float* v, int n, int Nq, int Nk, int C, int heads,
-                          float* out);
+                          const int32_t* kvlen, int flags, float* out);
 
 }  // namespace sdb

@@ -9,6 +9,8 @@ import torch
 
 from stable_diffusion_burn_b200 import synth, topology
 
+import attn_profiles as AP
+
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 UNET_TOL = 1.0e-3
@@ -62,24 +64,127 @@ def test_attention(ctx, n, Nq, Nk, C, heads):
             ctx.set_option("attn_split", 1)
 
 
+def _attn_ref(q, k, v, heads, split, kvlen=None, mask=None):
+    """fp64 attention on operands rounded the way the kernel consumes them: q / k exact with the split product, else fp16;
+    v fp16. kvlen: sample s sees only its first kvlen[s] keys."""
+    from oracle import sd_oracle as O
+    q64, k64 = ((torch.from_numpy(a).double() if split else torch.from_numpy(a).half().double()) for a in (q, k))
+    v64 = torch.from_numpy(v).half().double()
+    if kvlen is None:
+        return O.qkv_attention(q64, k64, v64, heads, mask=mask).numpy()
+    return np.concatenate([O.qkv_attention(q64[s:s + 1], k64[s:s + 1, :L], v64[s:s + 1, :L], heads, mask=mask).numpy()
+                           for s, L in enumerate(kvlen)])
+
+
+def _check_attn(name, out, ref):
+    e2, em = rel(out, ref), relmax(out, ref)
+    print(f"{name}: rel L2 {e2:.3e} max/max {em:.3e}")
+    assert np.isfinite(out).all() and e2 < 1e-3 and em < 2e-3, name
+
+
+def _kvlen_inputs(rng, n, Nq, Nk, C, lens):
+    """q, k, v with the rows past each sample's length zeroed, and k, v with those rows holding large finite values instead"""
+    q = rng.standard_normal((n, Nq, C)).astype(np.float32)
+    k = rng.standard_normal((n, Nk, C)).astype(np.float32)
+    v = rng.standard_normal((n, Nk, C)).astype(np.float32)
+    kj, vj = k.copy(), v.copy()
+    for s, L in enumerate(lens):
+        k[s, L:] = 0.0
+        v[s, L:] = 0.0
+        sign = lambda: rng.choice(np.float32([-1.0, 1.0]), (Nk - L, C))
+        kj[s, L:] = sign() * rng.uniform(6.0, 8.0, (Nk - L, C))
+        vj[s, L:] = sign() * rng.uniform(2.0e4, 3.0e4, (Nk - L, C))
+    return q, k, v, kj, vj
+
+
+# per-sample key lengths: n = len(lens); Nk is the padded key count of the batch
+ATTN_KVLEN = [  # Nq, Nk, C, heads, lens
+    (4096, 96, 320, 8, [2, 77]),  # level 0 of the guided (CFG) batch: unconditional | prompt keys, padded to 96
+    (1024, 96, 640, 8, [2, 77]),
+    (256, 96, 1280, 8, [1, 63, 64, 65, 77]),  # d = 160: both sides of the 64-key sub-tile boundary
+    (200, 300, 320, 8, [1, 128, 129, 300]),  # key-tile boundary and a partial last tile
+]
+
+
+@pytest.mark.parametrize("Nq,Nk,C,heads,lens", ATTN_KVLEN)
+def test_attention_kvlen(ctx, Nq, Nk, C, heads, lens):
+    """sample s attends only to its first lens[s] keys; whatever the rows past them hold (here up to |k| = 8, |v| = 3e4),
+    the output is bit-identical to the run where they are zero: masked keys are dropped by select before the max and the sum"""
+    rng = np.random.default_rng(Nq + Nk + C + len(lens))
+    q, k, v, kj, vj = _kvlen_inputs(rng, len(lens), Nq, Nk, C, lens)
+    d = C // heads
+    for split in ((1, 0) if d in (40, 80) else (1,)):
+        ctx.set_option("attn_split", split)
+        try:
+            out = ctx.test_attention(q, k, v, heads, kvlen=lens)
+            junk = ctx.test_attention(q, kj, vj, heads, kvlen=lens)
+        finally:
+            ctx.set_option("attn_split", 1)
+        _check_attn(f"kvlen {lens} d={d} split={split}", out, _attn_ref(q, k, v, heads, split and d in (40, 80), kvlen=lens))
+        assert np.array_equal(out, junk), (lens, split)
+
+
+def test_attention_rejects_bad_arguments(ctx):
+    from stable_diffusion_burn_b200._lib import SdbError
+    q = np.zeros((2, 8, 320), np.float32)
+    kv = np.zeros((2, 16, 320), np.float32)
+    for lens in ([0, 16], [1, 17], [-1, 4]):  # the kernel would clamp these; the entry refuses them
+        with pytest.raises(SdbError, match="kvlen"):
+            ctx.test_attention(q, kv, kv, 8, kvlen=lens)
+    # the causal mask is applied inside the first key tile only: longer causal sequences are refused on the host
+    x = np.zeros((2, 129, 768), np.float32)
+    for vt in (True, False):
+        with pytest.raises(SdbError, match="at most 128 keys"):
+            ctx.test_attention(x, x, x, 12, causal=True, v_transposed=vt)
+
+
+@pytest.mark.parametrize("L", [1, 2, 8, 20, 77])
+def test_attention_clip(ctx, L):
+    """the CLIP text encoder's attention: d = 64, causal, V transposed, single fp16 q / k"""
+    from oracle import sd_oracle as O
+    rng = np.random.default_rng(100 + L)
+    n, C, heads = 2, 768, 12
+    q, k, v = (rng.standard_normal((n, L, C)).astype(np.float32) for _ in range(3))
+    out = ctx.test_attention(q, k, v, heads, causal=True, v_transposed=True)
+    _check_attn(f"clip L={L}", out, _attn_ref(q, k, v, heads, False, mask=O.attn_decoder_mask(L, torch.float64)))
+
+
+RESCALE = [(p, d) for p, (_, dims) in AP.PROFILES.items() for d in dims]
+
+
+@pytest.mark.parametrize("profile,d", RESCALE)
+def test_attention_rescale(ctx, profile, d):
+    """logit profiles that make the lazy rescale of the running maximum fire (or stay off) in known ways
+    (tests/attn_profiles.py; tests/test_attn_profiles_cpu.py checks each profile against the kernel's rule)"""
+    q, k, v = AP.make_case(profile, d)
+    _check_attn(f"rescale {profile} d={d}", ctx.test_attention(q, k, v, AP.HEADS), _attn_ref(q, k, v, AP.HEADS, d in (40, 80)))
+
+
 def test_attention_register_split_bit_identical(ctx):
     """option attn_regsplit = 1: the launches run a register-split variant (setmaxnreg moves registers from the TMA producer
     warpgroup to the softmax warpgroups). Same arithmetic in the same order -> bit-identical to the variant without it."""
     rng = np.random.default_rng(11)
-    for n, Nq, Nk, C, heads in [(1, 4096, 4096, 320, 8), (2, 1024, 1024, 640, 8), (2, 256, 77, 320, 8), (1, 200, 300, 640, 8)]:
-        q = rng.standard_normal((n, Nq, C)).astype(np.float32)
-        k = rng.standard_normal((n, Nk, C)).astype(np.float32)
-        v = rng.standard_normal((n, Nk, C)).astype(np.float32)
+    cases = []  # name, q, k, v, heads, keyword arguments
+    for n, Nq, Nk, C, heads in [(1, 4096, 4096, 320, 8), (2, 1024, 1024, 640, 8), (2, 256, 77, 320, 8), (1, 200, 300, 640, 8),
+                                (2, 256, 300, 1280, 8)]:
+        q, k, v = (rng.standard_normal((n, N, C)).astype(np.float32) for N in (Nq, Nk, Nk))
+        cases.append((f"{n}x{Nq}x{Nk} C={C}", q, k, v, heads, {}))
+    q, k, v = (rng.standard_normal((2, 77, 768)).astype(np.float32) for _ in range(3))
+    cases.append(("clip", q, k, v, 12, dict(causal=True, v_transposed=True)))
+    q, _, _, kj, vj = _kvlen_inputs(rng, 2, 4096, 96, 320, [2, 77])
+    cases.append(("kvlen", q, kj, vj, 8, dict(kvlen=[2, 77])))
+    cases.append(("rescale creep", *AP.make_case("creep", 40), AP.HEADS, {}))
+    for name, q, k, v, heads, kw in cases:
         for split in (1, 0):  # split q / k operands (<48,2,QK3>) and the single-operand kernels (<48,2>, <80,2>)
             ctx.set_option("attn_split", split)
             try:
-                a = ctx.test_attention(q, k, v, heads)
+                a = ctx.test_attention(q, k, v, heads, **kw)
                 ctx.set_option("attn_regsplit", 1)
-                b = ctx.test_attention(q, k, v, heads)
+                b = ctx.test_attention(q, k, v, heads, **kw)
             finally:
                 ctx.set_option("attn_regsplit", 0)
                 ctx.set_option("attn_split", 1)
-            assert np.isfinite(a).all() and np.array_equal(a, b), (n, Nq, Nk, C, split)
+            assert np.isfinite(a).all() and np.array_equal(a, b), (name, split)
 
 
 # ------------------------------------------------------------------ UNet::forward
