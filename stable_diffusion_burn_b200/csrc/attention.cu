@@ -4,10 +4,12 @@
 //   softmax((q d^-1/4)(k d^-1/4)^T) v  ==  softmax(q k^T d^-1/2) v.
 //
 // One CTA = 128 query rows of one (sample, head). Warp roles:
-//   warpgroup 0    : TMA producer (warp 0) — the Q tile once, then K tiles [128 keys][d] and V tiles through an ST-stage ring
+//   warpgroup 0    : TMA producers — warp 0 the Q tile once, then K tiles [128 keys][d]; warp 1 the V tiles (ST-stage rings)
 //   warpgroups 1-2 : 64 query rows each. S = Q K^T with wgmma (Q and K from shared memory, S in registers: m64n128), running
 //                    max / sum in fp32 (exp2 with the d^-1/2 scale folded in), P converted in registers to the A fragment of
-//                    O += P V (wgmma with A from registers, O in registers), lazy O rescale, O / l written as fp16 hi(/lo)
+//                    O += P V (wgmma with A from registers, O in registers), lazy O rescale, O / l written as fp16 hi(/lo).
+//                    Software-pipelined: the softmax of one key tile runs while the tensor cores compute the P V product of the
+//                    previous one, and the two warpgroups take turns issuing their wgmmas (ping-pong on named barriers).
 #include "attention.cuh"
 
 #include <type_traits>
@@ -71,9 +73,10 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
   uint64_t* v_empty = v_full + ST;     // ST (one arrival per softmax warp)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  long long* const dbg = (p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) ? p.dbg : nullptr;
+  // stamps go through p.dbg (a kernel parameter) rather than a pointer copy that would hold two registers through the loop
+  const bool dbg = p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
   constexpr int DJ0 = 8;  // stamped key tiles: DJ0 .. DJ0+3
-  if (dbg && threadIdx.x == 0) dbg[255] = clock64();
+  if (dbg && threadIdx.x == 0) p.dbg[255] = clock64();
   pdl_trigger();
   const int q0 = blockIdx.x * 128;
   const int h = blockIdx.y;
@@ -103,7 +106,9 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
   // (setmaxnreg sits INSIDE the role branches: ptxas budgets the code after a join with the smaller of the two limits)
   if (warp < 4) {
     if (RS) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    // ======================================================================= TMA producer
+    // ======================================================================= TMA producers
+    // warp 0 loads Q and the K tiles, warp 1 the V tiles: the consumers free a K stage a whole softmax before the V stage of the
+    // same tile, so the next K load must not queue behind the wait for that V stage
     if (warp == 0 && elect_one()) {
       mbar_expect_tx(q_full, Cfg::Q_TILE);
 #pragma unroll
@@ -124,6 +129,11 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
             tma_load_2d(sK + st * Cfg::K_BYTES + Cfg::K_HALF + c * 16384, &mk_lo, &k_full[st], p.k_col0 + h * DPAD + c * 64,
                         s * p.k_rows_per_sample + j * 128);
         }
+      }
+    } else if (warp == 1 && elect_one()) {
+      for (int j = 0; j < T; ++j) {
+        const int st = j % ST;
+        const uint32_t ph = (j / ST) & 1;
         mbar_wait(&v_empty[st], ph ^ 1);
         mbar_expect_tx(&v_full[st], Cfg::V_TX);
         if (VMN) {
@@ -152,61 +162,99 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
     float o[DPAD / 2];
 #pragma unroll
     for (int i = 0; i < DPAD / 2; ++i) o[i] = 0.f;
-    auto sstamp = [&](int j, int k) {
-      if (dbg && threadIdx.x == 128 && j >= DJ0 && j < DJ0 + 4) dbg[(j - DJ0) * 8 + k] = clock64();
-    };
     const uint32_t qa = smem_u32(sQ) + wg * (64 * 128);
     // keys per S sub-tile: the 128-key tile in one m64n128 product, or for d = 160 in two m64n64 halves (S, P and O of a 128-key
     // product do not fit the registers beside an 80-register O: the wgmma would be serialised and the thread would spill)
     constexpr int KW = DPAD > 128 ? 64 : 128, NSUB = 128 / KW;
-    mbar_wait(q_full, 0);
-    for (int j = 0; j < T; ++j) {
-      const int st = j % ST;
-      const uint32_t ph = (j / ST) & 1;
-      sstamp(j, 0);
-      mbar_wait(&k_full[st], ph);
-      sstamp(j, 1);
-      int valid_tile[2];
+    // Software pipeline over the key sub-tiles u = 0 .. U-1 (keys [KW (u % NSUB), + KW) of tile u / NSUB). Iteration u issues
+    // S_u = Q K_u^T, then O += P_{u-1} V_{u-1}, waits for S_u alone and exponentiates it on the CUDA cores while the tensor cores
+    // run the P V product; then it waits for that product, rescales O and packs P_u for the next iteration. Each output element
+    // sees the operations of the serial schedule in the same order (O <- alpha_u O, then O += P_u V_u), with the same row
+    // maxima, exponent arguments and partial-sum folds: the result is bit-identical to computing the sub-tiles one at a time.
+    const int U = T * NSUB;
+    float sv[KW / 2];     // S_u, exponentiated in place (P_u in fp32)
+    uint32_t pa[KW / 4];  // P_{u-1} as fp16 pairs: the A fragments of the KW / 16 k-steps of P V, read by wgmmas in flight
+    float alpha[2];       // O rescale factor of the sub-tile just exponentiated (per row half)
+    // SDB_ATTN_DBG timeline of key tiles DJ0 .. DJ0+3 (their first sub-tile): 0 S issued, 1 S ready, 2 softmax done,
+    // 3 PV issued, 4 PV done
+    auto sstamp = [&](int u, int k) {
+      const int j = u / NSUB;
+      if (dbg && threadIdx.x == 128 && u % NSUB == 0 && j >= DJ0 && j < DJ0 + 4) p.dbg[(j - DJ0) * 8 + k] = clock64();
+    };
+    auto issue_s = [&](int u) {
+      const int j = u / NSUB, sub = u % NSUB, st = j % ST;
+      if (sub == 0) mbar_wait(&k_full[st], (j / ST) & 1);
+#pragma unroll
+      for (int i = 0; i < KW / 2; ++i) sv[i] = 0.f;
+      const uint32_t ka = smem_u32(sK + st * Cfg::K_BYTES) + sub * KW * 128;  // key rows [sub KW, sub KW + KW) of the tile
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < DPAD / 16; ++kk) {
+        const uint32_t off = (kk / 4) * 16384 + (kk % 4) * 32;
+        Wgmma<KW>::template ss<0>(sv, make_sdesc_sw128(qa + off), make_sdesc_sw128(ka + off), 1);
+        if (QK3) {  // + q_lo k_hi^T + q_hi k_lo^T
+          Wgmma<KW>::template ss<0>(sv, make_sdesc_sw128(qa + Cfg::Q_HALF + off), make_sdesc_sw128(ka + off), 1);
+          Wgmma<KW>::template ss<0>(sv, make_sdesc_sw128(qa + off), make_sdesc_sw128(ka + Cfg::K_HALF + off), 1);
+        }
+      }
+      wgmma_commit();
+      sstamp(u, 0);
+    };
+    auto s_ready = [&](int u) {  // after the wait for S_u: the K stage is free once its last sub-tile is multiplied
+      reg_fence(sv);
+      const int j = u / NSUB;
+      if (u % NSUB == NSUB - 1 && lane == 0) mbar_arrive(&k_empty[j % ST]);
+      sstamp(u, 1);
+    };
+    auto issue_pv = [&](int u) {
+      const int j = u / NSUB, sub = u % NSUB, st = j % ST;
+      if (sub == 0) mbar_wait(&v_full[st], (j / ST) & 1);
+      const uint32_t va = smem_u32(sV + st * Cfg::V_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < KW / 16; ++kk) {
+        const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+        const int kg = sub * (KW / 16) + kk;  // 16-key step inside the 128-key tile
+        // K-major V^T: 16 keys = 32 bytes inside a 128-byte row; MN-major V: 16 keys = 16 rows of 128 bytes
+        if (VMN)
+          Wgmma<DPAD>::template rs<1>(o, a, make_sdesc_sw128_mn(va + kg * 2048, Cfg::V_CHUNK), 1);
+        else
+          Wgmma<DPAD>::template rs<0>(o, a, make_sdesc_sw128(va + (kg / 4) * Cfg::V_CHUNK + (kg % 4) * 32), 1);
+      }
+      wgmma_commit();
+      sstamp(u, 3);
+    };
+    auto pv_done = [&](int u) {  // after the wait for P_u V_u: the V stage is free once its last sub-tile is multiplied
+      reg_fence(o);
+      const int j = u / NSUB;
+      if (u % NSUB == NSUB - 1 && lane == 0) mbar_arrive(&v_empty[j % ST]);
+      sstamp(u, 4);
+    };
+    // S_u -> P_u (fp32, in sv), alpha; running maximum and sum. Sub-tiles with every key valid for both rows (all but the last
+    // of a short sequence) take a copy of the code without the key mask: the same values, without a compare per element.
+    auto softmax = [&](int u) {
+      const int j = u / NSUB, sub = u % NSUB;
+      // valid keys of this sub-tile per row (<= 0: none), less this thread's column offset cl: column 8 (i / 4) + cl + i % 2 of
+      // element i is a valid key when 8 (i / 4) + i % 2 < vcl (compile-time left sides, no column registers)
+      int vcl[2];
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        valid_tile[hh] = min(128, kvlen - j * 128);
-        if (p.causal) valid_tile[hh] = max(1, min(valid_tile[hh], q0 + rw + 8 * hh - j * 128 + 1));  // additive -inf mask above the diagonal
+        int vt = min(128, kvlen - j * 128);
+        if (p.causal) vt = max(1, min(vt, q0 + rw + 8 * hh - j * 128 + 1));  // additive -inf mask above the diagonal
+        vcl[hh] = vt - sub * KW - cl;
       }
-#pragma unroll 1
-      for (int sub = 0; sub < NSUB; ++sub) {
-        float sv[KW / 2];
-#pragma unroll
-        for (int i = 0; i < KW / 2; ++i) sv[i] = 0.f;
-        const uint32_t ka = smem_u32(sK + st * Cfg::K_BYTES) + sub * KW * 128;  // key rows [sub KW, sub KW + KW) of the tile
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < DPAD / 16; ++kk) {
-          const uint32_t off = (kk / 4) * 16384 + (kk % 4) * 32;
-          Wgmma<KW>::template ss<0>(sv, make_sdesc_sw128(qa + off), make_sdesc_sw128(ka + off), 1);
-          if (QK3) {  // + q_lo k_hi^T + q_hi k_lo^T
-            Wgmma<KW>::template ss<0>(sv, make_sdesc_sw128(qa + Cfg::Q_HALF + off), make_sdesc_sw128(ka + off), 1);
-            Wgmma<KW>::template ss<0>(sv, make_sdesc_sw128(qa + off), make_sdesc_sw128(ka + Cfg::K_HALF + off), 1);
-          }
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        reg_fence(sv);
-        if (sub == NSUB - 1 && lane == 0) mbar_arrive(&k_empty[st]);
-        if (sub == 0) sstamp(j, 2);
-        int valid[2];  // valid keys of this sub-tile per row (<= 0: none)
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) valid[hh] = valid_tile[hh] - sub * KW;
-        const bool full = valid[0] >= KW && valid[1] >= KW;
+      auto run = [&](auto full_c) {
+        constexpr bool full = decltype(full_c)::value;
         // 4 independent max chains per row, then the 4 lanes that share a row
         float mxa[2][4];
 #pragma unroll
         for (int a = 0; a < 4; ++a) mxa[0][a] = mxa[1][a] = -INFINITY;
 #pragma unroll
         for (int i = 0; i < KW / 2; ++i) {
-          const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + cl + (i & 1);
-          if (full || col < valid[hh]) mxa[hh][(i >> 2) & 3] = fmaxf(mxa[hh][(i >> 2) & 3], sv[i]);
+          const int hh = (i >> 1) & 1;
+          if (full || 8 * (i >> 2) + (i & 1) < vcl[hh]) mxa[hh][(i >> 2) & 3] = fmaxf(mxa[hh][(i >> 2) & 3], sv[i]);
         }
-        float m_new[2], alpha[2];
+        float m_new[2];
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           float mx = fmaxf(fmaxf(mxa[hh][0], mxa[hh][1]), fmaxf(mxa[hh][2], mxa[hh][3]));
@@ -220,20 +268,19 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
           m_new[hh] = resc ? m_cand : m_run[hh];
           alpha[hh] = resc ? ex2(m_run[hh] - m_new[hh]) : 1.0f;  // 0 on the first tile
         }
-        if (sub == 0) sstamp(j, 3);
         float sum[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // independent partial row sums (ILP), folded in fixed order below
-        uint32_t pa[KW / 4];                        // P as fp16 pairs: the A fragments of the KW / 16 k-steps of P V
 #pragma unroll
         for (int i = 0; i < KW / 2; i += 2) {
-          const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + cl;
+          const int hh = (i >> 1) & 1, c8 = 8 * (i >> 2);
           float p0 = ex2(fmaf(sv[i], sl2, -m_new[hh]));
           float p1 = ex2(fmaf(sv[i + 1], sl2, -m_new[hh]));
           if (!full) {
-            p0 = (col < valid[hh]) ? p0 : 0.f;
-            p1 = (col + 1 < valid[hh]) ? p1 : 0.f;
+            p0 = (c8 < vcl[hh]) ? p0 : 0.f;
+            p1 = (c8 + 1 < vcl[hh]) ? p1 : 0.f;
           }
           sum[hh][(i >> 2) & 1] += p0 + p1;  // fp32 terms; the fp16 rounding of P is unbiased and averages out over the row
-          pa[i >> 1] = pack_h2(p0, p1);
+          sv[i] = p0;
+          sv[i + 1] = p1;
         }
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
@@ -243,34 +290,65 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
           l_run[hh] = l_run[hh] * alpha[hh] + t;
           m_run[hh] = m_new[hh];
         }
-        if (alpha[0] != 1.0f || alpha[1] != 1.0f) {
+      };
+      if (vcl[0] >= KW - cl && vcl[1] >= KW - cl)
+        run(std::true_type());
+      else
+        run(std::false_type());
+      sstamp(u, 2);
+    };
+    // once P_{u-1} V_{u-1} is done: O <- alpha_u O, and P_u to fp16 A fragments (pa is read by the P V wgmmas until then)
+    auto rescale_pack = [&]() {
+      if (alpha[0] != 1.0f || alpha[1] != 1.0f) {
 #pragma unroll
-          for (int i = 0; i < DPAD / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
-        }
-        if (sub == 0) {
-          sstamp(j, 4);
-          mbar_wait(&v_full[st], ph);
-          sstamp(j, 5);
-        }
-        const uint32_t va = smem_u32(sV + st * Cfg::V_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < KW / 16; ++kk) {
-          const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
-          const int kg = sub * (KW / 16) + kk;  // 16-key step inside the 128-key tile
-          // K-major V^T: 16 keys = 32 bytes inside a 128-byte row; MN-major V: 16 keys = 16 rows of 128 bytes
-          if (VMN)
-            Wgmma<DPAD>::template rs<1>(o, a, make_sdesc_sw128_mn(va + kg * 2048, Cfg::V_CHUNK), 1);
-          else
-            Wgmma<DPAD>::template rs<0>(o, a, make_sdesc_sw128(va + (kg / 4) * Cfg::V_CHUNK + (kg % 4) * 32), 1);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        reg_fence(o);
+        for (int i = 0; i < DPAD / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
       }
-      if (lane == 0) mbar_arrive(&v_empty[st]);
-      sstamp(j, 6);
+#pragma unroll
+      for (int i = 0; i < KW / 2; i += 2) pa[i >> 1] = pack_h2(sv[i], sv[i + 1]);
+    };
+
+    // Ping-pong of the two warpgroups (named barriers 2 and 3): a warpgroup issues the wgmmas of a round only after the other
+    // one has issued those of its previous round, so the tensor cores take the two in turn while the other exponentiates.
+    // Warpgroup 1 lets warpgroup 0 go first and skips its last hand-over, so no arrival is left pending at exit.
+    auto turn_begin = [&]() {
+      if (wg == 0)
+        asm volatile("bar.sync 2, 256;" ::: "memory");
+      else
+        asm volatile("bar.sync 3, 256;" ::: "memory");
+    };
+    auto turn_end = [&](bool last) {
+      if (wg == 0)
+        asm volatile("bar.arrive 3, 256;" ::: "memory");
+      else if (!last)
+        asm volatile("bar.arrive 2, 256;" ::: "memory");
+    };
+    if (wg == 1) turn_end(false);
+
+    mbar_wait(q_full, 0);
+    turn_begin();
+    issue_s(0);
+    turn_end(false);
+    wgmma_wait<0>();
+    s_ready(0);
+    softmax(0);
+    rescale_pack();
+    for (int u = 1; u < U; ++u) {
+      turn_begin();
+      issue_s(u);
+      issue_pv(u - 1);
+      turn_end(false);
+      wgmma_wait<1>();  // S_u; P_{u-1} V_{u-1} may still run
+      s_ready(u);
+      softmax(u);
+      wgmma_wait<0>();
+      pv_done(u - 1);
+      rescale_pack();
     }
+    turn_begin();
+    issue_pv(U - 1);
+    turn_end(true);
+    wgmma_wait<0>();
+    pv_done(U - 1);
     // ---- epilogue: O / l -> fp16 hi(/lo)
     const float inv_l[2] = {1.0f / l_run[0], 1.0f / l_run[1]};
 #pragma unroll

@@ -223,13 +223,15 @@ void run_attention(Ctx& c, const AttnOp& a) {
     attention_launch(am, p, c.stream);
   }
   if (dbg_on) {  // bring-up aid: per-key-tile timeline of CTA (0,0,0), cycles since kernel entry
+    // The consumer loop is software-pipelined: tile j's P V product is issued in the iteration of tile j + 1, after S_{j+1}, so
+    // "pv_issued" follows the next tile's "s_issued" and "pv_done" overlaps the next tile's softmax.
     SDB_CUDA(cudaStreamSynchronize(c.stream));
     const long long t0 = dbg_buf[255];
     auto rel = [&](int i) { return dbg_buf[i] ? dbg_buf[i] - t0 : -1; };
     fprintf(stderr, "attn_dbg nb=%d d=%d Nq=%d Nk=%d qk3=%d\n", a.nb, a.d, a.Nq, a.Nk, p.qk3);
     for (int jj = 0; jj < 4; ++jj)
-      fprintf(stderr, "  j=%d softmax warpgroup 0: start %lld k_ready %lld s_done %lld max %lld rescaled %lld v_ready %lld pv_done %lld\n",
-              8 + jj, rel(jj * 8 + 0), rel(jj * 8 + 1), rel(jj * 8 + 2), rel(jj * 8 + 3), rel(jj * 8 + 4), rel(jj * 8 + 5), rel(jj * 8 + 6));
+      fprintf(stderr, "  j=%d softmax warpgroup 0: s_issued %lld s_ready %lld softmax_done %lld pv_issued %lld pv_done %lld\n",
+              8 + jj, rel(jj * 8 + 0), rel(jj * 8 + 1), rel(jj * 8 + 2), rel(jj * 8 + 3), rel(jj * 8 + 4));
   }
 }
 

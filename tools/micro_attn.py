@@ -1,5 +1,6 @@
 """Timeline probe of the fused attention kernel. With SDB_ATTN_DBG=1 every launch prints clock64 stamps of CTA (0,0,0) for key
-tiles 8..11, taken by the first softmax warpgroup: tile start, K ready, S = QK^T done, row maxima, O rescaled, V ready, PV done.
+tiles 8..11, taken by the first softmax warpgroup: S = QK^T issued, S ready, softmax done, PV issued, PV done (the P V product
+of a tile is issued after the next tile's QK^T).
    SDB_ATTN_DBG=1 python tools/micro_attn.py [regsplit]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
