@@ -175,11 +175,12 @@ int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float*
                      const float* beta, const float* w1, const float* b1, int M, int K0, int C, int N, int passes, int geglu,
                      float* out);
 /* conv (3x3 pad 1 or 1x1) whose epilogue also leaves the GroupNorm statistics of its output, followed by the apply-only
- * GroupNorm(+SiLU) that consumes them (the ResBlock's conv_in -> norm_out -> SiLU chain, unet/mod.rs:716-725). NCHW fp32 in/out;
+ * GroupNorm(+SiLU) that consumes them (the ResBlock's conv_in -> norm_out -> SiLU chain, unet/mod.rs:716-725). stride 2 (3x3)
+ * is the UNet downsample conv, upsample = 1 (3x3) the folded nearest-2x + conv of the upsample blocks. NCHW fp32 in/out;
  * *slots = partial-statistics slots per image the GEMM wrote (> 0). */
 int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const float* bias, const float* gamma,
-                            const float* beta, int n, int cin, int H, int W, int cout, int ksize, int passes, int silu,
-                            float* y, int* slots);
+                            const float* beta, int n, int cin, int H, int W, int cout, int ksize, int stride, int upsample,
+                            int passes, int silu, float* y, int* slots);
 /* GroupNorm(32 groups)+optional SiLU, NCHW fp32 in/out. */
 int sdb_test_groupnorm(sdb_ctx* ctx, const float* x, const float* gamma, const float* beta, int n, int c,
                        int H, int W, int silu, float* y);
@@ -192,6 +193,25 @@ int sdb_test_layernorm(sdb_ctx* ctx, const float* x, const float* gamma, const f
  * stages it (q / k as single fp16 values in one matrix, V^T; needs Nq == Nk and C / heads a multiple of 16). */
 int sdb_test_attention(sdb_ctx* ctx, const float* q, const float* k, const float* v, int n, int Nq, int Nk,
                        int C, int heads, const int32_t* kvlen, int flags, float* out);
+/* One UNet ResBlock (unet/mod.rs:712-734) or, with emb_bias = NULL, VAE ResnetBlock (autoencoder/mod.rs:513-528) on
+ * cat([x0, x1]) (x1 NULL when c1 = 0), through the model's own staging, packing and launch choices. Host NCHW fp32 tensors;
+ * weights OIHW; skip_w [cout][c0 + c1][1][1] or NULL (then x0 is added and c0 must equal cout); emb_bias [cout] replaces conv1's
+ * bias (the model passes conv_in.bias + lin_embed(silu(emb))). flags: 1 / 2 = x0 / x1 are written by a producer that leaves
+ * GroupNorm statistics (a 3-pass identity conv: the block then sees hi + lo of the input, 22 bits); otherwise an fp32 tensor
+ * with an fp16 copy and no statistics. Outputs [n][cout][H][W]: out, out16 = its fp16 hi + lo copy (zero without the raw16
+ * option), out_norm = SiLU(GroupNorm(out; norm2)) staged from the statistics conv2 left. trace (64 ints): [0] GroupNorm
+ * stagings, [1..4] their path (1 fused, 2 apply from producer partials, 3 apply after the 64:1 pre-fold), [5] GEMMs, then 10 ints
+ * per GEMM: kind, N, BN, split-K, TN, TH, TW, extra-K channels, GroupNorm slots written, second-source channels. */
+int sdb_test_resblock(sdb_ctx* ctx, const float* x0, const float* x1, int n, int c0, int c1, int H, int W, int cout,
+                      const float* norm1_g, const float* norm1_b, const float* conv1_w, const float* conv1_b, const float* norm2_g,
+                      const float* norm2_b, const float* conv2_w, const float* conv2_b, const float* skip_w, const float* skip_b,
+                      const float* emb_bias, int passes, int flags, float* out, float* out16, float* out_norm, int32_t* trace);
+/* GroupNorm(32 groups)(+SiLU) of cat([x0, x1]) (x1 NULL when c1 = 0) as an fp16 hi + lo operand, returned NCHW as hi + lo.
+ * mode 0: statistics kernel over both sources + apply; 1: the fused statistics + apply kernel; 2: apply from the partials two
+ * producers left (3-pass identity convs, which pass hi + lo of the inputs), with the 64:1 pre-fold above 128 slots per image.
+ * trace as sdb_test_resblock. */
+int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n, int c0, int c1, int H, int W,
+                           const float* gamma, const float* beta, int silu, int mode, float* y, int32_t* trace);
 
 #ifdef __cplusplus
 }

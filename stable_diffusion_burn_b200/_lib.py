@@ -71,7 +71,12 @@ SIGNATURES = [
     ("sdb_test_ln_fold", C.c_int, [_ctx, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int,
                                    C.c_int, C.c_int, _f32p]),
     ("sdb_test_conv_groupnorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                          C.c_int, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int)]),
+                                          C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int)]),
+    ("sdb_test_resblock", C.c_int, [_ctx, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                    _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p,
+                                    C.c_int, C.c_int, _f32p, _f32p, _f32p, C.POINTER(C.c_int32)]),
+    ("sdb_test_groupnorm_cat", C.c_int, [_ctx, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, _f32p,
+                                         C.c_int, C.c_int, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_groupnorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_test_layernorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, _f32p]),
     ("sdb_test_attention", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -324,15 +329,65 @@ class Context:
                                              1 if geglu else 0, ptr(out)))
         return out
 
-    def test_conv_groupnorm(self, x, w, bias, gamma, beta, passes=3, silu=False):
+    def test_conv_groupnorm(self, x, w, bias, gamma, beta, passes=3, silu=False, stride=1, upsample=0):
         x = f32(x); w = f32(w); bias = f32(bias); gamma = f32(gamma); beta = f32(beta)
         n, cin, H, W = x.shape
         cout, _, k, _ = w.shape
-        y = np.empty((n, cout, H, W), np.float32)
+        Ho = 2 * H if upsample else (H // 2 if stride == 2 else H)
+        Wo = 2 * W if upsample else (W // 2 if stride == 2 else W)
+        y = np.empty((n, cout, Ho, Wo), np.float32)
         slots = C.c_int()
         self.check(self.lib.sdb_test_conv_groupnorm(self.h, ptr(x), ptr(w), ptr(bias), ptr(gamma), ptr(beta), n, cin, H, W, cout, k,
-                                                    passes, 1 if silu else 0, ptr(y), C.byref(slots)))
+                                                    stride, upsample, passes, 1 if silu else 0, ptr(y), C.byref(slots)))
         return y, slots.value
+
+    @staticmethod
+    def _decode_trace(t):
+        """trace ints of sdb_test_resblock / sdb_test_groupnorm_cat -> {"gn": [...], "gemms": [...]}"""
+        paths = {1: "fused", 2: "apply", 3: "apply+fold"}
+        keys = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1")
+        gemms = [dict(zip(keys, (int(v) for v in t[6 + 10 * i:16 + 10 * i]))) for i in range(min(int(t[5]), 5))]
+        return {"gn": [paths.get(int(v), int(v)) for v in t[1:1 + min(int(t[0]), 4)]], "gemms": gemms}
+
+    def test_resblock(self, x0, x1, norm1, conv1, norm2, conv2, skip=None, emb_bias=None, passes=1, x0_stats=True,
+                      x1_stats=True):
+        """One ResBlock (emb_bias given) or VAE ResnetBlock (emb_bias None) on cat([x0, x1]); norm* = (gamma, beta),
+        conv* / skip = (weight OIHW, bias). -> (out, out16, out_norm, trace): the block output, its fp16 hi + lo copy,
+        SiLU(GroupNorm(out; norm2)) from the statistics conv2 left, and what ran ({"gn": paths, "gemms": launch choices,
+        "skip": "merged" | "separate" | "none"})."""
+        x0 = f32(x0)
+        n, c0, H, W = x0.shape
+        x1 = f32(x1) if x1 is not None else None
+        c1 = 0 if x1 is None else x1.shape[1]
+        cout = conv1[0].shape[0]
+        keep = [f32(v) for v in (*norm1, *conv1, *norm2, *conv2)]
+        sk = [f32(v) for v in skip] if skip is not None else [None, None]
+        eb = f32(emb_bias) if emb_bias is not None else None
+        p = lambda a: None if a is None else ptr(a)
+        out, out16, outn = (np.empty((n, cout, H, W), np.float32) for _ in range(3))
+        trace = np.zeros(64, np.int32)
+        flags = (1 if x0_stats else 0) | (2 if (x1 is not None and x1_stats) else 0)
+        self.check(self.lib.sdb_test_resblock(self.h, ptr(x0), p(x1), n, c0, c1, H, W, cout, *(ptr(a) for a in keep), p(sk[0]),
+                                              p(sk[1]), p(eb), passes, flags, ptr(out), ptr(out16), ptr(outn),
+                                              trace.ctypes.data_as(C.POINTER(C.c_int32))))
+        tr = self._decode_trace(trace)
+        g = tr["gemms"]
+        tr["skip"] = "separate" if len(g) == 3 else ("merged" if g and g[-1]["xk"] > 0 else "none")
+        return out, out16, outn, tr
+
+    def test_groupnorm_cat(self, x0, x1, gamma, beta, silu=False, mode=0):
+        """GroupNorm(+SiLU) of cat([x0, x1]) as the fp16 hi + lo operand. mode 0: statistics kernel + apply, 1: fused kernel,
+        2: apply from identity-producer partials (inputs pass as hi + lo). -> (y NCHW, trace)"""
+        x0 = f32(x0)
+        n, c0, H, W = x0.shape
+        x1 = f32(x1) if x1 is not None else None
+        c1 = 0 if x1 is None else x1.shape[1]
+        g = f32(gamma); b = f32(beta)
+        y = np.empty((n, c0 + c1, H, W), np.float32)
+        trace = np.zeros(64, np.int32)
+        self.check(self.lib.sdb_test_groupnorm_cat(self.h, ptr(x0), None if x1 is None else ptr(x1), n, c0, c1, H, W, ptr(g), ptr(b),
+                                                   1 if silu else 0, int(mode), ptr(y), trace.ctypes.data_as(C.POINTER(C.c_int32))))
+        return y, self._decode_trace(trace)
 
     def test_groupnorm(self, x, gamma, beta, silu=False):
         x = f32(x); n, c, H, W = x.shape

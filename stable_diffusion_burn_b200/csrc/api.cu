@@ -690,11 +690,15 @@ int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float*
 }
 
 int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const float* bias, const float* gamma, const float* beta,
-                            int n, int cin, int H, int W, int cout, int ksize, int passes, int silu, float* y, int* used_epilogue_stats) {
+                            int n, int cin, int H, int W, int cout, int ksize, int stride, int upsample, int passes, int silu,
+                            float* y, int* used_epilogue_stats) {
   API_BEGIN(ctx)
   c.work.reset();
   SDB_CHECK(ksize == 1 || ksize == 3, "ksize");
-  const size_t xin = (size_t)n * cin * H * W, yout = (size_t)n * cout * H * W;
+  SDB_CHECK((stride == 1 && (upsample == 0 || (upsample == 1 && ksize == 3))) || (stride == 2 && ksize == 3 && !upsample),
+            "stride / upsample");
+  const int Ho = upsample ? 2 * H : (stride == 2 ? H / 2 : H), Wo = upsample ? 2 * W : (stride == 2 ? W / 2 : W);
+  const size_t xin = (size_t)n * cin * H * W, yout = (size_t)n * cout * Ho * Wo;
   auto up = [&](const float* h, size_t cnt) {
     float* d = c.work.get<float>(cnt);
     SDB_CUDA(cudaMemcpyAsync(d, h, sizeof(float) * cnt, cudaMemcpyHostToDevice, c.stream));
@@ -710,27 +714,35 @@ int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const 
   float* d_yh = c.work.get<float>(yout);
   float* d_y = c.work.get<float>(yout);
   nchw_to_nhwc_launch(d_x, n, cin, H, W, d_xh, c.stream);
+  // operand, packing and GEMM kind as the model's downsample (stride 2) and upsample convs use them (see sdb_test_conv2d)
   ActOp A;
   A.n = n, A.C = cin, A.H = H, A.W = W;
+  int kind = ksize == 1 ? G_CONV1 : G_CONV3, mode = 0;
+  if (stride == 2) kind = G_CONV3_S2, mode = PREP_PHASE2, A.P = 4, A.H = H / 2, A.W = W / 2;
+  if (upsample) kind = G_CONV3_UP2;
   A.p = Half2Ptr{c.work.get<__half>(xin), c.work.get<__half>(xin)};
-  prep_operand_launch(d_xh, cin, nullptr, 0, n, H, W, 0, nullptr, nullptr, nullptr, 0.f, A.p, c.stream);
+  prep_operand_launch(d_xh, cin, nullptr, 0, n, H, W, mode, nullptr, nullptr, nullptr, 0.f, A.p, c.stream);
   WeightOp Wp;
-  Wp.N = cout, Wp.K = ksize * ksize * cin;
-  Wp.p = Half2Ptr{c.work.get<__half>((size_t)cout * Wp.K), c.work.get<__half>((size_t)cout * Wp.K)};
-  pack_conv_launch(d_w, cout, cin, ksize, Wp.p, c.stream);
+  Wp.N = cout, Wp.K = (upsample ? 4 : ksize * ksize) * cin;
+  const size_t w_elems = (size_t)cout * Wp.K * (upsample ? 4 : 1);
+  Wp.p = Half2Ptr{c.work.get<__half>(w_elems), c.work.get<__half>(w_elems)};
+  if (upsample)
+    pack_conv_up2_launch(d_w, cout, cin, Wp.p, c.stream);
+  else
+    pack_conv_launch(d_w, cout, cin, ksize, Wp.p, c.stream);
   GnPart gn;
   gn.bucket = cout % 320 == 0 ? 10 : cout / 32;
-  gn.cap = std::max(3 * ((H * W + 127) / 128), 160);
+  gn.cap = std::max(3 * ((Ho * Wo + 127) / 128), 160);
   gn.buf = c.work.get<float>((size_t)n * gn.cap * (cout / gn.bucket) * 2);
   Epilogue ep;
   ep.out_f32 = d_conv, ep.bias = d_b, ep.gn = &gn;
-  run_gemm(c, ksize == 1 ? G_CONV1 : G_CONV3, A, nullptr, Wp, passes, ep);
+  run_gemm(c, kind, A, nullptr, Wp, passes, ep);
   if (used_epilogue_stats) *used_epilogue_stats = gn.slots;
   SDB_CHECK(gn.slots > 0, "the GEMM did not produce GroupNorm statistics for this shape");
   Half2Ptr o16{c.work.get<__half>(yout), c.work.get<__half>(yout)};
   GnSrc s0, s1;
   s0.x = d_conv, s0.C = cout, s0.part = gn.buf, s0.cap = gn.cap, s0.slots = gn.slots;
-  gn_apply_launch(s0, s1, gn.bucket, n, H, W, silu, d_g, d_be, 1e-5f, o16, c.stream);
+  gn_apply_launch(s0, s1, gn.bucket, n, Ho, Wo, silu, d_g, d_be, 1e-5f, o16, c.stream);
   std::vector<__half> hi(yout), lo(yout);
   SDB_CUDA(cudaMemcpyAsync(hi.data(), o16.hi, yout * 2, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, yout * 2, cudaMemcpyDeviceToHost, c.stream));
@@ -738,7 +750,7 @@ int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const 
   std::vector<float> nhwc(yout);
   for (size_t i = 0; i < yout; ++i) nhwc[i] = __half2float(hi[i]) + __half2float(lo[i]);
   SDB_CUDA(cudaMemcpyAsync(d_yh, nhwc.data(), yout * 4, cudaMemcpyHostToDevice, c.stream));
-  nhwc_to_nchw_launch(d_yh, n, cout, H, W, d_y, c.stream);
+  nhwc_to_nchw_launch(d_yh, n, cout, Ho, Wo, d_y, c.stream);
   SDB_CUDA(cudaMemcpyAsync(y, d_y, sizeof(float) * yout, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
   API_END
@@ -793,6 +805,25 @@ int sdb_test_attention(sdb_ctx* ctx, const float* q, const float* k, const float
   API_BEGIN(ctx)
   c.work.reset();
   model_test_attention(c, q, k, v, n, Nq, Nk, C, heads, kvlen, flags, out);
+  API_END
+}
+
+int sdb_test_resblock(sdb_ctx* ctx, const float* x0, const float* x1, int n, int c0, int c1, int H, int W, int cout,
+                      const float* norm1_g, const float* norm1_b, const float* conv1_w, const float* conv1_b, const float* norm2_g,
+                      const float* norm2_b, const float* conv2_w, const float* conv2_b, const float* skip_w, const float* skip_b,
+                      const float* emb_bias, int passes, int flags, float* out, float* out16, float* out_norm, int32_t* trace) {
+  API_BEGIN(ctx)
+  c.work.reset();
+  model_test_resblock(c, x0, x1, n, c0, c1, H, W, cout, norm1_g, norm1_b, conv1_w, conv1_b, norm2_g, norm2_b, conv2_w, conv2_b,
+                      skip_w, skip_b, emb_bias, passes, flags, out, out16, out_norm, trace);
+  API_END
+}
+
+int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n, int c0, int c1, int H, int W, const float* gamma,
+                           const float* beta, int silu, int mode, float* y, int32_t* trace) {
+  API_BEGIN(ctx)
+  c.work.reset();
+  model_test_groupnorm_cat(c, x0, x1, n, c0, c1, H, W, gamma, beta, silu, mode, y, trace);
   API_END
 }
 

@@ -363,6 +363,7 @@ struct Fwd {
       };
       src(x0, s0);
       if (x1) src(*x1, s1);
+      if (c.trace_on) c.gn_trace.push_back(x0.gn.slots > 128 || (x1 && x1->gn.slots > 128) ? GN_PATH_APPLY_FOLD : GN_PATH_APPLY);
       KernelScope ks(c, KC_PREP, 0, (double)nb * HW * C * (4.0 + 2.0 + (lo ? 2.0 : 0.0)));
       gn_apply_launch(s0, s1, x0.gn.bucket, nb, x0.H, x0.W, silu ? 1 : 0, nw.gamma, nw.beta, nw.eps, a.p, c.stream);
       return a;
@@ -371,6 +372,7 @@ struct Fwd {
     unsigned int* tk = gn_tickets + (size_t)gn_slot * nb * 2;
     gn_slot++;
     float* part = c.work.get<float>(gn_fused_partial_floats(nb, HW));
+    if (c.trace_on) c.gn_trace.push_back(GN_PATH_FUSED);
     KernelScope ks(c, KC_PREP, 0, (double)nb * HW * C * (8.0 + 2.0 + (lo ? 2.0 : 0.0)));
     gn_fused_launch(x0.p, x0.C, x1 ? x1->p : nullptr, x1 ? x1->C : 0, nb, x0.H, x0.W, silu ? 1 : 0, nw.gamma, nw.beta, nw.eps,
                     a.p, part, tk, c.stream);
@@ -1447,6 +1449,160 @@ void model_test_attention(Ctx& c, const float* q, const float* k, const float* v
   SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, lo.size() * 2, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
   for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
+}
+
+// ================================================================================ ResBlock / GroupNorm unit-test entries
+namespace {
+struct TraceScope {  // records the GEMM choices and GroupNorm paths of everything queued while it lives
+  Ctx& c;
+  explicit TraceScope(Ctx& c_) : c(c_) { c.gemm_trace.clear(), c.gn_trace.clear(), c.trace_on = true; }
+  ~TraceScope() { c.trace_on = false; }
+};
+}  // namespace
+
+static float* upload(Ctx& c, const float* h, size_t count) {
+  if (!h) return nullptr;
+  float* d = c.work.get<float>(count);
+  SDB_CUDA(cudaMemcpyAsync(d, h, count * 4, cudaMemcpyHostToDevice, c.stream));
+  return d;
+}
+
+static ConvW test_conv_weights(Ctx& c, Fwd& f, const float* w, const float* b, int cin, int cout, int k) {
+  SDB_CHECK(cin % 64 == 0 && cout % 32 == 0, "test conv: channels must be multiples of 64 (in) and 32 (out)");
+  ConvW cw;
+  cw.cin = cin, cw.cout = cout, cw.k = k;
+  cw.packed.p = f.half2((size_t)cout * k * k * cin, true);
+  cw.packed.N = cout, cw.packed.K = k * k * cin;
+  pack_conv_launch(upload(c, w, (size_t)cout * cin * k * k), cout, cin, k, cw.packed.p, c.stream);
+  cw.bias = upload(c, b, cout);
+  return cw;
+}
+
+// An NCHW host tensor staged as a model activation. stats = true: written by a 3-pass identity 3x3 conv with the epilogue a
+// ResBlock output gets (fp32, fp16 hi/lo copy, GroupNorm partials); the 3-pass product returns hi + lo of the input (22 bits,
+// exact in fp32). stats = false: the fp32 tensor and its fp16 copy without statistics, as the UNet's conv_in leaves it.
+static Act stage_activation(Fwd& f, const float* h, int C, int H, int W, bool stats) {
+  Ctx& c = f.c;
+  Act a = f.act16(H, W, C);
+  float* d = upload(c, h, a.count());
+  if (!stats) {
+    nchw_to_nhwc_launch(d, f.nb, C, H, W, a.p, c.stream);
+    if (a.raw16.hi) convert_f16_launch(a.p, (long long)a.count(), a.raw16, c.stream);
+    return a;
+  }
+  float* xh = c.work.get<float>(a.count());
+  nchw_to_nhwc_launch(d, f.nb, C, H, W, xh, c.stream);
+  ActOp A;
+  A.n = f.nb, A.H = H, A.W = W, A.C = C;
+  A.p = f.half2(a.count(), true);
+  convert_f16_launch(xh, (long long)a.count(), A.p, c.stream);
+  // identity weights [C][C][3][3]: a one at the centre tap of (i, i)
+  float* id = c.work.get<float>((size_t)C * C * 9);
+  SDB_CUDA(cudaMemsetAsync(id, 0, (size_t)C * C * 9 * 4, c.stream));
+  const std::vector<float> ones(C, 1.f);
+  SDB_CUDA(cudaMemcpy2DAsync(id + 4, (size_t)(C + 1) * 9 * 4, ones.data(), 4, 4, C, cudaMemcpyHostToDevice, c.stream));
+  WeightOp wid;
+  wid.p = f.half2((size_t)C * C * 9, true), wid.N = C, wid.K = 9 * C;
+  pack_conv_launch(id, C, C, 3, wid.p, c.stream);
+  Epilogue ep;
+  ep.out_f32 = a.p, ep.out_f16 = a.raw16, ep.gn = &a.gn;
+  run_gemm(c, G_CONV3, A, nullptr, wid, 3, ep);
+  return a;
+}
+
+// NHWC fp16 hi + lo (or nothing: zeros) -> NCHW fp32 on the host
+static void fetch_half2(Ctx& c, Half2Ptr p, int n, int C, int H, int W, float* out) {
+  const size_t cnt = (size_t)n * C * H * W;
+  std::vector<__half> hi(cnt), lo(cnt);
+  if (p.hi) SDB_CUDA(cudaMemcpyAsync(hi.data(), p.hi, cnt * 2, cudaMemcpyDeviceToHost, c.stream));
+  if (p.lo) SDB_CUDA(cudaMemcpyAsync(lo.data(), p.lo, cnt * 2, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  for (int s = 0; s < n; ++s)
+    for (int i = 0; i < H * W; ++i)
+      for (int ch = 0; ch < C; ++ch) {
+        const size_t src = ((size_t)s * H * W + i) * C + ch;
+        out[((size_t)s * C + ch) * H * W + i] = (p.hi ? __half2float(hi[src]) : 0.f) + (p.lo ? __half2float(lo[src]) : 0.f);
+      }
+}
+
+static void write_trace(const Ctx& c, int32_t* trace) {
+  std::fill(trace, trace + kTestTraceInts, 0);
+  trace[0] = (int)c.gn_trace.size();
+  for (size_t i = 0; i < c.gn_trace.size() && i < 4; ++i) trace[1 + i] = c.gn_trace[i];
+  trace[5] = (int)c.gemm_trace.size();
+  for (size_t i = 0; i < c.gemm_trace.size() && i < 5; ++i) {
+    const Ctx::GemmRecord& r = c.gemm_trace[i];
+    const int v[10] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels};
+    std::copy(v, v + 10, trace + 6 + 10 * i);
+  }
+}
+
+void model_test_resblock(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, int Cout,
+                         const float* n1g, const float* n1b, const float* w1, const float* b1, const float* n2g, const float* n2b,
+                         const float* w2, const float* b2, const float* wsk, const float* bsk, const float* emb_bias, int passes,
+                         int flags, float* out, float* out16, float* outn, int32_t* trace) {
+  SDB_CHECK(n >= 1 && H >= 1 && W >= 1 && C0 > 0 && C1 >= 0 && (C1 > 0) == (x1 != nullptr), "test_resblock: shapes");
+  SDB_CHECK(b1 && b2 && (!wsk || bsk) && (wsk || (!x1 && C0 == Cout)), "test_resblock: biases / skip (a block without one adds x0)");
+  SDB_CHECK((flags & ~3) == 0, "test_resblock: flags are 1 (x0 with producer statistics) | 2 (x1 with producer statistics)");
+  const int Cin = C0 + C1;
+  Fwd f(c, n);
+  f.init_sums(4);
+  NormW nw1, nw2;
+  nw1.c = Cin, nw1.gamma = upload(c, n1g, Cin), nw1.beta = upload(c, n1b, Cin);
+  nw2.c = Cout, nw2.gamma = upload(c, n2g, Cout), nw2.beta = upload(c, n2b, Cout);
+  const ConvW cw1 = test_conv_weights(c, f, w1, b1, Cin, Cout, 3), cw2 = test_conv_weights(c, f, w2, b2, Cout, Cout, 3);
+  ConvW sk;
+  float* bias_merged = nullptr;
+  if (wsk) {  // packed as pack_resblock / pack_resnet do
+    sk = test_conv_weights(c, f, wsk, bsk, Cin, Cout, 1);
+    bias_merged = c.work.get<float>(Cout);
+    add_vec_launch(cw2.bias, sk.bias, Cout, bias_merged, c.stream);
+  }
+  const float* d_emb = upload(c, emb_bias, Cout);
+  const Act a0 = stage_activation(f, x0, C0, H, W, flags & 1);
+  Act a1;
+  if (x1) a1 = stage_activation(f, x1, C1, H, W, flags & 2);
+  Act o = f.act16(H, W, Cout);
+  ActOp g;
+  {
+    TraceScope ts(c);
+    run_resblock(f, nw1, cw1, nw2, cw2, wsk ? &sk : nullptr, bias_merged, passes, a0, x1 ? &a1 : nullptr, d_emb, o);
+    g = f.gn_operand(o, nullptr, nw2, true, true);  // a consumer of the output: reads the partials conv_out left
+    write_trace(c, trace);
+  }
+  float* d = c.work.get<float>(o.count());
+  nhwc_to_nchw_launch(o.p, n, Cout, H, W, d, c.stream);
+  SDB_CUDA(cudaMemcpyAsync(out, d, o.count() * 4, cudaMemcpyDeviceToHost, c.stream));
+  fetch_half2(c, o.raw16, n, Cout, H, W, out16);
+  fetch_half2(c, g.p, n, Cout, H, W, outn);
+}
+
+void model_test_groupnorm_cat(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, const float* gamma,
+                              const float* beta, int silu, int mode, float* y, int32_t* trace) {
+  SDB_CHECK(n >= 1 && H >= 1 && W >= 1 && C0 > 0 && C1 >= 0 && (C1 > 0) == (x1 != nullptr), "test_groupnorm_cat: shapes");
+  SDB_CHECK(mode >= 0 && mode <= 2, "test_groupnorm_cat: mode is 0 (statistics kernel + apply), 1 (fused), 2 (producer partials)");
+  const int C = C0 + C1;
+  Fwd f(c, n);
+  f.init_sums(2);
+  NormW nw;
+  nw.c = C, nw.gamma = upload(c, gamma, C), nw.beta = upload(c, beta, C);
+  const Act a0 = stage_activation(f, x0, C0, H, W, mode == 2);
+  Act a1;
+  if (x1) a1 = stage_activation(f, x1, C1, H, W, mode == 2);
+  TraceScope ts(c);
+  ActOp g;
+  if (mode == 0) {
+    double* sums = c.work.get<double>((size_t)n * 64);
+    float* part = c.work.get<float>(gn_stats_partial_floats(n, H * W));
+    gn_stats_launch(a0.p, C0, x1 ? a1.p : nullptr, C1, n, H * W, sums, part, f.gn_tickets, c.stream);
+    g.p = f.half2((size_t)n * H * W * C, true);
+    prep_operand_launch(a0.p, C0, x1 ? a1.p : nullptr, C1, n, H, W, PREP_NORM | (silu ? PREP_SILU : 0), sums, nw.gamma, nw.beta,
+                        nw.eps, g.p, c.stream);
+  } else {
+    g = f.gn_operand(a0, x1 ? &a1 : nullptr, nw, silu != 0, true);
+  }
+  write_trace(c, trace);
+  fetch_half2(c, g.p, n, C, H, W, y);
 }
 
 }  // namespace sdb

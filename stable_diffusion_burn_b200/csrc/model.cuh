@@ -35,5 +35,13 @@ long long dump_tensor_read(const std::string& file, int ndim, int64_t* dims, std
 void model_load_dump_dir(Ctx& c, const char* root);
 void model_test_attention(Ctx& c, const float* q, const float* k, const float* v, int n, int Nq, int Nk, int C, int heads,
                           const int32_t* kvlen, int flags, float* out);
+// ResBlock / concat-GroupNorm test entries (sdb200.h: sdb_test_resblock, sdb_test_groupnorm_cat); trace = kTestTraceInts ints
+constexpr int kTestTraceInts = 64;
+void model_test_resblock(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, int Cout,
+                         const float* n1g, const float* n1b, const float* w1, const float* b1, const float* n2g, const float* n2b,
+                         const float* w2, const float* b2, const float* wsk, const float* bsk, const float* emb_bias, int passes,
+                         int flags, float* out, float* out16, float* outn, int32_t* trace);
+void model_test_groupnorm_cat(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, const float* gamma,
+                              const float* beta, int silu, int mode, float* y, int32_t* trace);
 
 }  // namespace sdb

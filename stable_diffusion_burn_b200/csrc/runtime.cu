@@ -252,6 +252,7 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
   ActOp a0 = a0in, a1;
   if (a1in) a1 = *a1in;
   int gn_rpi = ep.gn_rpi, gn_nimg = 0;
+  const int kind_in = kind;
   if (kind == G_CONV1) {  // a 1x1 conv over NHWC is a plain row-major GEMM
     gn_rpi = a0.H * a0.W;
     a0.W = a0.n * a0.H * a0.W, a0.H = 1, a0.n = 1;
@@ -396,6 +397,8 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
     gn->slots = ok ? slots : 0;
     if (!ok) gn = nullptr;
   }
+  if (c.trace_on)
+    c.gemm_trace.push_back({kind_in, w.N, BN, split, p.TN, p.TH, p.TW, p.xkc * 64, gn ? gn->slots : 0, a1in ? a1.C : 0});
   p.gn_part = gn ? gn->buf : nullptr;
   p.gn_cap = gn ? gn->cap : 0, p.gn_bucket = gn ? gn->bucket : 1;
   p.gn_rpi = gn ? gn_rpi : 0, p.gn_nimg = gn_nimg;

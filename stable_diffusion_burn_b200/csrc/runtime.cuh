@@ -36,6 +36,10 @@ struct TensorInfo {
   int fan_in = 1;
 };
 
+// which GroupNorm kernel staged an operand: statistics and apply in one launch, apply from producer partials, or apply after
+// the 64:1 pre-fold of more than 128 partial slots
+enum GnPath : int { GN_PATH_FUSED = 1, GN_PATH_APPLY = 2, GN_PATH_APPLY_FOLD = 3 };
+
 enum KernelClass : int {
   KC_GEMM = 0,
   KC_SPLITK,  // kept for the class table layout: the split-K fold now happens inside gemm_tc
@@ -152,6 +156,14 @@ struct Ctx {
   // SDB_DEBUG_SYNC=1: synchronise after every launch and report the failing op (bring-up aid)
   bool debug_sync = false;
   std::string dbg_label;
+  // launch record for the test entries (sdb_test_resblock): what run_gemm chose per GEMM and which GroupNorm path
+  // Fwd::gn_operand took, so a test can assert it reached the path it is meant to cover
+  struct GemmRecord {
+    int kind, N, BN, split, TN, TH, TW, xk_channels, gn_slots, a1_channels;
+  };
+  bool trace_on = false;
+  std::vector<GemmRecord> gemm_trace;
+  std::vector<int> gn_trace;  // GN_PATH_*
 
   float* master_ptr(const std::string& name);
   const TensorInfo& info(const std::string& name);

@@ -86,7 +86,9 @@ def test_groupnorm(ctx, n, c, H, W, silu):
 # n, cin, H, W, cout, ksize: plain tiles (one image per tile), two / four images per tile (8x8, 8x4), split-K (small grid, long
 # K), a 1x1 conv over flattened tokens, a VAE width (bucket = group size), an awkward 12x12 map (masked tile rows)
 GN_FROM_GEMM = [(2, 320, 32, 32, 320, 3), (2, 1280, 8, 8, 1280, 3), (4, 640, 8, 4, 640, 3), (2, 1280, 16, 16, 640, 3),
-                (2, 320, 16, 16, 640, 1), (2, 640, 8, 8, 320, 1), (1, 512, 32, 32, 512, 3), (1, 256, 64, 64, 128, 3), (2, 320, 12, 12, 320, 3)]
+                (2, 320, 16, 16, 640, 1), (2, 640, 8, 8, 320, 1), (1, 512, 32, 32, 512, 3), (1, 256, 64, 64, 128, 3), (2, 320, 12, 12, 320, 3),
+                # n = 3 on 8x8 maps: two images per tile with the second image of the last tile masked, without and with split-K
+                (3, 64, 8, 8, 320, 3), (3, 1280, 8, 8, 1280, 3)]
 
 
 @pytest.mark.parametrize("n,cin,H,W,cout,k", GN_FROM_GEMM)
@@ -104,6 +106,35 @@ def test_groupnorm_from_gemm_statistics(ctx, n, cin, H, W, cout, k, silu):
     out, slots = ctx.test_conv_groupnorm(x, w, b, g, be, passes=3, silu=silu)
     e = rel(out, ref.numpy())
     print(f"GN from GEMM statistics n={n} {cin}->{cout} {H}x{W} k={k}: {slots} slots/image, rel L2 {e:.3e}")
+    assert slots > 0 and e < 3e-5
+
+
+# n, cin, H, W, cout, stride, upsample: the UNet downsample convs (stride 2; the 16x16 -> 8x8 one packs two images per tile and
+# splits K) and the folded nearest-2x upsample convs, whose four output phases write separate partial slots
+GN_FROM_RESAMPLING_GEMM = [(2, 320, 32, 32, 320, 2, 0), (2, 640, 16, 16, 640, 2, 0), (1, 320, 64, 64, 320, 2, 0),
+                           (2, 1280, 8, 8, 1280, 1, 1), (2, 640, 16, 16, 640, 1, 1), (1, 512, 32, 32, 512, 1, 1),
+                           (3, 1280, 8, 8, 1280, 1, 1)]
+
+
+@pytest.mark.parametrize("n,cin,H,W,cout,stride,up", GN_FROM_RESAMPLING_GEMM)
+@pytest.mark.parametrize("silu", [False, True])
+def test_groupnorm_from_resampling_gemm_statistics(ctx, n, cin, H, W, cout, stride, up, silu):
+    """GroupNorm from the statistics the stride-2 and upsample conv epilogues leave (the UNet's downsample and upsample blocks)."""
+    x = rnd((n, cin, H, W), 56)
+    w = rnd((cout, cin, 3, 3), 57) / np.sqrt(cin * 9)
+    b = rnd((cout,), 58) * 0.5 + 0.3
+    g = 1 + 0.1 * rnd((cout,), 59); be = 0.1 * rnd((cout,), 60)
+    xt = torch.from_numpy(x).double()
+    if up:
+        xt = F.interpolate(xt, scale_factor=2, mode="nearest")
+    conv = F.conv2d(xt, torch.from_numpy(w).double(), torch.from_numpy(b).double(), stride=stride, padding=1)
+    ref = F.group_norm(conv, 32, torch.from_numpy(g).double(), torch.from_numpy(be).double(), 1e-5)
+    if silu:
+        ref = F.silu(ref)
+    out, slots = ctx.test_conv_groupnorm(x, w, b, g, be, passes=3, silu=silu, stride=stride, upsample=up)
+    assert out.shape == ref.shape
+    e = rel(out, ref.numpy())
+    print(f"GN from GEMM statistics n={n} {cin}->{cout} {H}x{W} stride={stride} up={up}: {slots} slots/image, rel L2 {e:.3e}")
     assert slots > 0 and e < 3e-5
 
 
