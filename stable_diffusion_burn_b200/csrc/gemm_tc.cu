@@ -669,18 +669,23 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
 }
 
 // ------------------------------------------------------------------ launcher
+// Opt-in maximum of dynamic shared memory per block on sm_90 (227 KB); the kernel adds 1 KB of alignment pad and two 8-byte
+// barriers per stage to the ring.
+static constexpr int SMEM_OPTIN_MAX = 227 * 1024;
 template <int BN, int PASSES>
 constexpr int pick_stages() {
-  // as many stages as fit in ~200 KB, capped at 8
+  // as many stages as fit in the opt-in maximum, capped at 8. The 3-pass BN = 160 tile (72 KB stages, the bulk of the
+  // UNet's tensor work) needs 3: with one wgmma group in flight a freed slot then has two stages of products, not one, to be
+  // refilled in, and its mainloop keeps the tensor pipe busy (DESIGN.md §4, "Measured").
   constexpr int per = StageLayout<BN, PASSES>::BYTES;
-  constexpr int n = (200 * 1024) / per;
+  constexpr int n = (SMEM_OPTIN_MAX - 1024) / (per + 2 * 8);
   return n > 8 ? 8 : n;
 }
 
 template <int BN, int PASSES, int STAGES, int EPI>
 static void launch_epi(const GemmMaps& maps, const GemmParams& p, cudaStream_t stream) {
   constexpr int smem = region_bytes<BN, PASSES, STAGES>() + 2 * STAGES * 8 + 1024;
-  static_assert(smem <= 227 * 1024, "shared memory per block");
+  static_assert(smem <= SMEM_OPTIN_MAX, "shared memory per block");
   static_assert(4 * BN * 8 <= AccLayout<BN>::GN_BYTES && 2 * (EW * 32) * 4 * 16 <= AccLayout<BN>::GN_BYTES,
                 "GroupNorm column sums must fit in the scratch after the accumulator image");
   static DeviceOnce once;
