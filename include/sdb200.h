@@ -122,6 +122,25 @@ int sdb_clip_forward_dev(sdb_ctx* ctx, const int32_t* d_tokens, int n, int L, fl
 int sdb_encode_image(sdb_ctx* ctx, const float* img, int n, int H, int W, float* latent);
 int sdb_encode_image_dev(sdb_ctx* ctx, const float* d_img, int n, int H, int W, float* d_latent, void* stream);
 
+/* ---- image-to-image / masked inpainting (DESIGN.md §7 f5) -------------------------------------------------------------- */
+/* The reference has no img2img; this is built from its own parts: encode_image (src/model/autoencoder/mod.rs:60-66), the latent
+ * scale 0.18215 of latent_to_image (src/model/stablediffusion/mod.rs:71) and the schedule and DDIM step of sample_latent (:111,
+ * :123-156). image u8 [n,8H,8W,3] HWC RGB (the format sdb_sample_image returns) -> x = v/127.5 - 1 -> z0 = 0.18215 *
+ * encode_image(x). Of the N timesteps (0..1000).rev().step_by(1000/n_steps), the last k = floor(strength * N) run, from
+ * t0 = ts[N-k], on the start latent sqrt(abar[t0]) z0 + sqrt(1 - abar[t0]) noise. strength must be finite, in (0, 1], and give
+ * k >= 1 (strength >= 1/N). mask (optional) u8 [n,8H,8W]: 255 = regenerate, 0 = keep, in between blends; it is reduced to one
+ * weight per latent cell, w = (sum of the 8x8 block) / (64*255), and after every step x = w x + (1-w) (sqrt(a_prev) z0 +
+ * sqrt(1 - a_prev) noise), so the kept region ends as exactly z0. noise [n,4,H,W]; NULL = the N(0,1) stream keyed by `seed`
+ * that sdb_sample_image starts from. Outputs: latent_out [n,4,H,W] and / or rgb_out [n,8H,8W,3]; at least one must be set.
+ * H, W are latent sizes with the constraints of sampling (multiples of 8, (H/8)*(W/8) a multiple of 8). */
+int sdb_img2img(sdb_ctx* ctx, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
+                const float* uncond, int Lu, double guidance_scale, int n_steps, const float* noise, uint64_t seed, int H, int W,
+                float* latent_out, uint8_t* rgb_out);
+/* device-pointer variant: d_noise is required (as d_init_latent is for sdb_sample_image_dev). */
+int sdb_img2img_dev(sdb_ctx* ctx, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
+                    int L, const float* d_uncond, int Lu, double guidance_scale, int n_steps, const float* d_noise, int H, int W,
+                    float* d_latent_out, uint8_t* d_rgb_out, void* stream);
+
 /* ---- hot path, device buffers (zero-copy callers) ------------------------------------------ */
 int sdb_unet_forward_dev(sdb_ctx* ctx, const float* d_x, int32_t timestep, const float* d_context,
                          int n, int H, int W, int L, float* d_out, void* stream);

@@ -44,6 +44,14 @@ extern "C" {
     fn sdb_forward_diffuser(ctx: *mut SdbCtx, latent: *const f32, timestep: i32, context: *const f32, n: c_int, l: c_int,
                             uncond: *const f32, lu: c_int, guidance_scale: f64, h: c_int, w: c_int, pred: *mut f32,
                             out_uncond: *mut f32, out_cond: *mut f32) -> c_int;
+    fn sdb_img2img(ctx: *mut SdbCtx, image: *const u8, mask: *const u8, strength: f64, context: *const f32, n: c_int, l: c_int,
+                   uncond: *const f32, lu: c_int, guidance_scale: f64, n_steps: c_int, noise: *const f32, seed: u64, h: c_int,
+                   w: c_int, latent_out: *mut f32, rgb_out: *mut u8) -> c_int;
+    #[allow(dead_code)]
+    fn sdb_img2img_dev(ctx: *mut SdbCtx, d_image: *const c_void, d_mask: *const c_void, strength: f64, d_context: *const c_void,
+                       n: c_int, l: c_int, d_uncond: *const c_void, lu: c_int, guidance_scale: f64, n_steps: c_int,
+                       d_noise: *const c_void, h: c_int, w: c_int, d_latent_out: *mut c_void, d_rgb_out: *mut c_void,
+                       stream: *mut c_void) -> c_int;
     fn sdb_nccl_unique_id(id128: *mut c_void) -> c_int;
     fn sdb_broadcast_weights(ctx: *mut SdbCtx, id128: *const c_void, rank: c_int, world: c_int) -> c_int;
     #[allow(dead_code)]
@@ -178,6 +186,30 @@ impl StableDiffusion {
                                  pred.as_mut_ptr(), std::ptr::null_mut(), std::ptr::null_mut())
         })?;
         Ok(pred)
+    }
+
+    /// Image-to-image / masked inpainting, an extension built from the reference's encode_image
+    /// (src/model/autoencoder/mod.rs:60-66) and the schedule and DDIM step of sample_latent (src/model/stablediffusion/mod.rs:123-156).
+    /// `image`: n RGB images of `height` x `width` (multiples of 64) as HWC u8, the format `sample_image` returns; `mask`:
+    /// n x height x width u8 (255 = regenerate, 0 = keep) or None; `strength` in (0, 1]: the last floor(strength * N) of the N
+    /// timesteps run. `noise = None` draws the latent `sample_image` would start from for `seed`.
+    #[allow(clippy::too_many_arguments)]
+    pub fn img2img(&self, image: &[u8], [n, height, width]: [usize; 3], mask: Option<&[u8]>, strength: f64, context: &[f32],
+                   l: usize, unconditional_context: &[f32], lu: usize, unconditional_guidance_scale: f64, n_steps: usize,
+                   noise: Option<&[f32]>, seed: u64) -> Result<Vec<Vec<u8>>, SdbError> {
+        let (h, w) = (height / 8, width / 8);
+        if image.len() != n * height * width * 3 || mask.map_or(false, |m| m.len() != n * height * width)
+            || noise.map_or(false, |z| z.len() != n * 4 * h * w) {
+            return Err(SdbError("img2img: buffer sizes do not match [n, height, width]".into()));
+        }
+        let mut rgb = vec![0u8; n * height * width * 3];
+        self.check(unsafe {
+            sdb_img2img(self.ctx, image.as_ptr(), mask.map_or(std::ptr::null(), |m| m.as_ptr()), strength, context.as_ptr(),
+                        n as c_int, l as c_int, unconditional_context.as_ptr(), lu as c_int, unconditional_guidance_scale,
+                        n_steps as c_int, noise.map_or(std::ptr::null(), |z| z.as_ptr()), seed, h as c_int, w as c_int,
+                        std::ptr::null_mut(), rgb.as_mut_ptr())
+        })?;
+        Ok(rgb.chunks(height * width * 3).map(|c| c.to_vec()).collect())
     }
 
     /// Multi-GPU init: rank 0 calls `nccl_unique_id()` and ships the 128 bytes to the other ranks by any means; every rank then

@@ -57,6 +57,10 @@ SIGNATURES = [
     ("sdb_decode_latent_dev", C.c_int, [_ctx, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     ("sdb_sample_image_dev", C.c_int, [_ctx, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_int,
                                        C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    ("sdb_img2img", C.c_int, [_ctx, _u8p, _u8p, C.c_double, _f32p, C.c_int, C.c_int, _f32p, C.c_int, C.c_double, C.c_int, _f32p,
+                              C.c_uint64, C.c_int, C.c_int, _f32p, _u8p]),
+    ("sdb_img2img_dev", C.c_int, [_ctx, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                  C.c_double, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("sdb_set_option", C.c_int, [_ctx, C.c_char_p, C.c_int]),
     ("sdb_profile_enable", C.c_int, [_ctx, C.c_int]),
     ("sdb_profile_reset", C.c_int, [_ctx]),
@@ -262,6 +266,36 @@ class Context:
                                              ptr(init_latent) if init_latent is not None else None, seed, H, W,
                                              rgb.ctypes.data_as(_u8p)))
         return rgb
+
+    def img2img(self, image, context, uncond, scale, n_steps, strength, mask=None, noise=None, seed=0, latent=False, rgb=True):
+        """Image-to-image / masked inpainting (include/sdb200.h: sdb_img2img). image u8 [n,8H,8W,3]; mask u8 [n,8H,8W]
+        (255 = regenerate, 0 = keep) or None; noise [n,4,H,W] or None (the seeded stream sample_image starts from).
+        -> the latent [n,4,H,W] and / or the u8 image [n,8H,8W,3]: a tuple (latent, rgb) when both are requested."""
+        if not (latent or rgb):
+            raise ValueError("request the latent, the image or both")
+        image = np.ascontiguousarray(image, dtype=np.uint8)
+        if image.ndim != 4 or image.shape[3] != 3 or image.shape[1] % 8 or image.shape[2] % 8:
+            raise ValueError("image must be u8 [n, 8H, 8W, 3]")
+        n, Hp, Wp, _ = image.shape
+        H, W = Hp // 8, Wp // 8
+        context = f32(context); uncond = f32(uncond)
+        if mask is not None:
+            mask = np.ascontiguousarray(mask, dtype=np.uint8)
+            if mask.shape != (n, Hp, Wp):
+                raise ValueError("mask must be u8 [n, 8H, 8W]")
+        if noise is not None:
+            noise = f32(noise)
+            if noise.shape != (n, 4, H, W):
+                raise ValueError("noise must be [n, 4, H, W]")
+        lat = np.empty((n, 4, H, W), np.float32) if latent else None
+        out = np.empty((n, Hp, Wp, 3), np.uint8) if rgb else None
+        self.check(self.lib.sdb_img2img(self.h, image.ctypes.data_as(_u8p), None if mask is None else mask.ctypes.data_as(_u8p),
+                                        float(strength), ptr(context), n, context.shape[1], ptr(uncond), uncond.shape[0],
+                                        float(scale), int(n_steps), None if noise is None else ptr(noise), int(seed), H, W,
+                                        None if lat is None else ptr(lat), None if out is None else out.ctypes.data_as(_u8p)))
+        if latent and rgb:
+            return lat, out
+        return lat if latent else out
 
     # ---- profiling
     def profile(self, on=True):

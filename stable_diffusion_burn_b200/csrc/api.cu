@@ -345,6 +345,26 @@ int sdb_sample_image_dev(sdb_ctx* ctx, const float* d_context, int n, int L, con
   API_END
 }
 
+int sdb_img2img(sdb_ctx* ctx, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
+                const float* uncond, int Lu, double guidance_scale, int n_steps, const float* noise, uint64_t seed, int H, int W,
+                float* latent_out, uint8_t* rgb_out) {
+  API_BEGIN(ctx)
+  need_final(c);
+  model_img2img_host(c, image, mask, strength, context, n, L, uncond, Lu, guidance_scale, n_steps, noise, seed, H, W, latent_out,
+                     rgb_out);
+  API_END
+}
+
+int sdb_img2img_dev(sdb_ctx* ctx, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
+                    int L, const float* d_uncond, int Lu, double guidance_scale, int n_steps, const float* d_noise, int H, int W,
+                    float* d_latent_out, uint8_t* d_rgb_out, void* stream) {
+  API_BEGIN(ctx)
+  need_final(c);
+  model_img2img_dev(c, d_image, d_mask, strength, d_context, n, L, d_uncond, Lu, guidance_scale, n_steps, d_noise, H, W,
+                    d_latent_out, d_rgb_out, (cudaStream_t)stream);
+  API_END
+}
+
 int sdb_forward_diffuser(sdb_ctx* ctx, const float* latent, int32_t timestep, const float* context, int n, int L,
                          const float* uncond, int Lu, double guidance_scale, int H, int W, float* pred, float* out_uncond,
                          float* out_cond) {

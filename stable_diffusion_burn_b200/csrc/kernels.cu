@@ -1072,24 +1072,96 @@ void add_vec_launch(const float* a, const float* b, int n, float* y, cudaStream_
 }
 
 // ============================================================ sampler elementwise
+// BLEND (masked img2img): the step's result nl is blended with the known latent noised to the step's target level,
+// x = w nl + (1 - w) (sqrt(a_prev) z0 + sqrt(1 - a_prev) eps), w = mask[sample][pixel % plane]. nl is the same expression in
+// both instantiations, so an all-ones mask reproduces the unmasked step bit for bit; the blend is written with _rn intrinsics
+// (no FMA contraction) so that a test can restate it exactly in float32.
+template <bool BLEND>
 __global__ void cfg_ddim_kernel(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
                                 long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
-                                float dir_coef) {
+                                float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
+                                const float* __restrict__ w, int plane) {
   pdl_enter();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) {
     const float u = eu[i], c = ec[i];
     const float pred = u + (c - u) * scale;               // stablediffusion/mod.rs:190-191
     const float x0 = (lat[i] - pred * sqrt_1m_at) / sqrt_at;  // :152
-    const float nl = x0 * sqrt_aprev + pred * dir_coef;   // :153-155 (sigma = 0)
+    float nl = x0 * sqrt_aprev + pred * dir_coef;         // :153-155 (sigma = 0)
+    if constexpr (BLEND) {
+      const int p = (int)(i % plane);
+      const float wi = w[(i / (4ll * plane)) * plane + p];
+      const float known = __fadd_rn(__fmul_rn(sqrt_aprev, z0[i]), __fmul_rn(dir_coef, e0[i]));
+      nl = __fadd_rn(__fmul_rn(wi, nl), __fmul_rn(__fsub_rn(1.0f, wi), known));
+    }
     lat[i] = nl;
     lat[i + count] = nl;  // the UNet input batch holds the latent twice (uncond half | cond half)
   }
 }
 void cfg_ddim_launch(const float* eps_u, const float* eps_c, float* latent, long long count, float scale,
-                     float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st) {
+                     float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
+                     const float* z0, const float* eps0, const float* w, int plane) {
   int grid = (int)((count + 255) / 256);
   if (grid > g_num_sms * 8) grid = g_num_sms * 8;
-  launch_k(cfg_ddim_kernel, dim3(grid), dim3(256), 0, st, eps_u, eps_c, latent, count, scale, sqrt_one_minus_at, sqrt_at, sqrt_aprev, dir_coef);
+  if (w)
+    launch_k(cfg_ddim_kernel<true>, dim3(grid), dim3(256), 0, st, eps_u, eps_c, latent, count, scale, sqrt_one_minus_at, sqrt_at,
+             sqrt_aprev, dir_coef, z0, eps0, w, plane);
+  else
+    launch_k(cfg_ddim_kernel<false>, dim3(grid), dim3(256), 0, st, eps_u, eps_c, latent, count, scale, sqrt_one_minus_at, sqrt_at,
+             sqrt_aprev, dir_coef, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, 0);
+  SDB_CUDA(cudaGetLastError());
+}
+
+// ============================================================ img2img staging
+// u8 HWC RGB [nb][Hp][Wp][3] -> the encoder's input [nb][4][Hp][Wp], x = v / 127.5 - 1 (the inverse of latent_to_image's
+// (x + 1) / 2 * 255), fourth plane zero
+__global__ void u8_to_enc_input_kernel(const uint8_t* __restrict__ rgb, long long plane, long long total, float* __restrict__ out) {
+  pdl_enter();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long p = i % plane, r = i / plane;
+    const int ch = (int)(r % 4);
+    const long long s = r / 4;
+    out[i] = ch == 3 ? 0.f : __fsub_rn(__fdiv_rn((float)rgb[(s * plane + p) * 3 + ch], 127.5f), 1.0f);
+  }
+}
+void u8_to_enc_input_launch(const uint8_t* rgb, int nb, int Hp, int Wp, float* out, cudaStream_t st) {
+  const long long plane = (long long)Hp * Wp, total = (long long)nb * 4 * plane;
+  int grid = (int)((total + 255) / 256);
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
+  launch_k(u8_to_enc_input_kernel, dim3(grid), dim3(256), 0, st, rgb, plane, total, out);
+  SDB_CUDA(cudaGetLastError());
+}
+
+// Once per img2img call. Latent elements i < count: z0 *= 0.18215 in place, start latent sa z0 + sb eps into both halves of the
+// UNet input batch. Then, with a mask, one thread per latent cell j < n*H*W: w = (sum of the 8x8 mask block) / (64 * 255).
+__global__ void img2img_prep_kernel(float* __restrict__ z0, const float* __restrict__ eps, float* __restrict__ xb, long long count,
+                                    float sa, float sb, const uint8_t* __restrict__ mask, float* __restrict__ w, int H, int W) {
+  pdl_enter();
+  const long long cells = mask ? count / 4 : 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count + cells; i += (long long)gridDim.x * blockDim.x) {
+    if (i < count) {
+      const float z = __fmul_rn(z0[i], 0.18215f);
+      const float x = __fadd_rn(__fmul_rn(sa, z), __fmul_rn(sb, eps[i]));
+      z0[i] = z;
+      xb[i] = x;
+      xb[i + count] = x;
+    } else {
+      const long long j = i - count;
+      const int x = (int)(j % W), y = (int)((j / W) % H);
+      const long long s = j / ((long long)H * W);
+      const uint8_t* m = mask + (s * 8 * H + 8 * y) * 8 * W + 8 * x;
+      int sum = 0;
+      for (int r = 0; r < 8; ++r)
+        for (int q = 0; q < 8; ++q) sum += m[(long long)r * 8 * W + q];
+      w[j] = __fdiv_rn((float)sum, 16320.0f);
+    }
+  }
+}
+void img2img_prep_launch(float* z0, const float* eps, float* xb, long long count, float sa, float sb, const uint8_t* mask, float* w,
+                         int H, int W, cudaStream_t st) {
+  const long long total = count + (mask ? count / 4 : 0);
+  int grid = (int)((total + 255) / 256);
+  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
+  launch_k(img2img_prep_kernel, dim3(grid), dim3(256), 0, st, z0, eps, xb, count, sa, sb, mask, w, H, W);
   SDB_CUDA(cudaGetLastError());
 }
 

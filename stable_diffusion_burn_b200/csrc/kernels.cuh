@@ -93,8 +93,16 @@ void embed_tokens_launch(const int* tok, const float* E, const float* Pos, int n
 // ---- sampler elementwise (reference stablediffusion/mod.rs:152-156, 190-191)
 // pred = u + (c-u)*scale ; x0 = (lat - pred*sqrt(1-a_t))/sqrt(a_t) ; lat' = x0*sqrt(a_prev) + pred*sqrt(1-a_prev)
 // latent holds 2*count floats: the update is written to both halves (uncond | cond inputs of the next step)
+// w != null (masked img2img): lat' = w lat' + (1 - w) (sqrt(a_prev) z0 + sqrt(1 - a_prev) eps0), w [n][plane] per latent cell
 void cfg_ddim_launch(const float* eps_u, const float* eps_c, float* latent, long long count, float scale,
-                     float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st);
+                     float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
+                     const float* z0 = nullptr, const float* eps0 = nullptr, const float* w = nullptr, int plane = 0);
+// ---- img2img staging: u8 HWC RGB [nb][Hp][Wp][3] -> encoder input [nb][4][Hp][Wp], v / 127.5 - 1, fourth plane zero
+void u8_to_enc_input_launch(const uint8_t* rgb, int nb, int Hp, int Wp, float* out, cudaStream_t st);
+// z0 [count] *= 0.18215 in place; xb[0..count) = xb[count..2count) = sa z0 + sb eps; mask (optional, u8 [n][8H][8W]) ->
+// w [n][H][W] = 8x8 block sum / 16320
+void img2img_prep_launch(float* z0, const float* eps, float* xb, long long count, float sa, float sb, const uint8_t* mask, float* w,
+                         int H, int W, cudaStream_t st);
 // pred = u + (c - u) * scale alone (forward_diffuser without the DDIM update)
 void cfg_combine_launch(const float* eps_u, const float* eps_c, long long count, float scale, float* pred, cudaStream_t st);
 // u8 = trunc(clamp((img+1)/2*255, 0, 255)), NCHW fp32 -> NHWC u8 (reference stablediffusion/mod.rs:79-97)

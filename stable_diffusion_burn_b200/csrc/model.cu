@@ -1055,17 +1055,38 @@ void model_latent_to_image_host(Ctx& c, const float* latent, int n, int H, int W
   SDB_CUDA(cudaStreamSynchronize(c.stream));
 }
 
-// sample_latent + latent_to_image (stablediffusion/mod.rs:51-160). The conditional and unconditional UNet
-// evaluations of a step (forward_diffuser :162-192) run as ONE batch-2n pass: weights stream from HBM once.
-void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale,
-                      int n_steps, const float* d_init_latent, int H, int W, float* d_latent_out, uint8_t* d_rgb,
-                      cudaStream_t caller) {
-  Model& m = M(c);
+static void check_sample_args(int n, int L, int Lu, int n_steps, int H, int W) {
   SDB_CHECK(n >= 1 && L >= 1 && Lu >= 1, "sample arguments");
   SDB_CHECK(n_steps >= 1 && n_steps <= 1000, "n_steps must be in [1,1000] (step_by(0) panics in the reference)");
   SDB_CHECK(H % 8 == 0 && W % 8 == 0, "latent size must be a multiple of 8");
   SDB_CHECK(((H / 8) * (W / 8)) % 8 == 0, "unsupported latent size: (H/8)*(W/8) must be a multiple of 8");
-  StreamJoin join(c, caller);
+}
+
+// timesteps (stablediffusion/mod.rs:111,123): (0..1000).rev().step_by(1000 / n_steps)
+static std::vector<int> ddim_timesteps(int n_steps) {
+  std::vector<int> ts;
+  for (int t = 999; t >= 0; t -= 1000 / n_steps) ts.push_back(t);
+  return ts;
+}
+
+namespace {
+struct Img2ImgIn {  // what the sampler loop needs to start part way down the schedule from an encoded image
+  float* z0 = nullptr;          // [n,4,H,W] encoder output; scaled by 0.18215 in place by the preparation kernel
+  const float* eps = nullptr;   // [n,4,H,W] the noise
+  const uint8_t* mask = nullptr;  // [n,8H,8W] or null
+  float* w = nullptr;           // [n,H,W] latent mask (written when mask is set)
+  float sa = 0.f, sb = 0.f;     // sqrt(abar[t0]), sqrt(1 - abar[t0])
+};
+}  // namespace
+
+// sample_latent + latent_to_image (stablediffusion/mod.rs:51-160) from schedule index `first` on. The conditional and
+// unconditional UNet evaluations of a step (forward_diffuser :162-192) run as ONE batch-2n pass: weights stream from HBM once.
+// ii == null: txt2img from d_init_latent. Otherwise the start latent and (with a mask) the per-step blend come from ii.
+// Runs on c.stream; the caller joins the streams.
+static void sample_loop(Ctx& c, const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale, int n_steps,
+                        int first, const float* d_init_latent, const Img2ImgIn* ii, int H, int W, float* d_latent_out,
+                        uint8_t* d_rgb) {
+  Model& m = M(c);
   c.work.reset();
   const int nb = 2 * n;
   const int Lpad = round_up(std::max(L, Lu), 32);
@@ -1081,12 +1102,16 @@ void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float*
     SDB_CUDA(cudaMemcpyAsync(ctxp + (size_t)i * Lpad * 768, d_uncond, (size_t)Lu * 768 * 4, cudaMemcpyDeviceToDevice, c.stream));
   SDB_CUDA(cudaMemcpy2DAsync(ctxp + (size_t)n * Lpad * 768, (size_t)Lpad * 768 * 4, d_context, (size_t)L * 768 * 4,
                              (size_t)L * 768 * 4, n, cudaMemcpyDeviceToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(xb, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(xb + le, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
-  // timesteps (stablediffusion/mod.rs:111,123): (0..1000).rev().step_by(1000 / n_steps)
+  if (!ii) {
+    SDB_CUDA(cudaMemcpyAsync(xb, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
+    SDB_CUDA(cudaMemcpyAsync(xb + le, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
+  } else {
+    KernelScope ks(c, KC_ELEMENTWISE);
+    img2img_prep_launch(ii->z0, ii->eps, xb, (long long)le, ii->sa, ii->sb, ii->mask, ii->w, H, W, c.stream);
+  }
   const int step = 1000 / n_steps;
-  std::vector<int> ts;
-  for (int t = 999; t >= 0; t -= step) ts.push_back(t);
+  std::vector<int> ts = ddim_timesteps(n_steps);
+  ts.erase(ts.begin(), ts.begin() + first);  // img2img runs the last k timesteps only
   std::vector<int> lens(nb);
   for (int i = 0; i < nb; ++i) lens[i] = i < n ? Lu : L;
   SDB_CUDA(cudaMemcpyAsync(d_t, ts.data(), ts.size() * 4, cudaMemcpyHostToDevice, c.stream));
@@ -1125,8 +1150,9 @@ void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float*
   int64_t graph_launches = 0;
   if (use_graph) {
     for (auto& g : m.graphs)
-      if (g.key == key && g.io[0] == (void*)xb && g.io[1] == (void*)eps && g.io[2] == (void*)cs.kv[0].kv) exec = g.exec,
-          graph_launches = (int64_t)(intptr_t)g.io[3];
+      if (g.key == key && g.io[0] == (void*)xb && g.io[1] == (void*)eps && g.io[2] == (void*)cs.kv[0].kv &&
+          g.io[4] == (void*)(uintptr_t)work_mark)  // the step's own temporaries start at work_mark
+        exec = g.exec, graph_launches = (int64_t)(intptr_t)g.io[3];
     if (!exec) {
       // warm-up pass outside capture (sets kernel attributes), then capture
       SDB_CUDA(cudaMemcpyAsync(d_tcur, d_t, 4, cudaMemcpyDeviceToDevice, c.stream));
@@ -1151,6 +1177,7 @@ void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float*
       ge.key = key, ge.exec = exec;
       memset(ge.io, 0, sizeof(ge.io));
       ge.io[0] = xb, ge.io[1] = eps, ge.io[2] = cs.kv[0].kv, ge.io[3] = (void*)(intptr_t)graph_launches;
+      ge.io[4] = (void*)(uintptr_t)work_mark;
       m.graphs.push_back(ge);
     }
   }
@@ -1168,12 +1195,22 @@ void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float*
       unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all);
     }
     KernelScope ks(c, KC_ELEMENTWISE);
+    const bool blend = ii && ii->mask;
     cfg_ddim_launch(eps, eps + le, xb, (long long)le, (float)scale, (float)std::sqrt(1.0 - a_t), (float)std::sqrt(a_t),
-                    (float)std::sqrt(a_prev), (float)std::sqrt(1.0 - a_prev), c.stream);
+                    (float)std::sqrt(a_prev), (float)std::sqrt(1.0 - a_prev), c.stream, blend ? ii->z0 : nullptr,
+                    blend ? ii->eps : nullptr, blend ? ii->w : nullptr, H * W);
   }
   c.work.off = work_mark;
   if (d_latent_out) SDB_CUDA(cudaMemcpyAsync(d_latent_out, xb, le * 4, cudaMemcpyDeviceToDevice, c.stream));
   if (d_rgb) latent_to_image_dev(c, xb, n, H, W, d_rgb);
+}
+
+void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale,
+                      int n_steps, const float* d_init_latent, int H, int W, float* d_latent_out, uint8_t* d_rgb,
+                      cudaStream_t caller) {
+  check_sample_args(n, L, Lu, n_steps, H, W);
+  StreamJoin join(c, caller);
+  sample_loop(c, d_context, n, L, d_uncond, Lu, scale, n_steps, 0, d_init_latent, nullptr, H, W, d_latent_out, d_rgb);
 }
 
 void model_sample_host(Ctx& c, const float* context, int n, int L, const float* uncond, int Lu, double scale, int n_steps,
@@ -1191,6 +1228,90 @@ void model_sample_host(Ctx& c, const float* context, int n, int L, const float* 
   else
     randn_launch(d_l, (long long)le, seed, c.stream);
   model_sample_dev(c, d_c, n, L, d_u, Lu, scale, n_steps, d_l, H, W, d_lo, d_r, c.stream);
+  if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
+  if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+// ================================================================================ image-to-image / inpainting (DESIGN §7 f5)
+// The schedule index img2img starts from: k = floor(strength * N) of the N timesteps run, the last k of them.
+static int img2img_first(double strength, int n_steps) {
+  SDB_CHECK(std::isfinite(strength) && strength > 0.0 && strength <= 1.0, "img2img: strength must be finite and in (0, 1]");
+  const int N = (int)ddim_timesteps(n_steps).size();
+  const int k = (int)std::floor(strength * (double)N);
+  char msg[160];
+  snprintf(msg, sizeof(msg), "img2img: strength %.17g runs none of the %d timesteps; the smallest valid strength is 1/%d = %.17g",
+           strength, N, N, 1.0 / N);
+  SDB_CHECK(k >= 1, msg);
+  return N - k;
+}
+
+static void check_img2img_args(int n, int L, int Lu, int n_steps, int H, int W, const void* image, const void* context,
+                               const void* uncond, const void* latent_out, const void* rgb) {
+  check_sample_args(n, L, Lu, n_steps, H, W);
+  SDB_CHECK(image && context && uncond, "img2img: null image, context or uncond");
+  SDB_CHECK(latent_out || rgb, "img2img: request the latent, the image or both");
+}
+
+// Encoder (chunks of 4 images, as model_encode_dev) -> z0 in an io slot -> sampler loop from t0 = ts[N - k] -> decode.
+// z0 and the latent mask live in io slots, not in the work arena: the arena prefix up to the loop's work_mark is laid out
+// exactly as txt2img lays it out, so no cached step graph can see img2img data where it expects its own temporaries.
+void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
+                       int L, const float* d_uncond, int Lu, double scale, int n_steps, const float* d_noise, int H, int W,
+                       float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
+  Model& m = M(c);
+  check_img2img_args(n, L, Lu, n_steps, H, W, d_image, d_context, d_uncond, d_latent_out, d_rgb);
+  SDB_CHECK(d_noise, "img2img: the device entry needs the noise latent");
+  const int first = img2img_first(strength, n_steps);
+  const double abar = (double)m.alphas_host[ddim_timesteps(n_steps)[first]];  // read as f32, widened (mod.rs:124-140)
+  Img2ImgIn ii;
+  ii.sa = (float)std::sqrt(abar), ii.sb = (float)std::sqrt(1.0 - abar);
+  ii.eps = d_noise, ii.mask = d_mask;
+  StreamJoin join(c, caller);
+  const size_t le = (size_t)n * 4 * H * W;
+  ii.z0 = (float*)c.io(kIoImg2ImgZ0, le * 4);
+  if (d_mask) ii.w = (float*)c.io(kIoImg2ImgW, (size_t)n * H * W * 4);
+  c.work.reset();
+  const int Hp = 8 * H, Wp = 8 * W;
+  const size_t plane = (size_t)Hp * Wp;
+  for (int i0 = 0; i0 < n; i0 += 4) {
+    const int nb = std::min(4, n - i0);
+    const size_t mark = c.work.off;
+    float* img4 = c.work.get<float>((size_t)nb * 4 * plane);
+    {
+      KernelScope ks(c, KC_ELEMENTWISE);
+      u8_to_enc_input_launch(d_image + (size_t)i0 * 3 * plane, nb, Hp, Wp, img4, c.stream);
+    }
+    Fwd f(c, nb);
+    vae_encode(f, img4, Hp, Wp, ii.z0 + (size_t)i0 * 4 * H * W);
+    c.work.off = mark;
+  }
+  sample_loop(c, d_context, n, L, d_uncond, Lu, scale, n_steps, first, nullptr, &ii, H, W, d_latent_out, d_rgb);
+}
+
+void model_img2img_host(Ctx& c, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
+                        const float* uncond, int Lu, double scale, int n_steps, const float* noise, uint64_t seed, int H, int W,
+                        float* latent_out, uint8_t* rgb) {
+  check_img2img_args(n, L, Lu, n_steps, H, W, image, context, uncond, latent_out, rgb);
+  img2img_first(strength, n_steps);  // reject before staging anything
+  const size_t le = (size_t)n * 4 * H * W, ce = (size_t)n * L * 768, ue = (size_t)Lu * 768, re = (size_t)n * 3 * 64 * H * W,
+               me = (size_t)n * 64 * H * W;
+  float* d_c = (float*)c.io(0, ce * 4);
+  float* d_u = (float*)c.io(1, ue * 4);
+  float* d_n = (float*)c.io(2, le * 4);
+  float* d_lo = latent_out ? (float*)c.io(3, le * 4) : nullptr;
+  uint8_t* d_r = rgb ? (uint8_t*)c.io(4, re) : nullptr;
+  uint8_t* d_i = (uint8_t*)c.io(5, re);
+  uint8_t* d_m = mask ? (uint8_t*)c.io(6, me) : nullptr;
+  SDB_CUDA(cudaMemcpyAsync(d_c, context, ce * 4, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(d_u, uncond, ue * 4, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(d_i, image, re, cudaMemcpyHostToDevice, c.stream));
+  if (mask) SDB_CUDA(cudaMemcpyAsync(d_m, mask, me, cudaMemcpyHostToDevice, c.stream));
+  if (noise)
+    SDB_CUDA(cudaMemcpyAsync(d_n, noise, le * 4, cudaMemcpyHostToDevice, c.stream));
+  else
+    randn_launch(d_n, (long long)le, seed, c.stream);  // the latent txt2img would start from for this seed
+  model_img2img_dev(c, d_i, d_m, strength, d_c, n, L, d_u, Lu, scale, n_steps, d_n, H, W, d_lo, d_r, c.stream);
   if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
   if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));

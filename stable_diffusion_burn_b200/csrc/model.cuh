@@ -23,6 +23,13 @@ void model_sample_host(Ctx& c, const float* context, int n, int L, const float* 
 void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale,
                       int n_steps, const float* d_init_latent, int H, int W, float* d_latent_out, uint8_t* d_rgb,
                       cudaStream_t caller);
+// image-to-image / masked inpainting (DESIGN §7 f5): image u8 [n,8H,8W,3], mask u8 [n,8H,8W] or null, noise [n,4,H,W]
+void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
+                       int L, const float* d_uncond, int Lu, double scale, int n_steps, const float* d_noise, int H, int W,
+                       float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller);
+void model_img2img_host(Ctx& c, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
+                        const float* uncond, int Lu, double scale, int n_steps, const float* noise, uint64_t seed, int H, int W,
+                        float* latent_out, uint8_t* rgb);
 void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const float* d_context, int n, int L, const float* d_uncond,
                                 int Lu, double scale, int H, int W, float* d_pred, float* d_u, float* d_c, cudaStream_t caller);
 void model_forward_diffuser_host(Ctx& c, const float* latent, int t, const float* context, int n, int L, const float* uncond,

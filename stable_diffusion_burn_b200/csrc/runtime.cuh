@@ -113,6 +113,9 @@ struct MetaCheck {
   bool must_be_absent = false;  // e.g. a bias file on a bias-less Linear
 };
 
+constexpr int kIoImg2ImgZ0 = 8;  // encoded image latent z0 [n,4,H,W]
+constexpr int kIoImg2ImgW = 9;   // latent mask w [n,H,W]
+
 struct Ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -144,11 +147,12 @@ struct Ctx {
   double cls_ms[KC_COUNT] = {0}, cls_flops[KC_COUNT] = {0}, cls_bytes[KC_COUNT] = {0};
   double cls_issued[KC_COUNT] = {0};  // tensor-core FLOPs actually issued (x passes for split-fp16 products)
   int64_t cls_launches[KC_COUNT] = {0};
-  // grow-only device staging for the host-buffer entry points (no cudaMalloc/cudaFree per call: each is a device-wide sync)
+  // grow-only device staging for the host-buffer entry points (no cudaMalloc/cudaFree per call: each is a device-wide sync).
+  // Slots 0..6: host-entry staging; kIoImg2Img*: buffers the img2img device entry keeps outside the work arena.
   struct IoBuf {
     void* p = nullptr;
     size_t cap = 0;
-  } iobuf[6];
+  } iobuf[10];
   void* io(int slot, size_t bytes);
   void io_destroy();
   void* model = nullptr;  // Model* (model.cu)

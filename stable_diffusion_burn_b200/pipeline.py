@@ -106,6 +106,15 @@ class StableDiffusion:
         return self.ctx.sample_latent(context, unconditional_context, unconditional_guidance_scale, n_steps,
                                       init_latent=init_latent, seed=seed, H=height // 8, W=width // 8)
 
+    def img2img(self, image, context, unconditional_context, unconditional_guidance_scale: float, n_steps: int,
+                strength: float, mask=None, noise=None, seed: int = 0):
+        """Image-to-image / masked inpainting (an extension: the reference has none; DESIGN.md §7 f5). image u8
+        [n, height, width, 3] HWC RGB, the format sample_image returns; mask u8 [n, height, width] (255 = regenerate,
+        0 = keep) or None; strength in (0, 1]. -> list of n flat uint8 arrays of height*width*3, like sample_image."""
+        rgb = self.ctx.img2img(image, context, unconditional_context, unconditional_guidance_scale, n_steps, strength,
+                               mask=mask, noise=noise, seed=seed)
+        return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
+
     def latent_to_image(self, latent):
         rgb = self.ctx.latent_to_image(latent)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
