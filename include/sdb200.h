@@ -86,8 +86,8 @@ int sdb_unet_forward(sdb_ctx* ctx, const float* x, int32_t timestep, const float
                      int n, int H, int W, int L, float* out);
 /* Autoencoder::decode_latent (src/model/autoencoder/mod.rs:68-71): latent [n,4,H,W] -> img [n,3,8H,8W]. */
 int sdb_decode_latent(sdb_ctx* ctx, const float* latent, int n, int H, int W, float* img);
-/* StableDiffusion::sample_latent (src/model/stablediffusion/mod.rs:102-160), DDIM eta=0 with
- * classifier-free guidance (forward_diffuser :162-192). context [n,L,768]; uncond [Lu,768] is
+/* StableDiffusion::sample_latent (src/model/stablediffusion/mod.rs:102-160), DDIM eta=0 (the default sampler; see
+ * sdb_set_sampler) with classifier-free guidance (forward_diffuser :162-192). context [n,L,768]; uncond [Lu,768] is
  * broadcast over the batch. init_latent [n,4,H,W] (the reference draws it from an unseeded RNG,
  * :115-121); if NULL an internal Philox N(0,1) stream keyed by `seed` is used. */
 int sdb_sample_latent(sdb_ctx* ctx, const float* context, int n, int L, const float* uncond, int Lu,
@@ -140,6 +140,21 @@ int sdb_img2img(sdb_ctx* ctx, const uint8_t* image, const uint8_t* mask, double 
 int sdb_img2img_dev(sdb_ctx* ctx, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
                     int L, const float* d_uncond, int Lu, double guidance_scale, int n_steps, const float* d_noise, int H, int W,
                     float* d_latent_out, uint8_t* d_rgb_out, void* stream);
+
+/* ---- sampler (DESIGN.md §7 f6) ------------------------------------------------------------------------------------------ */
+/* The reference samples with DDIM at eta = 0 only (src/model/stablediffusion/mod.rs:119, sigma = 0). The sampler is context
+ * state, read by sdb_sample_latent, sdb_sample_image, sdb_sample_image_dev, sdb_img2img and sdb_img2img_dev (not by
+ * sdb_forward_diffuser or sdb_unet_forward); the schedule, the UNet step and the decode are the same for every sampler.
+ * SDB_SAMPLER_DDIM with eta in [0, 1] (finite): DDIM (Song et al. 2021, eq. 16), s = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a'),
+ *   x' = sqrt(a') x0 + sqrt(1 - a' - s^2) eps + s z. eta = 0 (the default) is the reference's sampler, unchanged to the bit.
+ *   z is N(0,1) keyed by (noise_seed, timestep value, element index in the call's [n,4,H,W] latent): a batch member's noise
+ *   depends on its position in the call.
+ * SDB_SAMPLER_DPMPP_2M (eta must be 0): DPM-Solver++(2M) (Lu et al. 2022), data prediction, second order from the second step
+ *   a call runs; the final step returns x0. A context starts with (SDB_SAMPLER_DDIM, 0.0, 0). Invalid arguments are an error
+ *   and leave the setting unchanged. */
+#define SDB_SAMPLER_DDIM 0
+#define SDB_SAMPLER_DPMPP_2M 1
+int sdb_set_sampler(sdb_ctx* ctx, int kind, double eta, uint64_t noise_seed);
 
 /* ---- hot path, device buffers (zero-copy callers) ------------------------------------------ */
 int sdb_unet_forward_dev(sdb_ctx* ctx, const float* d_x, int32_t timestep, const float* d_context,
@@ -231,6 +246,9 @@ int sdb_test_resblock(sdb_ctx* ctx, const float* x0, const float* x1, int n, int
  * trace as sdb_test_resblock. */
 int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n, int c0, int c1, int H, int W,
                            const float* gamma, const float* beta, int silu, int mode, float* y, int32_t* trace);
+/* The first `count` values of stochastic DDIM's noise z at timestep t (0 <= t < 1000) for noise_seed, as the fused sampler step
+ * draws them (see sdb_set_sampler). Host buffer out [count]. */
+int sdb_test_step_noise(sdb_ctx* ctx, uint64_t noise_seed, int t, int64_t count, float* out);
 
 #ifdef __cplusplus
 }

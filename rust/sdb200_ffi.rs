@@ -52,6 +52,7 @@ extern "C" {
                        n: c_int, l: c_int, d_uncond: *const c_void, lu: c_int, guidance_scale: f64, n_steps: c_int,
                        d_noise: *const c_void, h: c_int, w: c_int, d_latent_out: *mut c_void, d_rgb_out: *mut c_void,
                        stream: *mut c_void) -> c_int;
+    fn sdb_set_sampler(ctx: *mut SdbCtx, kind: c_int, eta: f64, noise_seed: u64) -> c_int;
     fn sdb_nccl_unique_id(id128: *mut c_void) -> c_int;
     fn sdb_broadcast_weights(ctx: *mut SdbCtx, id128: *const c_void, rank: c_int, world: c_int) -> c_int;
     #[allow(dead_code)]
@@ -62,6 +63,16 @@ extern "C" {
 
 #[derive(Debug)]
 pub struct SdbError(pub String);
+
+const SDB_SAMPLER_DDIM: c_int = 0;
+const SDB_SAMPLER_DPMPP_2M: c_int = 1;
+
+/// The sampler of the sampling calls (include/sdb200.h: sdb_set_sampler).
+#[derive(Clone, Copy, Debug)]
+pub enum Sampler {
+    Ddim { eta: f64 },
+    DpmPp2M,
+}
 
 pub struct StableDiffusion {
     ctx: *mut SdbCtx,
@@ -210,6 +221,17 @@ impl StableDiffusion {
                         std::ptr::null_mut(), rgb.as_mut_ptr())
         })?;
         Ok(rgb.chunks(height * width * 3).map(|c| c.to_vec()).collect())
+    }
+
+    /// The sampler of `sample_image` / `sample_latent` / `img2img` until changed (an extension: the reference samples with DDIM at
+    /// eta = 0, src/model/stablediffusion/mod.rs:119). `Sampler::Ddim { eta }` with eta in [0, 1] (0 = the reference's sampler,
+    /// the default) or `Sampler::DpmPp2M` (DPM-Solver++(2M), good at 10-15 steps); `noise_seed` keys stochastic DDIM's noise.
+    pub fn set_sampler(&self, sampler: Sampler, noise_seed: u64) -> Result<(), SdbError> {
+        let (kind, eta) = match sampler {
+            Sampler::Ddim { eta } => (SDB_SAMPLER_DDIM, eta),
+            Sampler::DpmPp2M => (SDB_SAMPLER_DPMPP_2M, 0.0),
+        };
+        self.check(unsafe { sdb_set_sampler(self.ctx, kind, eta, noise_seed) })
     }
 
     /// Multi-GPU init: rank 0 calls `nccl_unique_id()` and ships the 128 bytes to the other ranks by any means; every rank then

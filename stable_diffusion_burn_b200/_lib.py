@@ -61,6 +61,7 @@ SIGNATURES = [
                               C.c_uint64, C.c_int, C.c_int, _f32p, _u8p]),
     ("sdb_img2img_dev", C.c_int, [_ctx, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                   C.c_double, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("sdb_set_sampler", C.c_int, [_ctx, C.c_int, C.c_double, C.c_uint64]),
     ("sdb_set_option", C.c_int, [_ctx, C.c_char_p, C.c_int]),
     ("sdb_profile_enable", C.c_int, [_ctx, C.c_int]),
     ("sdb_profile_reset", C.c_int, [_ctx]),
@@ -81,6 +82,7 @@ SIGNATURES = [
                                     C.c_int, C.c_int, _f32p, _f32p, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_groupnorm_cat", C.c_int, [_ctx, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, _f32p,
                                          C.c_int, C.c_int, _f32p, C.POINTER(C.c_int32)]),
+    ("sdb_test_step_noise", C.c_int, [_ctx, C.c_uint64, C.c_int, C.c_int64, _f32p]),
     ("sdb_test_groupnorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_test_layernorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, _f32p]),
     ("sdb_test_attention", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -180,6 +182,17 @@ class Context:
 
     def set_option(self, key, value):
         self.check(self.lib.sdb_set_option(self.h, key.encode(), int(value)))
+
+    SAMPLERS = {"ddim": 0, "dpmpp_2m": 1}  # SDB_SAMPLER_DDIM, SDB_SAMPLER_DPMPP_2M
+
+    def set_sampler(self, kind=0, eta=0.0, noise_seed=0):
+        """Sampler of every sampling entry until changed (include/sdb200.h: sdb_set_sampler; DESIGN.md §7 f6). kind: 0 / "ddim"
+        (eta in [0, 1]) or 1 / "dpmpp_2m" (eta 0). noise_seed keys stochastic DDIM's per-step noise."""
+        if isinstance(kind, str):
+            if kind not in self.SAMPLERS:
+                raise ValueError(f"unknown sampler {kind!r}: one of {', '.join(self.SAMPLERS)}")
+            kind = self.SAMPLERS[kind]
+        self.check(self.lib.sdb_set_sampler(self.h, int(kind), float(eta), int(noise_seed)))
 
     # ---- hot path (host buffers)
     def unet_forward(self, x, t, context):
@@ -429,6 +442,12 @@ class Context:
         g = f32(gamma); b = f32(beta)
         self.check(self.lib.sdb_test_groupnorm(self.h, ptr(x), ptr(g), ptr(b), n, c, H, W, 1 if silu else 0, ptr(y)))
         return y
+
+    def test_step_noise(self, noise_seed, t, count):
+        """stochastic DDIM's noise z at timestep t: the first `count` values (numpy mirror: synth.step_noise)."""
+        out = np.empty(int(count), np.float32)
+        self.check(self.lib.sdb_test_step_noise(self.h, int(noise_seed), int(t), int(count), ptr(out)))
+        return out
 
     def test_layernorm(self, x, gamma, beta):
         x = f32(x); rows, c = x.shape

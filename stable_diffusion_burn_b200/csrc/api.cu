@@ -414,6 +414,20 @@ int sdb_clip_forward_dev(sdb_ctx* ctx, const int32_t* d_tokens, int n, int L, fl
   API_END
 }
 
+// ------------------------------------------------------------------------------ sampler (DESIGN.md §7 f6)
+int sdb_set_sampler(sdb_ctx* ctx, int kind, double eta, uint64_t noise_seed) {
+  API_BEGIN(ctx)
+  char msg[160];
+  snprintf(msg, sizeof(msg), "sampler: unknown kind %d (SDB_SAMPLER_DDIM = 0, SDB_SAMPLER_DPMPP_2M = 1)", kind);
+  SDB_CHECK(kind == SDB_SAMPLER_DDIM || kind == SDB_SAMPLER_DPMPP_2M, msg);
+  snprintf(msg, sizeof(msg), "sampler: eta %.17g must be finite and in [0, 1]", eta);
+  SDB_CHECK(std::isfinite(eta) && eta >= 0.0 && eta <= 1.0, msg);
+  snprintf(msg, sizeof(msg), "sampler: DPM-Solver++(2M) is deterministic; eta %.17g must be 0", eta);
+  SDB_CHECK(kind != SDB_SAMPLER_DPMPP_2M || eta == 0.0, msg);
+  c.sampler_kind = kind, c.sampler_eta = eta, c.sampler_noise_seed = noise_seed;
+  API_END
+}
+
 // ------------------------------------------------------------------------------ options / profiling
 int sdb_set_option(sdb_ctx* ctx, const char* key, int value) {
   API_BEGIN(ctx)
@@ -844,6 +858,17 @@ int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n
   API_BEGIN(ctx)
   c.work.reset();
   model_test_groupnorm_cat(c, x0, x1, n, c0, c1, H, W, gamma, beta, silu, mode, y, trace);
+  API_END
+}
+
+int sdb_test_step_noise(sdb_ctx* ctx, uint64_t noise_seed, int t, int64_t count, float* out) {
+  API_BEGIN(ctx)
+  SDB_CHECK(out && count >= 1, "step_noise: null output or count < 1");
+  SDB_CHECK(t >= 0 && t < 1000, "step_noise: timestep must be in [0, 1000)");
+  float* d = (float*)c.io(0, (size_t)count * 4);
+  step_noise_launch(d, (long long)count, noise_seed, t, c.stream);
+  SDB_CUDA(cudaMemcpyAsync(out, d, (size_t)count * 4, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
   API_END
 }
 

@@ -1072,30 +1072,94 @@ void add_vec_launch(const float* a, const float* b, int n, float* y, cudaStream_
 }
 
 // ============================================================ sampler elementwise
+__host__ __device__ __forceinline__ uint32_t mix32(uint32_t x) {
+  x ^= x >> 16;
+  x *= 0x85EBCA6Bu;
+  x ^= x >> 13;
+  x *= 0xC2B2AE35u;
+  x ^= x >> 16;
+  return x;
+}
+// Counter-hash Box-Muller N(0,1): element i of the stream keyed by (k0, k1). The init latent (randn_launch) and the per-step
+// noise of stochastic DDIM (step_noise_keys) are both this function, evaluated in registers where they are consumed.
+__device__ __forceinline__ float randn_at(long long i, uint32_t k0, uint32_t k1) {
+  const uint32_t a = mix32((uint32_t)i ^ k0), b = mix32(((uint32_t)i * 0x9E3779B9u) ^ k1);
+  const float u1 = ((a >> 8) + 1) * (1.0f / 16777216.0f);  // (0,1]
+  const float u2 = (b >> 8) * (1.0f / 16777216.0f);
+  return sqrtf(-2.0f * logf(u1)) * cosf(6.283185307179586f * u2);
+}
+
+// One fused guidance + update step of the sampler (DESIGN §7 f5, f6), per latent element i < count:
+//   pred = u + (c - u) scale, x0 = (x - sqrt(1 - a_t) pred) / sqrt(a_t)                        (every kind)
+//   STEP_DDIM        x' = sqrt(a_prev) x0 + dir_coef pred                        (eta = 0: sample_latent's own step)
+//   STEP_DDIM_ETA    x' = sqrt(a_prev) x0 + dir_coef pred + s z,  z = randn_at(i, k0, k1)
+//   STEP_DPMPP_2M    D = x0 (first order) or c1 x0 - c2 x0_prev (second order); x0_prev <- x0; x' = cx x + cd D
 // BLEND (masked img2img): the step's result nl is blended with the known latent noised to the step's target level,
 // x = w nl + (1 - w) (sqrt(a_prev) z0 + sqrt(1 - a_prev) eps), w = mask[sample][pixel % plane]. nl is the same expression in
-// both instantiations, so an all-ones mask reproduces the unmasked step bit for bit; the blend is written with _rn intrinsics
-// (no FMA contraction) so that a test can restate it exactly in float32.
-template <bool BLEND>
-__global__ void cfg_ddim_kernel(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
-                                long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
-                                float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
-                                const float* __restrict__ w, int plane) {
+// both instantiations, so an all-ones mask reproduces the unmasked step bit for bit. The blend and the new samplers' updates
+// are written with _rn intrinsics (no FMA contraction) so that a test can restate them exactly in float32. STEP_DDIM is the
+// expression sample_latent has always used; its kernel keeps the argument list and the instructions it had.
+template <int KIND, bool BLEND>
+__device__ __forceinline__ void cfg_step(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
+                                         long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
+                                         float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
+                                         const float* __restrict__ w, int plane, const SamplerStep& s) {
   pdl_enter();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) {
     const float u = eu[i], c = ec[i];
     const float pred = u + (c - u) * scale;               // stablediffusion/mod.rs:190-191
-    const float x0 = (lat[i] - pred * sqrt_1m_at) / sqrt_at;  // :152
-    float nl = x0 * sqrt_aprev + pred * dir_coef;         // :153-155 (sigma = 0)
+    const float x = lat[i];
+    const float x0 = (x - pred * sqrt_1m_at) / sqrt_at;   // :152
+    float nl;
+    if constexpr (KIND == STEP_DDIM) {
+      nl = x0 * sqrt_aprev + pred * dir_coef;             // :153-155 (sigma = 0)
+    } else if constexpr (KIND == STEP_DDIM_ETA) {         // :153-155 with sigma = s
+      nl = __fadd_rn(__fadd_rn(__fmul_rn(sqrt_aprev, x0), __fmul_rn(dir_coef, pred)), __fmul_rn(s.s, randn_at(i, s.k0, s.k1)));
+    } else {
+      const float d = s.second ? __fsub_rn(__fmul_rn(s.c1, x0), __fmul_rn(s.c2, s.hist[i])) : x0;
+      s.hist[i] = x0;
+      nl = __fadd_rn(__fmul_rn(s.cx, x), __fmul_rn(s.cd, d));
+    }
     if constexpr (BLEND) {
+      const float ka = KIND == STEP_DDIM ? sqrt_aprev : s.ka, kb = KIND == STEP_DDIM ? dir_coef : s.kb;
       const int p = (int)(i % plane);
       const float wi = w[(i / (4ll * plane)) * plane + p];
-      const float known = __fadd_rn(__fmul_rn(sqrt_aprev, z0[i]), __fmul_rn(dir_coef, e0[i]));
+      const float known = __fadd_rn(__fmul_rn(ka, z0[i]), __fmul_rn(kb, e0[i]));
       nl = __fadd_rn(__fmul_rn(wi, nl), __fmul_rn(__fsub_rn(1.0f, wi), known));
     }
     lat[i] = nl;
     lat[i + count] = nl;  // the UNet input batch holds the latent twice (uncond half | cond half)
   }
+}
+template <bool BLEND>
+__global__ void cfg_ddim_kernel(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
+                                long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
+                                float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
+                                const float* __restrict__ w, int plane) {
+  cfg_step<STEP_DDIM, BLEND>(eu, ec, lat, count, scale, sqrt_1m_at, sqrt_at, sqrt_aprev, dir_coef, z0, e0, w, plane, SamplerStep{});
+}
+template <int KIND, bool BLEND>
+__global__ void cfg_sampler_kernel(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
+                                   long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
+                                   float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
+                                   const float* __restrict__ w, int plane, const SamplerStep s) {
+  cfg_step<KIND, BLEND>(eu, ec, lat, count, scale, sqrt_1m_at, sqrt_at, sqrt_aprev, dir_coef, z0, e0, w, plane, s);
+}
+void cfg_sampler_launch(int kind, const SamplerStep& s, const float* eps_u, const float* eps_c, float* latent, long long count,
+                        float scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
+                        const float* z0, const float* eps0, const float* w, int plane) {
+  SDB_CHECK(kind == STEP_DDIM_ETA || kind == STEP_DPMPP_2M, "cfg_sampler_launch: kind");
+  int grid = (int)((count + 255) / 256);
+  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
+  auto go = [&](auto kernel) {
+    launch_k(kernel, dim3(grid), dim3(256), 0, st, eps_u, eps_c, latent, count, scale, sqrt_one_minus_at, sqrt_at, sqrt_aprev,
+             dir_coef, z0, eps0, w, plane, s);
+  };
+  if (kind == STEP_DDIM_ETA)
+    w ? go(cfg_sampler_kernel<STEP_DDIM_ETA, true>) : go(cfg_sampler_kernel<STEP_DDIM_ETA, false>);
+  else
+    w ? go(cfg_sampler_kernel<STEP_DPMPP_2M, true>) : go(cfg_sampler_kernel<STEP_DPMPP_2M, false>);
+  SDB_CUDA(cudaGetLastError());
 }
 void cfg_ddim_launch(const float* eps_u, const float* eps_c, float* latent, long long count, float scale,
                      float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
@@ -1201,27 +1265,29 @@ void to_rgb8_launch(const float* img_nchw, int n, int H, int W, uint8_t* rgb, cu
 }
 
 
-__device__ __forceinline__ uint32_t mix32(uint32_t x) {
-  x ^= x >> 16;
-  x *= 0x85EBCA6Bu;
-  x ^= x >> 13;
-  x *= 0xC2B2AE35u;
-  x ^= x >> 16;
-  return x;
-}
 __global__ void randn_kernel(float* __restrict__ x, long long count, uint32_t k0, uint32_t k1) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) {
-    const uint32_t a = mix32((uint32_t)i ^ k0), b = mix32(((uint32_t)i * 0x9E3779B9u) ^ k1);
-    const float u1 = ((a >> 8) + 1) * (1.0f / 16777216.0f);  // (0,1]
-    const float u2 = (b >> 8) * (1.0f / 16777216.0f);
-    x[i] = sqrtf(-2.0f * logf(u1)) * cosf(6.283185307179586f * u2);
-  }
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x)
+    x[i] = randn_at(i, k0, k1);
 }
-void randn_launch(float* x, long long count, uint64_t seed, cudaStream_t st) {
+static void randn_keys_launch(float* x, long long count, uint32_t k0, uint32_t k1, cudaStream_t st) {
   int grid = (int)((count + 255) / 256);
   if (grid > g_num_sms * 8) grid = g_num_sms * 8;
-  randn_kernel<<<grid, 256, 0, st>>>(x, count, (uint32_t)seed * 2654435761u + 1u, (uint32_t)(seed >> 32) ^ 0x5bd1e995u);
+  randn_kernel<<<grid, 256, 0, st>>>(x, count, k0, k1);
   SDB_CUDA(cudaGetLastError());
+}
+void randn_launch(float* x, long long count, uint64_t seed, cudaStream_t st) {
+  randn_keys_launch(x, count, (uint32_t)seed * 2654435761u + 1u, (uint32_t)(seed >> 32) ^ 0x5bd1e995u, st);
+}
+// The init-latent keys of the seed, mixed with the timestep. k1 also takes k0: seeds that differ in their low word only would
+// otherwise share k1, hence the angle of every Box-Muller pair, and their streams would correlate (at pi/4).
+void step_noise_keys(uint64_t seed, int t, uint32_t* k0, uint32_t* k1) {
+  *k0 = ((uint32_t)seed * 2654435761u + 1u) ^ mix32(0x3C6EF372u + (uint32_t)t);
+  *k1 = ((uint32_t)(seed >> 32) ^ 0x5bd1e995u) ^ mix32(*k0 ^ 0xA54FF53Au);
+}
+void step_noise_launch(float* x, long long count, uint64_t seed, int t, cudaStream_t st) {
+  uint32_t k0, k1;
+  step_noise_keys(seed, t, &k0, &k1);
+  randn_keys_launch(x, count, k0, k1, st);
 }
 
 // ============================================================ weight packing

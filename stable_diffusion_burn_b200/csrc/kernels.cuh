@@ -97,6 +97,20 @@ void embed_tokens_launch(const int* tok, const float* E, const float* Pos, int n
 void cfg_ddim_launch(const float* eps_u, const float* eps_c, float* latent, long long count, float scale,
                      float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
                      const float* z0 = nullptr, const float* eps0 = nullptr, const float* w = nullptr, int plane = 0);
+// The other updates of the same fused step (DESIGN §7 f6), one launch per step like cfg_ddim_launch, which is STEP_DDIM.
+enum : int { STEP_DDIM = 0, STEP_DDIM_ETA = 1, STEP_DPMPP_2M = 2 };
+struct SamplerStep {   // per-step scalars, computed on the host in double and passed as f32
+  float* hist = nullptr;      // STEP_DPMPP_2M: x0 of the previous step [count]; read when `second`, always overwritten
+  float cx = 0.f, cd = 0.f;   // STEP_DPMPP_2M: x' = cx x + cd D
+  float c1 = 0.f, c2 = 0.f;   // STEP_DPMPP_2M, second order: D = c1 x0 - c2 x0_prev
+  int second = 0;
+  float s = 0.f;              // STEP_DDIM_ETA: x' = sqrt(a_prev) x0 + dir_coef pred + s z
+  uint32_t k0 = 0, k1 = 0;    // STEP_DDIM_ETA: key of z (step_noise_keys)
+  float ka = 0.f, kb = 0.f;   // blend: known = ka z0 + kb eps0 (sqrt(a_prev), sqrt(1 - a_prev))
+};
+void cfg_sampler_launch(int kind, const SamplerStep& s, const float* eps_u, const float* eps_c, float* latent, long long count,
+                        float scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
+                        const float* z0, const float* eps0, const float* w, int plane);
 // ---- img2img staging: u8 HWC RGB [nb][Hp][Wp][3] -> encoder input [nb][4][Hp][Wp], v / 127.5 - 1, fourth plane zero
 void u8_to_enc_input_launch(const uint8_t* rgb, int nb, int Hp, int Wp, float* out, cudaStream_t st);
 // z0 [count] *= 0.18215 in place; xb[0..count) = xb[count..2count) = sa z0 + sb eps; mask (optional, u8 [n][8H][8W]) ->
@@ -111,6 +125,10 @@ void quant_conv_slice_launch(const float* x, const float* w, const float* b, int
 void add_vec_launch(const float* a, const float* b, int n, float* y, cudaStream_t st);
 // N(0,1) latents from a Philox-like counter hash (used only when the caller passes no init latent)
 void randn_launch(float* x, long long count, uint64_t seed, cudaStream_t st);
+// Stochastic DDIM's per-step noise: the same generator keyed by (noise_seed, timestep value), element i of the call's latent
+// (numpy mirror: synth.step_noise). step_noise_launch writes the stream the fused step draws in registers.
+void step_noise_keys(uint64_t seed, int t, uint32_t* k0, uint32_t* k1);
+void step_noise_launch(float* x, long long count, uint64_t seed, int t, cudaStream_t st);
 
 // ---- row softmax for the 1-head VAE attention: P = softmax(S*scale) rows -> fp16 hi(/lo)
 void softmax_rows_launch(const float* S, long long rows, int cols, float scale, Half2Ptr out, cudaStream_t st);

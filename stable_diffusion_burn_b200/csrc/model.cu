@@ -8,6 +8,8 @@
 // Activations are NHWC fp32 (residual stream); GEMM operands are staged as fp16 hi(/lo) tensors.
 #include "model.cuh"
 
+#include "../../include/sdb200.h"
+
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -1181,6 +1183,11 @@ static void sample_loop(Ctx& c, const float* d_context, int n, int L, const floa
       m.graphs.push_back(ge);
     }
   }
+  // the sampler (DESIGN §7 f6): DDIM with eta = 0 is sample_latent's own step and keeps its kernel
+  const bool dpm = c.sampler_kind == SDB_SAMPLER_DPMPP_2M;
+  const int kind = dpm ? STEP_DPMPP_2M : (c.sampler_eta != 0.0 ? STEP_DDIM_ETA : STEP_DDIM);
+  float* hist = dpm ? (float*)c.io(kIoSamplerHist, le * 4) : nullptr;
+  double h_prev = 0.0;  // DPM++: h of the previous step this call ran (none before the first)
   for (size_t i = 0; i < ts.size(); ++i) {
     const int t = ts[i];
     // alphas are read as f32 and widened to f64 (stablediffusion/mod.rs:124-140)
@@ -1196,9 +1203,39 @@ static void sample_loop(Ctx& c, const float* d_context, int n, int L, const floa
     }
     KernelScope ks(c, KC_ELEMENTWISE);
     const bool blend = ii && ii->mask;
-    cfg_ddim_launch(eps, eps + le, xb, (long long)le, (float)scale, (float)std::sqrt(1.0 - a_t), (float)std::sqrt(a_t),
-                    (float)std::sqrt(a_prev), (float)std::sqrt(1.0 - a_prev), c.stream, blend ? ii->z0 : nullptr,
-                    blend ? ii->eps : nullptr, blend ? ii->w : nullptr, H * W);
+    double dir = std::sqrt(1.0 - a_prev);
+    SamplerStep s;
+    if (kind != STEP_DDIM) {
+      s.ka = (float)std::sqrt(a_prev), s.kb = (float)dir;
+      if (kind == STEP_DDIM_ETA) {  // Song et al. 2021 eq. 16; s = 0 on the final step (a_prev = 1)
+        const double sig = c.sampler_eta * std::sqrt((1.0 - a_prev) / (1.0 - a_t)) * std::sqrt(1.0 - a_t / a_prev);
+        dir = std::sqrt(std::max(0.0, 1.0 - a_prev - sig * sig));
+        s.s = (float)sig;
+        step_noise_keys(c.sampler_noise_seed, t, &s.k0, &s.k1);
+      } else if (t < step) {  // DPM++ final step: sigma' = 0, h = inf: first order, x' = x0
+        s.cx = 0.f, s.cd = 1.f;
+      } else {  // DPM-Solver++(2M) (Lu et al. 2022), data prediction, lambda = ln(alpha / sigma)
+        const double lam = std::log(std::sqrt(a_t) / std::sqrt(1.0 - a_t));
+        const double lam_next = std::log(std::sqrt(a_prev) / std::sqrt(1.0 - a_prev));
+        const double h = lam_next - lam;
+        s.cx = (float)(std::sqrt(1.0 - a_prev) / std::sqrt(1.0 - a_t));
+        s.cd = (float)(-std::sqrt(a_prev) * std::expm1(-h));
+        if (i > 0) {  // second order: the first step a call runs has no history
+          const double c2 = 1.0 / (2.0 * (h_prev / h));
+          s.second = 1, s.c1 = (float)(1.0 + c2), s.c2 = (float)c2;
+        }
+        h_prev = h;
+      }
+      s.hist = hist;
+    }
+    if (kind == STEP_DDIM)
+      cfg_ddim_launch(eps, eps + le, xb, (long long)le, (float)scale, (float)std::sqrt(1.0 - a_t), (float)std::sqrt(a_t),
+                      (float)std::sqrt(a_prev), (float)dir, c.stream, blend ? ii->z0 : nullptr, blend ? ii->eps : nullptr,
+                      blend ? ii->w : nullptr, H * W);
+    else
+      cfg_sampler_launch(kind, s, eps, eps + le, xb, (long long)le, (float)scale, (float)std::sqrt(1.0 - a_t),
+                         (float)std::sqrt(a_t), (float)std::sqrt(a_prev), (float)dir, c.stream, blend ? ii->z0 : nullptr,
+                         blend ? ii->eps : nullptr, blend ? ii->w : nullptr, H * W);
   }
   c.work.off = work_mark;
   if (d_latent_out) SDB_CUDA(cudaMemcpyAsync(d_latent_out, xb, le * 4, cudaMemcpyDeviceToDevice, c.stream));

@@ -115,6 +115,7 @@ struct MetaCheck {
 
 constexpr int kIoImg2ImgZ0 = 8;  // encoded image latent z0 [n,4,H,W]
 constexpr int kIoImg2ImgW = 9;   // latent mask w [n,H,W]
+constexpr int kIoSamplerHist = 10;  // DPM-Solver++(2M): x0 of the previous step [n,4,H,W]
 
 struct Ctx {
   int device = 0;
@@ -140,6 +141,10 @@ struct Ctx {
   int opt_emb_hoist = 1;    // sample_latent computes the time-embedding rows of every timestep once per call (not once per step)
   int opt_prefetch_w = 0;   // 1: weight-bound GEMMs (<= 4 M tiles) prefetch their weight strip into L2 ahead of griddepcontrol.wait.
   int opt_gn_epilogue = 1;  // GroupNorm statistics produced by the GEMM epilogue that writes the tensor (no stats pass, no rendezvous)
+  // sampler of the sampling entries (sdb_set_sampler, DESIGN §7 f6): SDB_SAMPLER_DDIM with eta, or SDB_SAMPLER_DPMPP_2M
+  int sampler_kind = 0;
+  double sampler_eta = 0.0;
+  uint64_t sampler_noise_seed = 0;
   // profiling
   bool profiling = false;
   std::vector<ProfEvent> prof;
@@ -148,11 +153,11 @@ struct Ctx {
   double cls_issued[KC_COUNT] = {0};  // tensor-core FLOPs actually issued (x passes for split-fp16 products)
   int64_t cls_launches[KC_COUNT] = {0};
   // grow-only device staging for the host-buffer entry points (no cudaMalloc/cudaFree per call: each is a device-wide sync).
-  // Slots 0..6: host-entry staging; kIoImg2Img*: buffers the img2img device entry keeps outside the work arena.
+  // Slots 0..6: host-entry staging; kIoImg2Img*, kIoSamplerHist: buffers the sampling entries keep outside the work arena.
   struct IoBuf {
     void* p = nullptr;
     size_t cap = 0;
-  } iobuf[10];
+  } iobuf[11];
   void* io(int slot, size_t bytes);
   void io_destroy();
   void* model = nullptr;  // Model* (model.cu)

@@ -13,6 +13,8 @@ Differences forced by the tier (documented in DESIGN.md): the initial latent is 
 """
 from __future__ import annotations
 
+import contextlib
+
 import numpy as np
 
 from ._lib import Context
@@ -94,25 +96,41 @@ class StableDiffusion:
         return self
 
     # ---- hot path
+    # sampler / eta / noise_seed (an extension, DESIGN.md §7 f6): "ddim" (eta in [0, 1]; eta = 0 is the reference's sampler) or
+    # "dpmpp_2m" (DPM-Solver++(2M), eta = 0). They hold for the one call; the context's default sampler is restored after it.
+    @contextlib.contextmanager
+    def _sampler(self, sampler, eta, noise_seed):
+        self.ctx.set_sampler(sampler, eta, noise_seed)
+        try:
+            yield
+        finally:
+            self.ctx.set_sampler(0, 0.0, 0)
+
     def sample_image(self, context, unconditional_context, unconditional_guidance_scale: float, n_steps: int,
-                     init_latent=None, seed: int = 0, height: int = 512, width: int = 512):
+                     init_latent=None, seed: int = 0, height: int = 512, width: int = 512, sampler: str = "ddim",
+                     eta: float = 0.0, noise_seed: int = 0):
         """-> list of n flat uint8 arrays of H*W*3 (HWC RGB), like the reference's Vec<Vec<u8>>."""
-        rgb = self.ctx.sample_image(context, unconditional_context, unconditional_guidance_scale, n_steps,
-                                    init_latent=init_latent, seed=seed, H=height // 8, W=width // 8)
+        with self._sampler(sampler, eta, noise_seed):
+            rgb = self.ctx.sample_image(context, unconditional_context, unconditional_guidance_scale, n_steps,
+                                        init_latent=init_latent, seed=seed, H=height // 8, W=width // 8)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
 
     def sample_latent(self, context, unconditional_context, unconditional_guidance_scale: float, n_steps: int,
-                      init_latent=None, seed: int = 0, height: int = 512, width: int = 512) -> np.ndarray:
-        return self.ctx.sample_latent(context, unconditional_context, unconditional_guidance_scale, n_steps,
-                                      init_latent=init_latent, seed=seed, H=height // 8, W=width // 8)
+                      init_latent=None, seed: int = 0, height: int = 512, width: int = 512, sampler: str = "ddim",
+                      eta: float = 0.0, noise_seed: int = 0) -> np.ndarray:
+        with self._sampler(sampler, eta, noise_seed):
+            return self.ctx.sample_latent(context, unconditional_context, unconditional_guidance_scale, n_steps,
+                                          init_latent=init_latent, seed=seed, H=height // 8, W=width // 8)
 
     def img2img(self, image, context, unconditional_context, unconditional_guidance_scale: float, n_steps: int,
-                strength: float, mask=None, noise=None, seed: int = 0):
+                strength: float, mask=None, noise=None, seed: int = 0, sampler: str = "ddim", eta: float = 0.0,
+                noise_seed: int = 0):
         """Image-to-image / masked inpainting (an extension: the reference has none; DESIGN.md §7 f5). image u8
         [n, height, width, 3] HWC RGB, the format sample_image returns; mask u8 [n, height, width] (255 = regenerate,
         0 = keep) or None; strength in (0, 1]. -> list of n flat uint8 arrays of height*width*3, like sample_image."""
-        rgb = self.ctx.img2img(image, context, unconditional_context, unconditional_guidance_scale, n_steps, strength,
-                               mask=mask, noise=noise, seed=seed)
+        with self._sampler(sampler, eta, noise_seed):
+            rgb = self.ctx.img2img(image, context, unconditional_context, unconditional_guidance_scale, n_steps, strength,
+                                   mask=mask, noise=noise, seed=seed)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
 
     def latent_to_image(self, latent):

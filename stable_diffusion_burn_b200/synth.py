@@ -150,6 +150,36 @@ def make_latent(n: int, h: int, w: int, seed: int = 1234) -> np.ndarray:
     return out
 
 
+def randn_stream(count: int, k0: int, k1: int) -> np.ndarray:
+    """The device's counter-hash Box-Muller N(0,1) stream (csrc/kernels.cu: randn_at), element i of `count`:
+    u1 = ((mix32(i ^ k0) >> 8) + 1) 2^-24, u2 = (mix32(i * 0x9E3779B9 ^ k1) >> 8) 2^-24, sqrt(-2 ln u1) cos(2 pi u2) in float32.
+    u1 and u2 are exact; the device's logf / cosf and numpy's differ by a few ulp."""
+    i = np.arange(count, dtype=np.uint64).astype(np.uint32)
+    with np.errstate(over="ignore"):
+        a = _mix32(i ^ np.uint32(k0))
+        b = _mix32((i * np.uint32(0x9E3779B9)) ^ np.uint32(k1))
+    u1 = ((a >> np.uint32(8)) + np.uint32(1)).astype(np.float32) * np.float32(1.0 / 16777216.0)
+    u2 = (b >> np.uint32(8)).astype(np.float32) * np.float32(1.0 / 16777216.0)
+    r = np.sqrt(np.float32(-2.0) * np.log(u1))
+    return (r * np.cos(np.float32(6.283185307179586) * u2)).astype(np.float32)
+
+
+def step_noise_keys(noise_seed: int, t: int):
+    """Key of stochastic DDIM's noise at timestep t (csrc/kernels.cu: step_noise_keys): the init-latent key of noise_seed mixed
+    with the timestep value; k1 also takes k0, so that seeds differing in their low word only do not share k1 (the angle of every
+    Box-Muller pair)."""
+    k0 = (((noise_seed & 0xFFFFFFFF) * 2654435761 + 1) & 0xFFFFFFFF) ^ _mix32_scalar(0x3C6EF372 + t)
+    k1 = (((noise_seed >> 32) & 0xFFFFFFFF) ^ 0x5BD1E995) ^ _mix32_scalar(k0 ^ 0xA54FF53A)
+    return k0, k1
+
+
+def step_noise(noise_seed: int, t: int, shape) -> np.ndarray:
+    """Stochastic DDIM's per-step noise z [shape] at timestep t, keyed by (noise_seed, t, flat element index in the call's
+    [n,4,H,W] latent): a batch member's noise depends on its position in the call. Mirror of sdb_test_step_noise."""
+    n = int(np.prod(shape))
+    return randn_stream(n, *step_noise_keys(noise_seed, t)).reshape(shape)
+
+
 def make_context(n: int, L: int, seed: int = 77) -> np.ndarray:
     """Stand-in for CLIP output [n,L,768]: N(0,1) rows normalised to zero mean / unit variance."""
     g = np.random.Generator(np.random.Philox(seed))
