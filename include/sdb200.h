@@ -246,6 +246,21 @@ int sdb_test_resblock(sdb_ctx* ctx, const float* x0, const float* x1, int n, int
  * trace as sdb_test_resblock. */
 int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n, int c0, int c1, int H, int W,
                            const float* gamma, const float* beta, int silu, int mode, float* y, int32_t* trace);
+/* One of the UNet's 16 SpatialTransformers (unet/mod.rs:461-481), index = its position in execution order (0..5 input blocks,
+ * 6 middle block, 7..15 output blocks), run on the weights sdb_finalize_weights packed, with the model's own launch sequence.
+ * Needs finalized weights. x [n][c][H][W] (c must be the block's width; H * W a multiple of 8) is staged as a ResBlock leaves it (a
+ * 3-pass identity conv: the block sees hi + lo of x, with GroupNorm partials). context [n][lmax][768] with per-sample lengths
+ * lens[n] in [1, lmax] goes through the context K/V preparation of the sampling entries (zero padded to a multiple of 32).
+ * flags: 1 = the output carries an fp16 hi + lo copy (else out16 is zero). Outputs: out, out16 [n][C][H][W]; out_norm =
+ * SiLU(GroupNorm(out; the block's own norm)) staged the way the next ResBlock stages its input; taps_y [4][n*H*W][C] = the residual
+ * stream (hi + lo) after proj_in, attn1, attn2 and the MLP; taps_ln [3][n*H*W][2] = (sum, sum of squares) per token row that
+ * norm1 / norm2 / norm3 read. trace (160 ints): [0] GroupNorm stagings, [1..4] their path (as sdb_test_resblock), [5] GEMMs, then
+ * 12 ints per GEMM: kind, N, BN, split-K, TN, TH, TW, extra-K channels, GroupNorm slots written, second-source channels, passes,
+ * epilogue roles (1 LayerNorm statistics, 2 LayerNorm-consuming, 4 GEGLU, 8 fp16-pair residual, 16 fp32 residual, 32 GroupNorm
+ * partials); [126] attention launches, then 5 ints each from [127]: dpad, Nq, Nk, split q / k (hi + lo), per-sample lengths. */
+int sdb_test_spatial_transformer(sdb_ctx* ctx, int index, const float* x, int n, int c, int H, int W, const float* context,
+                                 int lmax, const int32_t* lens, int flags, float* out, float* out16, float* out_norm, float* taps_y,
+                                 float* taps_ln, int32_t* trace);
 /* The first `count` values of stochastic DDIM's noise z at timestep t (0 <= t < 1000) for noise_seed, as the fused sampler step
  * draws them (see sdb_set_sampler). Host buffer out [count]. */
 int sdb_test_step_noise(sdb_ctx* ctx, uint64_t noise_seed, int t, int64_t count, float* out);

@@ -82,6 +82,9 @@ SIGNATURES = [
                                     C.c_int, C.c_int, _f32p, _f32p, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_groupnorm_cat", C.c_int, [_ctx, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, _f32p,
                                          C.c_int, C.c_int, _f32p, C.POINTER(C.c_int32)]),
+    ("sdb_test_spatial_transformer", C.c_int, [_ctx, C.c_int, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, C.c_int,
+                                               C.POINTER(C.c_int32), C.c_int, _f32p, _f32p, _f32p, _f32p, _f32p,
+                                               C.POINTER(C.c_int32)]),
     ("sdb_test_step_noise", C.c_int, [_ctx, C.c_uint64, C.c_int, C.c_int64, _f32p]),
     ("sdb_test_groupnorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_test_layernorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, _f32p]),
@@ -435,6 +438,37 @@ class Context:
         self.check(self.lib.sdb_test_groupnorm_cat(self.h, ptr(x0), None if x1 is None else ptr(x1), n, c0, c1, H, W, ptr(g), ptr(b),
                                                    1 if silu else 0, int(mode), ptr(y), trace.ctypes.data_as(C.POINTER(C.c_int32))))
         return y, self._decode_trace(trace)
+
+    _EPI_ROLES = ("lns", "lnc", "geglu", "res16", "res32", "gn")
+
+    def test_spatial_transformer(self, index, x, context, lens, act16=True):
+        """The UNet's SpatialTransformer number `index` (execution order, 0..15) on its finalized weights. x [n, C, H, W];
+        context [n, Lmax, 768] with per-sample lengths lens [n]. -> dict: out, out16 (its fp16 hi + lo copy, zero unless act16),
+        out_norm = SiLU(GroupNorm(out; the block's norm)), y [4, n*H*W, C] (the residual stream after proj_in, attn1, attn2, MLP),
+        ln [3, n*H*W, 2] (the row sums norm1..3 read), trace ({"gn": paths, "gemms": [...], "attn": [...]})."""
+        x = f32(x); context = f32(context)
+        n, c, H, W = x.shape
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        assert context.shape[0] == n and context.shape[2] == 768 and lens.shape == (n,)
+        out, out16, outn = (np.empty((n, c, H, W), np.float32) for _ in range(3))
+        y = np.empty((4, n * H * W, c), np.float32)
+        ln = np.empty((3, n * H * W, 2), np.float32)
+        t = np.zeros(160, np.int32)
+        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
+        self.check(self.lib.sdb_test_spatial_transformer(self.h, int(index), ptr(x), n, c, H, W, ptr(context), context.shape[1],
+                                                         i32(lens), 1 if act16 else 0, ptr(out), ptr(out16), ptr(outn), ptr(y),
+                                                         ptr(ln), i32(t)))
+        paths = {1: "fused", 2: "apply", 3: "apply+fold"}
+        keys = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1", "passes")
+        gemms = []
+        for i in range(min(int(t[5]), 10)):
+            g = dict(zip(keys, (int(v) for v in t[6 + 12 * i:17 + 12 * i])))
+            g["epi"] = {r for b, r in enumerate(self._EPI_ROLES) if int(t[17 + 12 * i]) >> b & 1}
+            gemms.append(g)
+        attn = [dict(zip(("dpad", "Nq", "Nk", "qk3", "kvlen"), (int(v) for v in t[127 + 5 * i:132 + 5 * i])))
+                for i in range(min(int(t[126]), 4))]
+        tr = {"gn": [paths.get(int(v), int(v)) for v in t[1:1 + min(int(t[0]), 4)]], "gemms": gemms, "attn": attn}
+        return dict(out=out, out16=out16, out_norm=outn, y=y, ln=ln, trace=tr)
 
     def test_groupnorm(self, x, gamma, beta, silu=False):
         x = f32(x); n, c, H, W = x.shape

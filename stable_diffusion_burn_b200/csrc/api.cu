@@ -861,6 +861,16 @@ int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n
   API_END
 }
 
+int sdb_test_spatial_transformer(sdb_ctx* ctx, int index, const float* x, int n, int ch, int H, int W, const float* context,
+                                 int lmax, const int32_t* lens, int flags, float* out, float* out16, float* out_norm, float* taps_y,
+                                 float* taps_ln, int32_t* trace) {
+  API_BEGIN(ctx)
+  need_final(c);
+  c.work.reset();
+  model_test_spatial_transformer(c, index, x, n, ch, H, W, context, lmax, lens, flags, out, out16, out_norm, taps_y, taps_ln, trace);
+  API_END
+}
+
 int sdb_test_step_noise(sdb_ctx* ctx, uint64_t noise_seed, int t, int64_t count, float* out) {
   API_BEGIN(ctx)
   SDB_CHECK(out && count >= 1, "step_noise: null output or count < 1");

@@ -464,12 +464,20 @@ struct CtxState {
   std::vector<CtxKV> kv; // one per SpatialTransformer in execution order
 };
 
+// device copies of the block's intermediate state (sdb_test_spatial_transformer), taken in stream order before the next stage
+// rewrites it: y [Mt][C] as hi + lo after proj_in, attn1, attn2 and the MLP, and the LayerNorm row statistics [Mt][ln_slots(C)][2]
+// that norm1 / norm2 / norm3 read
+struct StTaps {
+  Half2Ptr y[4];
+  float* ln[3];
+};
+
 // reference unet/mod.rs:461-481 + 521-527 + 641-653 + 551-592
 // The block's residual stream y lives as an fp16 hi + lo pair (22 significant bits; no fp32 copy): every GEMM that reads it as
 // an operand takes the pair as it is, every GEMM that adds to it reads and rewrites the pair in place. The three LayerNorms have
 // no launch (see pack_st): the producers of y leave row statistics, the consumers normalise in their epilogue.
 static void run_spatial_transformer(Fwd& f, SpatialTransformerW& s, const CtxState& cs, const CtxKV& kv, const Act& x,
-                                    Act& out) {
+                                    Act& out, const StTaps* taps = nullptr) {
   Ctx& c = f.c;
   const size_t mark = c.work.off;
   const int P = s.passes;
@@ -484,11 +492,19 @@ static void run_spatial_transformer(Fwd& f, SpatialTransformerW& s, const CtxSta
   float* st1 = c.work.get<float>((size_t)Mt * ls * 2);
   float* st2 = c.work.get<float>((size_t)Mt * ls * 2);
   float* st3 = c.work.get<float>((size_t)Mt * ls * 2);
+  // taps: y after stage i and the LayerNorm statistics it left (none after the MLP)
+  auto tap = [&](int i, const float* st) {
+    if (!taps) return;
+    SDB_CUDA(cudaMemcpyAsync(taps->y[i].hi, y16.hi, (size_t)Mt * C * 2, cudaMemcpyDeviceToDevice, c.stream));
+    SDB_CUDA(cudaMemcpyAsync(taps->y[i].lo, y16.lo, (size_t)Mt * C * 2, cudaMemcpyDeviceToDevice, c.stream));
+    if (st) SDB_CUDA(cudaMemcpyAsync(taps->ln[i], st, (size_t)Mt * ls * 2 * 4, cudaMemcpyDeviceToDevice, c.stream));
+  };
   {
     Epilogue ep;
     ep.out_f16 = y16, ep.bias = s.proj_in.bias, ep.ln_out = st1;
     run_gemm(c, G_CONV1, a, nullptr, s.proj_in.packed, P, ep);
   }
+  tap(0, st1);
   Half2Ptr o16 = f.half2((size_t)Mt * C, lo);
   auto ln_consume = [&](Epilogue& ep, const float* stats, const NormW& nw, const float* u_hi, const float* u_full, const float* v) {
     ep.ln_in = stats, ep.ln_in_slots = ls, ep.ln_C = C, ep.ln_eps = nw.eps, ep.ln_u_hi = u_hi, ep.ln_u_full = u_full, ep.bias = v;
@@ -520,6 +536,7 @@ static void run_spatial_transformer(Fwd& f, SpatialTransformerW& s, const CtxSta
     ep.out_f16 = y16, ep.residual16 = y16, ep.bias = s.attn1.out.bias, ep.ln_out = st2;
     run_gemm(c, G_LINEAR, f.rows_operand(o16, Mt, C), nullptr, s.w_o1, P, ep);
   }
+  tap(1, st2);
   // ---- cross attention: x += out(attn(q = LN2(x), k,v = context))
   __half* q2 = c.work.get<__half>((size_t)Mt * hd);
   __half* q2_lo = qk_split ? c.work.get<__half>((size_t)Mt * hd) : nullptr;
@@ -545,6 +562,7 @@ static void run_spatial_transformer(Fwd& f, SpatialTransformerW& s, const CtxSta
     ep.out_f16 = y16, ep.residual16 = y16, ep.bias = s.attn2.out.bias, ep.ln_out = st3;
     run_gemm(c, G_LINEAR, f.rows_operand(o16, Mt, C), nullptr, s.w_o2, P, ep);
   }
+  tap(2, st3);
   // ---- GEGLU MLP: x += lin(x_a * gelu(gate)), LN3 folded into the GEGLU projection
   const int Pm = c.opt_mlp_passes ? c.opt_mlp_passes : P;  // pass policy of the MLP pair (DESIGN.md "precision")
   Half2Ptr g16 = f.half2((size_t)Mt * 4 * C, Pm >= 2 || c.opt_precision >= 2);
@@ -559,6 +577,7 @@ static void run_spatial_transformer(Fwd& f, SpatialTransformerW& s, const CtxSta
     ep.out_f16 = y16, ep.residual16 = y16, ep.bias = s.ff.bias;
     run_gemm(c, G_LINEAR, f.rows_operand(g16, Mt, 4 * C), nullptr, s.ff.packed, Pm, ep);
   }
+  tap(3, nullptr);
   // ---- proj_out + residual with the block input
   {
     Epilogue ep;
@@ -1613,7 +1632,7 @@ void model_test_attention(Ctx& c, const float* q, const float* k, const float* v
 namespace {
 struct TraceScope {  // records the GEMM choices and GroupNorm paths of everything queued while it lives
   Ctx& c;
-  explicit TraceScope(Ctx& c_) : c(c_) { c.gemm_trace.clear(), c.gn_trace.clear(), c.trace_on = true; }
+  explicit TraceScope(Ctx& c_) : c(c_) { c.gemm_trace.clear(), c.attn_trace.clear(), c.gn_trace.clear(), c.trace_on = true; }
   ~TraceScope() { c.trace_on = false; }
 };
 }  // namespace
@@ -1664,7 +1683,16 @@ static Act stage_activation(Fwd& f, const float* h, int C, int H, int W, bool st
   pack_conv_launch(id, C, C, 3, wid.p, c.stream);
   Epilogue ep;
   ep.out_f32 = a.p, ep.out_f16 = a.raw16, ep.gn = &a.gn;
-  run_gemm(c, G_CONV3, A, nullptr, wid, 3, ep);
+  // 3 passes whatever the precision option forces on the block under test: the staging must hand on hi + lo of the input
+  const int prec = c.opt_precision;
+  c.opt_precision = 0;
+  try {
+    run_gemm(c, G_CONV3, A, nullptr, wid, 3, ep);
+  } catch (...) {
+    c.opt_precision = prec;
+    throw;
+  }
+  c.opt_precision = prec;
   return a;
 }
 
@@ -1761,6 +1789,84 @@ void model_test_groupnorm_cat(Ctx& c, const float* x0, const float* x1, int n, i
   }
   write_trace(c, trace);
   fetch_half2(c, g.p, n, C, H, W, y);
+}
+
+// ================================================================================ SpatialTransformer unit-test entry
+void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, int Cx, int H, int W, const float* context, int Lmax,
+                                    const int32_t* lens, int flags, float* out, float* out16, float* out_norm, float* taps_y,
+                                    float* taps_ln, int32_t* trace) {
+  Model& m = M(c);
+  SDB_CHECK(index >= 0 && index < (int)m.sts.size(), "test_spatial_transformer: index is the execution-order position 0..15");
+  SDB_CHECK(n >= 1 && H >= 1 && W >= 1 && Lmax >= 1 && x && context && lens, "test_spatial_transformer: arguments");
+  SDB_CHECK((H * W) % 8 == 0, "unsupported latent size: H*W must be a multiple of 8");  // the UNet's (H/8)*(W/8) rule
+  SDB_CHECK((flags & ~1) == 0, "test_spatial_transformer: flags are 1 (the output carries an fp16 hi + lo copy)");
+  for (int s = 0; s < n; ++s) SDB_CHECK(lens[s] >= 1 && lens[s] <= Lmax, "test_spatial_transformer: lengths must lie in [1, Lmax]");
+  SpatialTransformerW& st = *m.sts[index];
+  SDB_CHECK(Cx == st.c, "test_spatial_transformer: x must have the block's channel count (" + std::to_string(st.c) + ")");
+  const int C = st.c, HW = H * W, ls = ln_slots(C);
+  const long long Mt = (long long)n * HW;
+  Fwd f(c, n);
+  f.init_sums(4);
+  // context [n][Lpad][768], zero padded, per-sample lengths: as model_unet_forward_dev / the sampling entries stage it
+  const int Lpad = round_up(Lmax, 32);
+  float* ctxp = c.work.get<float>((size_t)n * Lpad * 768);
+  int* d_len = c.work.get<int>(n);
+  SDB_CUDA(cudaMemsetAsync(ctxp, 0, (size_t)n * Lpad * 768 * 4, c.stream));
+  SDB_CUDA(cudaMemcpy2DAsync(ctxp, (size_t)Lpad * 768 * 4, context, (size_t)Lmax * 768 * 4, (size_t)Lmax * 768 * 4, n,
+                             cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(d_len, lens, 4 * n, cudaMemcpyHostToDevice, c.stream));
+  CtxState cs;
+  prepare_context(f, ctxp, Lpad, d_len, cs);
+  const Act a = stage_activation(f, x, C, H, W, true);
+  Act o = (flags & 1) ? f.act16(H, W, C) : f.act(H, W, C);
+  StTaps taps;
+  for (Half2Ptr& y : taps.y) y = f.half2((size_t)Mt * C, true);
+  for (float*& l : taps.ln) l = c.work.get<float>((size_t)Mt * ls * 2);
+  ActOp g;
+  {
+    TraceScope ts(c);
+    run_spatial_transformer(f, st, cs, cs.kv[index], a, o, &taps);
+    g = f.gn_operand(o, nullptr, st.norm, true, true);  // a consumer of the output, as the next ResBlock's norm_in stages it
+    std::fill(trace, trace + kStTraceInts, 0);
+    trace[0] = (int)c.gn_trace.size();
+    for (size_t i = 0; i < c.gn_trace.size() && i < 4; ++i) trace[1 + i] = c.gn_trace[i];
+    trace[5] = (int)c.gemm_trace.size();
+    for (size_t i = 0; i < c.gemm_trace.size() && i < 10; ++i) {
+      const Ctx::GemmRecord& r = c.gemm_trace[i];
+      const int v[12] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels, r.passes, r.epi};
+      std::copy(v, v + 12, trace + 6 + 12 * i);
+    }
+    trace[126] = (int)c.attn_trace.size();
+    for (size_t i = 0; i < c.attn_trace.size() && i < 4; ++i) {
+      const Ctx::AttnRecord& r = c.attn_trace[i];
+      const int v[5] = {r.dpad, r.Nq, r.Nk, r.qk3, r.kvlen};
+      std::copy(v, v + 5, trace + 127 + 5 * i);
+    }
+  }
+  float* d = c.work.get<float>(o.count());
+  nhwc_to_nchw_launch(o.p, n, C, H, W, d, c.stream);
+  SDB_CUDA(cudaMemcpyAsync(out, d, o.count() * 4, cudaMemcpyDeviceToHost, c.stream));
+  fetch_half2(c, o.raw16, n, C, H, W, out16);
+  fetch_half2(c, g.p, n, C, H, W, out_norm);
+  // taps: y as [Mt][C] hi + lo, the statistics folded over their slots in index order (as the consuming epilogue adds them)
+  const size_t cnt = (size_t)Mt * C;
+  std::vector<__half> hi(cnt), lo(cnt);
+  for (int i = 0; i < 4; ++i) {
+    SDB_CUDA(cudaMemcpyAsync(hi.data(), taps.y[i].hi, cnt * 2, cudaMemcpyDeviceToHost, c.stream));
+    SDB_CUDA(cudaMemcpyAsync(lo.data(), taps.y[i].lo, cnt * 2, cudaMemcpyDeviceToHost, c.stream));
+    SDB_CUDA(cudaStreamSynchronize(c.stream));
+    for (size_t e = 0; e < cnt; ++e) taps_y[i * cnt + e] = __half2float(hi[e]) + __half2float(lo[e]);
+  }
+  std::vector<float> sl((size_t)Mt * ls * 2);
+  for (int i = 0; i < 3; ++i) {
+    SDB_CUDA(cudaMemcpyAsync(sl.data(), taps.ln[i], sl.size() * 4, cudaMemcpyDeviceToHost, c.stream));
+    SDB_CUDA(cudaStreamSynchronize(c.stream));
+    for (long long r = 0; r < Mt; ++r) {
+      float sm = 0.f, sq = 0.f;
+      for (int k = 0; k < ls; ++k) sm += sl[(r * ls + k) * 2], sq += sl[(r * ls + k) * 2 + 1];
+      taps_ln[(i * Mt + r) * 2] = sm, taps_ln[(i * Mt + r) * 2 + 1] = sq;
+    }
+  }
 }
 
 }  // namespace sdb

@@ -50,5 +50,10 @@ void model_test_resblock(Ctx& c, const float* x0, const float* x1, int n, int C0
                          int flags, float* out, float* out16, float* outn, int32_t* trace);
 void model_test_groupnorm_cat(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, const float* gamma,
                               const float* beta, int silu, int mode, float* y, int32_t* trace);
+// SpatialTransformer test entry (sdb200.h: sdb_test_spatial_transformer); trace = kStTraceInts ints
+constexpr int kStTraceInts = 160;
+void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, int C, int H, int W, const float* context, int Lmax,
+                                    const int32_t* lens, int flags, float* out, float* out16, float* out_norm, float* taps_y,
+                                    float* taps_ln, int32_t* trace);
 
 }  // namespace sdb

@@ -218,6 +218,7 @@ void run_attention(Ctx& c, const AttnOp& a) {
     memset(dbg_buf, 0, 256 * sizeof(long long));
     p.dbg = dbg_buf;
   }
+  if (c.trace_on) c.attn_trace.push_back({a.dpad, a.Nq, a.Nk, p.qk3, a.kvlen ? 1 : 0});
   {
     KernelScope ks(c, KC_ATTN, flops, 0);
     attention_launch(am, p, c.stream);
@@ -397,8 +398,11 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
     gn->slots = ok ? slots : 0;
     if (!ok) gn = nullptr;
   }
-  if (c.trace_on)
-    c.gemm_trace.push_back({kind_in, w.N, BN, split, p.TN, p.TH, p.TW, p.xkc * 64, gn ? gn->slots : 0, a1in ? a1.C : 0});
+  if (c.trace_on) {
+    const int epi = (ep.ln_out ? EPI_ROLE_LNS : 0) | (ep.ln_in ? EPI_ROLE_LNC : 0) | (ep.geglu ? EPI_ROLE_GEGLU : 0) |
+                    (ep.residual16.hi ? EPI_ROLE_RES16 : 0) | (ep.residual ? EPI_ROLE_RES32 : 0) | (gn ? EPI_ROLE_GN : 0);
+    c.gemm_trace.push_back({kind_in, w.N, BN, split, p.TN, p.TH, p.TW, p.xkc * 64, gn ? gn->slots : 0, a1in ? a1.C : 0, passes, epi});
+  }
   p.gn_part = gn ? gn->buf : nullptr;
   p.gn_cap = gn ? gn->cap : 0, p.gn_bucket = gn ? gn->bucket : 1;
   p.gn_rpi = gn ? gn_rpi : 0, p.gn_nimg = gn_nimg;

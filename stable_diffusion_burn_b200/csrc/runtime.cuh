@@ -39,6 +39,9 @@ struct TensorInfo {
 // which GroupNorm kernel staged an operand: statistics and apply in one launch, apply from producer partials, or apply after
 // the 64:1 pre-fold of more than 128 partial slots
 enum GnPath : int { GN_PATH_FUSED = 1, GN_PATH_APPLY = 2, GN_PATH_APPLY_FOLD = 3 };
+// epilogue roles of a recorded GEMM (Ctx::GemmRecord::epi): LayerNorm statistics out, LayerNorm-consuming correction, GEGLU,
+// fp16-pair residual, fp32 residual, GroupNorm partials out
+enum EpiRole : int { EPI_ROLE_LNS = 1, EPI_ROLE_LNC = 2, EPI_ROLE_GEGLU = 4, EPI_ROLE_RES16 = 8, EPI_ROLE_RES32 = 16, EPI_ROLE_GN = 32 };
 
 enum KernelClass : int {
   KC_GEMM = 0,
@@ -165,13 +168,18 @@ struct Ctx {
   // SDB_DEBUG_SYNC=1: synchronise after every launch and report the failing op (bring-up aid)
   bool debug_sync = false;
   std::string dbg_label;
-  // launch record for the test entries (sdb_test_resblock): what run_gemm chose per GEMM and which GroupNorm path
-  // Fwd::gn_operand took, so a test can assert it reached the path it is meant to cover
+  // launch record for the test entries (sdb_test_resblock, sdb_test_spatial_transformer): what run_gemm chose per GEMM, what
+  // run_attention launched and which GroupNorm path Fwd::gn_operand took, so a test can assert it reached the path it is meant
+  // to cover. epi: EPI_ROLE_* bits of the epilogue (gn only when the statistics were really written)
   struct GemmRecord {
-    int kind, N, BN, split, TN, TH, TW, xk_channels, gn_slots, a1_channels;
+    int kind, N, BN, split, TN, TH, TW, xk_channels, gn_slots, a1_channels, passes, epi;
+  };
+  struct AttnRecord {
+    int dpad, Nq, Nk, qk3, kvlen;
   };
   bool trace_on = false;
   std::vector<GemmRecord> gemm_trace;
+  std::vector<AttnRecord> attn_trace;
   std::vector<int> gn_trace;  // GN_PATH_*
 
   float* master_ptr(const std::string& name);
