@@ -148,13 +148,50 @@ int sdb_img2img_dev(sdb_ctx* ctx, const uint8_t* d_image, const uint8_t* d_mask,
  * SDB_SAMPLER_DDIM with eta in [0, 1] (finite): DDIM (Song et al. 2021, eq. 16), s = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a'),
  *   x' = sqrt(a') x0 + sqrt(1 - a' - s^2) eps + s z. eta = 0 (the default) is the reference's sampler, unchanged to the bit.
  *   z is N(0,1) keyed by (noise_seed, timestep value, element index in the call's [n,4,H,W] latent): a batch member's noise
- *   depends on its position in the call.
+ *   depends on its position in the call (the sdb_*_batch entries key it per sample instead).
  * SDB_SAMPLER_DPMPP_2M (eta must be 0): DPM-Solver++(2M) (Lu et al. 2022), data prediction, second order from the second step
  *   a call runs; the final step returns x0. A context starts with (SDB_SAMPLER_DDIM, 0.0, 0). Invalid arguments are an error
  *   and leave the setting unchanged. */
 #define SDB_SAMPLER_DDIM 0
 #define SDB_SAMPLER_DPMPP_2M 1
 int sdb_set_sampler(sdb_ctx* ctx, int kind, double eta, uint64_t noise_seed);
+
+/* ---- batches of different requests (DESIGN.md §7 f7) --------------------------------------------------------------------- */
+/* One call samples n requests that differ in prompt length, negative prompt, guidance scale and seed, as one batch-2n UNet pass
+ * per step (the weights stream from HBM once per step for all of them). Sample i gives what request i gives as a call of its
+ * own at n = 1: its own context_len[i] prompt rows and uncond_len[i] negative rows (rows past a length are never read, so the
+ * caller's pad rows may hold anything), its own scale (cast to float), the init latent / img2img noise sdb_sample_image draws
+ * for seed[i] at n = 1, and stochastic-DDIM noise keyed by (noise_seed[i], timestep, element index within the sample). It
+ * matches that single call to rounding: split-K choices of the UNet's GEMMs depend on the batch size. The sampler
+ * (sdb_set_sampler), n_steps, strength, H and W hold for the whole call. The context is padded to the longest length any
+ * sample reads, rounded up to 32, whatever the strides L and Lu: a generous stride costs nothing.
+ * Errors (the field, the sample index and the value are named; nothing is changed): n < 1, L or Lu < 1, a length outside
+ * [1, stride], a non-finite scale, a NULL context / uncond / guidance_scale, a NULL seed when no init latent / noise is given. */
+typedef struct sdb_batch {
+  int n;
+  int L;                           /* row stride of context */
+  const float* context;            /* [n][L][768] */
+  const int32_t* context_len;      /* [n]: sample i reads rows [0, context_len[i]); NULL = L for every sample */
+  int Lu;                          /* row stride of uncond */
+  const float* uncond;             /* [n][Lu][768]: one negative / unconditional context per sample */
+  const int32_t* uncond_len;       /* [n]; NULL = Lu for every sample */
+  const double* guidance_scale;    /* [n], finite */
+  const uint64_t* seed;            /* [n]: init latent (txt2img) / noise (img2img) of sample i; unused with an explicit one */
+  const uint64_t* noise_seed;      /* [n]: stochastic-DDIM step noise of sample i; NULL = the sdb_set_sampler noise_seed */
+} sdb_batch;
+/* sdb_sample_latent / sdb_sample_image over a batch. init_latent [n,4,H,W] or NULL (= from the seeds). latent_out [n,4,H,W]
+ * and / or rgb_out [n,8H,8W,3]; at least one must be set. */
+int sdb_sample_batch(sdb_ctx* ctx, const sdb_batch* batch, int n_steps, const float* init_latent, int H, int W,
+                     float* latent_out, uint8_t* rgb_out);
+/* sdb_img2img over a batch: image u8 [n,8H,8W,3], mask u8 [n,8H,8W] or NULL, noise [n,4,H,W] or NULL (= from the seeds). */
+int sdb_img2img_batch(sdb_ctx* ctx, const sdb_batch* batch, const uint8_t* image, const uint8_t* mask, double strength,
+                      int n_steps, const float* noise, int H, int W, float* latent_out, uint8_t* rgb_out);
+/* device-pointer variants: context, uncond, image, mask, init latent / noise and the outputs are device buffers; the lengths,
+ * scales and seeds stay host arrays. Asynchronous on `stream`. */
+int sdb_sample_batch_dev(sdb_ctx* ctx, const sdb_batch* batch, int n_steps, const float* d_init_latent, int H, int W,
+                         float* d_latent_out, uint8_t* d_rgb_out, void* stream);
+int sdb_img2img_batch_dev(sdb_ctx* ctx, const sdb_batch* batch, const uint8_t* d_image, const uint8_t* d_mask, double strength,
+                          int n_steps, const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb_out, void* stream);
 
 /* ---- hot path, device buffers (zero-copy callers) ------------------------------------------ */
 int sdb_unet_forward_dev(sdb_ctx* ctx, const float* d_x, int32_t timestep, const float* d_context,

@@ -22,6 +22,21 @@ pub struct SdbCtx {
     _private: [u8; 0],
 }
 
+/// include/sdb200.h: sdb_batch — n different requests of one sampling call (DESIGN.md §7 f7).
+#[repr(C)]
+pub struct SdbBatch {
+    pub n: c_int,
+    pub l: c_int,
+    pub context: *const f32,
+    pub context_len: *const i32,
+    pub lu: c_int,
+    pub uncond: *const f32,
+    pub uncond_len: *const i32,
+    pub guidance_scale: *const f64,
+    pub seed: *const u64,
+    pub noise_seed: *const u64,
+}
+
 extern "C" {
     fn sdb_create(device: c_int, out: *mut *mut SdbCtx) -> c_int;
     fn sdb_destroy(ctx: *mut SdbCtx) -> c_int;
@@ -53,6 +68,10 @@ extern "C" {
                        d_noise: *const c_void, h: c_int, w: c_int, d_latent_out: *mut c_void, d_rgb_out: *mut c_void,
                        stream: *mut c_void) -> c_int;
     fn sdb_set_sampler(ctx: *mut SdbCtx, kind: c_int, eta: f64, noise_seed: u64) -> c_int;
+    fn sdb_sample_batch(ctx: *mut SdbCtx, batch: *const SdbBatch, n_steps: c_int, init_latent: *const f32, h: c_int, w: c_int,
+                        latent_out: *mut f32, rgb_out: *mut u8) -> c_int;
+    fn sdb_img2img_batch(ctx: *mut SdbCtx, batch: *const SdbBatch, image: *const u8, mask: *const u8, strength: f64, n_steps: c_int,
+                         noise: *const f32, h: c_int, w: c_int, latent_out: *mut f32, rgb_out: *mut u8) -> c_int;
     fn sdb_nccl_unique_id(id128: *mut c_void) -> c_int;
     fn sdb_broadcast_weights(ctx: *mut SdbCtx, id128: *const c_void, rank: c_int, world: c_int) -> c_int;
     #[allow(dead_code)]
@@ -234,6 +253,44 @@ impl StableDiffusion {
         self.check(unsafe { sdb_set_sampler(self.ctx, kind, eta, noise_seed) })
     }
 
+    /// n different requests in one call (an extension, DESIGN.md §7 f7): request i is (`contexts[i]` = L_i x 768 floats,
+    /// `unconditional_contexts[i]` = Lu_i x 768, `guidance_scales[i]`, `seeds[i]`) and gives, to rounding, what `sample_image`
+    /// gives for it alone, while every step runs one UNet pass for all of them. `noise_seeds` keys stochastic DDIM per request
+    /// (None = the `set_sampler` seed). The sampler and `n_steps` hold for the whole call. 512 x 512 like `sample_image`.
+    pub fn sample_batch(&self, contexts: &[&[f32]], unconditional_contexts: &[&[f32]], guidance_scales: &[f64], n_steps: usize,
+                        seeds: &[u64], noise_seeds: Option<&[u64]>) -> Result<Vec<Vec<u8>>, SdbError> {
+        let (h, w) = (64usize, 64usize);
+        let packed = Packed::new(contexts, unconditional_contexts, guidance_scales, Some(seeds), noise_seeds)?;
+        let mut rgb = vec![0u8; packed.n * 8 * h * 8 * w * 3];
+        self.check(unsafe {
+            sdb_sample_batch(self.ctx, &packed.batch(), n_steps as c_int, std::ptr::null(), h as c_int, w as c_int,
+                             std::ptr::null_mut(), rgb.as_mut_ptr())
+        })?;
+        Ok(rgb.chunks(8 * h * 8 * w * 3).map(|c| c.to_vec()).collect())
+    }
+
+    /// `img2img` over n different requests (arguments as `sample_batch`; `image`, `mask` as `img2img`). `noise = None` draws each
+    /// request's noise from its seed.
+    #[allow(clippy::too_many_arguments)]
+    pub fn img2img_batch(&self, image: &[u8], [height, width]: [usize; 2], mask: Option<&[u8]>, strength: f64, contexts: &[&[f32]],
+                         unconditional_contexts: &[&[f32]], guidance_scales: &[f64], n_steps: usize, noise: Option<&[f32]>,
+                         seeds: Option<&[u64]>, noise_seeds: Option<&[u64]>) -> Result<Vec<Vec<u8>>, SdbError> {
+        let (h, w) = (height / 8, width / 8);
+        let packed = Packed::new(contexts, unconditional_contexts, guidance_scales, seeds, noise_seeds)?;
+        let n = packed.n;
+        if image.len() != n * height * width * 3 || mask.map_or(false, |m| m.len() != n * height * width)
+            || noise.map_or(false, |z| z.len() != n * 4 * h * w) {
+            return Err(SdbError("img2img_batch: buffer sizes do not match [n, height, width]".into()));
+        }
+        let mut rgb = vec![0u8; n * height * width * 3];
+        self.check(unsafe {
+            sdb_img2img_batch(self.ctx, &packed.batch(), image.as_ptr(), mask.map_or(std::ptr::null(), |m| m.as_ptr()), strength,
+                              n_steps as c_int, noise.map_or(std::ptr::null(), |z| z.as_ptr()), h as c_int, w as c_int,
+                              std::ptr::null_mut(), rgb.as_mut_ptr())
+        })?;
+        Ok(rgb.chunks(height * width * 3).map(|c| c.to_vec()).collect())
+    }
+
     /// Multi-GPU init: rank 0 calls `nccl_unique_id()` and ships the 128 bytes to the other ranks by any means; every rank then
     /// calls `broadcast_weights(&id, rank, world)` (one ncclBroadcast of the weight arena from rank 0) and `finalize_weights()`.
     pub fn nccl_unique_id() -> Result<[u8; 128], SdbError> {
@@ -245,6 +302,55 @@ impl StableDiffusion {
     }
     pub fn broadcast_weights(&self, id: &[u8; 128], rank: usize, world: usize) -> Result<(), SdbError> {
         self.check(unsafe { sdb_broadcast_weights(self.ctx, id.as_ptr() as *const c_void, rank as c_int, world as c_int) })
+    }
+}
+
+/// The requests of a batch call padded to the longest prompt / negative (rows past a request's length are zero and never read).
+struct Packed {
+    n: usize,
+    l: usize,
+    lu: usize,
+    context: Vec<f32>,
+    context_len: Vec<i32>,
+    uncond: Vec<f32>,
+    uncond_len: Vec<i32>,
+    scales: Vec<f64>,
+    seeds: Option<Vec<u64>>,
+    noise_seeds: Option<Vec<u64>>,
+}
+
+impl Packed {
+    fn new(contexts: &[&[f32]], uncond: &[&[f32]], scales: &[f64], seeds: Option<&[u64]>, noise_seeds: Option<&[u64]>)
+           -> Result<Self, SdbError> {
+        let n = contexts.len();
+        if n == 0 || uncond.len() != n || scales.len() != n || seeds.map_or(false, |s| s.len() != n)
+            || noise_seeds.map_or(false, |s| s.len() != n) {
+            return Err(SdbError("batch: every per-request list must hold the same number (>= 1) of requests".into()));
+        }
+        if contexts.iter().chain(uncond.iter()).any(|c| c.is_empty() || c.len() % 768 != 0) {
+            return Err(SdbError("batch: every context must be a non-empty multiple of 768 floats".into()));
+        }
+        let pad = |rows: &[&[f32]]| {
+            let lmax = rows.iter().map(|c| c.len() / 768).max().unwrap_or(1);
+            let mut out = vec![0f32; n * lmax * 768];
+            for (i, c) in rows.iter().enumerate() {
+                out[i * lmax * 768..i * lmax * 768 + c.len()].copy_from_slice(c);
+            }
+            (lmax, out, rows.iter().map(|c| (c.len() / 768) as i32).collect::<Vec<_>>())
+        };
+        let (l, context, context_len) = pad(contexts);
+        let (lu, uncond, uncond_len) = pad(uncond);
+        Ok(Self { n, l, lu, context, context_len, uncond, uncond_len, scales: scales.to_vec(), seeds: seeds.map(|s| s.to_vec()),
+                  noise_seeds: noise_seeds.map(|s| s.to_vec()) })
+    }
+
+    fn batch(&self) -> SdbBatch {
+        SdbBatch {
+            n: self.n as c_int, l: self.l as c_int, context: self.context.as_ptr(), context_len: self.context_len.as_ptr(),
+            lu: self.lu as c_int, uncond: self.uncond.as_ptr(), uncond_len: self.uncond_len.as_ptr(),
+            guidance_scale: self.scales.as_ptr(), seed: self.seeds.as_ref().map_or(std::ptr::null(), |s| s.as_ptr()),
+            noise_seed: self.noise_seeds.as_ref().map_or(std::ptr::null(), |s| s.as_ptr()),
+        }
     }
 }
 

@@ -18,6 +18,17 @@ _u8p = C.POINTER(C.c_uint8)
 _i64p = C.POINTER(C.c_int64)
 _ctx = C.c_void_p
 
+
+class SdbBatch(C.Structure):
+    """include/sdb200.h: sdb_batch (DESIGN.md §7 f7)."""
+    _fields_ = [("n", C.c_int), ("L", C.c_int), ("context", C.c_void_p), ("context_len", C.POINTER(C.c_int32)),
+                ("Lu", C.c_int), ("uncond", C.c_void_p), ("uncond_len", C.POINTER(C.c_int32)),
+                ("guidance_scale", C.POINTER(C.c_double)), ("seed", C.POINTER(C.c_uint64)),
+                ("noise_seed", C.POINTER(C.c_uint64))]
+
+
+_batchp = C.POINTER(SdbBatch)
+
 # (name, restype, argtypes) — every symbol declared in include/sdb200.h
 SIGNATURES = [
     ("sdb_create", C.c_int, [C.c_int, C.POINTER(_ctx)]),
@@ -62,6 +73,12 @@ SIGNATURES = [
     ("sdb_img2img_dev", C.c_int, [_ctx, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                   C.c_double, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("sdb_set_sampler", C.c_int, [_ctx, C.c_int, C.c_double, C.c_uint64]),
+    ("sdb_sample_batch", C.c_int, [_ctx, _batchp, C.c_int, _f32p, C.c_int, C.c_int, _f32p, _u8p]),
+    ("sdb_sample_batch_dev", C.c_int, [_ctx, _batchp, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]),
+    ("sdb_img2img_batch", C.c_int, [_ctx, _batchp, _u8p, _u8p, C.c_double, C.c_int, _f32p, C.c_int, C.c_int, _f32p, _u8p]),
+    ("sdb_img2img_batch_dev", C.c_int, [_ctx, _batchp, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_int,
+                                        C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("sdb_set_option", C.c_int, [_ctx, C.c_char_p, C.c_int]),
     ("sdb_profile_enable", C.c_int, [_ctx, C.c_int]),
     ("sdb_profile_reset", C.c_int, [_ctx]),
@@ -121,6 +138,65 @@ def ptr(a: np.ndarray):
 
 class SdbError(RuntimeError):
     pass
+
+
+def _rows(a, what):
+    a = f32(a)
+    if a.ndim == 3 and a.shape[0] == 1:
+        a = a[0]
+    if a.ndim != 2 or a.shape[1] != 768 or a.shape[0] < 1:
+        raise ValueError(f"{what} must be [L, 768] or [1, L, 768] with L >= 1, got {a.shape}")
+    return a
+
+
+def pack_batch(contexts, unconds, scales, seeds=None, noise_seeds=None):
+    """The arrays of an sdb_batch (DESIGN.md §7 f7) from n requests. contexts: list of [L_i, 768] or [1, L_i, 768]; unconds: one
+    [Lu, 768] (or [1, Lu, 768]) array shared by every request, or a list of n; scales: a number or a list of n; seeds,
+    noise_seeds: lists of n or None. -> dict of context [n, Lmax, 768] and uncond [n, Lumax, 768] (rows past a request's length
+    zero), context_len / uncond_len int32 [n], scale float64 [n], seed / noise_seed uint64 [n] or None."""
+    if isinstance(contexts, np.ndarray) or not len(contexts):
+        raise ValueError("contexts must be a non-empty list of [L, 768] arrays")
+    ctx = [_rows(a, f"contexts[{i}]") for i, a in enumerate(contexts)]
+    n = len(ctx)
+    if isinstance(unconds, np.ndarray):
+        unc = [_rows(unconds, "uncond")] * n
+    else:
+        unc = [_rows(a, f"unconds[{i}]") for i, a in enumerate(unconds)]
+        if len(unc) != n:
+            raise ValueError(f"{len(unc)} unconditional contexts for {n} requests")
+
+    def per_request(v, what, dtype):
+        if v is None:
+            return None
+        a = np.array([v] * n if np.ndim(v) == 0 else v, dtype)
+        if a.shape != (n,):
+            raise ValueError(f"{what} must be one value or a list of {n}, got shape {a.shape}")
+        return a
+
+    scale = per_request(scales, "scales", np.float64)
+    if scale is None or not np.isfinite(scale).all():
+        raise ValueError("scales must be finite")
+
+    def stack(rows):
+        out = np.zeros((n, max(a.shape[0] for a in rows), 768), np.float32)
+        for i, a in enumerate(rows):
+            out[i, :a.shape[0]] = a
+        return out, np.array([a.shape[0] for a in rows], np.int32)
+
+    context, context_len = stack(ctx)
+    uncond, uncond_len = stack(unc)
+    return dict(context=context, context_len=context_len, uncond=uncond, uncond_len=uncond_len, scale=scale,
+                seed=per_request(seeds, "seeds", np.uint64), noise_seed=per_request(noise_seeds, "noise_seeds", np.uint64))
+
+
+def batch_struct(b, context_ptr=None, uncond_ptr=None):
+    """An SdbBatch over the arrays of pack_batch (kept alive by the caller). context_ptr / uncond_ptr: device addresses that
+    replace the host arrays (the _dev entries)."""
+    p = lambda a, t: None if a is None else a.ctypes.data_as(C.POINTER(t))
+    n, L, _ = b["context"].shape
+    return SdbBatch(n, L, context_ptr or b["context"].ctypes.data, p(b["context_len"], C.c_int32), b["uncond"].shape[1],
+                    uncond_ptr or b["uncond"].ctypes.data, p(b["uncond_len"], C.c_int32), p(b["scale"], C.c_double),
+                    p(b["seed"], C.c_uint64), p(b["noise_seed"], C.c_uint64))
 
 
 class Context:
@@ -309,6 +385,60 @@ class Context:
                                         float(strength), ptr(context), n, context.shape[1], ptr(uncond), uncond.shape[0],
                                         float(scale), int(n_steps), None if noise is None else ptr(noise), int(seed), H, W,
                                         None if lat is None else ptr(lat), None if out is None else out.ctypes.data_as(_u8p)))
+        if latent and rgb:
+            return lat, out
+        return lat if latent else out
+
+    def sample_batch(self, contexts, unconds, scales, n_steps, seeds=None, noise_seeds=None, init_latent=None, H=64, W=64,
+                     latent=False, rgb=True):
+        """n different requests in one call (include/sdb200.h: sdb_sample_batch; pack_batch for the arguments). init_latent
+        [n,4,H,W] or None (each request's latent from its seed). -> the latent [n,4,H,W] and / or the u8 image [n,8H,8W,3]: a
+        tuple (latent, rgb) when both are requested."""
+        if not (latent or rgb):
+            raise ValueError("request the latent, the image or both")
+        b = pack_batch(contexts, unconds, scales, seeds, noise_seeds)
+        n = b["context"].shape[0]
+        if init_latent is not None:
+            init_latent = f32(init_latent)
+            if init_latent.ndim != 4 or init_latent.shape[:2] != (n, 4):
+                raise ValueError("init_latent must be [n, 4, H, W]")
+            H, W = init_latent.shape[2:]
+        lat = np.empty((n, 4, H, W), np.float32) if latent else None
+        out = np.empty((n, 8 * H, 8 * W, 3), np.uint8) if rgb else None
+        self.check(self.lib.sdb_sample_batch(self.h, C.byref(batch_struct(b)), int(n_steps),
+                                             None if init_latent is None else ptr(init_latent), H, W,
+                                             None if lat is None else ptr(lat), None if out is None else out.ctypes.data_as(_u8p)))
+        if latent and rgb:
+            return lat, out
+        return lat if latent else out
+
+    def img2img_batch(self, image, contexts, unconds, scales, n_steps, strength, mask=None, noise=None, seeds=None,
+                      noise_seeds=None, latent=False, rgb=True):
+        """n different requests of image-to-image / inpainting in one call (include/sdb200.h: sdb_img2img_batch). image u8
+        [n,8H,8W,3]; mask u8 [n,8H,8W] or None; noise [n,4,H,W] or None (each request's noise from its seed)."""
+        if not (latent or rgb):
+            raise ValueError("request the latent, the image or both")
+        b = pack_batch(contexts, unconds, scales, seeds, noise_seeds)
+        n = b["context"].shape[0]
+        image = np.ascontiguousarray(image, dtype=np.uint8)
+        if image.ndim != 4 or image.shape[0] != n or image.shape[3] != 3 or image.shape[1] % 8 or image.shape[2] % 8:
+            raise ValueError("image must be u8 [n, 8H, 8W, 3]")
+        Hp, Wp = image.shape[1:3]
+        H, W = Hp // 8, Wp // 8
+        if mask is not None:
+            mask = np.ascontiguousarray(mask, dtype=np.uint8)
+            if mask.shape != (n, Hp, Wp):
+                raise ValueError("mask must be u8 [n, 8H, 8W]")
+        if noise is not None:
+            noise = f32(noise)
+            if noise.shape != (n, 4, H, W):
+                raise ValueError("noise must be [n, 4, H, W]")
+        lat = np.empty((n, 4, H, W), np.float32) if latent else None
+        out = np.empty((n, Hp, Wp, 3), np.uint8) if rgb else None
+        self.check(self.lib.sdb_img2img_batch(self.h, C.byref(batch_struct(b)), image.ctypes.data_as(_u8p),
+                                              None if mask is None else mask.ctypes.data_as(_u8p), float(strength), int(n_steps),
+                                              None if noise is None else ptr(noise), H, W, None if lat is None else ptr(lat),
+                                              None if out is None else out.ctypes.data_as(_u8p)))
         if latent and rgb:
             return lat, out
         return lat if latent else out

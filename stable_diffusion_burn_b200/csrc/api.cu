@@ -365,6 +365,39 @@ int sdb_img2img_dev(sdb_ctx* ctx, const uint8_t* d_image, const uint8_t* d_mask,
   API_END
 }
 
+int sdb_sample_batch(sdb_ctx* ctx, const sdb_batch* batch, int n_steps, const float* init_latent, int H, int W, float* latent_out,
+                     uint8_t* rgb_out) {
+  API_BEGIN(ctx)
+  need_final(c);
+  model_sample_batch_host(c, batch, n_steps, init_latent, H, W, latent_out, rgb_out);
+  API_END
+}
+
+int sdb_sample_batch_dev(sdb_ctx* ctx, const sdb_batch* batch, int n_steps, const float* d_init_latent, int H, int W,
+                         float* d_latent_out, uint8_t* d_rgb_out, void* stream) {
+  API_BEGIN(ctx)
+  need_final(c);
+  model_sample_batch_dev(c, batch, n_steps, d_init_latent, H, W, d_latent_out, d_rgb_out, (cudaStream_t)stream);
+  API_END
+}
+
+int sdb_img2img_batch(sdb_ctx* ctx, const sdb_batch* batch, const uint8_t* image, const uint8_t* mask, double strength,
+                      int n_steps, const float* noise, int H, int W, float* latent_out, uint8_t* rgb_out) {
+  API_BEGIN(ctx)
+  need_final(c);
+  model_img2img_batch_host(c, batch, image, mask, strength, n_steps, noise, H, W, latent_out, rgb_out);
+  API_END
+}
+
+int sdb_img2img_batch_dev(sdb_ctx* ctx, const sdb_batch* batch, const uint8_t* d_image, const uint8_t* d_mask, double strength,
+                          int n_steps, const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb_out, void* stream) {
+  API_BEGIN(ctx)
+  need_final(c);
+  model_img2img_batch_dev(c, batch, d_image, d_mask, strength, n_steps, d_noise, H, W, d_latent_out, d_rgb_out,
+                          (cudaStream_t)stream);
+  API_END
+}
+
 int sdb_forward_diffuser(sdb_ctx* ctx, const float* latent, int32_t timestep, const float* context, int n, int L,
                          const float* uncond, int Lu, double guidance_scale, int H, int W, float* pred, float* out_uncond,
                          float* out_cond) {

@@ -1089,6 +1089,18 @@ __device__ __forceinline__ float randn_at(long long i, uint32_t k0, uint32_t k1)
   return sqrtf(-2.0f * logf(u1)) * cosf(6.283185307179586f * u2);
 }
 
+// The init-latent keys of a seed (randn_launch)
+__host__ __device__ __forceinline__ void init_noise_keys(uint64_t seed, uint32_t* k0, uint32_t* k1) {
+  *k0 = (uint32_t)seed * 2654435761u + 1u;
+  *k1 = (uint32_t)(seed >> 32) ^ 0x5bd1e995u;
+}
+// The init-latent keys of the seed, mixed with the timestep. k1 also takes k0: seeds that differ in their low word only would
+// otherwise share k1, hence the angle of every Box-Muller pair, and their streams would correlate (at pi/4).
+__host__ __device__ void step_noise_keys(uint64_t seed, int t, uint32_t* k0, uint32_t* k1) {
+  *k0 = ((uint32_t)seed * 2654435761u + 1u) ^ mix32(0x3C6EF372u + (uint32_t)t);
+  *k1 = ((uint32_t)(seed >> 32) ^ 0x5bd1e995u) ^ mix32(*k0 ^ 0xA54FF53Au);
+}
+
 // One fused guidance + update step of the sampler (DESIGN §7 f5, f6), per latent element i < count:
 //   pred = u + (c - u) scale, x0 = (x - sqrt(1 - a_t) pred) / sqrt(a_t)                        (every kind)
 //   STEP_DDIM        x' = sqrt(a_prev) x0 + dir_coef pred                        (eta = 0: sample_latent's own step)
@@ -1099,7 +1111,9 @@ __device__ __forceinline__ float randn_at(long long i, uint32_t k0, uint32_t k1)
 // both instantiations, so an all-ones mask reproduces the unmasked step bit for bit. The blend and the new samplers' updates
 // are written with _rn intrinsics (no FMA contraction) so that a test can restate them exactly in float32. STEP_DDIM is the
 // expression sample_latent has always used; its kernel keeps the argument list and the instructions it had.
-template <int KIND, bool BLEND>
+// PER_SAMPLE (a batch of different requests, DESIGN §7 f7): the scale and the eta noise key of sample i / (4 plane) come from
+// s.scales / s.noise_seeds, and z is drawn at the index within the sample. The arithmetic is the same expression.
+template <int KIND, bool BLEND, bool PER_SAMPLE = false>
 __device__ __forceinline__ void cfg_step(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
                                          long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
                                          float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
@@ -1107,14 +1121,25 @@ __device__ __forceinline__ void cfg_step(const float* __restrict__ eu, const flo
   pdl_enter();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) {
     const float u = eu[i], c = ec[i];
-    const float pred = u + (c - u) * scale;               // stablediffusion/mod.rs:190-191
+    float sc = scale;
+    long long zi = i;  // index of z in its stream
+    uint32_t k0 = s.k0, k1 = s.k1;
+    if constexpr (PER_SAMPLE) {
+      const long long smp = i / (4ll * plane);
+      sc = s.scales[smp];
+      if constexpr (KIND == STEP_DDIM_ETA) {
+        zi = i - smp * 4ll * plane;
+        step_noise_keys(s.noise_seeds[smp], s.t, &k0, &k1);
+      }
+    }
+    const float pred = u + (c - u) * sc;                  // stablediffusion/mod.rs:190-191
     const float x = lat[i];
     const float x0 = (x - pred * sqrt_1m_at) / sqrt_at;   // :152
     float nl;
     if constexpr (KIND == STEP_DDIM) {
       nl = x0 * sqrt_aprev + pred * dir_coef;             // :153-155 (sigma = 0)
     } else if constexpr (KIND == STEP_DDIM_ETA) {         // :153-155 with sigma = s
-      nl = __fadd_rn(__fadd_rn(__fmul_rn(sqrt_aprev, x0), __fmul_rn(dir_coef, pred)), __fmul_rn(s.s, randn_at(i, s.k0, s.k1)));
+      nl = __fadd_rn(__fadd_rn(__fmul_rn(sqrt_aprev, x0), __fmul_rn(dir_coef, pred)), __fmul_rn(s.s, randn_at(zi, k0, k1)));
     } else {
       const float d = s.second ? __fsub_rn(__fmul_rn(s.c1, x0), __fmul_rn(s.c2, s.hist[i])) : x0;
       s.hist[i] = x0;
@@ -1138,27 +1163,37 @@ __global__ void cfg_ddim_kernel(const float* __restrict__ eu, const float* __res
                                 const float* __restrict__ w, int plane) {
   cfg_step<STEP_DDIM, BLEND>(eu, ec, lat, count, scale, sqrt_1m_at, sqrt_at, sqrt_aprev, dir_coef, z0, e0, w, plane, SamplerStep{});
 }
-template <int KIND, bool BLEND>
+template <int KIND, bool BLEND, bool PER_SAMPLE>
 __global__ void cfg_sampler_kernel(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
                                    long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
                                    float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
                                    const float* __restrict__ w, int plane, const SamplerStep s) {
-  cfg_step<KIND, BLEND>(eu, ec, lat, count, scale, sqrt_1m_at, sqrt_at, sqrt_aprev, dir_coef, z0, e0, w, plane, s);
+  cfg_step<KIND, BLEND, PER_SAMPLE>(eu, ec, lat, count, scale, sqrt_1m_at, sqrt_at, sqrt_aprev, dir_coef, z0, e0, w, plane, s);
 }
 void cfg_sampler_launch(int kind, const SamplerStep& s, const float* eps_u, const float* eps_c, float* latent, long long count,
                         float scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
                         const float* z0, const float* eps0, const float* w, int plane) {
-  SDB_CHECK(kind == STEP_DDIM_ETA || kind == STEP_DPMPP_2M, "cfg_sampler_launch: kind");
+  const bool per_sample = s.scales != nullptr;
+  SDB_CHECK(kind == STEP_DDIM_ETA || kind == STEP_DPMPP_2M || (kind == STEP_DDIM && per_sample), "cfg_sampler_launch: kind");
+  SDB_CHECK(!per_sample || (plane > 0 && (kind != STEP_DDIM_ETA || s.noise_seeds)), "cfg_sampler_launch: per-sample inputs");
   int grid = (int)((count + 255) / 256);
   if (grid > g_num_sms * 8) grid = g_num_sms * 8;
   auto go = [&](auto kernel) {
     launch_k(kernel, dim3(grid), dim3(256), 0, st, eps_u, eps_c, latent, count, scale, sqrt_one_minus_at, sqrt_at, sqrt_aprev,
              dir_coef, z0, eps0, w, plane, s);
   };
-  if (kind == STEP_DDIM_ETA)
-    w ? go(cfg_sampler_kernel<STEP_DDIM_ETA, true>) : go(cfg_sampler_kernel<STEP_DDIM_ETA, false>);
-  else
-    w ? go(cfg_sampler_kernel<STEP_DPMPP_2M, true>) : go(cfg_sampler_kernel<STEP_DPMPP_2M, false>);
+  if (per_sample) {
+    if (kind == STEP_DDIM)
+      w ? go(cfg_sampler_kernel<STEP_DDIM, true, true>) : go(cfg_sampler_kernel<STEP_DDIM, false, true>);
+    else if (kind == STEP_DDIM_ETA)
+      w ? go(cfg_sampler_kernel<STEP_DDIM_ETA, true, true>) : go(cfg_sampler_kernel<STEP_DDIM_ETA, false, true>);
+    else
+      w ? go(cfg_sampler_kernel<STEP_DPMPP_2M, true, true>) : go(cfg_sampler_kernel<STEP_DPMPP_2M, false, true>);
+  } else if (kind == STEP_DDIM_ETA) {
+    w ? go(cfg_sampler_kernel<STEP_DDIM_ETA, true, false>) : go(cfg_sampler_kernel<STEP_DDIM_ETA, false, false>);
+  } else {
+    w ? go(cfg_sampler_kernel<STEP_DPMPP_2M, true, false>) : go(cfg_sampler_kernel<STEP_DPMPP_2M, false, false>);
+  }
   SDB_CUDA(cudaGetLastError());
 }
 void cfg_ddim_launch(const float* eps_u, const float* eps_c, float* latent, long long count, float scale,
@@ -1276,13 +1311,47 @@ static void randn_keys_launch(float* x, long long count, uint32_t k0, uint32_t k
   SDB_CUDA(cudaGetLastError());
 }
 void randn_launch(float* x, long long count, uint64_t seed, cudaStream_t st) {
-  randn_keys_launch(x, count, (uint32_t)seed * 2654435761u + 1u, (uint32_t)(seed >> 32) ^ 0x5bd1e995u, st);
+  uint32_t k0, k1;
+  init_noise_keys(seed, &k0, &k1);
+  randn_keys_launch(x, count, k0, k1, st);
 }
-// The init-latent keys of the seed, mixed with the timestep. k1 also takes k0: seeds that differ in their low word only would
-// otherwise share k1, hence the angle of every Box-Muller pair, and their streams would correlate (at pi/4).
-void step_noise_keys(uint64_t seed, int t, uint32_t* k0, uint32_t* k1) {
-  *k0 = ((uint32_t)seed * 2654435761u + 1u) ^ mix32(0x3C6EF372u + (uint32_t)t);
-  *k1 = ((uint32_t)(seed >> 32) ^ 0x5bd1e995u) ^ mix32(*k0 ^ 0xA54FF53Au);
+__global__ void randn_seeds_kernel(float* __restrict__ x, long long per, long long count, const uint64_t* __restrict__ seeds) {
+  pdl_enter();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) {
+    const long long s = i / per;
+    uint32_t k0, k1;
+    init_noise_keys(seeds[s], &k0, &k1);
+    x[i] = randn_at(i - s * per, k0, k1);
+  }
+}
+void randn_seeds_launch(float* x, int n, long long per, const uint64_t* seeds, cudaStream_t st) {
+  const long long count = (long long)n * per;
+  int grid = (int)((count + 255) / 256);
+  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
+  launch_k(randn_seeds_kernel, dim3(grid), dim3(256), 0, st, x, per, count, seeds);
+  SDB_CUDA(cudaGetLastError());
+}
+
+__global__ void stage_cfg_context_kernel(const float* __restrict__ cond, int L, const float* __restrict__ uncond, long long ustride,
+                                         const int* __restrict__ lens, int n, int Lpad, long long total, float* __restrict__ out) {
+  pdl_enter();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int col = (int)(i % 768);
+    const long long rr = i / 768;
+    const int r = (int)(rr % Lpad), b = (int)(rr / Lpad);
+    float v = 0.f;
+    if (r < lens[b])
+      v = b < n ? uncond[b * ustride + (long long)r * 768 + col] : cond[((long long)(b - n) * L + r) * 768 + col];
+    out[i] = v;
+  }
+}
+void stage_cfg_context_launch(const float* cond, int L, const float* uncond, long long ustride, const int* lens, int n, int Lpad,
+                              float* out, cudaStream_t st) {
+  const long long total = 2ll * n * Lpad * 768;
+  int grid = (int)((total + 255) / 256);
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
+  launch_k(stage_cfg_context_kernel, dim3(grid), dim3(256), 0, st, cond, L, uncond, ustride, lens, n, Lpad, total, out);
+  SDB_CUDA(cudaGetLastError());
 }
 void step_noise_launch(float* x, long long count, uint64_t seed, int t, cudaStream_t st) {
   uint32_t k0, k1;

@@ -107,6 +107,12 @@ struct SamplerStep {   // per-step scalars, computed on the host in double and p
   float s = 0.f;              // STEP_DDIM_ETA: x' = sqrt(a_prev) x0 + dir_coef pred + s z
   uint32_t k0 = 0, k1 = 0;    // STEP_DDIM_ETA: key of z (step_noise_keys)
   float ka = 0.f, kb = 0.f;   // blend: known = ka z0 + kb eps0 (sqrt(a_prev), sqrt(1 - a_prev))
+  // per-sample inputs of a batch of different requests (DESIGN §7 f7). scales != null selects the per-sample instantiations:
+  // sample s = i / (4 plane) takes scales[s] instead of `scale`, and STEP_DDIM_ETA draws z at the index within the sample,
+  // keyed by step_noise_keys(noise_seeds[s], t) instead of (k0, k1). Any kind, STEP_DDIM included, may run per sample.
+  const float* scales = nullptr;         // device [n]
+  const uint64_t* noise_seeds = nullptr;  // device [n]
+  int t = 0;                             // timestep value of the step
 };
 void cfg_sampler_launch(int kind, const SamplerStep& s, const float* eps_u, const float* eps_c, float* latent, long long count,
                         float scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
@@ -127,8 +133,17 @@ void add_vec_launch(const float* a, const float* b, int n, float* y, cudaStream_
 void randn_launch(float* x, long long count, uint64_t seed, cudaStream_t st);
 // Stochastic DDIM's per-step noise: the same generator keyed by (noise_seed, timestep value), element i of the call's latent
 // (numpy mirror: synth.step_noise). step_noise_launch writes the stream the fused step draws in registers.
-void step_noise_keys(uint64_t seed, int t, uint32_t* k0, uint32_t* k1);
+__host__ __device__ void step_noise_keys(uint64_t seed, int t, uint32_t* k0, uint32_t* k1);
 void step_noise_launch(float* x, long long count, uint64_t seed, int t, cudaStream_t st);
+// One seed per sample (DESIGN §7 f7): x [n][per], sample s is the stream randn_launch(seeds[s]) draws at n = 1, element j < per
+// at index j. seeds: device [n]. At n = 1 it is randn_launch bit for bit.
+void randn_seeds_launch(float* x, int n, long long per, const uint64_t* seeds, cudaStream_t st);
+// The CFG context of a sampling call: out [2n][Lpad][768], samples [0, n) the unconditional rows, [n, 2n) the prompt rows.
+// Row r of out sample b is copied when r < lens[b] (device [2n]: uncond lengths, then cond lengths) and zero otherwise, so the
+// caller's pad rows are never read. cond [n][L][768]; uncond [n][Lu][768] with ustride = Lu * 768, or [Lu][768] with ustride 0
+// (one negative broadcast over the batch).
+void stage_cfg_context_launch(const float* cond, int L, const float* uncond, long long ustride, const int* lens, int n, int Lpad,
+                              float* out, cudaStream_t st);
 
 // ---- row softmax for the 1-head VAE attention: P = softmax(S*scale) rows -> fp16 hi(/lo)
 void softmax_rows_launch(const float* S, long long rows, int cols, float scale, Half2Ptr out, cudaStream_t st);

@@ -1098,19 +1098,45 @@ struct Img2ImgIn {  // what the sampler loop needs to start part way down the sc
   float* w = nullptr;           // [n,H,W] latent mask (written when mask is set)
   float sa = 0.f, sb = 0.f;     // sqrt(abar[t0]), sqrt(1 - abar[t0])
 };
+
+// The n requests of a sampling call (DESIGN §7 f7). The single-request entries describe a uniform batch: every sample reads the L
+// prompt rows and the one broadcast negative, under one scale, and eta noise runs over the call's flat latent. The batch entries
+// give each sample its own prompt length, negative, scale and noise seed.
+struct Batch {
+  int n = 0;
+  const float* cond = nullptr;    // device [n][L][768]
+  int L = 0;
+  const float* uncond = nullptr;  // device [n][Lu][768] (ustride = Lu * 768) or [Lu][768] broadcast (ustride = 0)
+  int Lu = 0;
+  long long ustride = 0;
+  std::vector<int> len, ulen;     // [n] prompt / negative rows sample i reads
+  double scale = 0.0;             // uniform guidance scale (d_scale null)
+  const float* d_scale = nullptr;          // device [n]: per-sample scales; selects the per-sample fused step
+  const uint64_t* d_noise_seed = nullptr;  // device [n]: eta noise seeds of the per-sample step
+};
+
+Batch uniform_batch(const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale) {
+  Batch b;
+  b.n = n, b.cond = d_context, b.L = L, b.uncond = d_uncond, b.Lu = Lu, b.scale = scale;
+  b.len.assign(n, L), b.ulen.assign(n, Lu);
+  return b;
+}
 }  // namespace
 
 // sample_latent + latent_to_image (stablediffusion/mod.rs:51-160) from schedule index `first` on. The conditional and
 // unconditional UNet evaluations of a step (forward_diffuser :162-192) run as ONE batch-2n pass: weights stream from HBM once.
 // ii == null: txt2img from d_init_latent. Otherwise the start latent and (with a mask) the per-step blend come from ii.
 // Runs on c.stream; the caller joins the streams.
-static void sample_loop(Ctx& c, const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale, int n_steps,
-                        int first, const float* d_init_latent, const Img2ImgIn* ii, int H, int W, float* d_latent_out,
-                        uint8_t* d_rgb) {
+static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const float* d_init_latent, const Img2ImgIn* ii, int H,
+                        int W, float* d_latent_out, uint8_t* d_rgb) {
   Model& m = M(c);
   c.work.reset();
+  const int n = b.n;
   const int nb = 2 * n;
-  const int Lpad = round_up(std::max(L, Lu), 32);
+  // padded to the longest row count any sample reads, not to the caller's strides: the step graph is keyed on Lpad
+  int lmax = 1;
+  for (int i = 0; i < n; ++i) lmax = std::max(lmax, std::max(b.len[i], b.ulen[i]));
+  const int Lpad = round_up(lmax, 32);
   const size_t le = (size_t)n * 4 * H * W;
   // batch layout: samples [0,n) = unconditional context, [n,2n) = prompt context
   float* ctxp = c.work.get<float>((size_t)nb * Lpad * 768);
@@ -1118,11 +1144,13 @@ static void sample_loop(Ctx& c, const float* d_context, int n, int L, const floa
   float* eps = c.work.get<float>(2 * le);
   int* d_t = c.work.get<int>(1024);
   int* d_len = c.work.get<int>(nb);
-  SDB_CUDA(cudaMemsetAsync(ctxp, 0, (size_t)nb * Lpad * 768 * 4, c.stream));
-  for (int i = 0; i < n; ++i)
-    SDB_CUDA(cudaMemcpyAsync(ctxp + (size_t)i * Lpad * 768, d_uncond, (size_t)Lu * 768 * 4, cudaMemcpyDeviceToDevice, c.stream));
-  SDB_CUDA(cudaMemcpy2DAsync(ctxp + (size_t)n * Lpad * 768, (size_t)Lpad * 768 * 4, d_context, (size_t)L * 768 * 4,
-                             (size_t)L * 768 * 4, n, cudaMemcpyDeviceToDevice, c.stream));
+  std::vector<int> lens(nb);
+  for (int i = 0; i < nb; ++i) lens[i] = i < n ? b.ulen[i] : b.len[i - n];
+  SDB_CUDA(cudaMemcpyAsync(d_len, lens.data(), nb * 4, cudaMemcpyHostToDevice, c.stream));
+  {
+    KernelScope ks(c, KC_ELEMENTWISE);
+    stage_cfg_context_launch(b.cond, b.L, b.uncond, b.ustride, d_len, n, Lpad, ctxp, c.stream);
+  }
   if (!ii) {
     SDB_CUDA(cudaMemcpyAsync(xb, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
     SDB_CUDA(cudaMemcpyAsync(xb + le, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
@@ -1133,11 +1161,8 @@ static void sample_loop(Ctx& c, const float* d_context, int n, int L, const floa
   const int step = 1000 / n_steps;
   std::vector<int> ts = ddim_timesteps(n_steps);
   ts.erase(ts.begin(), ts.begin() + first);  // img2img runs the last k timesteps only
-  std::vector<int> lens(nb);
-  for (int i = 0; i < nb; ++i) lens[i] = i < n ? Lu : L;
   SDB_CUDA(cudaMemcpyAsync(d_t, ts.data(), ts.size() * 4, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_len, lens.data(), nb * 4, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));  // host staging buffers (ts, lens) must outlive the copies
 
   // time-embedding rows of every timestep of the schedule, once per call (unet/mod.rs:19-30, 115-118, 718-722 depend on t alone).
   // Fixed-size table indexed by the timestep value: the addresses of everything allocated after it do not depend on n_steps,
@@ -1247,14 +1272,16 @@ static void sample_loop(Ctx& c, const float* d_context, int n, int L, const floa
       }
       s.hist = hist;
     }
-    if (kind == STEP_DDIM)
-      cfg_ddim_launch(eps, eps + le, xb, (long long)le, (float)scale, (float)std::sqrt(1.0 - a_t), (float)std::sqrt(a_t),
+    if (kind == STEP_DDIM && !b.d_scale) {
+      cfg_ddim_launch(eps, eps + le, xb, (long long)le, (float)b.scale, (float)std::sqrt(1.0 - a_t), (float)std::sqrt(a_t),
                       (float)std::sqrt(a_prev), (float)dir, c.stream, blend ? ii->z0 : nullptr, blend ? ii->eps : nullptr,
                       blend ? ii->w : nullptr, H * W);
-    else
-      cfg_sampler_launch(kind, s, eps, eps + le, xb, (long long)le, (float)scale, (float)std::sqrt(1.0 - a_t),
+    } else {
+      s.scales = b.d_scale, s.noise_seeds = b.d_noise_seed, s.t = t;  // per-sample step (batch entries) when set
+      cfg_sampler_launch(kind, s, eps, eps + le, xb, (long long)le, (float)b.scale, (float)std::sqrt(1.0 - a_t),
                          (float)std::sqrt(a_t), (float)std::sqrt(a_prev), (float)dir, c.stream, blend ? ii->z0 : nullptr,
                          blend ? ii->eps : nullptr, blend ? ii->w : nullptr, H * W);
+    }
   }
   c.work.off = work_mark;
   if (d_latent_out) SDB_CUDA(cudaMemcpyAsync(d_latent_out, xb, le * 4, cudaMemcpyDeviceToDevice, c.stream));
@@ -1266,7 +1293,8 @@ void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float*
                       cudaStream_t caller) {
   check_sample_args(n, L, Lu, n_steps, H, W);
   StreamJoin join(c, caller);
-  sample_loop(c, d_context, n, L, d_uncond, Lu, scale, n_steps, 0, d_init_latent, nullptr, H, W, d_latent_out, d_rgb);
+  sample_loop(c, uniform_batch(d_context, n, L, d_uncond, Lu, scale), n_steps, 0, d_init_latent, nullptr, H, W, d_latent_out,
+              d_rgb);
 }
 
 void model_sample_host(Ctx& c, const float* context, int n, int L, const float* uncond, int Lu, double scale, int n_steps,
@@ -1312,18 +1340,16 @@ static void check_img2img_args(int n, int L, int Lu, int n_steps, int H, int W, 
 // Encoder (chunks of 4 images, as model_encode_dev) -> z0 in an io slot -> sampler loop from t0 = ts[N - k] -> decode.
 // z0 and the latent mask live in io slots, not in the work arena: the arena prefix up to the loop's work_mark is laid out
 // exactly as txt2img lays it out, so no cached step graph can see img2img data where it expects its own temporaries.
-void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
-                       int L, const float* d_uncond, int Lu, double scale, int n_steps, const float* d_noise, int H, int W,
-                       float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
+// Runs on c.stream; the caller has checked the arguments and joined the streams.
+static void img2img_run(Ctx& c, const Batch& b, const uint8_t* d_image, const uint8_t* d_mask, double strength, int n_steps,
+                        const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb) {
   Model& m = M(c);
-  check_img2img_args(n, L, Lu, n_steps, H, W, d_image, d_context, d_uncond, d_latent_out, d_rgb);
-  SDB_CHECK(d_noise, "img2img: the device entry needs the noise latent");
+  const int n = b.n;
   const int first = img2img_first(strength, n_steps);
   const double abar = (double)m.alphas_host[ddim_timesteps(n_steps)[first]];  // read as f32, widened (mod.rs:124-140)
   Img2ImgIn ii;
   ii.sa = (float)std::sqrt(abar), ii.sb = (float)std::sqrt(1.0 - abar);
   ii.eps = d_noise, ii.mask = d_mask;
-  StreamJoin join(c, caller);
   const size_t le = (size_t)n * 4 * H * W;
   ii.z0 = (float*)c.io(kIoImg2ImgZ0, le * 4);
   if (d_mask) ii.w = (float*)c.io(kIoImg2ImgW, (size_t)n * H * W * 4);
@@ -1342,7 +1368,18 @@ void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, do
     vae_encode(f, img4, Hp, Wp, ii.z0 + (size_t)i0 * 4 * H * W);
     c.work.off = mark;
   }
-  sample_loop(c, d_context, n, L, d_uncond, Lu, scale, n_steps, first, nullptr, &ii, H, W, d_latent_out, d_rgb);
+  sample_loop(c, b, n_steps, first, nullptr, &ii, H, W, d_latent_out, d_rgb);
+}
+
+void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
+                       int L, const float* d_uncond, int Lu, double scale, int n_steps, const float* d_noise, int H, int W,
+                       float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
+  check_img2img_args(n, L, Lu, n_steps, H, W, d_image, d_context, d_uncond, d_latent_out, d_rgb);
+  SDB_CHECK(d_noise, "img2img: the device entry needs the noise latent");
+  img2img_first(strength, n_steps);
+  StreamJoin join(c, caller);
+  img2img_run(c, uniform_batch(d_context, n, L, d_uncond, Lu, scale), d_image, d_mask, strength, n_steps, d_noise, H, W,
+              d_latent_out, d_rgb);
 }
 
 void model_img2img_host(Ctx& c, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
@@ -1368,6 +1405,150 @@ void model_img2img_host(Ctx& c, const uint8_t* image, const uint8_t* mask, doubl
   else
     randn_launch(d_n, (long long)le, seed, c.stream);  // the latent txt2img would start from for this seed
   model_img2img_dev(c, d_i, d_m, strength, d_c, n, L, d_u, Lu, scale, n_steps, d_n, H, W, d_lo, d_r, c.stream);
+  if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
+  if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+// ================================================================================ batches of different requests (DESIGN §7 f7)
+// Rejects a malformed descriptor before anything is staged, naming the field, the sample and the value.
+static void check_batch(const sdb_batch* b, bool need_seed) {
+  SDB_CHECK(b, "batch: null descriptor");
+  char msg[200];
+  snprintf(msg, sizeof(msg), "batch: n = %d must be >= 1", b->n);
+  SDB_CHECK(b->n >= 1, msg);
+  snprintf(msg, sizeof(msg), "batch: the row strides L = %d and Lu = %d must be >= 1", b->L, b->Lu);
+  SDB_CHECK(b->L >= 1 && b->Lu >= 1, msg);
+  SDB_CHECK(b->context, "batch: context is NULL");
+  SDB_CHECK(b->uncond, "batch: uncond is NULL");
+  SDB_CHECK(b->guidance_scale, "batch: guidance_scale is NULL");
+  SDB_CHECK(b->seed || !need_seed, "batch: seed is NULL and no init latent / noise is given");
+  for (int i = 0; i < b->n; ++i) {
+    const int l = b->context_len ? b->context_len[i] : b->L, lu = b->uncond_len ? b->uncond_len[i] : b->Lu;
+    snprintf(msg, sizeof(msg), "batch: context_len[%d] = %d is outside [1, L = %d]", i, l, b->L);
+    SDB_CHECK(l >= 1 && l <= b->L, msg);
+    snprintf(msg, sizeof(msg), "batch: uncond_len[%d] = %d is outside [1, Lu = %d]", i, lu, b->Lu);
+    SDB_CHECK(lu >= 1 && lu <= b->Lu, msg);
+    snprintf(msg, sizeof(msg), "batch: guidance_scale[%d] = %.17g is not finite", i, b->guidance_scale[i]);
+    SDB_CHECK(std::isfinite(b->guidance_scale[i]), msg);
+  }
+}
+
+namespace {
+struct BatchTab {  // the per-sample tables of a batch call on the device (io slot kIoBatchTab)
+  const uint64_t* seed;
+  const uint64_t* noise_seed;
+  const float* scale;
+};
+}  // namespace
+
+// Scales are cast to float as the single-request entries cast theirs; a NULL noise_seed array means the context's noise seed
+// (sdb_set_sampler) for every sample.
+static BatchTab upload_batch_tab(Ctx& c, const sdb_batch& b) {
+  const int n = b.n;
+  std::vector<uint64_t> u(2 * n);
+  std::vector<float> f(n);
+  for (int i = 0; i < n; ++i) {
+    u[i] = b.seed ? b.seed[i] : 0;
+    u[n + i] = b.noise_seed ? b.noise_seed[i] : c.sampler_noise_seed;
+    f[i] = (float)b.guidance_scale[i];
+  }
+  char* d = (char*)c.io(kIoBatchTab, (size_t)n * 20);
+  SDB_CUDA(cudaMemcpyAsync(d, u.data(), (size_t)n * 16, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(d + (size_t)n * 16, f.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));  // the host tables must outlive the copies
+  return {(const uint64_t*)d, (const uint64_t*)d + n, (const float*)(d + (size_t)n * 16)};
+}
+
+// the Batch of a descriptor whose context and uncond are device pointers
+static Batch batch_of(const sdb_batch& sb, const BatchTab& tab) {
+  Batch b;
+  b.n = sb.n, b.cond = sb.context, b.L = sb.L, b.uncond = sb.uncond, b.Lu = sb.Lu, b.ustride = (long long)sb.Lu * 768;
+  for (int i = 0; i < sb.n; ++i) {
+    b.len.push_back(sb.context_len ? sb.context_len[i] : sb.L);
+    b.ulen.push_back(sb.uncond_len ? sb.uncond_len[i] : sb.Lu);
+  }
+  b.d_scale = tab.scale, b.d_noise_seed = tab.noise_seed;
+  return b;
+}
+
+// [n,4,H,W] in io slot 2: sample i is the latent the single-request entries draw for seed[i] at n = 1
+static float* seeded_latent(Ctx& c, int n, int H, int W, const uint64_t* d_seed) {
+  float* d = (float*)c.io(2, (size_t)n * 4 * H * W * 4);
+  KernelScope ks(c, KC_ELEMENTWISE);
+  randn_seeds_launch(d, n, 4ll * H * W, d_seed, c.stream);
+  return d;
+}
+
+// copies a host descriptor's context and uncond to io slots 0 / 1 and points the device descriptor at them
+static sdb_batch stage_batch_host(Ctx& c, const sdb_batch& sb) {
+  sdb_batch db = sb;
+  const size_t ce = (size_t)sb.n * sb.L * 768, ue = (size_t)sb.n * sb.Lu * 768;
+  float* d_c = (float*)c.io(0, ce * 4);
+  float* d_u = (float*)c.io(1, ue * 4);
+  SDB_CUDA(cudaMemcpyAsync(d_c, sb.context, ce * 4, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(d_u, sb.uncond, ue * 4, cudaMemcpyHostToDevice, c.stream));
+  db.context = d_c, db.uncond = d_u;
+  return db;
+}
+
+void model_sample_batch_dev(Ctx& c, const sdb_batch* sb, int n_steps, const float* d_init_latent, int H, int W,
+                            float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
+  check_batch(sb, !d_init_latent);
+  check_sample_args(sb->n, sb->L, sb->Lu, n_steps, H, W);
+  SDB_CHECK(d_latent_out || d_rgb, "sample_batch: request the latent, the image or both");
+  StreamJoin join(c, caller);
+  const BatchTab tab = upload_batch_tab(c, *sb);
+  if (!d_init_latent) d_init_latent = seeded_latent(c, sb->n, H, W, tab.seed);
+  sample_loop(c, batch_of(*sb, tab), n_steps, 0, d_init_latent, nullptr, H, W, d_latent_out, d_rgb);
+}
+
+void model_sample_batch_host(Ctx& c, const sdb_batch* sb, int n_steps, const float* init_latent, int H, int W, float* latent_out,
+                             uint8_t* rgb) {
+  check_batch(sb, !init_latent);
+  check_sample_args(sb->n, sb->L, sb->Lu, n_steps, H, W);
+  SDB_CHECK(latent_out || rgb, "sample_batch: request the latent, the image or both");
+  const size_t le = (size_t)sb->n * 4 * H * W, re = (size_t)sb->n * 3 * 64 * H * W;
+  const sdb_batch db = stage_batch_host(c, *sb);
+  float* d_l = init_latent ? (float*)c.io(2, le * 4) : nullptr;
+  float* d_lo = latent_out ? (float*)c.io(3, le * 4) : nullptr;
+  uint8_t* d_r = rgb ? (uint8_t*)c.io(4, re) : nullptr;
+  if (init_latent) SDB_CUDA(cudaMemcpyAsync(d_l, init_latent, le * 4, cudaMemcpyHostToDevice, c.stream));
+  model_sample_batch_dev(c, &db, n_steps, d_l, H, W, d_lo, d_r, c.stream);
+  if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
+  if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+void model_img2img_batch_dev(Ctx& c, const sdb_batch* sb, const uint8_t* d_image, const uint8_t* d_mask, double strength,
+                             int n_steps, const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb,
+                             cudaStream_t caller) {
+  check_batch(sb, !d_noise);
+  check_img2img_args(sb->n, sb->L, sb->Lu, n_steps, H, W, d_image, sb->context, sb->uncond, d_latent_out, d_rgb);
+  img2img_first(strength, n_steps);
+  StreamJoin join(c, caller);
+  const BatchTab tab = upload_batch_tab(c, *sb);
+  if (!d_noise) d_noise = seeded_latent(c, sb->n, H, W, tab.seed);
+  img2img_run(c, batch_of(*sb, tab), d_image, d_mask, strength, n_steps, d_noise, H, W, d_latent_out, d_rgb);
+}
+
+void model_img2img_batch_host(Ctx& c, const sdb_batch* sb, const uint8_t* image, const uint8_t* mask, double strength,
+                              int n_steps, const float* noise, int H, int W, float* latent_out, uint8_t* rgb) {
+  check_batch(sb, !noise);
+  check_img2img_args(sb->n, sb->L, sb->Lu, n_steps, H, W, image, sb->context, sb->uncond, latent_out, rgb);
+  img2img_first(strength, n_steps);  // reject before staging anything
+  const int n = sb->n;
+  const size_t le = (size_t)n * 4 * H * W, re = (size_t)n * 3 * 64 * H * W, me = (size_t)n * 64 * H * W;
+  const sdb_batch db = stage_batch_host(c, *sb);
+  float* d_n = noise ? (float*)c.io(2, le * 4) : nullptr;
+  float* d_lo = latent_out ? (float*)c.io(3, le * 4) : nullptr;
+  uint8_t* d_r = rgb ? (uint8_t*)c.io(4, re) : nullptr;
+  uint8_t* d_i = (uint8_t*)c.io(5, re);
+  uint8_t* d_m = mask ? (uint8_t*)c.io(6, me) : nullptr;
+  SDB_CUDA(cudaMemcpyAsync(d_i, image, re, cudaMemcpyHostToDevice, c.stream));
+  if (mask) SDB_CUDA(cudaMemcpyAsync(d_m, mask, me, cudaMemcpyHostToDevice, c.stream));
+  if (noise) SDB_CUDA(cudaMemcpyAsync(d_n, noise, le * 4, cudaMemcpyHostToDevice, c.stream));
+  model_img2img_batch_dev(c, &db, d_i, d_m, strength, n_steps, d_n, H, W, d_lo, d_r, c.stream);
   if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
   if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));

@@ -1,5 +1,6 @@
 // model.cuh — the SD-v1.4 sampling graph on top of the kernels (UNet, VAE decoder, DDIM sampler).
 #pragma once
+#include "../../include/sdb200.h"
 #include "runtime.cuh"
 
 namespace sdb {
@@ -30,6 +31,16 @@ void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, do
 void model_img2img_host(Ctx& c, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
                         const float* uncond, int Lu, double scale, int n_steps, const float* noise, uint64_t seed, int H, int W,
                         float* latent_out, uint8_t* rgb);
+// batches of different requests (DESIGN §7 f7): sdb_batch with device (dev) or host (host) context / uncond
+void model_sample_batch_dev(Ctx& c, const sdb_batch* b, int n_steps, const float* d_init_latent, int H, int W,
+                            float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller);
+void model_sample_batch_host(Ctx& c, const sdb_batch* b, int n_steps, const float* init_latent, int H, int W, float* latent_out,
+                             uint8_t* rgb);
+void model_img2img_batch_dev(Ctx& c, const sdb_batch* b, const uint8_t* d_image, const uint8_t* d_mask, double strength,
+                             int n_steps, const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb,
+                             cudaStream_t caller);
+void model_img2img_batch_host(Ctx& c, const sdb_batch* b, const uint8_t* image, const uint8_t* mask, double strength,
+                              int n_steps, const float* noise, int H, int W, float* latent_out, uint8_t* rgb);
 void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const float* d_context, int n, int L, const float* d_uncond,
                                 int Lu, double scale, int H, int W, float* d_pred, float* d_u, float* d_c, cudaStream_t caller);
 void model_forward_diffuser_host(Ctx& c, const float* latent, int t, const float* context, int n, int L, const float* uncond,

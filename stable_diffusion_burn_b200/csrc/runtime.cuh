@@ -119,6 +119,7 @@ struct MetaCheck {
 constexpr int kIoImg2ImgZ0 = 8;  // encoded image latent z0 [n,4,H,W]
 constexpr int kIoImg2ImgW = 9;   // latent mask w [n,H,W]
 constexpr int kIoSamplerHist = 10;  // DPM-Solver++(2M): x0 of the previous step [n,4,H,W]
+constexpr int kIoBatchTab = 11;     // per-sample tables of a batch call: seeds, noise seeds [n] u64, guidance scales [n] f32
 
 struct Ctx {
   int device = 0;
@@ -156,11 +157,12 @@ struct Ctx {
   double cls_issued[KC_COUNT] = {0};  // tensor-core FLOPs actually issued (x passes for split-fp16 products)
   int64_t cls_launches[KC_COUNT] = {0};
   // grow-only device staging for the host-buffer entry points (no cudaMalloc/cudaFree per call: each is a device-wide sync).
-  // Slots 0..6: host-entry staging; kIoImg2Img*, kIoSamplerHist: buffers the sampling entries keep outside the work arena.
+  // Slots 0..6: host-entry staging; kIoImg2Img*, kIoSamplerHist, kIoBatchTab: buffers the sampling entries keep outside the
+  // work arena.
   struct IoBuf {
     void* p = nullptr;
     size_t cap = 0;
-  } iobuf[11];
+  } iobuf[12];
   void* io(int slot, size_t bytes);
   void io_destroy();
   void* model = nullptr;  // Model* (model.cu)

@@ -133,6 +133,27 @@ class StableDiffusion:
                                    mask=mask, noise=noise, seed=seed)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
 
+    # ---- batches of different requests (an extension, DESIGN.md §7 f7): one UNet pass per step for all of them
+    def sample_batch(self, contexts, unconditional_contexts, guidance_scales, n_steps: int, seeds, height: int = 512,
+                     width: int = 512, sampler: str = "ddim", eta: float = 0.0, noise_seeds=None):
+        """contexts: list of n [1, L_i, 768] (what `context` returns; lengths may differ); unconditional_contexts: one [Lu, 768]
+        shared by every request or a list of n; guidance_scales: one number or a list of n; seeds: list of n (request i gets the
+        image sample_image gives for seeds[i] alone, to rounding); noise_seeds: list of n keying eta > 0 noise per request, or None.
+        -> list of n flat uint8 arrays of height*width*3, like sample_image."""
+        with self._sampler(sampler, eta, 0):
+            rgb = self.ctx.sample_batch(contexts, unconditional_contexts, guidance_scales, n_steps, seeds=seeds,
+                                        noise_seeds=noise_seeds, H=height // 8, W=width // 8)
+        return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
+
+    def img2img_batch(self, images, contexts, unconditional_contexts, guidance_scales, n_steps: int, strength: float,
+                      masks=None, seeds=None, noise=None, sampler: str = "ddim", eta: float = 0.0, noise_seeds=None):
+        """img2img over a batch of different requests: images u8 [n, height, width, 3]; masks u8 [n, height, width] or None;
+        the other arguments as sample_batch. -> list of n flat uint8 arrays of height*width*3."""
+        with self._sampler(sampler, eta, 0):
+            rgb = self.ctx.img2img_batch(images, contexts, unconditional_contexts, guidance_scales, n_steps, strength, mask=masks,
+                                         noise=noise, seeds=seeds, noise_seeds=noise_seeds)
+        return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
+
     def latent_to_image(self, latent):
         rgb = self.ctx.latent_to_image(latent)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]

@@ -164,6 +164,17 @@ def randn_stream(count: int, k0: int, k1: int) -> np.ndarray:
     return (r * np.cos(np.float32(6.283185307179586) * u2)).astype(np.float32)
 
 
+def init_noise_keys(seed: int):
+    """Key of the init latent the sampling entries draw for `seed` (csrc/kernels.cu: init_noise_keys)."""
+    return ((seed & 0xFFFFFFFF) * 2654435761 + 1) & 0xFFFFFFFF, ((seed >> 32) & 0xFFFFFFFF) ^ 0x5BD1E995
+
+
+def seeded_latents(seeds, h: int, w: int) -> np.ndarray:
+    """The init latents [n,4,h,w] of a batch call (DESIGN.md §7 f7): request i is the stream the device draws for seeds[i] at
+    n = 1, element j < 4hw at index j (csrc/kernels.cu: randn_seeds_kernel). To a few ulp, like randn_stream."""
+    return np.stack([randn_stream(4 * h * w, *init_noise_keys(int(s))).reshape(4, h, w) for s in seeds])
+
+
 def step_noise_keys(noise_seed: int, t: int):
     """Key of stochastic DDIM's noise at timestep t (csrc/kernels.cu: step_noise_keys): the init-latent key of noise_seed mixed
     with the timestep value; k1 also takes k0, so that seeds differing in their low word only do not share k1 (the angle of every
