@@ -156,6 +156,38 @@ int sdb_img2img_dev(sdb_ctx* ctx, const uint8_t* d_image, const uint8_t* d_mask,
 #define SDB_SAMPLER_DPMPP_2M 1
 int sdb_set_sampler(sdb_ctx* ctx, int kind, double eta, uint64_t noise_seed);
 
+/* ---- LoRA adapters (DESIGN.md §7 f8) ------------------------------------------------------------------------------------- */
+/* An adapter (id >= 0) is a set of terms; a term targets one registry weight with down [r][fan-in] (fan-in = in for a Linear,
+ * in*k*k in OIHW order for a conv), up [out][r] and alpha (kohya lora_down / lora_up, PEFT lora_A / lora_B). The weights the
+ * packers read are W_eff = W + sum over adapters (ascending id) and their terms (in the order added) of s (up . down), with
+ * s = (float)(multiplier * alpha / r) computed in double; for a Linear the registry holds [in][out], so the delta is added
+ * transposed. Per element, each term's dot product runs in fp32 FMAs with k ascending, terms accumulate as tot = fmaf(s, d, tot)
+ * from 0, and W_eff = W + tot rounded once: with dyadic factors and power-of-two scales every step is exact.
+ * Targets: UNet ResBlock conv_in / conv_out / skip_connection / lin_embed, the down- and upsample convs, SpatialTransformer
+ * proj_in / proj_out, attn1 / attn2 query / key / value / out, mlp/geglu/proj and mlp/lin, and CLIP attn/{query,key,value,out}
+ * and mlp/fc1 / fc2. Norms, biases, embeddings, the VAE, unet/input_blocks/conv, unet/lin{1,2}_time_embed and unet/conv_out
+ * are rejected. The master arena stays the base (sdb_get_tensor returns base weights); adapters are per context (the weight
+ * broadcast carries the base only) and survive sdb_set_tensor, sdb_load_dump_dir, sdb_broadcast_weights and
+ * sdb_finalize_weights, which packs base + active adapters. Every change is pending until sdb_lora_apply (or a finalize); a
+ * compute call with pending changes fails. A malformed argument is rejected, naming the field and value, before any state
+ * changes. All adapters of a context apply to every sample of a batch. */
+/* Copies the factors of one term to the device. Rejects an unknown or non-target tensor, rank < 1, a NULL factor, a non-finite
+ * or non-positive alpha and a second term for the same (adapter, tensor). A new adapter starts at multiplier 1. */
+int sdb_lora_add(sdb_ctx* ctx, int adapter, const char* tensor, int rank, const float* down, const float* up, double alpha);
+/* multiplier (finite) of an existing adapter; 0 disables it without freeing its factors */
+int sdb_lora_scale(sdb_ctx* ctx, int adapter, double multiplier);
+/* removes one adapter (-1 = all) and frees its device factors */
+int sdb_lora_remove(sdb_ctx* ctx, int adapter);
+/* Synchronous. One merge launch writes W_eff of every weight whose active terms changed since the last apply or finalize; the
+ * packing unit of each (a ResBlock, a SpatialTransformer with its LayerNorm folds, a resample conv, the time-embedding table,
+ * a CLIP block with its folded out-projection bias) is re-packed into its own packed addresses and nothing else is touched.
+ * Cached step graphs stay valid. With no active term a weight packs from the base tensor itself, so removing every adapter and
+ * applying restores the base packing bit for bit. */
+int sdb_lora_apply(sdb_ctx* ctx);
+/* W_eff of a registry tensor as the packers read it after the last apply or finalize (the base tensor when no active term
+ * targets it); host buffer of count elements. */
+int sdb_get_merged_tensor(sdb_ctx* ctx, const char* tensor, float* host, int64_t count);
+
 /* ---- batches of different requests (DESIGN.md §7 f7) --------------------------------------------------------------------- */
 /* One call samples n requests that differ in prompt length, negative prompt, guidance scale and seed, as one batch-2n UNet pass
  * per step (the weights stream from HBM once per step for all of them). Sample i gives what request i gives as a call of its

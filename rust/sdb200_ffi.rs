@@ -68,6 +68,14 @@ extern "C" {
                        d_noise: *const c_void, h: c_int, w: c_int, d_latent_out: *mut c_void, d_rgb_out: *mut c_void,
                        stream: *mut c_void) -> c_int;
     fn sdb_set_sampler(ctx: *mut SdbCtx, kind: c_int, eta: f64, noise_seed: u64) -> c_int;
+    fn sdb_tensor_count(ctx: *mut SdbCtx) -> c_int;
+    fn sdb_tensor_info(ctx: *mut SdbCtx, index: c_int, name: *mut *const c_char, dims: *mut i64, ndim: *mut c_int) -> c_int;
+    fn sdb_lora_add(ctx: *mut SdbCtx, adapter: c_int, tensor: *const c_char, rank: c_int, down: *const f32, up: *const f32,
+                    alpha: f64) -> c_int;
+    fn sdb_lora_scale(ctx: *mut SdbCtx, adapter: c_int, multiplier: f64) -> c_int;
+    fn sdb_lora_remove(ctx: *mut SdbCtx, adapter: c_int) -> c_int;
+    fn sdb_lora_apply(ctx: *mut SdbCtx) -> c_int;
+    fn sdb_get_merged_tensor(ctx: *mut SdbCtx, tensor: *const c_char, host: *mut f32, count: i64) -> c_int;
     fn sdb_sample_batch(ctx: *mut SdbCtx, batch: *const SdbBatch, n_steps: c_int, init_latent: *const f32, h: c_int, w: c_int,
                         latent_out: *mut f32, rgb_out: *mut u8) -> c_int;
     fn sdb_img2img_batch(ctx: *mut SdbCtx, batch: *const SdbBatch, image: *const u8, mask: *const u8, strength: f64, n_steps: c_int,
@@ -251,6 +259,61 @@ impl StableDiffusion {
             Sampler::DpmPp2M => (SDB_SAMPLER_DPMPP_2M, 0.0),
         };
         self.check(unsafe { sdb_set_sampler(self.ctx, kind, eta, noise_seed) })
+    }
+
+    /// One term of LoRA adapter `adapter` (an extension, DESIGN.md §7 f8) on registry weight `tensor`: `down` = rank x fan-in
+    /// floats, `up` = out x rank floats, `alpha`. Pending until `lora_apply`; the lengths are checked here, the rest in C.
+    pub fn lora_add(&self, adapter: i32, tensor: &str, rank: usize, down: &[f32], up: &[f32], alpha: f64) -> Result<(), SdbError> {
+        // the C side reads rank * fan_in floats from `down` and out * rank from `up`: check both lengths against the registry
+        // shape first, so that a short slice is an error and never read past its end
+        let (out, fan_in) = self.lora_geometry(tensor)?;
+        if rank == 0 || down.len() != rank * fan_in || up.len() != out * rank {
+            return Err(SdbError(format!("lora_add {tensor}: rank {rank} needs down = {} and up = {} floats, got {} and {}",
+                                        rank * fan_in, out * rank, down.len(), up.len())));
+        }
+        let name = CString::new(tensor).map_err(|_| SdbError("tensor name contains NUL".into()))?;
+        self.check(unsafe { sdb_lora_add(self.ctx, adapter, name.as_ptr(), rank as c_int, down.as_ptr(), up.as_ptr(), alpha) })
+    }
+
+    /// (out, fan-in) of a registry weight: [in][out] for a Linear, OIHW for a conv.
+    fn lora_geometry(&self, tensor: &str) -> Result<(usize, usize), SdbError> {
+        let n = unsafe { sdb_tensor_count(self.ctx) };
+        for i in 0..n {
+            let mut name: *const c_char = std::ptr::null();
+            let mut dims = [0i64; 4];
+            let mut ndim: c_int = 0;
+            self.check(unsafe { sdb_tensor_info(self.ctx, i, &mut name, dims.as_mut_ptr(), &mut ndim) })?;
+            if unsafe { CStr::from_ptr(name) }.to_bytes() != tensor.as_bytes() {
+                continue;
+            }
+            return match ndim {
+                2 => Ok((dims[1] as usize, dims[0] as usize)),
+                4 => Ok((dims[0] as usize, (dims[1] * dims[2] * dims[3]) as usize)),
+                _ => Err(SdbError(format!("lora_add {tensor}: not a LoRA target (a {ndim}-d tensor)"))),
+            };
+        }
+        Err(SdbError(format!("lora_add: unknown tensor '{tensor}'")))
+    }
+
+    /// Multiplier of an adapter (0 disables it without freeing it). Pending until `lora_apply`.
+    pub fn lora_scale(&self, adapter: i32, multiplier: f64) -> Result<(), SdbError> {
+        self.check(unsafe { sdb_lora_scale(self.ctx, adapter, multiplier) })
+    }
+
+    /// Removes an adapter (-1 = all). Pending until `lora_apply`.
+    pub fn lora_remove(&self, adapter: i32) -> Result<(), SdbError> {
+        self.check(unsafe { sdb_lora_remove(self.ctx, adapter) })
+    }
+
+    /// Merges and re-packs the layers whose adapters changed; cached step graphs stay valid.
+    pub fn lora_apply(&self) -> Result<(), SdbError> {
+        self.check(unsafe { sdb_lora_apply(self.ctx) })
+    }
+
+    /// The merged weight the packers read (the base tensor when no active term targets it); `out` holds its element count.
+    pub fn get_merged_tensor(&self, tensor: &str, out: &mut [f32]) -> Result<(), SdbError> {
+        let name = CString::new(tensor).map_err(|_| SdbError("tensor name contains NUL".into()))?;
+        self.check(unsafe { sdb_get_merged_tensor(self.ctx, name.as_ptr(), out.as_mut_ptr(), out.len() as i64) })
     }
 
     /// n different requests in one call (an extension, DESIGN.md §7 f7): request i is (`contexts[i]` = L_i x 768 floats,

@@ -73,6 +73,11 @@ SIGNATURES = [
     ("sdb_img2img_dev", C.c_int, [_ctx, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                   C.c_double, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("sdb_set_sampler", C.c_int, [_ctx, C.c_int, C.c_double, C.c_uint64]),
+    ("sdb_lora_add", C.c_int, [_ctx, C.c_int, C.c_char_p, C.c_int, _f32p, _f32p, C.c_double]),
+    ("sdb_lora_scale", C.c_int, [_ctx, C.c_int, C.c_double]),
+    ("sdb_lora_remove", C.c_int, [_ctx, C.c_int]),
+    ("sdb_lora_apply", C.c_int, [_ctx]),
+    ("sdb_get_merged_tensor", C.c_int, [_ctx, C.c_char_p, _f32p, C.c_int64]),
     ("sdb_sample_batch", C.c_int, [_ctx, _batchp, C.c_int, _f32p, C.c_int, C.c_int, _f32p, _u8p]),
     ("sdb_sample_batch_dev", C.c_int, [_ctx, _batchp, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                        C.c_void_p]),
@@ -272,6 +277,46 @@ class Context:
                 raise ValueError(f"unknown sampler {kind!r}: one of {', '.join(self.SAMPLERS)}")
             kind = self.SAMPLERS[kind]
         self.check(self.lib.sdb_set_sampler(self.h, int(kind), float(eta), int(noise_seed)))
+
+    # ---- LoRA adapters (include/sdb200.h: sdb_lora_*; DESIGN.md §7 f8)
+    def lora_add(self, adapter, tensor, down, up, alpha):
+        """One term of adapter `adapter`: registry weight `tensor`, down [r, fan-in] (a conv's [r, in, k, k] is flattened), up
+        [out, r] (or [out, r, 1, 1]), alpha. Pending until lora_apply."""
+        down = f32(down); up = f32(up)
+        r = down.shape[0] if down.ndim else 0
+        down = down.reshape(r, -1) if r else down
+        up = up.reshape(up.shape[0], -1) if up.ndim else up
+        if up.ndim != 2 or up.shape[1] != r:
+            raise ValueError(f"lora_add {tensor}: up {up.shape} does not match rank {r} of down {down.shape}")
+        if getattr(self, "_shapes", None) is None:  # one registry walk per context, not one per term
+            self._shapes = dict(self.tensor_list())
+        shape = self._shapes.get(tensor)
+        if shape is not None:
+            out, fan_in = (shape[1], shape[0]) if len(shape) == 2 else (shape[0], int(np.prod(shape[1:])))
+            if down.shape[1] != fan_in or up.shape[0] != out:
+                raise ValueError(f"lora_add {tensor}: down {down.shape} / up {up.shape} do not fit a weight of {out} outputs "
+                                 f"and fan-in {fan_in}")
+        self.check(self.lib.sdb_lora_add(self.h, int(adapter), tensor.encode(), int(r), ptr(down), ptr(up), float(alpha)))
+        self._lora_ids = self.lora_adapters() | {int(adapter)}
+
+    def lora_scale(self, adapter, multiplier):
+        self.check(self.lib.sdb_lora_scale(self.h, int(adapter), float(multiplier)))
+
+    def lora_remove(self, adapter=-1):
+        self.check(self.lib.sdb_lora_remove(self.h, int(adapter)))
+        self._lora_ids = set() if int(adapter) == -1 else self.lora_adapters() - {int(adapter)}
+
+    def lora_adapters(self) -> set:
+        """Ids of the adapters added through this Context and not removed."""
+        return set(getattr(self, "_lora_ids", ()))
+
+    def lora_apply(self):
+        self.check(self.lib.sdb_lora_apply(self.h))
+
+    def get_merged_tensor(self, name, shape):
+        a = np.empty(shape, np.float32)
+        self.check(self.lib.sdb_get_merged_tensor(self.h, name.encode(), ptr(a), a.size))
+        return a
 
     # ---- hot path (host buffers)
     def unet_forward(self, x, t, context):

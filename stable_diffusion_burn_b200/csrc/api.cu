@@ -279,7 +279,10 @@ int sdb_finalize_weights(sdb_ctx* ctx) {
 }
 
 // ------------------------------------------------------------------------------ hot path
-static void need_final(Ctx& c) { SDB_CHECK(c.finalized, "call sdb_finalize_weights first"); }
+static void need_final(Ctx& c) {
+  SDB_CHECK(c.finalized, "call sdb_finalize_weights first");
+  SDB_CHECK(!model_lora_pending(c), "LoRA adapter changes are pending: call sdb_lora_apply first");
+}
 
 int sdb_unet_forward(sdb_ctx* ctx, const float* x, int32_t timestep, const float* context, int n, int H, int W, int L,
                      float* out) {
@@ -458,6 +461,37 @@ int sdb_set_sampler(sdb_ctx* ctx, int kind, double eta, uint64_t noise_seed) {
   snprintf(msg, sizeof(msg), "sampler: DPM-Solver++(2M) is deterministic; eta %.17g must be 0", eta);
   SDB_CHECK(kind != SDB_SAMPLER_DPMPP_2M || eta == 0.0, msg);
   c.sampler_kind = kind, c.sampler_eta = eta, c.sampler_noise_seed = noise_seed;
+  API_END
+}
+
+// ------------------------------------------------------------------------------ LoRA adapters (DESIGN.md §7 f8)
+int sdb_lora_add(sdb_ctx* ctx, int adapter, const char* tensor, int rank, const float* down, const float* up, double alpha) {
+  API_BEGIN(ctx)
+  model_lora_add(c, adapter, tensor, rank, down, up, alpha);
+  API_END
+}
+
+int sdb_lora_scale(sdb_ctx* ctx, int adapter, double multiplier) {
+  API_BEGIN(ctx)
+  model_lora_scale(c, adapter, multiplier);
+  API_END
+}
+
+int sdb_lora_remove(sdb_ctx* ctx, int adapter) {
+  API_BEGIN(ctx)
+  model_lora_remove(c, adapter);
+  API_END
+}
+
+int sdb_lora_apply(sdb_ctx* ctx) {
+  API_BEGIN(ctx)
+  model_lora_apply(c);
+  API_END
+}
+
+int sdb_get_merged_tensor(sdb_ctx* ctx, const char* tensor, float* host, int64_t count) {
+  API_BEGIN(ctx)
+  model_get_merged_tensor(c, tensor, host, count);
   API_END
 }
 

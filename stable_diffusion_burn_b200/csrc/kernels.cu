@@ -1599,4 +1599,88 @@ void synth_fill_table_launch(float* base, const SynthDesc* d_desc, int ntensors,
   SDB_CUDA(cudaGetLastError());
 }
 
+// ============================================================ LoRA merge (DESIGN §7 f8)
+// One CTA = one 64 x 64 tile of one tensor's W_eff (tile -> tensor by binary search over the tile prefix sums). For each term the
+// up / down chunks of 32 ranks are staged in shared memory as [k][64 rows] and [k][64 cols]; a thread owns rows ty + 16 i and
+// cols tx + 16 j (i, j < 4), so for a fixed (i, j) a half-warp reads and writes 16 consecutive elements of the row-major tensor.
+// The term's dot product d runs k-ascending in fp32 FMAs and folds into tot with one more FMA: the order is fixed, so the
+// result is reproducible, and with dyadic factors exact.
+constexpr int kLoraTile = 64, kLoraKc = 32;
+__global__ void __launch_bounds__(256)
+lora_merge_kernel(const LoraTensorDesc* __restrict__ tens, int ntensors, const LoraTermDesc* __restrict__ terms) {
+  __shared__ float sa[kLoraKc][kLoraTile + 1];  // [k][row of the tile]
+  __shared__ float sb[kLoraKc][kLoraTile + 1];  // [k][col of the tile]
+  const long long tile = blockIdx.x;
+  int lo = 0, hi = ntensors - 1;
+  while (lo < hi) {  // last tensor whose first tile is <= tile
+    const int mid = (lo + hi + 1) >> 1;
+    if (tens[mid].tile0 <= tile) lo = mid; else hi = mid - 1;
+  }
+  const LoraTensorDesc t = tens[lo];
+  const int tl = (int)(tile - t.tile0);
+  const int row0 = (tl / t.tiles_c) * kLoraTile, col0 = (tl % t.tiles_c) * kLoraTile;
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  // conv: rows index out (up), cols index fan-in (down); Linear [in][out]: rows index fan-in (down), cols index out (up)
+  const int fan_in = t.transposed ? t.rows : t.cols;
+  float tot[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) tot[i][j] = 0.f;
+  for (int q = 0; q < t.nterms; ++q) {
+    const LoraTermDesc tm = terms[t.term0 + q];
+    float (*su)[kLoraTile + 1] = t.transposed ? sb : sa;  // where the up chunk goes
+    float (*sd)[kLoraTile + 1] = t.transposed ? sa : sb;  // where the down chunk goes
+    const int u0 = t.transposed ? col0 : row0, d0 = t.transposed ? row0 : col0;
+    const int u_lim = t.transposed ? t.cols : t.rows, d_lim = t.transposed ? t.rows : t.cols;
+    float d[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) d[i][j] = 0.f;
+    for (int k0 = 0; k0 < tm.r; k0 += kLoraKc) {
+      const int kc = min(kLoraKc, tm.r - k0);
+      __syncthreads();  // the previous chunk has been consumed
+      for (int e = threadIdx.x; e < kLoraKc * kLoraTile; e += 256) {
+        const int kk = e % kLoraKc, i = e / kLoraKc;  // up [out][r]: consecutive threads walk k
+        su[kk][i] = (kk < kc && u0 + i < u_lim) ? tm.up[(long long)(u0 + i) * tm.r + k0 + kk] : 0.f;
+        const int kd = e / kLoraTile, id = e % kLoraTile;  // down [r][fan-in]: consecutive threads walk fan-in
+        sd[kd][id] = (kd < kc && d0 + id < d_lim) ? tm.down[(long long)(k0 + kd) * fan_in + d0 + id] : 0.f;
+      }
+      __syncthreads();
+      for (int kk = 0; kk < kc; ++kk) {
+        float a[4], b[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) a[i] = sa[kk][ty + 16 * i], b[i] = sb[kk][tx + 16 * i];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) d[i][j] = __fmaf_rn(a[i], b[j], d[i][j]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) tot[i][j] = __fmaf_rn(tm.s, d[i][j], tot[i][j]);
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = row0 + ty + 16 * i;
+    if (r >= t.rows) continue;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int cc = col0 + tx + 16 * j;
+      if (cc < t.cols) {
+        const long long idx = (long long)r * t.cols + cc;
+        t.out[idx] = __fadd_rn(t.base[idx], tot[i][j]);
+      }
+    }
+  }
+}
+void lora_merge_launch(const LoraTensorDesc* d_tensors, int ntensors, const LoraTermDesc* d_terms, long long ntiles, cudaStream_t st) {
+  SDB_CHECK(ntiles > 0 && ntiles < (1LL << 31), "lora merge: tile count");
+  lora_merge_kernel<<<(unsigned)ntiles, 256, 0, st>>>(d_tensors, ntensors, d_terms);
+  SDB_CUDA(cudaGetLastError());
+}
+
 }  // namespace sdb

@@ -175,4 +175,24 @@ struct SynthDesc {
 };
 void synth_fill_table_launch(float* base, const SynthDesc* d_desc, int ntensors, long long nchunks, cudaStream_t st);
 
+// ---- LoRA merge (DESIGN §7 f8): W_eff = W + sum_t s_t (up_t . down_t), every changed tensor in ONE launch.
+// A tensor is stored [rows][cols]: a conv OIHW weight is [out][fan-in] (transposed = 0), a Linear weight of the registry is
+// [in][out] (transposed = 1). up_t [out][r_t], down_t [r_t][fan-in]. Per element: d = fmaf(up[o][k], down[k][f], d) with k
+// ascending from d = 0, tot = fmaf(s_t, d, tot) over the tensor's terms in table order from tot = 0, W_eff = W + tot (one rounding).
+struct LoraTensorDesc {
+  const float* base;
+  float* out;
+  int rows, cols, transposed;
+  int term0, nterms;  // the tensor's terms: [term0, term0 + nterms) of the term table
+  int tiles_c;        // 64-wide tiles along cols
+  long long tile0;    // index of the tensor's first 64 x 64 tile (prefix sums over the table)
+};
+struct LoraTermDesc {
+  const float* down;
+  const float* up;
+  int r;
+  float s;
+};
+void lora_merge_launch(const LoraTensorDesc* d_tensors, int ntensors, const LoraTermDesc* d_terms, long long ntiles, cudaStream_t st);
+
 }  // namespace sdb

@@ -41,31 +41,41 @@ static Half2Ptr alloc_half2(Arena& a, size_t count) {
 static float* mptr(Ctx& c, int idx) {
   return idx < 0 ? nullptr : reinterpret_cast<float*>(c.master.base) + c.tensors[idx].offset;
 }
+// the weight a packer reads: the LoRA-merged W_eff of a tensor with an active adapter term, else the master copy. Packing only:
+// every run-time read goes through mptr and sees the base weights.
+static float* wsrc(Ctx& c, int idx) {
+  if (idx >= 0) {
+    const auto& eff = M(c).lora.eff;
+    auto it = eff.find(idx);
+    if (it != eff.end()) return it->second;
+  }
+  return mptr(c, idx);
+}
 
 static void pack_conv(Ctx& c, ConvW& w, bool up2 = false) {
   w.bias = mptr(c, w.bi);
   if (w.cin % 64 != 0 || w.cout % 32 != 0) {  // CUDA-core convs
     if (w.cout <= 8 && w.k == 3 && w.cin % 4 == 0) {
       w.w_small = c.packed.get<float>((size_t)w.cout * 9 * w.cin);
-      pack_small_cout_launch(mptr(c, w.wi), w.cout, w.cin, w.w_small, c.stream);
+      pack_small_cout_launch(wsrc(c, w.wi), w.cout, w.cin, w.w_small, c.stream);
     }
     return;
   }
   if (up2) {
     w.packed.p = alloc_half2(c.packed, (size_t)16 * w.cout * w.cin);
     w.packed.N = w.cout, w.packed.K = 4 * w.cin;
-    pack_conv_up2_launch(mptr(c, w.wi), w.cout, w.cin, w.packed.p, c.stream);
+    pack_conv_up2_launch(wsrc(c, w.wi), w.cout, w.cin, w.packed.p, c.stream);
   } else {
     w.packed.p = alloc_half2(c.packed, (size_t)w.cout * w.k * w.k * w.cin);
     w.packed.N = w.cout, w.packed.K = w.k * w.k * w.cin;
-    pack_conv_launch(mptr(c, w.wi), w.cout, w.cin, w.k, w.packed.p, c.stream);
+    pack_conv_launch(wsrc(c, w.wi), w.cout, w.cin, w.k, w.packed.p, c.stream);
   }
 }
 static void pack_lin(Ctx& c, LinW& w) {
   w.bias = mptr(c, w.bi);
   w.packed.p = alloc_half2(c.packed, (size_t)w.out * w.in);
   w.packed.N = w.out, w.packed.K = w.in;
-  pack_linear_launch(mptr(c, w.wi), w.in, w.out, w.packed.p, 0, c.stream);
+  pack_linear_launch(wsrc(c, w.wi), w.in, w.out, w.packed.p, 0, c.stream);
 }
 static void pack_norm(Ctx& c, NormW& n) {
   n.gamma = mptr(c, n.gi), n.beta = mptr(c, n.bi);
@@ -78,7 +88,7 @@ static void pack_norm(Ctx& c, NormW& n) {
 static void pack_heads(Ctx& c, const LinW& src, int heads, int d, int dpad, Half2Ptr dst, int row_offset,
                        const float* in_scale = nullptr) {
   for (int h = 0; h < heads; ++h)
-    pack_linear_launch(mptr(c, src.wi), src.in, d, dst, row_offset + h * dpad, c.stream, src.out, h * d, in_scale);
+    pack_linear_launch(wsrc(c, src.wi), src.in, d, dst, row_offset + h * dpad, c.stream, src.out, h * d, in_scale);
 }
 
 static void pack_resblock(Ctx& c, ResBlockW& r, int passes) {
@@ -129,7 +139,7 @@ static void pack_st(Ctx& c, SpatialTransformerW& s, int passes) {
   s.w_geglu.p = alloc_half2(c.packed, (size_t)8 * s.c * s.c), s.w_geglu.N = 8 * s.c, s.w_geglu.K = s.c;
   s.geglu_bias = c.packed.get<float>((size_t)8 * s.c);
   fold(s.w_geglu, s.u_geglu_hi, s.u_geglu_full, s.v_geglu, [&](Half2Ptr dst, const float* sc) {
-    pack_geglu_launch(mptr(c, s.geglu.wi), mptr(c, s.geglu.bi), s.c, 4 * s.c, 64, dst, dst.hi == s.w_geglu.p.hi ? s.geglu_bias : nullptr,
+    pack_geglu_launch(wsrc(c, s.geglu.wi), mptr(c, s.geglu.bi), s.c, 4 * s.c, 64, dst, dst.hi == s.w_geglu.p.hi ? s.geglu_bias : nullptr,
                       c.stream, sc);
   }, s.ln3);
   add_vec_launch(s.v_geglu, s.geglu_bias, 8 * s.c, s.v_geglu, c.stream);  // v = beta^T W + b (packed order)
@@ -148,52 +158,16 @@ static void pack_resnet(Ctx& c, ResnetW& r, int passes) {
   }
 }
 
-void model_finalize(Ctx& c) {
+// fused time-embedding projection: every lin_embed side by side, bias = lin bias + conv_in bias
+static void pack_emb(Ctx& c) {
   Model& m = M(c);
-  model_invalidate_graphs(c);
-  c.packed.reset();
-  SDB_CUDA(cudaMemsetAsync(c.packed.base, 0, c.packed.cap, c.stream));  // head-pad rows must be zero
-  // ---- UNet
-  m.lin1_time.bias = mptr(c, m.lin1_time.bi), m.lin2_time.bias = mptr(c, m.lin2_time.bi);
-  auto pack_block = [&](UNetBlockW& b) {
-    const int p = g_level_passes[std::min(b.level, 3)];
-    switch (b.kind) {
-      case BK_CONV:
-        pack_conv(c, b.conv);
-        break;
-      case BK_DOWN:
-        pack_conv(c, b.conv), b.conv.passes = p;
-        break;
-      case BK_R:
-        pack_resblock(c, b.res, p);
-        break;
-      case BK_RT:
-        pack_resblock(c, b.res, p), pack_st(c, b.st, p);
-        break;
-      case BK_RU:
-      case BK_RTU:
-        pack_resblock(c, b.res, p);
-        if (b.kind == BK_RTU) pack_st(c, b.st, p);
-        pack_conv(c, b.conv, /*up2=*/true);
-        b.conv.passes = g_level_passes[std::max(b.level - 1, 0)];  // the conv runs at the upsampled resolution
-        break;
-    }
-  };
-  for (auto& b : m.in_blocks) pack_block(b);
-  pack_resblock(c, m.mid_res1, g_level_passes[3]);
-  pack_st(c, m.mid_st, g_level_passes[3]);
-  pack_resblock(c, m.mid_res2, g_level_passes[3]);
-  for (auto& b : m.out_blocks) pack_block(b);
-  pack_norm(c, m.norm_out);
-  pack_conv(c, m.conv_out);
-  // fused time-embedding projection: every lin_embed side by side, bias = lin bias + conv_in bias
   m.emb_total = 0;
   for (ResBlockW* r : m.resblocks) r->emb_off = m.emb_total, m.emb_total += r->cout;
   m.emb_w_all = c.packed.get<float>((size_t)1280 * m.emb_total);
   m.emb_b_all = c.packed.get<float>(m.emb_total);
   std::vector<float> hb(m.emb_total), t1, t2;
   for (ResBlockW* r : m.resblocks) {
-    SDB_CUDA(cudaMemcpy2DAsync(m.emb_w_all + r->emb_off, (size_t)m.emb_total * 4, mptr(c, r->lin_embed.wi),
+    SDB_CUDA(cudaMemcpy2DAsync(m.emb_w_all + r->emb_off, (size_t)m.emb_total * 4, wsrc(c, r->lin_embed.wi),
                                (size_t)r->cout * 4, (size_t)r->cout * 4, 1280, cudaMemcpyDeviceToDevice, c.stream));
     t1.resize(r->cout), t2.resize(r->cout);
     SDB_CUDA(cudaMemcpyAsync(t1.data(), mptr(c, r->lin_embed.bi), r->cout * 4, cudaMemcpyDeviceToHost, c.stream));
@@ -202,6 +176,126 @@ void model_finalize(Ctx& c) {
     for (int i = 0; i < r->cout; ++i) hb[r->emb_off + i] = t1[i] + t2[i];
   }
   SDB_CUDA(cudaMemcpyAsync(m.emb_b_all, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice, c.stream));
+}
+static void pack_clip_block(Ctx& c, ClipBlockW& cb) {
+  pack_norm(c, cb.attn_ln), pack_norm(c, cb.mlp_ln);
+  cb.w_qk.p = alloc_half2(c.packed, (size_t)2 * 768 * 768), cb.w_qk.N = 1536, cb.w_qk.K = 768;
+  pack_linear_launch(wsrc(c, cb.query.wi), 768, 768, cb.w_qk.p, 0, c.stream);
+  pack_linear_launch(wsrc(c, cb.key.wi), 768, 768, cb.w_qk.p, 768, c.stream);
+  cb.bias_qk = c.packed.get<float>(1536);
+  SDB_CUDA(cudaMemcpyAsync(cb.bias_qk, mptr(c, cb.query.bi), 768 * 4, cudaMemcpyDeviceToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(cb.bias_qk + 768, mptr(c, cb.key.bi), 768 * 4, cudaMemcpyDeviceToDevice, c.stream));
+  pack_lin(c, cb.value), pack_lin(c, cb.out), pack_lin(c, cb.fc1), pack_lin(c, cb.fc2);
+  // softmax rows sum to one, so P.(V + 1 b_v^T) = P.V + b_v^T: fold the value bias into the out-projection bias
+  cb.bias_out = c.packed.get<float>(768);
+  gemv_launch(mptr(c, cb.value.bi), wsrc(c, cb.out.wi), mptr(c, cb.out.bi), 768, 768, cb.bias_out, c.stream);
+}
+
+static void pack_unit(Ctx& c, PackUnit& u) {
+  switch (u.kind) {
+    case U_RES:
+      pack_resblock(c, *u.res, u.passes);
+      break;
+    case U_ST:
+      pack_st(c, *u.st, u.passes);
+      break;
+    case U_CONV:
+    case U_UP:
+      pack_conv(c, *u.conv, /*up2=*/u.kind == U_UP);
+      if (u.passes) u.conv->passes = u.passes;
+      break;
+    case U_EMB:
+      pack_emb(c);
+      break;
+    case U_CLIP:
+      pack_clip_block(c, *u.clip);
+      break;
+  }
+}
+
+// The packing units in finalize order and the LoRA target -> unit map (DESIGN §7 f8), built once from the weight tree.
+static void build_units(Model& m) {
+  if (!m.units.empty()) return;
+  auto add = [&](PackUnit u, std::initializer_list<int> targets) {
+    for (int t : targets)
+      if (t >= 0) m.lora_target[t] = (int)m.units.size();
+    m.units.push_back(u);
+  };
+  auto res = [&](ResBlockW& r, int p) {
+    PackUnit u;
+    u.kind = U_RES, u.res = &r, u.passes = p;
+    add(u, {r.conv_in.wi, r.conv_out.wi, r.has_skip ? r.skip.wi : -1});
+  };
+  auto st = [&](SpatialTransformerW& s, int p) {
+    PackUnit u;
+    u.kind = U_ST, u.st = &s, u.passes = p;
+    add(u, {s.proj_in.wi, s.proj_out.wi, s.attn1.query.wi, s.attn1.key.wi, s.attn1.value.wi, s.attn1.out.wi, s.attn2.query.wi,
+            s.attn2.key.wi, s.attn2.value.wi, s.attn2.out.wi, s.geglu.wi, s.ff.wi});
+  };
+  auto block = [&](UNetBlockW& b) {
+    const int p = g_level_passes[std::min(b.level, 3)];
+    PackUnit u;
+    u.conv = &b.conv;
+    switch (b.kind) {
+      case BK_CONV:  // unet/input_blocks/conv runs on CUDA cores from the master arena: no packed copy, not a target
+        u.kind = U_CONV;
+        add(u, {});
+        break;
+      case BK_DOWN:
+        u.kind = U_CONV, u.passes = p;
+        add(u, {b.conv.wi});
+        break;
+      case BK_R:
+        res(b.res, p);
+        break;
+      case BK_RT:
+        res(b.res, p), st(b.st, p);
+        break;
+      case BK_RU:
+      case BK_RTU:
+        res(b.res, p);
+        if (b.kind == BK_RTU) st(b.st, p);
+        u.kind = U_UP, u.passes = g_level_passes[std::max(b.level - 1, 0)];  // the conv runs at the upsampled resolution
+        add(u, {b.conv.wi});
+        break;
+    }
+  };
+  for (auto& b : m.in_blocks) block(b);
+  res(m.mid_res1, g_level_passes[3]), st(m.mid_st, g_level_passes[3]), res(m.mid_res2, g_level_passes[3]);
+  for (auto& b : m.out_blocks) block(b);
+  m.unit_emb = (int)m.units.size();
+  PackUnit e;
+  e.kind = U_EMB;
+  m.units.push_back(e);
+  for (ResBlockW* r : m.resblocks) m.lora_target[r->lin_embed.wi] = m.unit_emb;
+  for (ClipBlockW& cb : m.clip.blocks) {
+    PackUnit u;
+    u.kind = U_CLIP, u.clip = &cb;
+    add(u, {cb.query.wi, cb.key.wi, cb.value.wi, cb.out.wi, cb.fc1.wi, cb.fc2.wi});
+  }
+}
+
+static void run_unit(Ctx& c, PackUnit& u) {
+  u.off0 = c.packed.off;
+  pack_unit(c, u);
+  u.off1 = c.packed.off;
+}
+
+static void lora_merge_all(Ctx& c);
+
+void model_finalize(Ctx& c) {
+  Model& m = M(c);
+  model_invalidate_graphs(c);
+  build_units(m);
+  lora_merge_all(c);  // W_eff of every tensor with an active adapter term, on the current base
+  c.packed.reset();
+  SDB_CUDA(cudaMemsetAsync(c.packed.base, 0, c.packed.cap, c.stream));  // head-pad rows must be zero
+  // ---- UNet
+  m.lin1_time.bias = mptr(c, m.lin1_time.bi), m.lin2_time.bias = mptr(c, m.lin2_time.bi);
+  for (int i = 0; i < m.unit_emb; ++i) run_unit(c, m.units[i]);
+  pack_norm(c, m.norm_out);
+  pack_conv(c, m.conv_out);
+  run_unit(c, m.units[m.unit_emb]);
   // ---- VAE decoder
   pack_conv(c, m.post_quant), pack_conv(c, m.vae_conv_in), pack_conv(c, m.vae_conv_out);
   pack_resnet(c, m.mid_block1, g_vae_passes_lowres), pack_resnet(c, m.mid_block2, g_vae_passes_lowres);
@@ -232,19 +326,7 @@ void model_finalize(Ctx& c) {
     pack_norm(c, e.norm_out);
   }
   // ---- CLIP text encoder
-  for (ClipBlockW& cb : m.clip.blocks) {
-    pack_norm(c, cb.attn_ln), pack_norm(c, cb.mlp_ln);
-    cb.w_qk.p = alloc_half2(c.packed, (size_t)2 * 768 * 768), cb.w_qk.N = 1536, cb.w_qk.K = 768;
-    pack_linear_launch(mptr(c, cb.query.wi), 768, 768, cb.w_qk.p, 0, c.stream);
-    pack_linear_launch(mptr(c, cb.key.wi), 768, 768, cb.w_qk.p, 768, c.stream);
-    cb.bias_qk = c.packed.get<float>(1536);
-    SDB_CUDA(cudaMemcpyAsync(cb.bias_qk, mptr(c, cb.query.bi), 768 * 4, cudaMemcpyDeviceToDevice, c.stream));
-    SDB_CUDA(cudaMemcpyAsync(cb.bias_qk + 768, mptr(c, cb.key.bi), 768 * 4, cudaMemcpyDeviceToDevice, c.stream));
-    pack_lin(c, cb.value), pack_lin(c, cb.out), pack_lin(c, cb.fc1), pack_lin(c, cb.fc2);
-    // softmax rows sum to one, so P.(V + 1 b_v^T) = P.V + b_v^T: fold the value bias into the out-projection bias
-    cb.bias_out = c.packed.get<float>(768);
-    gemv_launch(mptr(c, cb.value.bi), mptr(c, cb.out.wi), mptr(c, cb.out.bi), 768, 768, cb.bias_out, c.stream);
-  }
+  for (size_t i = m.unit_emb + 1; i < m.units.size(); ++i) run_unit(c, m.units[i]);
   pack_norm(c, m.clip.ln_final);
   // ---- schedule
   m.alphas_host.resize(1000);
@@ -260,6 +342,256 @@ void model_invalidate_graphs(Ctx& c) {
   for (auto& g : m.graphs)
     if (g.exec) cudaGraphExecDestroy(g.exec);
   m.graphs.clear();
+}
+
+// ================================================================================ LoRA adapters (DESIGN §7 f8)
+struct ActiveTerm {
+  const LoraTerm* t;
+  float s;
+};
+using ActiveMap = std::unordered_map<int, std::vector<ActiveTerm>>;
+// tensor -> its active terms in accumulation order (adapters by ascending id, terms in the order they were added)
+static ActiveMap lora_active(const Model& m) {
+  ActiveMap out;
+  for (const auto& a : m.lora.adapters) {
+    if (a.second.multiplier == 0.0) continue;
+    for (const LoraTerm& t : a.second.terms) out[t.tensor].push_back({&t, (float)(a.second.multiplier * t.alpha / t.rank)});
+  }
+  return out;
+}
+static std::vector<std::pair<uint64_t, float>> lora_sig(const ActiveMap& act, int tensor) {
+  std::vector<std::pair<uint64_t, float>> s;
+  auto it = act.find(tensor);
+  if (it != act.end())
+    for (const ActiveTerm& a : it->second) s.push_back({a.t->serial, a.s});
+  return s;
+}
+// out (rows, cols) of a target weight as stored, and its fan-in
+static void lora_geometry(const TensorInfo& t, int& rows, int& cols, int& out, int& fan_in, bool& lin) {
+  lin = t.kind == K_LIN_W;
+  rows = (int)t.dims[0], cols = (int)(t.count / t.dims[0]);
+  out = lin ? cols : rows, fan_in = lin ? rows : cols;
+}
+
+// Tensors whose active terms differ from what was last merged (a term added, removed or rescaled), ascending.
+static std::vector<int> lora_changed(const LoraState& L, const ActiveMap& act) {
+  std::vector<int> cand;
+  for (auto& a : act) cand.push_back(a.first);
+  for (auto& a : L.applied)
+    if (!act.count(a.first)) cand.push_back(a.first);
+  std::sort(cand.begin(), cand.end());
+  std::vector<int> changed;
+  for (int t : cand) {
+    auto ap = L.applied.find(t);
+    if (ap == L.applied.end() || ap->second != lora_sig(act, t)) changed.push_back(t);
+  }
+  return changed;
+}
+
+// Writes W_eff of `tensors` in one lora_merge_launch into their buffers (allocated by lora_add, so nothing is allocated here) and
+// returns after the device has finished; only then are the merged tensors pointed at their W_eff. A tensor without an active term
+// drops its W_eff: the packers then read the base. The caller records `applied` once the packing has been updated too.
+static void lora_merge(Ctx& c, const std::vector<int>& tensors, const ActiveMap& act) {
+  LoraState& L = M(c).lora;
+  std::vector<LoraTensorDesc> td;
+  std::vector<LoraTermDesc> tt;
+  std::vector<int> merged;
+  long long tiles = 0;
+  for (int idx : tensors) {
+    auto it = act.find(idx);
+    if (it == act.end()) continue;
+    const TensorInfo& ti = c.tensors[idx];
+    LoraTensorDesc d;
+    int o, f;
+    bool lin;
+    lora_geometry(ti, d.rows, d.cols, o, f, lin);
+    d.base = mptr(c, idx), d.out = L.buf.at(idx), d.transposed = lin;
+    d.term0 = (int)tt.size(), d.nterms = (int)it->second.size();
+    d.tiles_c = (d.cols + 63) / 64;
+    d.tile0 = tiles;
+    tiles += (long long)((d.rows + 63) / 64) * d.tiles_c;
+    for (const ActiveTerm& a : it->second) tt.push_back({a.t->down, a.t->up, a.t->rank, a.s});
+    td.push_back(d);
+    merged.push_back(idx);
+  }
+  if (!td.empty()) {
+    SDB_CUDA(cudaStreamSynchronize(c.stream));  // the tables live in the work arena
+    c.work.reset();
+    LoraTensorDesc* d_td = c.work.get<LoraTensorDesc>(td.size());
+    LoraTermDesc* d_tt = c.work.get<LoraTermDesc>(tt.size());
+    SDB_CUDA(cudaMemcpyAsync(d_td, td.data(), td.size() * sizeof(LoraTensorDesc), cudaMemcpyHostToDevice, c.stream));
+    SDB_CUDA(cudaMemcpyAsync(d_tt, tt.data(), tt.size() * sizeof(LoraTermDesc), cudaMemcpyHostToDevice, c.stream));
+    lora_merge_launch(d_td, (int)td.size(), d_tt, tiles, c.stream);
+    SDB_CUDA(cudaStreamSynchronize(c.stream));
+    c.work.reset();
+  }
+  for (int idx : tensors) L.eff.erase(idx);
+  for (int idx : merged) L.eff[idx] = L.buf.at(idx);
+}
+static void lora_record(LoraState& L, const std::vector<int>& tensors, const ActiveMap& act) {
+  for (int idx : tensors) {
+    auto s = lora_sig(act, idx);
+    if (s.empty())
+      L.applied.erase(idx);
+    else
+      L.applied[idx] = std::move(s);
+  }
+}
+
+static void lora_merge_all(Ctx& c) {
+  LoraState& L = M(c).lora;
+  const ActiveMap act = lora_active(M(c));
+  std::vector<int> ts;
+  for (auto& a : act) ts.push_back(a.first);
+  for (auto& e : L.eff)
+    if (!act.count(e.first)) ts.push_back(e.first);
+  for (auto& a : L.applied)
+    if (!act.count(a.first)) ts.push_back(a.first);
+  std::sort(ts.begin(), ts.end());
+  ts.erase(std::unique(ts.begin(), ts.end()), ts.end());
+  lora_merge(c, ts, act);
+  lora_record(L, ts, act);
+  L.pending = false;
+}
+
+// `pending` is set by every add / scale / remove; whether anything really differs from what was merged is settled here, so an add
+// undone by a remove leaves nothing pending.
+bool model_lora_pending(Ctx& c) {
+  LoraState& L = M(c).lora;
+  if (L.pending && lora_changed(L, lora_active(M(c))).empty()) L.pending = false;
+  return L.pending;
+}
+
+void model_lora_add(Ctx& c, int adapter, const char* tensor, int rank, const float* down, const float* up, double alpha) {
+  Model& m = M(c);
+  build_units(m);
+  char msg[512];
+  snprintf(msg, sizeof(msg), "lora_add: adapter %d must be >= 0", adapter);
+  SDB_CHECK(adapter >= 0, msg);
+  SDB_CHECK(tensor, "lora_add: tensor is NULL");
+  auto it = c.index.find(tensor);
+  snprintf(msg, sizeof(msg), "lora_add: unknown tensor '%s'", tensor);
+  SDB_CHECK(it != c.index.end(), msg);
+  const int idx = it->second;
+  snprintf(msg, sizeof(msg),
+           "lora_add: tensor '%s' is not a LoRA target (targets: the packed UNet ResBlock, SpatialTransformer and resample "
+           "weights and the CLIP attention / MLP weights; not norms, biases, embeddings, the VAE, unet/input_blocks/conv, "
+           "unet/lin{1,2}_time_embed or unet/conv_out)", tensor);
+  SDB_CHECK(m.lora_target.count(idx), msg);
+  snprintf(msg, sizeof(msg), "lora_add: rank %d must be >= 1", rank);
+  SDB_CHECK(rank >= 1, msg);
+  SDB_CHECK(down, "lora_add: down is NULL");
+  SDB_CHECK(up, "lora_add: up is NULL");
+  snprintf(msg, sizeof(msg), "lora_add: alpha %.17g must be finite and > 0", alpha);
+  SDB_CHECK(std::isfinite(alpha) && alpha > 0.0, msg);
+  auto ad = m.lora.adapters.find(adapter);
+  if (ad != m.lora.adapters.end())
+    for (const LoraTerm& t : ad->second.terms) {
+      snprintf(msg, sizeof(msg), "lora_add: adapter %d already has a term for '%s'", adapter, tensor);
+      SDB_CHECK(t.tensor != idx, msg);
+    }
+  int rows, cols, out, fan_in;
+  bool lin;
+  lora_geometry(c.tensors[idx], rows, cols, out, fan_in, lin);
+  LoraTerm t;
+  t.tensor = idx, t.rank = rank, t.alpha = alpha;
+  // the tensor's W_eff buffer is allocated with its first term and kept until no term targets it, so that neither an apply
+  // nor a scale to 0 and back allocates or frees device memory (each cudaMalloc / cudaFree synchronises the device)
+  float* wbuf = nullptr;
+  const bool new_buf = !m.lora.buf.count(idx);
+  try {
+    SDB_CUDA(cudaMalloc(&t.down, (size_t)rank * fan_in * sizeof(float)));
+    SDB_CUDA(cudaMalloc(&t.up, (size_t)out * rank * sizeof(float)));
+    if (new_buf) SDB_CUDA(cudaMalloc(&wbuf, c.tensors[idx].count * sizeof(float)));
+    SDB_CUDA(cudaMemcpy(t.down, down, (size_t)rank * fan_in * sizeof(float), cudaMemcpyHostToDevice));
+    SDB_CUDA(cudaMemcpy(t.up, up, (size_t)out * rank * sizeof(float), cudaMemcpyHostToDevice));
+  } catch (...) {
+    cudaFree(t.down), cudaFree(t.up), cudaFree(wbuf);
+    throw;
+  }
+  if (new_buf) m.lora.buf[idx] = wbuf;
+  t.serial = m.lora.next_serial++;
+  m.lora.adapters[adapter].terms.push_back(t);
+  m.lora.pending = true;
+}
+
+void model_lora_scale(Ctx& c, int adapter, double multiplier) {
+  LoraState& L = M(c).lora;
+  char msg[160];
+  auto it = L.adapters.find(adapter);
+  snprintf(msg, sizeof(msg), "lora_scale: no adapter %d", adapter);
+  SDB_CHECK(it != L.adapters.end(), msg);
+  snprintf(msg, sizeof(msg), "lora_scale: multiplier %.17g must be finite", multiplier);
+  SDB_CHECK(std::isfinite(multiplier), msg);
+  it->second.multiplier = multiplier;
+  L.pending = true;
+}
+
+void model_lora_remove(Ctx& c, int adapter) {
+  LoraState& L = M(c).lora;
+  char msg[160];
+  snprintf(msg, sizeof(msg), "lora_remove: no adapter %d (-1 removes all)", adapter);
+  SDB_CHECK(adapter == -1 || L.adapters.count(adapter), msg);
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  for (auto it = L.adapters.begin(); it != L.adapters.end();) {
+    if (adapter != -1 && it->first != adapter) {
+      ++it;
+      continue;
+    }
+    for (LoraTerm& t : it->second.terms) cudaFree(t.down), cudaFree(t.up);
+    it = L.adapters.erase(it);
+  }
+  std::unordered_set<int> targeted;
+  for (const auto& a : L.adapters)
+    for (const LoraTerm& t : a.second.terms) targeted.insert(t.tensor);
+  for (auto it = L.buf.begin(); it != L.buf.end();) {
+    if (targeted.count(it->first)) {
+      ++it;
+      continue;
+    }
+    L.eff.erase(it->first);  // its packing is re-made from the base by the next apply or finalize
+    cudaFree(it->second);
+    it = L.buf.erase(it);
+  }
+  L.pending = true;
+}
+
+void model_lora_apply(Ctx& c) {
+  Model& m = M(c);
+  build_units(m);
+  SDB_CUDA(cudaStreamSynchronize(c.stream));  // nothing queued may still read the packed weights about to be rewritten
+  const ActiveMap act = lora_active(m);
+  const std::vector<int> changed = lora_changed(m.lora, act);
+  lora_merge(c, changed, act);
+  if (c.finalized) {
+    // re-run the packing unit of every changed tensor into its own packed addresses; the step graphs captured those addresses
+    // and stay valid. Head-pad rows are never written by the packers and stay zero.
+    std::vector<int> units;
+    for (int t : changed) units.push_back(m.lora_target.at(t));
+    std::sort(units.begin(), units.end());
+    units.erase(std::unique(units.begin(), units.end()), units.end());
+    const size_t off = c.packed.off;
+    for (int ui : units) {
+      PackUnit& u = m.units[ui];
+      c.packed.off = u.off0;
+      pack_unit(c, u);
+      SDB_CHECK(c.packed.off == u.off1, "lora_apply: a re-packed unit did not end where finalize left it");
+    }
+    c.packed.off = off;
+    SDB_CUDA(cudaStreamSynchronize(c.stream));
+    c.work.reset();
+  }
+  lora_record(m.lora, changed, act);  // only now: a failure above leaves these tensors changed for the next apply
+  m.lora.pending = false;
+}
+
+void model_get_merged_tensor(Ctx& c, const char* tensor, float* host, int64_t count) {
+  SDB_CHECK(tensor && host, "get_merged_tensor: null argument");
+  const TensorInfo& t = c.info(tensor);
+  SDB_CHECK(count == t.count, "get_merged_tensor: element count mismatch");
+  SDB_CHECK(!model_lora_pending(c), "get_merged_tensor: adapter changes are pending: call sdb_lora_apply first");
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  SDB_CUDA(cudaMemcpy(host, wsrc(c, c.index.at(tensor)), t.count * sizeof(float), cudaMemcpyDeviceToHost));
 }
 
 // ================================================================================ forward helpers

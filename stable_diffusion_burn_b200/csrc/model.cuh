@@ -10,6 +10,13 @@ void model_destroy(Ctx& c);
 void model_init_synthetic(Ctx& c, uint32_t seed);
 void model_finalize(Ctx& c);  // packs weights into kernel layouts
 void model_invalidate_graphs(Ctx& c);
+// LoRA adapters (DESIGN §7 f8; include/sdb200.h: sdb_lora_*)
+void model_lora_add(Ctx& c, int adapter, const char* tensor, int rank, const float* down, const float* up, double alpha);
+void model_lora_scale(Ctx& c, int adapter, double multiplier);
+void model_lora_remove(Ctx& c, int adapter);  // -1 = all
+void model_lora_apply(Ctx& c);
+bool model_lora_pending(Ctx& c);
+void model_get_merged_tensor(Ctx& c, const char* tensor, float* host, int64_t count);
 
 void model_unet_forward_host(Ctx& c, const float* x, int t, const float* context, int n, int H, int W, int L, float* out);
 void model_unet_forward_dev(Ctx& c, const float* d_x, int t, const float* d_context, int n, int H, int W, int L,

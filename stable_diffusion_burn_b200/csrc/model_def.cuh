@@ -1,6 +1,7 @@
 // model_def.cuh — weight tree of the hot path. Tensor names are the reference's dump-dir paths
 // (src/model/unet/load.rs:213-306, src/model/autoencoder/load.rs:16-198).
 #pragma once
+#include <map>
 #include <memory>
 
 #include "runtime.cuh"
@@ -116,6 +117,46 @@ struct ClipW {
   NormW ln_final;
 };
 
+// One packing unit of model_finalize: what sdb_lora_apply re-packs, in place, when one of its weights changes (DESIGN §7 f8).
+// off0 / off1: the packed arena offsets at the unit's start and end, recorded by the last finalize.
+enum PackUnitKind : int { U_RES = 0, U_ST, U_CONV, U_UP, U_EMB, U_CLIP };
+struct PackUnit {
+  int kind = U_RES;
+  ResBlockW* res = nullptr;
+  SpatialTransformerW* st = nullptr;
+  ConvW* conv = nullptr;
+  ClipBlockW* clip = nullptr;
+  int passes = 0;  // U_CONV / U_UP: the conv's pass count (0 = left as it is)
+  size_t off0 = 0, off1 = 0;
+};
+
+// LoRA adapters of a context (DESIGN §7 f8). Factors and effective weights live in their own device allocations, outside the
+// master, packed and work arenas.
+struct LoraTerm {
+  int tensor = -1, rank = 0;
+  float* down = nullptr;  // device [rank][fan-in]
+  float* up = nullptr;    // device [out][rank]
+  double alpha = 0.0;
+  uint64_t serial = 0;    // unique per added term: a removed and re-added term counts as a change
+};
+struct LoraAdapter {
+  double multiplier = 1.0;
+  std::vector<LoraTerm> terms;  // in the order they were added
+};
+struct LoraState {
+  std::map<int, LoraAdapter> adapters;               // ascending id = accumulation order
+  std::unordered_map<int, float*> buf;               // tensor -> W_eff buffer (device), while any term targets the tensor
+  std::unordered_map<int, float*> eff;               // tensor -> its buf, for tensors with an active term as of the last merge
+  std::unordered_map<int, std::vector<std::pair<uint64_t, float>>> applied;  // tensor -> (term serial, scale) merged into eff
+  uint64_t next_serial = 1;
+  bool pending = false;  // an add / scale / remove since the last apply or finalize (model_lora_pending settles it)
+  ~LoraState() {
+    for (auto& a : adapters)
+      for (LoraTerm& t : a.second.terms) cudaFree(t.down), cudaFree(t.up);
+    for (auto& e : buf) cudaFree(e.second);
+  }
+};
+
 struct Model {
   ClipW clip;
   EncoderW enc;
@@ -147,6 +188,11 @@ struct Model {
     void* io[8];
   };
   std::vector<GraphEntry> graphs;
+  // packing units in finalize order: the UNet blocks, then the time-embedding table (unit_emb), then the CLIP blocks
+  std::vector<PackUnit> units;
+  int unit_emb = -1;
+  std::unordered_map<int, int> lora_target;  // LoRA target tensor -> index of the unit that packs it
+  LoraState lora;
 };
 
 }  // namespace sdb

@@ -95,6 +95,39 @@ class StableDiffusion:
         self.ctx.finalize_weights()
         return self
 
+    # ---- LoRA adapters (an extension, DESIGN.md §7 f8): merged into the packed weights, shared by every sample of a call
+    def load_lora(self, path, adapter: int, multiplier: float = 1.0):
+        """Reads a kohya or diffusers/PEFT .safetensors LoRA file into adapter id `adapter` (>= 0, not in use) and applies it."""
+        from .lora import lora_terms, read_safetensors
+        if int(adapter) in self.ctx.lora_adapters():
+            raise ValueError(f"load_lora: adapter {adapter} is in use: unload_lora({adapter}) first or pick another id")
+        terms = lora_terms(read_safetensors(path))
+        if not terms:
+            raise ValueError(f"{path}: no LoRA terms")
+        try:
+            for reg, down, up, alpha in terms:
+                self.ctx.lora_add(adapter, reg, down, up, alpha)
+            self.ctx.lora_scale(adapter, multiplier)
+        except Exception:
+            # the adapter is new: removing it undoes every add, and nothing else that is pending gets applied
+            if int(adapter) in self.ctx.lora_adapters():
+                self.ctx.lora_remove(adapter)
+            raise
+        self.ctx.lora_apply()
+        return self
+
+    def set_lora_scale(self, adapter: int, multiplier: float):
+        """Rescales a loaded adapter (0 disables it and keeps it loaded) and applies the change."""
+        self.ctx.lora_scale(adapter, multiplier)
+        self.ctx.lora_apply()
+        return self
+
+    def unload_lora(self, adapter: int = -1):
+        """Removes one adapter (-1: all) and applies the change."""
+        self.ctx.lora_remove(adapter)
+        self.ctx.lora_apply()
+        return self
+
     # ---- hot path
     # sampler / eta / noise_seed (an extension, DESIGN.md §7 f6): "ddim" (eta in [0, 1]; eta = 0 is the reference's sampler) or
     # "dpmpp_2m" (DPM-Solver++(2M), eta = 0). They hold for the one call; the context's default sampler is restored after it.

@@ -141,6 +141,24 @@ def realistic_stats(params: dict, seed: int = 7) -> dict:
     return out
 
 
+def make_lora(targets, rank: int, seed: int = 0, alpha=None) -> list:
+    """A seeded synthetic LoRA adapter (DESIGN.md §7 f8): for each registry weight name in `targets`, counter-hash factors
+    down [rank][fan-in] ~ U(-1, 1) and up [out][rank] ~ U(-1, 1) * b, with b chosen so that the RMS of s (up . down) is about
+    0.3 of the synthetic weight's RMS (1 / sqrt(fan-in)). alpha defaults to rank (s = 1). -> [(name, down, up, alpha)]."""
+    shapes = {n: (s, k) for n, s, k, _ in topology.all_params()}
+    out = []
+    for name in targets:
+        shape, kind = shapes[name]
+        o, f = (shape[1], shape[0]) if kind == "lin_w" else (shape[0], int(np.prod(shape[1:])))
+        a = float(rank if alpha is None else alpha)
+        s = a / rank
+        b = np.float32(0.3 * 3.0 / (math.sqrt(rank) * math.sqrt(f) * s))  # RMS(up.down) = sqrt(r) * (1/sqrt3) * (b/sqrt3)
+        down = (uniform01(name + "#lora_down", rank * f, seed) * np.float32(2.0) - np.float32(1.0)).reshape(rank, f)
+        up = ((uniform01(name + "#lora_up", o * rank, seed) * np.float32(2.0) - np.float32(1.0)) * b).reshape(o, rank)
+        out.append((name, down.astype(np.float32), up.astype(np.float32), a))
+    return out
+
+
 # ---------------------------------------------------------------- inputs ----
 def make_latent(n: int, h: int, w: int, seed: int = 1234) -> np.ndarray:
     """N(0,1) init latent [n,4,h,w]; image i uses stream seed+i (SURVEY §8d)."""
