@@ -33,6 +33,12 @@ typedef struct sdb_ctx sdb_ctx;
 /* Replaces device selection + StableDiffusionConfig::init (src/bin/sample/main.rs:59-83,
  * src/model/stablediffusion/mod.rs:22-39). */
 int sdb_create(int device, sdb_ctx** out);
+/* A context for an inpainting checkpoint (SD-1.5-inpainting and the like; DESIGN.md §7 f9). Its registry is sdb_create's except
+ * unet/input_blocks/conv/weight, [320,9,3,3] (and its n_channels_in 9): the UNet reads cat(latent, latent mask, masked-image
+ * latent). On such a context sdb_img2img[_dev] and sdb_img2img_batch[_dev] need the mask and condition the UNet on it with no
+ * blend; sdb_unet_forward[_dev] and sdb_forward_diffuser[_dev] take x / latent [n,9,H,W] and return [n,4,H,W]; the text-to-image
+ * entries fail (use sdb_img2img with an all-255 mask at strength 1). Loading a conv_in of the other width fails. */
+int sdb_create_inpaint(int device, sdb_ctx** out);
 int sdb_destroy(sdb_ctx* ctx);
 /* ctx may be NULL: returns the last error of the calling thread (e.g. a failed sdb_create). */
 const char* sdb_last_error(sdb_ctx* ctx);
@@ -132,7 +138,11 @@ int sdb_encode_image_dev(sdb_ctx* ctx, const float* d_img, int n, int H, int W, 
  * weight per latent cell, w = (sum of the 8x8 block) / (64*255), and after every step x = w x + (1-w) (sqrt(a_prev) z0 +
  * sqrt(1 - a_prev) noise), so the kept region ends as exactly z0. noise [n,4,H,W]; NULL = the N(0,1) stream keyed by `seed`
  * that sdb_sample_image starts from. Outputs: latent_out [n,4,H,W] and / or rgb_out [n,8H,8W,3]; at least one must be set.
- * H, W are latent sizes with the constraints of sampling (multiples of 8, (H/8)*(W/8) a multiple of 8). */
+ * H, W are latent sizes with the constraints of sampling (multiples of 8, (H/8)*(W/8) a multiple of 8).
+ * On a 9-channel context (sdb_create_inpaint; DESIGN.md §7 f9) the mask is required and binary, m = (mask >= 128); the masked
+ * image x_m = m ? 0 : x gives z_m = 0.18215 * encode_image(x_m), the latent mask is the nearest pick m[8h][8w], and both CFG
+ * halves of every UNet pass read cat(x_t, latent mask, z_m). The start latent and the strength rule are the above, z0 from the
+ * unmasked image; each step is the sampler's update with no blend. */
 int sdb_img2img(sdb_ctx* ctx, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
                 const float* uncond, int Lu, double guidance_scale, int n_steps, const float* noise, uint64_t seed, int H, int W,
                 float* latent_out, uint8_t* rgb_out);

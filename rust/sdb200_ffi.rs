@@ -39,6 +39,7 @@ pub struct SdbBatch {
 
 extern "C" {
     fn sdb_create(device: c_int, out: *mut *mut SdbCtx) -> c_int;
+    fn sdb_create_inpaint(device: c_int, out: *mut *mut SdbCtx) -> c_int;
     fn sdb_destroy(ctx: *mut SdbCtx) -> c_int;
     fn sdb_last_error(ctx: *mut SdbCtx) -> *const c_char;
     fn sdb_set_tensor(ctx: *mut SdbCtx, name: *const c_char, host: *const f32, dims: *const i64, ndim: c_int) -> c_int;
@@ -110,6 +111,17 @@ impl StableDiffusion {
     pub fn new(device: i32) -> Result<Self, SdbError> {
         let mut ctx = std::ptr::null_mut();
         let rc = unsafe { sdb_create(device, &mut ctx) };
+        if rc != 0 {
+            return Err(SdbError(unsafe { CStr::from_ptr(sdb_last_error(std::ptr::null_mut())) }.to_string_lossy().into()));
+        }
+        Ok(Self { ctx })
+    }
+
+    /// A context for an inpainting checkpoint: a 9-channel `conv_in` reading latent | mask | masked-image latent (DESIGN.md §7 f9).
+    /// `img2img` then needs the mask; the text-to-image calls fail.
+    pub fn new_inpaint(device: i32) -> Result<Self, SdbError> {
+        let mut ctx = std::ptr::null_mut();
+        let rc = unsafe { sdb_create_inpaint(device, &mut ctx) };
         if rc != 0 {
             return Err(SdbError(unsafe { CStr::from_ptr(sdb_last_error(std::ptr::null_mut())) }.to_string_lossy().into()));
         }

@@ -32,6 +32,7 @@ _batchp = C.POINTER(SdbBatch)
 # (name, restype, argtypes) — every symbol declared in include/sdb200.h
 SIGNATURES = [
     ("sdb_create", C.c_int, [C.c_int, C.POINTER(_ctx)]),
+    ("sdb_create_inpaint", C.c_int, [C.c_int, C.POINTER(_ctx)]),
     ("sdb_destroy", C.c_int, [_ctx]),
     ("sdb_last_error", C.c_char_p, [_ctx]),
     ("sdb_version", C.c_char_p, []),
@@ -205,12 +206,12 @@ def batch_struct(b, context_ptr=None, uncond_ptr=None):
 
 
 class Context:
-    """Owns one sdb_ctx (one CUDA device)."""
+    """Owns one sdb_ctx (one CUDA device). inpaint=True: a 9-channel inpainting UNet (sdb_create_inpaint, DESIGN.md §7 f9)."""
 
-    def __init__(self, device: int = 0):
+    def __init__(self, device: int = 0, inpaint: bool = False):
         self.lib = load()
         h = _ctx()
-        rc = self.lib.sdb_create(device, C.byref(h))
+        rc = (self.lib.sdb_create_inpaint if inpaint else self.lib.sdb_create)(device, C.byref(h))
         if rc != 0:
             raise SdbError(self.lib.sdb_last_error(None).decode())
         self.h = h
@@ -241,6 +242,12 @@ class Context:
             self.check(self.lib.sdb_tensor_info(self.h, i, C.byref(name), dims, C.byref(nd)))
             out.append((name.value.decode(), tuple(int(dims[j]) for j in range(nd.value))))
         return out
+
+    def unet_in_channels(self) -> int:
+        """4, or 9 on an inpainting context: read from the registry's unet/input_blocks/conv/weight."""
+        if getattr(self, "_cin", None) is None:
+            self._cin = next(s[1] for n, s in self.tensor_list() if n == "unet/input_blocks/conv/weight")
+        return self._cin
 
     def set_tensor(self, name, arr):
         a = f32(arr)
@@ -320,18 +327,24 @@ class Context:
 
     # ---- hot path (host buffers)
     def unet_forward(self, x, t, context):
+        """x [n,4,H,W] ([n,9,H,W] = latent | mask | masked-image latent on an inpainting context) -> [n,4,H,W]."""
         x = f32(x); context = f32(context)
-        n, _, H, W = x.shape
+        n, ch, H, W = x.shape
+        if ch != self.unet_in_channels():
+            raise ValueError(f"x has {ch} channels; this context's UNet takes {self.unet_in_channels()}")
         L = context.shape[1]
-        out = np.empty_like(x)
+        out = np.empty((n, 4, H, W), np.float32)
         self.check(self.lib.sdb_unet_forward(self.h, ptr(x), int(t), ptr(context), n, H, W, L, ptr(out)))
         return out
 
     def forward_diffuser(self, latent, t, context, uncond, scale):
-        """-> (pred, uncond UNet output, cond UNet output), each [n,4,H,W]."""
+        """latent [n,4,H,W] ([n,9,H,W] on an inpainting context) -> (pred, uncond UNet output, cond UNet output), each
+        [n,4,H,W]."""
         latent = f32(latent); context = f32(context); uncond = f32(uncond)
-        n, _, H, W = latent.shape
-        outs = [np.empty_like(latent) for _ in range(3)]
+        n, ch, H, W = latent.shape
+        if ch != self.unet_in_channels():
+            raise ValueError(f"latent has {ch} channels; this context's UNet takes {self.unet_in_channels()}")
+        outs = [np.empty((n, 4, H, W), np.float32) for _ in range(3)]
         self.check(self.lib.sdb_forward_diffuser(self.h, ptr(latent), int(t), ptr(context), n, context.shape[1], ptr(uncond),
                                                  uncond.shape[0], float(scale), H, W, ptr(outs[0]), ptr(outs[1]), ptr(outs[2])))
         return tuple(outs)
@@ -406,7 +419,8 @@ class Context:
 
     def img2img(self, image, context, uncond, scale, n_steps, strength, mask=None, noise=None, seed=0, latent=False, rgb=True):
         """Image-to-image / masked inpainting (include/sdb200.h: sdb_img2img). image u8 [n,8H,8W,3]; mask u8 [n,8H,8W]
-        (255 = regenerate, 0 = keep) or None; noise [n,4,H,W] or None (the seeded stream sample_image starts from).
+        (255 = regenerate, 0 = keep) or None; noise [n,4,H,W] or None (the seeded stream sample_image starts from). On an
+        inpainting context the mask is required and binary (>= 128 regenerates) and conditions the UNet instead of a blend.
         -> the latent [n,4,H,W] and / or the u8 image [n,8H,8W,3]: a tuple (latent, rgb) when both are requested."""
         if not (latent or rgb):
             raise ValueError("request the latent, the image or both")
@@ -460,7 +474,8 @@ class Context:
     def img2img_batch(self, image, contexts, unconds, scales, n_steps, strength, mask=None, noise=None, seeds=None,
                       noise_seeds=None, latent=False, rgb=True):
         """n different requests of image-to-image / inpainting in one call (include/sdb200.h: sdb_img2img_batch). image u8
-        [n,8H,8W,3]; mask u8 [n,8H,8W] or None; noise [n,4,H,W] or None (each request's noise from its seed)."""
+        [n,8H,8W,3]; mask u8 [n,8H,8W] or None (required on an inpainting context); noise [n,4,H,W] or None (each request's
+        noise from its seed)."""
         if not (latent or rgb):
             raise ValueError("request the latent, the image or both")
         b = pack_batch(contexts, unconds, scales, seeds, noise_seeds)

@@ -94,7 +94,7 @@ extern "C" {
 
 const char* sdb_version(void) { return "sdb200 0.2.0 sm_90a"; }
 
-int sdb_create(int device, sdb_ctx** out) {
+static int create(int device, int unet_cin, sdb_ctx** out) {
   if (!out) {
     g_err = "null out pointer";
     return 1;
@@ -117,6 +117,7 @@ int sdb_create(int device, sdb_ctx** out) {
     g_num_sms = prop.multiProcessorCount;
     h = new sdb_ctx();
     h->c.device = device;
+    h->c.unet_cin = unet_cin;
     h->c.debug_sync = getenv("SDB_DEBUG_SYNC") && atoi(getenv("SDB_DEBUG_SYNC")) != 0;
     if (getenv("SDB_PDL")) g_pdl_enabled = atoi(getenv("SDB_PDL")) != 0, g_pdl_late = atoi(getenv("SDB_PDL")) == 2;
     SDB_CUDA(cudaStreamCreateWithFlags(&h->c.stream, cudaStreamNonBlocking));
@@ -129,6 +130,10 @@ int sdb_create(int device, sdb_ctx** out) {
     return 1;
   }
 }
+
+int sdb_create(int device, sdb_ctx** out) { return create(device, 4, out); }
+
+int sdb_create_inpaint(int device, sdb_ctx** out) { return create(device, 9, out); }
 
 int sdb_destroy(sdb_ctx* ctx) {
   ctx_teardown(ctx);
@@ -155,6 +160,7 @@ int sdb_set_tensor(sdb_ctx* ctx, const char* name, const float* host, const int6
   API_BEGIN(ctx)
   SDB_CHECK(name && host && dims, "null argument");
   const TensorInfo& t = c.info(name);
+  if (t.name == "unet/input_blocks/conv/weight") check_conv_in_shape(c, "set_tensor", ndim, dims);
   SDB_CHECK(ndim == t.ndim, std::string("rank mismatch for ") + name);
   for (int i = 0; i < ndim; ++i) SDB_CHECK(dims[i] == t.dims[i], std::string("shape mismatch for ") + name);
   SDB_CUDA(cudaMemcpyAsync(c.master_ptr(name), host, t.count * sizeof(float), cudaMemcpyHostToDevice, c.stream));

@@ -93,6 +93,12 @@ void model_load_dump_dir(Ctx& c, const char* root_c) {
   // load_stable_diffusion (src/model/stablediffusion/load.rs:20-21)
   SDB_CHECK(read_scalar(root + "/n_steps.npy", v), "missing file " + root + "/n_steps.npy");
   SDB_CHECK(v == 1000.f, "n_steps must be 1000 (the sampler's schedule length)");
+  // a 4- / 9-channel conv_in that does not fit this context gets a message naming the create entry to use, before the
+  // configuration scalar unet/input_blocks/conv/n_channels_in reports it as a plain topology difference
+  if (npy_read_f32(root + "/unet/input_blocks/conv/weight.npy", buf) && buf.size() >= 4) {
+    const int64_t d[4] = {(int64_t)buf[0], (int64_t)buf[1], (int64_t)buf[2], (int64_t)buf[3]};
+    check_conv_in_shape(c, root, 4, d);
+  }
   // configuration scalars recorded while the registry was built
   for (const MetaCheck& m : c.meta) {
     const std::string file = root + "/" + m.relpath + ".npy";

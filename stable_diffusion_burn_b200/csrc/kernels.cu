@@ -744,6 +744,70 @@ void conv3x3_cin4_launch(const float* x_nchw, int n, int H, int W, const float* 
   SDB_CUDA(cudaGetLastError());
 }
 
+// ============================================================ conv 3x3, Cin = 9: the inpainting UNet's conv_in (DESIGN §7 f9)
+// The conv3x3_cin4 scheme over 81 taps. Channels 0-3 come from x (sample stride xs), channels 4-8 from cond (sample stride cs,
+// sample index modulo cmod: the two CFG halves of a step read one copy). The taps accumulate in OIHW order from the bias, as
+// conv3x3_cin4_kernel does, so zero weights on channels 4-8 give its result bit for bit. Weights [81][Cout] fill 101 KB of shared
+// memory and every CTA stages all of them: PIX output pixels per CTA amortise that staging.
+template <int PIX>
+__global__ void __launch_bounds__(256)
+conv3x3_cin9_kernel(const float* __restrict__ x, long long xs, const float* __restrict__ cond, long long cs, int cmod, int H, int W,
+                    const float* __restrict__ w, const float* __restrict__ b, int Cout, float* __restrict__ y,
+                    __half* __restrict__ y_hi, __half* __restrict__ y_lo) {
+  pdl_enter();
+  extern __shared__ float sm[];
+  float* s_w = sm;                  // [81][Cout]
+  float* s_in = sm + 81 * Cout;     // [PIX][81]
+  const int n = blockIdx.y;
+  const int HW = H * W;
+  const int p0 = blockIdx.x * PIX;
+  for (int i = threadIdx.x; i < 81 * Cout; i += blockDim.x) {
+    const int k = i / Cout, co = i % Cout;  // k = ci*9 + tap (OIHW inner order)
+    s_w[i] = w[(size_t)co * 81 + k];
+  }
+  const float* xn = x + (size_t)n * xs;
+  const float* cn = cond + (size_t)(n % cmod) * cs - (size_t)4 * HW;  // channel ci >= 4 at cn + ci*HW
+  for (int i = threadIdx.x; i < PIX * 81; i += blockDim.x) {
+    const int pl = i / 81, k = i % 81;
+    const int ci = k / 9, tap = k % 9;
+    const int p = p0 + pl;
+    float v = 0.f;
+    if (p < HW) {
+      const int h = p / W + tap / 3 - 1, ww = p % W + tap % 3 - 1;
+      if (h >= 0 && h < H && ww >= 0 && ww < W) v = (ci < 4 ? xn : cn)[(size_t)ci * HW + (size_t)h * W + ww];
+    }
+    s_in[i] = v;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < PIX * Cout; i += blockDim.x) {
+    const int pl = i / Cout, co = i % Cout;
+    const int p = p0 + pl;
+    if (p >= HW) continue;
+    float acc = b ? b[co] : 0.f;
+#pragma unroll 9
+    for (int k = 0; k < 81; ++k) acc += s_in[pl * 81 + k] * s_w[k * Cout + co];
+    const size_t o = ((size_t)n * HW + p) * Cout + co;
+    y[o] = acc;
+    if (y_hi) {
+      const __half h = __float2half_rn(acc);
+      y_hi[o] = h;
+      if (y_lo) y_lo[o] = __float2half_rn(acc - __half2float(h));
+    }
+  }
+}
+void conv3x3_cin9_launch(const float* x, long long x_stride, const float* cond, long long cond_stride, int cond_mod, int n, int H,
+                         int W, const float* w, const float* b, int Cout, float* y, Half2Ptr y16, cudaStream_t st) {
+  constexpr int PIX = kConvCin9Pix;
+  const size_t smem = (size_t)(81 * Cout + PIX * 81) * sizeof(float);
+  static DeviceOnce once;
+  if (once.first())
+    SDB_CUDA(cudaFuncSetAttribute(conv3x3_cin9_kernel<PIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  dim3 grid(ceil_div(H * W, PIX), n);
+  launch_k(conv3x3_cin9_kernel<PIX>, grid, dim3(256), smem, st, x, x_stride, cond, cond_stride, cond_mod, H, W, w, b, Cout, y,
+           y16.hi, y16.lo);
+  SDB_CUDA(cudaGetLastError());
+}
+
 // ============================================================ conv 3x3, Cout <= 8, fused GroupNorm + SiLU (fp32, CUDA cores)
 // The last conv of the UNet (320 -> 4), of the VAE decoder (128 -> 3 at 512x512: 134 MB of input) and of the encoder (512 -> 8).
 // HBM-bound by construction (Cout is tiny), so the kernel is organised around reading x ONCE with wide coalesced loads:
@@ -902,6 +966,31 @@ __global__ void quant_conv_slice_kernel(const float* __restrict__ x, const float
 void quant_conv_slice_launch(const float* x, const float* w, const float* b, int n, int HW, float* y, cudaStream_t st) {
   dim3 grid(std::min(ceil_div(HW, 256), 1024), n);
   quant_conv_slice_kernel<<<grid, 256, 0, st>>>(x, w, b, HW, y);
+  SDB_CUDA(cudaGetLastError());
+}
+
+// quant_conv_slice_kernel writing fl(y * scale) at a per-sample stride: the inpainting path's masked-image latent lands scaled
+// in channels 1-4 of the conditioning tensor [n,5,HW] (ys = 5 HW) in the encoder's own launch
+__global__ void quant_conv_slice_scaled_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
+                                               int HW, long long ys, float scale, float* __restrict__ y) {
+  const int n = blockIdx.y;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += gridDim.x * blockDim.x) {
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = x[((size_t)n * 8 + j) * HW + p];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      float acc = b[c];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc += w[c * 8 + j] * v[j];
+      y[(size_t)n * ys + (size_t)c * HW + p] = __fmul_rn(acc, scale);
+    }
+  }
+}
+void quant_conv_slice_scaled_launch(const float* x, const float* w, const float* b, int n, int HW, long long y_stride, float scale,
+                                    float* y, cudaStream_t st) {
+  dim3 grid(std::min(ceil_div(HW, 256), 1024), n);
+  quant_conv_slice_scaled_kernel<<<grid, 256, 0, st>>>(x, w, b, HW, y_stride, scale, y);
   SDB_CUDA(cudaGetLastError());
 }
 
@@ -1261,6 +1350,39 @@ void img2img_prep_launch(float* z0, const float* eps, float* xb, long long count
   int grid = (int)((total + 255) / 256);
   if (grid > g_num_sms * 8) grid = g_num_sms * 8;
   launch_k(img2img_prep_kernel, dim3(grid), dim3(256), 0, st, z0, eps, xb, count, sa, sb, mask, w, H, W);
+  SDB_CUDA(cudaGetLastError());
+}
+
+// 9-channel inpainting (DESIGN §7 f9), once per call. Elements i < nb*4*plane: the encoder input of the masked image,
+// x_m = (mask >= 128) ? 0 : fl(fl(v / 127.5) - 1), fourth plane zero (u8_to_enc_input's layout). Then one thread per latent cell
+// j < nb*H*W: the latent mask m[8h][8w] >= 128 (nearest pick), 1 or 0, into channel 0 of cond [nb,5,H,W].
+__global__ void inpaint_prep_kernel(const uint8_t* __restrict__ rgb, const uint8_t* __restrict__ mask, int Hp, int Wp, long long count,
+                                    float* __restrict__ out, float* __restrict__ cond) {
+  pdl_enter();
+  const long long plane = (long long)Hp * Wp;
+  const int H = Hp / 8, W = Wp / 8;
+  const long long cells = count / (4 * 64);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count + cells; i += (long long)gridDim.x * blockDim.x) {
+    if (i < count) {
+      const long long p = i % plane, r = i / plane;
+      const int ch = (int)(r % 4);
+      const long long s = r / 4;
+      const bool hole = mask[s * plane + p] >= 128;
+      out[i] = (ch == 3 || hole) ? 0.f : __fsub_rn(__fdiv_rn((float)rgb[(s * plane + p) * 3 + ch], 127.5f), 1.0f);
+    } else {
+      const long long j = i - count;
+      const int xx = (int)(j % W), yy = (int)((j / W) % H);
+      const long long s = j / ((long long)H * W);
+      cond[s * 5 * H * W + (long long)yy * W + xx] = mask[s * plane + (long long)(8 * yy) * Wp + 8 * xx] >= 128 ? 1.f : 0.f;
+    }
+  }
+}
+void inpaint_prep_launch(const uint8_t* rgb, const uint8_t* mask, int nb, int Hp, int Wp, float* enc_in, float* cond,
+                         cudaStream_t st) {
+  const long long count = (long long)nb * 4 * Hp * Wp, total = count + count / 256;
+  int grid = (int)((total + 255) / 256);
+  if (grid > g_num_sms * 16) grid = g_num_sms * 16;
+  launch_k(inpaint_prep_kernel, dim3(grid), dim3(256), 0, st, rgb, mask, Hp, Wp, count, enc_in, cond);
   SDB_CUDA(cudaGetLastError());
 }
 

@@ -68,6 +68,11 @@ void nhwc_to_nchw_launch(const float* x, int n, int C, int H, int W, float* y, c
 // pre: optional 1x1 4->4 conv (post_quant_conv) with scalar input scale applied to the input first.
 void conv3x3_cin4_launch(const float* x_nchw, int n, int H, int W, const float* w, const float* b, int Cout,
                          const float* pre_w, const float* pre_b, float pre_scale, float* y, Half2Ptr y16, cudaStream_t st);
+// the 9-channel inpainting UNet's conv_in (DESIGN §7 f9): channels 0-3 from x (sample stride x_stride), 4-8 from cond (sample stride
+// cond_stride, sample index modulo cond_mod); kConvCin9Pix output pixels per CTA
+constexpr int kConvCin9Pix = 32;
+void conv3x3_cin9_launch(const float* x, long long x_stride, const float* cond, long long cond_stride, int cond_mod, int n, int H,
+                         int W, const float* w, const float* b, int Cout, float* y, Half2Ptr y16, cudaStream_t st);
 // 3x3 pad 1, Cout <= 4, input NHWC fp32 with fused GroupNorm+SiLU; output NCHW fp32 [n,Cout,H,W];
 // weights repacked [Cout][9][C] fp32.
 void conv3x3_small_cout_launch(const float* x, int n, int H, int W, int C, const double* sums, const float* gamma,
@@ -119,6 +124,9 @@ void cfg_sampler_launch(int kind, const SamplerStep& s, const float* eps_u, cons
                         const float* z0, const float* eps0, const float* w, int plane);
 // ---- img2img staging: u8 HWC RGB [nb][Hp][Wp][3] -> encoder input [nb][4][Hp][Wp], v / 127.5 - 1, fourth plane zero
 void u8_to_enc_input_launch(const uint8_t* rgb, int nb, int Hp, int Wp, float* out, cudaStream_t st);
+// 9-channel inpainting: the masked image's encoder input [nb,4,Hp,Wp] and the latent mask into channel 0 of cond [nb,5,Hp/8,Wp/8]
+void inpaint_prep_launch(const uint8_t* rgb, const uint8_t* mask, int nb, int Hp, int Wp, float* enc_in, float* cond,
+                         cudaStream_t st);
 // z0 [count] *= 0.18215 in place; xb[0..count) = xb[count..2count) = sa z0 + sb eps; mask (optional, u8 [n][8H][8W]) ->
 // w [n][H][W] = 8x8 block sum / 16320
 void img2img_prep_launch(float* z0, const float* eps, float* xb, long long count, float sa, float sb, const uint8_t* mask, float* w,
@@ -128,6 +136,9 @@ void cfg_combine_launch(const float* eps_u, const float* eps_c, long long count,
 // u8 = trunc(clamp((img+1)/2*255, 0, 255)), NCHW fp32 -> NHWC u8 (reference stablediffusion/mod.rs:79-97)
 void to_rgb8_launch(const float* img_nchw, int n, int H, int W, uint8_t* rgb, cudaStream_t st);
 void quant_conv_slice_launch(const float* x, const float* w, const float* b, int n, int HW, float* y, cudaStream_t st);
+// the same, writing fl(y * scale) at sample stride y_stride (the inpainting conditioning tensor)
+void quant_conv_slice_scaled_launch(const float* x, const float* w, const float* b, int n, int HW, long long y_stride, float scale,
+                                    float* y, cudaStream_t st);
 void add_vec_launch(const float* a, const float* b, int n, float* y, cudaStream_t st);
 // N(0,1) latents from a Philox-like counter hash (used only when the caller passes no init latent)
 void randn_launch(float* x, long long count, uint64_t seed, cudaStream_t st);

@@ -949,11 +949,16 @@ static void prepare_context(Fwd& f, const float* d_ctx /*[nb][Lpad][768] zero pa
 
 // ================================================================================ UNet::forward
 struct UNetIO {
-  const float* x;      // [nb,4,H,W] NCHW
+  const float* x;      // [nb,4,H,W] NCHW (sample stride x_stride)
   const int* t_dev;    // device scalar timestep
   float* out;          // [nb,4,H,W] NCHW
   int H, W;
   const float* emb_all = nullptr;  // [1000][emb_total] rows precomputed per timestep value (sample_latent), or null
+  // 9-channel conv_in (DESIGN §7 f9): input channels 4-8 of sample i at cond + (i % cond_mod) * cond_stride
+  long long x_stride = 0;
+  const float* cond = nullptr;
+  long long cond_stride = 0;
+  int cond_mod = 1;
 };
 
 static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
@@ -994,9 +999,13 @@ static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
     switch (b.kind) {
       case BK_CONV: {
         o = f.act16(H, W, b.cout);
-        KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * H * W * 36.0 * b.cout);
-        conv3x3_cin4_launch(io.x, f.nb, H, W, mptr(c, b.conv.wi), b.conv.bias, b.cout, nullptr, nullptr, 1.f, o.p, o.raw16,
-                            c.stream);
+        KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * H * W * 9.0 * b.cin * b.cout);
+        if (b.cin == 9)
+          conv3x3_cin9_launch(io.x, io.x_stride, io.cond, io.cond_stride, io.cond_mod, f.nb, H, W, mptr(c, b.conv.wi), b.conv.bias,
+                              b.cout, o.p, o.raw16, c.stream);
+        else
+          conv3x3_cin4_launch(io.x, f.nb, H, W, mptr(c, b.conv.wi), b.conv.bias, b.cout, nullptr, nullptr, 1.f, o.p, o.raw16,
+                              c.stream);
         break;
       }
       case BK_DOWN: {  // unet/mod.rs:412-427: 3x3 stride 2 pad 1
@@ -1203,8 +1212,9 @@ static void vae_decode(Fwd& f, const float* d_latent, int H, int W, float pre_sc
 
 // ================================================================================ VAE encoder (SURVEY §8f row f4)
 // Autoencoder::encode_image (autoencoder/mod.rs:60-66): Encoder::forward (:133-145) -> quant_conv -> channels [0,4).
-// d_img4: the image with a zero fourth plane [nb][4][H][W]; d_latent [nb][4][H/8][W/8].
-static void vae_encode(Fwd& f, const float* d_img4, int H, int W, float* d_latent) {
+// d_img4: the image with a zero fourth plane [nb][4][H][W]; d_latent [nb][4][H/8][W/8], or with out_stride > 0 sample i at
+// d_latent + i * out_stride, scaled by out_scale (the inpainting conditioning tensor).
+static void vae_encode(Fwd& f, const float* d_img4, int H, int W, float* d_latent, long long out_stride = 0, float out_scale = 1.f) {
   Ctx& c = f.c;
   EncoderW& e = f.m.enc;
   const size_t mark0 = c.work.off;
@@ -1254,7 +1264,10 @@ static void vae_encode(Fwd& f, const float* d_img4, int H, int W, float* d_laten
   }
   {
     KernelScope ks(c, KC_ELEMENTWISE);
-    quant_conv_slice_launch(y8, mptr(c, e.quant.wi), e.quant.bias, f.nb, H * W, d_latent, c.stream);
+    if (out_stride)
+      quant_conv_slice_scaled_launch(y8, mptr(c, e.quant.wi), e.quant.bias, f.nb, H * W, out_stride, out_scale, d_latent, c.stream);
+    else
+      quant_conv_slice_launch(y8, mptr(c, e.quant.wi), e.quant.bias, f.nb, H * W, d_latent, c.stream);
   }
   c.work.off = mark0;
 }
@@ -1283,8 +1296,11 @@ struct StreamJoin {  // run on c.stream ordered after / before the caller's stre
 }  // namespace
 
 // UNet pass over nb samples with per-sample context lengths. d_ctx_padded [nb][Lpad][768].
+// A 9-channel UNet reads d_x [nb,4,H,W] and d_cond [nb/2,5,H,W] (both CFG halves of a step share it), or with d_cond null
+// d_x [nb,9,H,W].
 static void unet_pass(Ctx& c, int nb, const float* d_x, const int* d_t, const float* d_ctx_padded, int Lpad, int* d_kvlen,
-                      int H, int W, float* d_out, const CtxState* shared_cs, const float* emb_all = nullptr) {
+                      int H, int W, float* d_out, const CtxState* shared_cs, const float* emb_all = nullptr,
+                      const float* d_cond = nullptr) {
   Fwd f(c, nb);
   const size_t mark = c.work.off;
   CtxState local;
@@ -1295,6 +1311,13 @@ static void unet_pass(Ctx& c, int nb, const float* d_x, const int* d_t, const fl
   }
   UNetIO io{d_x, d_t, d_out, H, W};
   io.emb_all = emb_all;
+  const long long hw = (long long)H * W;
+  if (c.unet_cin == 9) {
+    if (d_cond)
+      io.x_stride = 4 * hw, io.cond = d_cond, io.cond_stride = 5 * hw, io.cond_mod = nb / 2;
+    else
+      io.x_stride = 9 * hw, io.cond = d_x + 4 * hw, io.cond_stride = 9 * hw, io.cond_mod = nb;
+  }
   unet_forward(f, io, *cs);
   c.work.off = mark;
 }
@@ -1322,11 +1345,11 @@ void model_unet_forward_dev(Ctx& c, const float* d_x, int t, const float* d_cont
 }
 
 void model_unet_forward_host(Ctx& c, const float* x, int t, const float* context, int n, int H, int W, int L, float* out) {
-  const size_t xe = (size_t)n * 4 * H * W, ce = (size_t)n * L * 768;
-  float* d_x = (float*)c.io(0, xe * 4);
+  const size_t xe = (size_t)n * 4 * H * W, ie = (size_t)n * c.unet_cin * H * W, ce = (size_t)n * L * 768;
+  float* d_x = (float*)c.io(0, ie * 4);
   float* d_c = (float*)c.io(1, ce * 4);
   float* d_o = (float*)c.io(2, xe * 4);
-  SDB_CUDA(cudaMemcpyAsync(d_x, x, xe * 4, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(d_x, x, ie * 4, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaMemcpyAsync(d_c, context, ce * 4, cudaMemcpyHostToDevice, c.stream));
   model_unet_forward_dev(c, d_x, t, d_c, n, H, W, L, d_o, c.stream);
   SDB_CUDA(cudaMemcpyAsync(out, d_o, xe * 4, cudaMemcpyDeviceToHost, c.stream));
@@ -1408,6 +1431,13 @@ void model_latent_to_image_host(Ctx& c, const float* latent, int n, int H, int W
   SDB_CUDA(cudaStreamSynchronize(c.stream));
 }
 
+// a 9-channel UNet (sdb_create_inpaint) reads a mask and a masked-image latent that text-to-image does not have
+static void check_txt2img(const Ctx& c) {
+  SDB_CHECK(c.unet_cin == 4,
+            "sample: this context runs a 9-channel inpainting UNet (sdb_create_inpaint), which needs a mask and an image; for "
+            "text-to-image call sdb_img2img with an all-255 mask at strength 1");
+}
+
 static void check_sample_args(int n, int L, int Lu, int n_steps, int H, int W) {
   SDB_CHECK(n >= 1 && L >= 1 && Lu >= 1, "sample arguments");
   SDB_CHECK(n_steps >= 1 && n_steps <= 1000, "n_steps must be in [1,1000] (step_by(0) panics in the reference)");
@@ -1429,6 +1459,7 @@ struct Img2ImgIn {  // what the sampler loop needs to start part way down the sc
   const uint8_t* mask = nullptr;  // [n,8H,8W] or null
   float* w = nullptr;           // [n,H,W] latent mask (written when mask is set)
   float sa = 0.f, sb = 0.f;     // sqrt(abar[t0]), sqrt(1 - abar[t0])
+  const float* cond = nullptr;  // 9-channel UNet (DESIGN §7 f9): [n,5,H,W] latent mask | z_m, read by conv_in; no blend then
 };
 
 // The n requests of a sampling call (DESIGN §7 f7). The single-request entries describe a uniform batch: every sample reads the L
@@ -1457,8 +1488,8 @@ Batch uniform_batch(const float* d_context, int n, int L, const float* d_uncond,
 
 // sample_latent + latent_to_image (stablediffusion/mod.rs:51-160) from schedule index `first` on. The conditional and
 // unconditional UNet evaluations of a step (forward_diffuser :162-192) run as ONE batch-2n pass: weights stream from HBM once.
-// ii == null: txt2img from d_init_latent. Otherwise the start latent and (with a mask) the per-step blend come from ii.
-// Runs on c.stream; the caller joins the streams.
+// ii == null: txt2img from d_init_latent. Otherwise the start latent and (with a mask) the per-step blend come from ii; a
+// 9-channel UNet reads ii->cond instead of blending. Runs on c.stream; the caller joins the streams.
 static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const float* d_init_latent, const Img2ImgIn* ii, int H,
                         int W, float* d_latent_out, uint8_t* d_rgb) {
   Model& m = M(c);
@@ -1522,6 +1553,7 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const fl
   const long long key = ((long long)nb << 48) ^ ((long long)H << 36) ^ ((long long)W << 24) ^ ((long long)Lpad << 8) ^
                         (long long)(c.opt_precision & 3);
   const bool use_graph = c.opt_graphs && !c.profiling;
+  const float* cond = ii ? ii->cond : nullptr;  // an io slot that can grow and move between calls: part of the graph match
   int* d_tcur = c.work.get<int>(1);
   const size_t work_mark = c.work.off;
   cudaGraphExec_t exec = nullptr;
@@ -1529,18 +1561,19 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const fl
   if (use_graph) {
     for (auto& g : m.graphs)
       if (g.key == key && g.io[0] == (void*)xb && g.io[1] == (void*)eps && g.io[2] == (void*)cs.kv[0].kv &&
-          g.io[4] == (void*)(uintptr_t)work_mark)  // the step's own temporaries start at work_mark
+          g.io[4] == (void*)(uintptr_t)work_mark &&  // the step's own temporaries start at work_mark
+          g.io[5] == (const void*)cond)
         exec = g.exec, graph_launches = (int64_t)(intptr_t)g.io[3];
     if (!exec) {
       // warm-up pass outside capture (sets kernel attributes), then capture
       SDB_CUDA(cudaMemcpyAsync(d_tcur, d_t, 4, cudaMemcpyDeviceToDevice, c.stream));
-      unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all);
+      unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all, cond);
       SDB_CUDA(cudaStreamSynchronize(c.stream));
       const int64_t before = c.launches;
       cudaGraph_t graph;
       SDB_CUDA(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
       try {
-        unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all);
+        unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all, cond);
       } catch (...) {
         cudaGraph_t g2;
         cudaStreamEndCapture(c.stream, &g2);
@@ -1556,6 +1589,7 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const fl
       memset(ge.io, 0, sizeof(ge.io));
       ge.io[0] = xb, ge.io[1] = eps, ge.io[2] = cs.kv[0].kv, ge.io[3] = (void*)(intptr_t)graph_launches;
       ge.io[4] = (void*)(uintptr_t)work_mark;
+      ge.io[5] = (void*)cond;
       m.graphs.push_back(ge);
     }
   }
@@ -1575,10 +1609,10 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const fl
       c.launches += graph_launches;
     } else {
       c.work.off = work_mark;
-      unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all);
+      unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all, cond);
     }
     KernelScope ks(c, KC_ELEMENTWISE);
-    const bool blend = ii && ii->mask;
+    const bool blend = ii && ii->mask && !ii->cond;
     double dir = std::sqrt(1.0 - a_prev);
     SamplerStep s;
     if (kind != STEP_DDIM) {
@@ -1623,6 +1657,7 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const fl
 void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale,
                       int n_steps, const float* d_init_latent, int H, int W, float* d_latent_out, uint8_t* d_rgb,
                       cudaStream_t caller) {
+  check_txt2img(c);
   check_sample_args(n, L, Lu, n_steps, H, W);
   StreamJoin join(c, caller);
   sample_loop(c, uniform_batch(d_context, n, L, d_uncond, Lu, scale), n_steps, 0, d_init_latent, nullptr, H, W, d_latent_out,
@@ -1631,6 +1666,7 @@ void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float*
 
 void model_sample_host(Ctx& c, const float* context, int n, int L, const float* uncond, int Lu, double scale, int n_steps,
                        const float* init_latent, uint64_t seed, int H, int W, float* latent_out, uint8_t* rgb) {
+  check_txt2img(c);
   const size_t le = (size_t)n * 4 * H * W, ce = (size_t)n * L * 768, ue = (size_t)Lu * 768, re = (size_t)n * 3 * 64 * H * W;
   float* d_c = (float*)c.io(0, ce * 4);
   float* d_u = (float*)c.io(1, ue * 4);
@@ -1662,16 +1698,20 @@ static int img2img_first(double strength, int n_steps) {
   return N - k;
 }
 
-static void check_img2img_args(int n, int L, int Lu, int n_steps, int H, int W, const void* image, const void* context,
-                               const void* uncond, const void* latent_out, const void* rgb) {
+static void check_img2img_args(const Ctx& c, int n, int L, int Lu, int n_steps, int H, int W, const void* image, const void* mask,
+                               const void* context, const void* uncond, const void* latent_out, const void* rgb) {
   check_sample_args(n, L, Lu, n_steps, H, W);
   SDB_CHECK(image && context && uncond, "img2img: null image, context or uncond");
+  SDB_CHECK(mask || c.unet_cin == 4, "img2img: the mask is NULL; a 9-channel inpainting UNet (sdb_create_inpaint) needs one");
   SDB_CHECK(latent_out || rgb, "img2img: request the latent, the image or both");
 }
 
 // Encoder (chunks of 4 images, as model_encode_dev) -> z0 in an io slot -> sampler loop from t0 = ts[N - k] -> decode.
 // z0 and the latent mask live in io slots, not in the work arena: the arena prefix up to the loop's work_mark is laid out
 // exactly as txt2img lays it out, so no cached step graph can see img2img data where it expects its own temporaries.
+// A 9-channel UNet (DESIGN §7 f9) gets no blend: inpaint_prep writes the masked image's encoder input and the latent mask, and
+// a second encoder pass (the same chunks) writes z_m, so the conditioning tensor [n,5,H,W] (io slot kIoInpaintCond) holds
+// m_lat | z_m for conv_in.
 // Runs on c.stream; the caller has checked the arguments and joined the streams.
 static void img2img_run(Ctx& c, const Batch& b, const uint8_t* d_image, const uint8_t* d_mask, double strength, int n_steps,
                         const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb) {
@@ -1681,10 +1721,12 @@ static void img2img_run(Ctx& c, const Batch& b, const uint8_t* d_image, const ui
   const double abar = (double)m.alphas_host[ddim_timesteps(n_steps)[first]];  // read as f32, widened (mod.rs:124-140)
   Img2ImgIn ii;
   ii.sa = (float)std::sqrt(abar), ii.sb = (float)std::sqrt(1.0 - abar);
-  ii.eps = d_noise, ii.mask = d_mask;
+  const bool inpaint = c.unet_cin == 9;
+  ii.eps = d_noise, ii.mask = inpaint ? nullptr : d_mask;
   const size_t le = (size_t)n * 4 * H * W;
   ii.z0 = (float*)c.io(kIoImg2ImgZ0, le * 4);
-  if (d_mask) ii.w = (float*)c.io(kIoImg2ImgW, (size_t)n * H * W * 4);
+  if (ii.mask) ii.w = (float*)c.io(kIoImg2ImgW, (size_t)n * H * W * 4);
+  float* cond = inpaint ? (float*)c.io(kIoInpaintCond, (size_t)n * 5 * H * W * 4) : nullptr;
   c.work.reset();
   const int Hp = 8 * H, Wp = 8 * W;
   const size_t plane = (size_t)Hp * Wp;
@@ -1700,13 +1742,28 @@ static void img2img_run(Ctx& c, const Batch& b, const uint8_t* d_image, const ui
     vae_encode(f, img4, Hp, Wp, ii.z0 + (size_t)i0 * 4 * H * W);
     c.work.off = mark;
   }
+  if (inpaint) {
+    float* enc_in = c.work.get<float>((size_t)n * 4 * plane);
+    {
+      KernelScope ks(c, KC_ELEMENTWISE);
+      inpaint_prep_launch(d_image, d_mask, n, Hp, Wp, enc_in, cond, c.stream);
+    }
+    for (int i0 = 0; i0 < n; i0 += 4) {
+      const int nb = std::min(4, n - i0);
+      const size_t mark = c.work.off;
+      Fwd f(c, nb);
+      vae_encode(f, enc_in + (size_t)i0 * 4 * plane, Hp, Wp, cond + ((size_t)i0 * 5 + 1) * H * W, 5ll * H * W, 0.18215f);
+      c.work.off = mark;
+    }
+    ii.cond = cond;
+  }
   sample_loop(c, b, n_steps, first, nullptr, &ii, H, W, d_latent_out, d_rgb);
 }
 
 void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
                        int L, const float* d_uncond, int Lu, double scale, int n_steps, const float* d_noise, int H, int W,
                        float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
-  check_img2img_args(n, L, Lu, n_steps, H, W, d_image, d_context, d_uncond, d_latent_out, d_rgb);
+  check_img2img_args(c, n, L, Lu, n_steps, H, W, d_image, d_mask, d_context, d_uncond, d_latent_out, d_rgb);
   SDB_CHECK(d_noise, "img2img: the device entry needs the noise latent");
   img2img_first(strength, n_steps);
   StreamJoin join(c, caller);
@@ -1717,7 +1774,7 @@ void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, do
 void model_img2img_host(Ctx& c, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
                         const float* uncond, int Lu, double scale, int n_steps, const float* noise, uint64_t seed, int H, int W,
                         float* latent_out, uint8_t* rgb) {
-  check_img2img_args(n, L, Lu, n_steps, H, W, image, context, uncond, latent_out, rgb);
+  check_img2img_args(c, n, L, Lu, n_steps, H, W, image, mask, context, uncond, latent_out, rgb);
   img2img_first(strength, n_steps);  // reject before staging anything
   const size_t le = (size_t)n * 4 * H * W, ce = (size_t)n * L * 768, ue = (size_t)Lu * 768, re = (size_t)n * 3 * 64 * H * W,
                me = (size_t)n * 64 * H * W;
@@ -1826,6 +1883,7 @@ static sdb_batch stage_batch_host(Ctx& c, const sdb_batch& sb) {
 
 void model_sample_batch_dev(Ctx& c, const sdb_batch* sb, int n_steps, const float* d_init_latent, int H, int W,
                             float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
+  check_txt2img(c);
   check_batch(sb, !d_init_latent);
   check_sample_args(sb->n, sb->L, sb->Lu, n_steps, H, W);
   SDB_CHECK(d_latent_out || d_rgb, "sample_batch: request the latent, the image or both");
@@ -1837,6 +1895,7 @@ void model_sample_batch_dev(Ctx& c, const sdb_batch* sb, int n_steps, const floa
 
 void model_sample_batch_host(Ctx& c, const sdb_batch* sb, int n_steps, const float* init_latent, int H, int W, float* latent_out,
                              uint8_t* rgb) {
+  check_txt2img(c);
   check_batch(sb, !init_latent);
   check_sample_args(sb->n, sb->L, sb->Lu, n_steps, H, W);
   SDB_CHECK(latent_out || rgb, "sample_batch: request the latent, the image or both");
@@ -1856,7 +1915,7 @@ void model_img2img_batch_dev(Ctx& c, const sdb_batch* sb, const uint8_t* d_image
                              int n_steps, const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb,
                              cudaStream_t caller) {
   check_batch(sb, !d_noise);
-  check_img2img_args(sb->n, sb->L, sb->Lu, n_steps, H, W, d_image, sb->context, sb->uncond, d_latent_out, d_rgb);
+  check_img2img_args(c, sb->n, sb->L, sb->Lu, n_steps, H, W, d_image, d_mask, sb->context, sb->uncond, d_latent_out, d_rgb);
   img2img_first(strength, n_steps);
   StreamJoin join(c, caller);
   const BatchTab tab = upload_batch_tab(c, *sb);
@@ -1867,7 +1926,7 @@ void model_img2img_batch_dev(Ctx& c, const sdb_batch* sb, const uint8_t* d_image
 void model_img2img_batch_host(Ctx& c, const sdb_batch* sb, const uint8_t* image, const uint8_t* mask, double strength,
                               int n_steps, const float* noise, int H, int W, float* latent_out, uint8_t* rgb) {
   check_batch(sb, !noise);
-  check_img2img_args(sb->n, sb->L, sb->Lu, n_steps, H, W, image, sb->context, sb->uncond, latent_out, rgb);
+  check_img2img_args(c, sb->n, sb->L, sb->Lu, n_steps, H, W, image, mask, sb->context, sb->uncond, latent_out, rgb);
   img2img_first(strength, n_steps);  // reject before staging anything
   const int n = sb->n;
   const size_t le = (size_t)n * 4 * H * W, re = (size_t)n * 3 * 64 * H * W, me = (size_t)n * 64 * H * W;
@@ -1896,9 +1955,9 @@ void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const floa
   c.work.reset();
   const int nb = 2 * n;
   const int Lpad = round_up(std::max(L, Lu), 32);
-  const size_t le = (size_t)n * 4 * H * W;
+  const size_t le = (size_t)n * 4 * H * W, li = (size_t)n * c.unet_cin * H * W;  // output / input latent elements
   float* ctxp = c.work.get<float>((size_t)nb * Lpad * 768);
-  float* xb = c.work.get<float>(2 * le);
+  float* xb = c.work.get<float>(2 * li);
   float* eps = c.work.get<float>(2 * le);
   int* d_t = c.work.get<int>(1);
   int* d_len = c.work.get<int>(nb);
@@ -1907,8 +1966,8 @@ void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const floa
     SDB_CUDA(cudaMemcpyAsync(ctxp + (size_t)i * Lpad * 768, d_uncond, (size_t)Lu * 768 * 4, cudaMemcpyDeviceToDevice, c.stream));
   SDB_CUDA(cudaMemcpy2DAsync(ctxp + (size_t)n * Lpad * 768, (size_t)Lpad * 768 * 4, d_context, (size_t)L * 768 * 4,
                              (size_t)L * 768 * 4, n, cudaMemcpyDeviceToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(xb, d_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(xb + le, d_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(xb, d_latent, li * 4, cudaMemcpyDeviceToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(xb + li, d_latent, li * 4, cudaMemcpyDeviceToDevice, c.stream));
   std::vector<int> lens(nb);
   for (int i = 0; i < nb; ++i) lens[i] = i < n ? Lu : L;
   SDB_CUDA(cudaMemcpyAsync(d_t, &t, 4, cudaMemcpyHostToDevice, c.stream));
@@ -1925,12 +1984,12 @@ void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const floa
 
 void model_forward_diffuser_host(Ctx& c, const float* latent, int t, const float* context, int n, int L, const float* uncond,
                                  int Lu, double scale, int H, int W, float* pred, float* out_u, float* out_c) {
-  const size_t le = (size_t)n * 4 * H * W, ce = (size_t)n * L * 768, ue = (size_t)Lu * 768;
-  float* d_l = (float*)c.io(0, le * 4);
+  const size_t le = (size_t)n * 4 * H * W, li = (size_t)n * c.unet_cin * H * W, ce = (size_t)n * L * 768, ue = (size_t)Lu * 768;
+  float* d_l = (float*)c.io(0, li * 4);
   float* d_c = (float*)c.io(1, ce * 4);
   float* d_u = (float*)c.io(2, ue * 4);
   float* d_o = (float*)c.io(3, 3 * le * 4);
-  SDB_CUDA(cudaMemcpyAsync(d_l, latent, le * 4, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(d_l, latent, li * 4, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaMemcpyAsync(d_c, context, ce * 4, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaMemcpyAsync(d_u, uncond, ue * 4, cudaMemcpyHostToDevice, c.stream));
   model_forward_diffuser_dev(c, d_l, t, d_c, n, L, d_u, Lu, scale, H, W, d_o, d_o + le, d_o + 2 * le, c.stream);

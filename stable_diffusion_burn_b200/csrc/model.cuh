@@ -6,6 +6,8 @@
 namespace sdb {
 
 void model_create(Ctx& c);   // builds the tensor registry, allocates arenas
+// rejects a unet/input_blocks/conv/weight of [320,C,3,3] with C != c.unet_cin, naming both shapes and the create entry to use
+void check_conv_in_shape(const Ctx& c, const std::string& what, int ndim, const int64_t* dims);
 void model_destroy(Ctx& c);
 void model_init_synthetic(Ctx& c, uint32_t seed);
 void model_finalize(Ctx& c);  // packs weights into kernel layouts

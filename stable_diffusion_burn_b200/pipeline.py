@@ -25,7 +25,8 @@ class UNet:
         self._c = ctx
 
     def forward(self, x: np.ndarray, timesteps, context: np.ndarray) -> np.ndarray:
-        """x [n,4,H,W]; timesteps Int[1] (one t for the batch); context [n,L,768] -> [n,4,H,W]."""
+        """x [n,4,H,W] (an inpainting UNet: [n,9,H,W] = latent | mask | masked-image latent); timesteps Int[1] (one t for
+        the batch); context [n,L,768] -> [n,4,H,W]."""
         ts = np.asarray(timesteps).reshape(-1)
         if ts.size != 1:
             raise ValueError("timesteps must hold exactly one value (reference: Tensor<B,1,Int> of length 1)")
@@ -59,10 +60,11 @@ class CLIP:
 
 
 class StableDiffusion:
-    """Owns the device context; `diffusion`, `autoencoder` and `clip` mirror the reference's fields."""
+    """Owns the device context; `diffusion`, `autoencoder` and `clip` mirror the reference's fields. inpaint=True holds an
+    inpainting checkpoint (a 9-channel UNet, DESIGN.md §7 f9): img2img then needs a mask, and the txt2img calls fail."""
 
-    def __init__(self, device: int = 0):
-        self.ctx = Context(device)
+    def __init__(self, device: int = 0, inpaint: bool = False):
+        self.ctx = Context(device, inpaint=inpaint)
         self.diffusion = UNet(self.ctx)
         self.autoencoder = Autoencoder(self.ctx)
         self.clip = CLIP(self.ctx)
@@ -160,7 +162,9 @@ class StableDiffusion:
                 noise_seed: int = 0):
         """Image-to-image / masked inpainting (an extension: the reference has none; DESIGN.md §7 f5). image u8
         [n, height, width, 3] HWC RGB, the format sample_image returns; mask u8 [n, height, width] (255 = regenerate,
-        0 = keep) or None; strength in (0, 1]. -> list of n flat uint8 arrays of height*width*3, like sample_image."""
+        0 = keep) or None; strength in (0, 1]. With inpaint=True the mask is required, binary (>= 128 regenerates), and
+        conditions the UNet, which sees the masked image, instead of a blend after each step. -> list of n flat uint8 arrays of
+        height*width*3, like sample_image."""
         with self._sampler(sampler, eta, noise_seed):
             rgb = self.ctx.img2img(image, context, unconditional_context, unconditional_guidance_scale, n_steps, strength,
                                    mask=mask, noise=noise, seed=seed)

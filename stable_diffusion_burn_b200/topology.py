@@ -107,12 +107,18 @@ def _unet_block(out, name, kind, cin, cout):
         raise ValueError(kind)
 
 
-def unet_params(prefix="unet"):
+def unet_params(prefix="unet", in_channels=4):
+    """in_channels: 4 (SD-v1) or 9 (an inpainting UNet: conv_in reads latent | mask | masked-image latent, DESIGN.md §7 f9)."""
+    if in_channels not in (4, 9):
+        raise ValueError(f"in_channels must be 4 or 9, got {in_channels}")
     out = []
     _lin(out, f"{prefix}/lin1_time_embed", 320, EMB_DIM)
     _lin(out, f"{prefix}/lin2_time_embed", EMB_DIM, EMB_DIM)
-    for f, kind, cin, cout in UNET_INPUT_BLOCKS:
-        _unet_block(out, f"{prefix}/input_blocks/{f}", kind, cin, cout)
+    for i, (f, kind, cin, cout) in enumerate(UNET_INPUT_BLOCKS):
+        _unet_block(out, f"{prefix}/input_blocks/{f}", kind, in_channels if i == 0 else cin, cout)
+    # conv_in's bias keeps the 4-channel fan-in: only the weight of a 9-channel registry differs (its synthetic stream too)
+    b = next(i for i, e in enumerate(out) if e[0] == f"{prefix}/input_blocks/conv/bias")
+    out[b] = out[b][:3] + (4 * 9,)
     # middle: ResTransformerRes(1280,1280,1280,768,8) unet/mod.rs:58, 328-351
     m = f"{prefix}/middle_block"
     _resblock(out, f"{m}/res1", 1280, 1280)
@@ -209,8 +215,9 @@ def clip_params(prefix="clip"):
     return out
 
 
-def all_params():
-    return unet_params() + vae_decoder_params() + clip_params() + vae_encoder_params()
+def all_params(inpaint=False):
+    """The registry in sdb_create's order; inpaint=True: sdb_create_inpaint's (a 9-channel unet/input_blocks/conv)."""
+    return unet_params(in_channels=9 if inpaint else 4) + vae_decoder_params() + clip_params() + vae_encoder_params()
 
 
 if __name__ == "__main__":
