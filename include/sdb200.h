@@ -37,8 +37,14 @@ int sdb_create(int device, sdb_ctx** out);
  * unet/input_blocks/conv/weight, [320,9,3,3] (and its n_channels_in 9): the UNet reads cat(latent, latent mask, masked-image
  * latent). On such a context sdb_img2img[_dev] and sdb_img2img_batch[_dev] need the mask and condition the UNet on it with no
  * blend; sdb_unet_forward[_dev] and sdb_forward_diffuser[_dev] take x / latent [n,9,H,W] and return [n,4,H,W]; the text-to-image
- * entries fail (use sdb_img2img with an all-255 mask at strength 1). Loading a conv_in of the other width fails. */
+ * entries fail (use sdb_img2img with an all-255 mask at strength 1). Loading a conv_in of another width fails. */
 int sdb_create_inpaint(int device, sdb_ctx** out);
+/* A context for an InstructPix2Pix checkpoint (timbrooks/instruct-pix2pix; DESIGN.md §7 f10). Its registry is sdb_create's except
+ * unet/input_blocks/conv/weight, [320,8,3,3] (and its n_channels_in 8): the UNet reads cat(latent, image latent). Such a context
+ * edits images with sdb_edit_image[_dev]; sdb_unet_forward[_dev] takes x [n,8,H,W] and returns [n,4,H,W]. The text-to-image
+ * entries, sdb_img2img[_dev], the sdb_*_batch entries and sdb_forward_diffuser[_dev] (two-way guidance) fail, naming
+ * sdb_edit_image. Loading a conv_in of another width fails. */
+int sdb_create_pix2pix(int device, sdb_ctx** out);
 int sdb_destroy(sdb_ctx* ctx);
 /* ctx may be NULL: returns the last error of the calling thread (e.g. a failed sdb_create). */
 const char* sdb_last_error(sdb_ctx* ctx);
@@ -151,9 +157,28 @@ int sdb_img2img_dev(sdb_ctx* ctx, const uint8_t* d_image, const uint8_t* d_mask,
                     int L, const float* d_uncond, int Lu, double guidance_scale, int n_steps, const float* d_noise, int H, int W,
                     float* d_latent_out, uint8_t* d_rgb_out, void* stream);
 
+/* ---- InstructPix2Pix image editing (DESIGN.md §7 f10) ------------------------------------------------------------------ */
+/* Edits n images by instruction on an 8-channel context (sdb_create_pix2pix), as the original edit_cli.py and diffusers'
+ * StableDiffusionInstructPix2PixPipeline do. image u8 [n,8H,8W,3] HWC RGB -> x = v/127.5 - 1 -> the image latent
+ * c_I = encode_image(x), UNSCALED (the posterior mode; no 0.18215). Sampling runs the full schedule from t = 999 (no strength)
+ * on init_latent [n,4,H,W]; NULL = the N(0,1) stream keyed by `seed` that sdb_sample_image starts from. Each step is one
+ * batch-3n UNet pass over the groups, in this order,
+ *   e_U = UNet(cat(x_t, 0), t, uncond)   e_I = UNet(cat(x_t, c_I), t, uncond)   e_T = UNet(cat(x_t, c_I), t, context)
+ * combined as pred = e_U + text_scale (e_T - e_I) + image_scale (e_I - e_U) (both finite; all three passes always run), then
+ * the context's sampler (sdb_set_sampler) updates the latent with no blend. context [n,L,768]; uncond [Lu,768], one negative
+ * broadcast over the batch. Outputs: latent_out [n,4,H,W] and / or rgb_out [n,8H,8W,3]; at least one must be set. H, W are
+ * latent sizes with the constraints of sampling. Fails on a 4- or 9-channel context, naming sdb_create_pix2pix. */
+int sdb_edit_image(sdb_ctx* ctx, const uint8_t* image, const float* context, int n, int L, const float* uncond, int Lu,
+                   double text_scale, double image_scale, int n_steps, const float* init_latent, uint64_t seed, int H, int W,
+                   float* latent_out, uint8_t* rgb_out);
+/* device-pointer variant: d_init_latent is required; runs ordered after, and before the rest of, `stream`. */
+int sdb_edit_image_dev(sdb_ctx* ctx, const uint8_t* d_image, const float* d_context, int n, int L, const float* d_uncond, int Lu,
+                       double text_scale, double image_scale, int n_steps, const float* d_init_latent, int H, int W,
+                       float* d_latent_out, uint8_t* d_rgb_out, void* stream);
+
 /* ---- sampler (DESIGN.md §7 f6) ------------------------------------------------------------------------------------------ */
 /* The reference samples with DDIM at eta = 0 only (src/model/stablediffusion/mod.rs:119, sigma = 0). The sampler is context
- * state, read by sdb_sample_latent, sdb_sample_image, sdb_sample_image_dev, sdb_img2img and sdb_img2img_dev (not by
+ * state, read by sdb_sample_latent, sdb_sample_image, sdb_sample_image_dev, sdb_img2img[_dev] and sdb_edit_image[_dev] (not by
  * sdb_forward_diffuser or sdb_unet_forward); the schedule, the UNet step and the decode are the same for every sampler.
  * SDB_SAMPLER_DDIM with eta in [0, 1] (finite): DDIM (Song et al. 2021, eq. 16), s = eta sqrt((1-a')/(1-a)) sqrt(1 - a/a'),
  *   x' = sqrt(a') x0 + sqrt(1 - a' - s^2) eps + s z. eta = 0 (the default) is the reference's sampler, unchanged to the bit.

@@ -40,6 +40,7 @@ pub struct SdbBatch {
 extern "C" {
     fn sdb_create(device: c_int, out: *mut *mut SdbCtx) -> c_int;
     fn sdb_create_inpaint(device: c_int, out: *mut *mut SdbCtx) -> c_int;
+    fn sdb_create_pix2pix(device: c_int, out: *mut *mut SdbCtx) -> c_int;
     fn sdb_destroy(ctx: *mut SdbCtx) -> c_int;
     fn sdb_last_error(ctx: *mut SdbCtx) -> *const c_char;
     fn sdb_set_tensor(ctx: *mut SdbCtx, name: *const c_char, host: *const f32, dims: *const i64, ndim: c_int) -> c_int;
@@ -68,6 +69,14 @@ extern "C" {
                        n: c_int, l: c_int, d_uncond: *const c_void, lu: c_int, guidance_scale: f64, n_steps: c_int,
                        d_noise: *const c_void, h: c_int, w: c_int, d_latent_out: *mut c_void, d_rgb_out: *mut c_void,
                        stream: *mut c_void) -> c_int;
+    fn sdb_edit_image(ctx: *mut SdbCtx, image: *const u8, context: *const f32, n: c_int, l: c_int, uncond: *const f32, lu: c_int,
+                      text_scale: f64, image_scale: f64, n_steps: c_int, init_latent: *const f32, seed: u64, h: c_int, w: c_int,
+                      latent_out: *mut f32, rgb_out: *mut u8) -> c_int;
+    #[allow(dead_code)]
+    fn sdb_edit_image_dev(ctx: *mut SdbCtx, d_image: *const c_void, d_context: *const c_void, n: c_int, l: c_int,
+                          d_uncond: *const c_void, lu: c_int, text_scale: f64, image_scale: f64, n_steps: c_int,
+                          d_init_latent: *const c_void, h: c_int, w: c_int, d_latent_out: *mut c_void, d_rgb_out: *mut c_void,
+                          stream: *mut c_void) -> c_int;
     fn sdb_set_sampler(ctx: *mut SdbCtx, kind: c_int, eta: f64, noise_seed: u64) -> c_int;
     fn sdb_tensor_count(ctx: *mut SdbCtx) -> c_int;
     fn sdb_tensor_info(ctx: *mut SdbCtx, index: c_int, name: *mut *const c_char, dims: *mut i64, ndim: *mut c_int) -> c_int;
@@ -122,6 +131,17 @@ impl StableDiffusion {
     pub fn new_inpaint(device: i32) -> Result<Self, SdbError> {
         let mut ctx = std::ptr::null_mut();
         let rc = unsafe { sdb_create_inpaint(device, &mut ctx) };
+        if rc != 0 {
+            return Err(SdbError(unsafe { CStr::from_ptr(sdb_last_error(std::ptr::null_mut())) }.to_string_lossy().into()));
+        }
+        Ok(Self { ctx })
+    }
+
+    /// A context for an InstructPix2Pix checkpoint: an 8-channel `conv_in` reading latent | image latent (DESIGN.md §7 f10).
+    /// `edit_image` is then the sampling call; the text-to-image, `img2img` and batch calls fail.
+    pub fn new_pix2pix(device: i32) -> Result<Self, SdbError> {
+        let mut ctx = std::ptr::null_mut();
+        let rc = unsafe { sdb_create_pix2pix(device, &mut ctx) };
         if rc != 0 {
             return Err(SdbError(unsafe { CStr::from_ptr(sdb_last_error(std::ptr::null_mut())) }.to_string_lossy().into()));
         }
@@ -258,6 +278,30 @@ impl StableDiffusion {
                         n as c_int, l as c_int, unconditional_context.as_ptr(), lu as c_int, unconditional_guidance_scale,
                         n_steps as c_int, noise.map_or(std::ptr::null(), |z| z.as_ptr()), seed, h as c_int, w as c_int,
                         std::ptr::null_mut(), rgb.as_mut_ptr())
+        })?;
+        Ok(rgb.chunks(height * width * 3).map(|c| c.to_vec()).collect())
+    }
+
+    /// InstructPix2Pix editing on a `new_pix2pix` context (DESIGN.md §7 f10). `image`: n RGB images of `height` x `width`
+    /// (multiples of 64) as HWC u8, the format `sample_image` returns; `context`: n instructions of `l` rows; every step runs the
+    /// UNet on (no image, negative), (image, negative) and (image, instruction) and combines them with `text_scale` and
+    /// `image_scale` (7.5 and 1.5 in the original pipeline). `init_latent = None` draws the latent `sample_image` would start
+    /// from for `seed`.
+    #[allow(clippy::too_many_arguments)]
+    pub fn edit_image(&self, image: &[u8], [n, height, width]: [usize; 3], context: &[f32], l: usize,
+                      unconditional_context: &[f32], lu: usize, text_scale: f64, image_scale: f64, n_steps: usize,
+                      init_latent: Option<&[f32]>, seed: u64) -> Result<Vec<Vec<u8>>, SdbError> {
+        let (h, w) = (height / 8, width / 8);
+        if image.len() != n * height * width * 3 || context.len() != n * l * 768
+            || init_latent.map_or(false, |z| z.len() != n * 4 * h * w) {
+            return Err(SdbError("edit_image: buffer sizes do not match [n, height, width] and [n, l, 768]".into()));
+        }
+        let mut rgb = vec![0u8; n * height * width * 3];
+        self.check(unsafe {
+            sdb_edit_image(self.ctx, image.as_ptr(), context.as_ptr(), n as c_int, l as c_int, unconditional_context.as_ptr(),
+                           lu as c_int, text_scale, image_scale, n_steps as c_int,
+                           init_latent.map_or(std::ptr::null(), |z| z.as_ptr()), seed, h as c_int, w as c_int,
+                           std::ptr::null_mut(), rgb.as_mut_ptr())
         })?;
         Ok(rgb.chunks(height * width * 3).map(|c| c.to_vec()).collect())
     }

@@ -33,6 +33,7 @@ _batchp = C.POINTER(SdbBatch)
 SIGNATURES = [
     ("sdb_create", C.c_int, [C.c_int, C.POINTER(_ctx)]),
     ("sdb_create_inpaint", C.c_int, [C.c_int, C.POINTER(_ctx)]),
+    ("sdb_create_pix2pix", C.c_int, [C.c_int, C.POINTER(_ctx)]),
     ("sdb_destroy", C.c_int, [_ctx]),
     ("sdb_last_error", C.c_char_p, [_ctx]),
     ("sdb_version", C.c_char_p, []),
@@ -73,6 +74,10 @@ SIGNATURES = [
                               C.c_uint64, C.c_int, C.c_int, _f32p, _u8p]),
     ("sdb_img2img_dev", C.c_int, [_ctx, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                   C.c_double, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("sdb_edit_image", C.c_int, [_ctx, _u8p, _f32p, C.c_int, C.c_int, _f32p, C.c_int, C.c_double, C.c_double, C.c_int, _f32p,
+                                 C.c_uint64, C.c_int, C.c_int, _f32p, _u8p]),
+    ("sdb_edit_image_dev", C.c_int, [_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_double,
+                                     C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("sdb_set_sampler", C.c_int, [_ctx, C.c_int, C.c_double, C.c_uint64]),
     ("sdb_lora_add", C.c_int, [_ctx, C.c_int, C.c_char_p, C.c_int, _f32p, _f32p, C.c_double]),
     ("sdb_lora_scale", C.c_int, [_ctx, C.c_int, C.c_double]),
@@ -206,12 +211,16 @@ def batch_struct(b, context_ptr=None, uncond_ptr=None):
 
 
 class Context:
-    """Owns one sdb_ctx (one CUDA device). inpaint=True: a 9-channel inpainting UNet (sdb_create_inpaint, DESIGN.md §7 f9)."""
+    """Owns one sdb_ctx (one CUDA device). inpaint=True: a 9-channel inpainting UNet (sdb_create_inpaint, DESIGN.md §7 f9);
+    pix2pix=True: an 8-channel InstructPix2Pix UNet (sdb_create_pix2pix, f10)."""
 
-    def __init__(self, device: int = 0, inpaint: bool = False):
+    def __init__(self, device: int = 0, inpaint: bool = False, pix2pix: bool = False):
+        if inpaint and pix2pix:
+            raise ValueError("a context is either an inpainting (inpaint=True) or an InstructPix2Pix (pix2pix=True) one, not both")
         self.lib = load()
         h = _ctx()
-        rc = (self.lib.sdb_create_inpaint if inpaint else self.lib.sdb_create)(device, C.byref(h))
+        create = self.lib.sdb_create_inpaint if inpaint else (self.lib.sdb_create_pix2pix if pix2pix else self.lib.sdb_create)
+        rc = create(device, C.byref(h))
         if rc != 0:
             raise SdbError(self.lib.sdb_last_error(None).decode())
         self.h = h
@@ -244,7 +253,7 @@ class Context:
         return out
 
     def unet_in_channels(self) -> int:
-        """4, or 9 on an inpainting context: read from the registry's unet/input_blocks/conv/weight."""
+        """4, 9 on an inpainting context or 8 on an InstructPix2Pix one: read from the registry's unet/input_blocks/conv/weight."""
         if getattr(self, "_cin", None) is None:
             self._cin = next(s[1] for n, s in self.tensor_list() if n == "unet/input_blocks/conv/weight")
         return self._cin
@@ -327,7 +336,8 @@ class Context:
 
     # ---- hot path (host buffers)
     def unet_forward(self, x, t, context):
-        """x [n,4,H,W] ([n,9,H,W] = latent | mask | masked-image latent on an inpainting context) -> [n,4,H,W]."""
+        """x [n,4,H,W] ([n,9,H,W] = latent | mask | masked-image latent on an inpainting context, [n,8,H,W] = latent | image
+        latent on an InstructPix2Pix one) -> [n,4,H,W]."""
         x = f32(x); context = f32(context)
         n, ch, H, W = x.shape
         if ch != self.unet_in_channels():
@@ -444,6 +454,35 @@ class Context:
                                         float(strength), ptr(context), n, context.shape[1], ptr(uncond), uncond.shape[0],
                                         float(scale), int(n_steps), None if noise is None else ptr(noise), int(seed), H, W,
                                         None if lat is None else ptr(lat), None if out is None else out.ctypes.data_as(_u8p)))
+        if latent and rgb:
+            return lat, out
+        return lat if latent else out
+
+    def edit_image(self, image, context, uncond, text_scale, image_scale, n_steps, init_latent=None, seed=0, latent=False,
+                   rgb=True):
+        """InstructPix2Pix image editing on an 8-channel context (include/sdb200.h: sdb_edit_image). image u8 [n,8H,8W,3];
+        context [n,L,768]; uncond [Lu,768]; init_latent [n,4,H,W] or None (the seeded stream sample_image starts from).
+        -> the latent [n,4,H,W] and / or the u8 image [n,8H,8W,3]: a tuple (latent, rgb) when both are requested."""
+        if not (latent or rgb):
+            raise ValueError("request the latent, the image or both")
+        image = np.ascontiguousarray(image, dtype=np.uint8)
+        if image.ndim != 4 or image.shape[3] != 3 or image.shape[1] % 8 or image.shape[2] % 8:
+            raise ValueError("image must be u8 [n, 8H, 8W, 3]")
+        n, Hp, Wp, _ = image.shape
+        H, W = Hp // 8, Wp // 8
+        context = f32(context); uncond = f32(uncond)
+        if context.ndim != 3 or context.shape[0] != n:
+            raise ValueError("context must be [n, L, 768], one prompt per image")
+        if init_latent is not None:
+            init_latent = f32(init_latent)
+            if init_latent.shape != (n, 4, H, W):
+                raise ValueError("init_latent must be [n, 4, H, W]")
+        lat = np.empty((n, 4, H, W), np.float32) if latent else None
+        out = np.empty((n, Hp, Wp, 3), np.uint8) if rgb else None
+        self.check(self.lib.sdb_edit_image(self.h, image.ctypes.data_as(_u8p), ptr(context), n, context.shape[1], ptr(uncond),
+                                           uncond.shape[0], float(text_scale), float(image_scale), int(n_steps),
+                                           None if init_latent is None else ptr(init_latent), int(seed), H, W,
+                                           None if lat is None else ptr(lat), None if out is None else out.ctypes.data_as(_u8p)))
         if latent and rgb:
             return lat, out
         return lat if latent else out

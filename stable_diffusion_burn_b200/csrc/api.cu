@@ -135,6 +135,8 @@ int sdb_create(int device, sdb_ctx** out) { return create(device, 4, out); }
 
 int sdb_create_inpaint(int device, sdb_ctx** out) { return create(device, 9, out); }
 
+int sdb_create_pix2pix(int device, sdb_ctx** out) { return create(device, 8, out); }
+
 int sdb_destroy(sdb_ctx* ctx) {
   ctx_teardown(ctx);
   return 0;
@@ -371,6 +373,26 @@ int sdb_img2img_dev(sdb_ctx* ctx, const uint8_t* d_image, const uint8_t* d_mask,
   need_final(c);
   model_img2img_dev(c, d_image, d_mask, strength, d_context, n, L, d_uncond, Lu, guidance_scale, n_steps, d_noise, H, W,
                     d_latent_out, d_rgb_out, (cudaStream_t)stream);
+  API_END
+}
+
+int sdb_edit_image(sdb_ctx* ctx, const uint8_t* image, const float* context, int n, int L, const float* uncond, int Lu,
+                   double text_scale, double image_scale, int n_steps, const float* init_latent, uint64_t seed, int H, int W,
+                   float* latent_out, uint8_t* rgb_out) {
+  API_BEGIN(ctx)
+  need_final(c);
+  model_edit_host(c, image, context, n, L, uncond, Lu, text_scale, image_scale, n_steps, init_latent, seed, H, W, latent_out,
+                  rgb_out);
+  API_END
+}
+
+int sdb_edit_image_dev(sdb_ctx* ctx, const uint8_t* d_image, const float* d_context, int n, int L, const float* d_uncond, int Lu,
+                       double text_scale, double image_scale, int n_steps, const float* d_init_latent, int H, int W,
+                       float* d_latent_out, uint8_t* d_rgb_out, void* stream) {
+  API_BEGIN(ctx)
+  need_final(c);
+  model_edit_dev(c, d_image, d_context, n, L, d_uncond, Lu, text_scale, image_scale, n_steps, d_init_latent, H, W, d_latent_out,
+                 d_rgb_out, (cudaStream_t)stream);
   API_END
 }
 

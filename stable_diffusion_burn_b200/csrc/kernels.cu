@@ -744,31 +744,34 @@ void conv3x3_cin4_launch(const float* x_nchw, int n, int H, int W, const float* 
   SDB_CUDA(cudaGetLastError());
 }
 
-// ============================================================ conv 3x3, Cin = 9: the inpainting UNet's conv_in (DESIGN §7 f9)
-// The conv3x3_cin4 scheme over 81 taps. Channels 0-3 come from x (sample stride xs), channels 4-8 from cond (sample stride cs,
-// sample index modulo cmod: the two CFG halves of a step read one copy). The taps accumulate in OIHW order from the bias, as
-// conv3x3_cin4_kernel does, so zero weights on channels 4-8 give its result bit for bit. Weights [81][Cout] fill 101 KB of shared
-// memory and every CTA stages all of them: PIX output pixels per CTA amortise that staging.
-template <int PIX>
+// ============================================================ conv 3x3, Cin = 8 or 9: a conditioned UNet's conv_in
+// The conv3x3_cin4 scheme over CIN*9 taps: the inpainting UNet (CIN 9, DESIGN §7 f9) and the InstructPix2Pix UNet (CIN 8, f10).
+// Channels 0-3 come from x (sample stride xs), channels 4..CIN-1 from cond (sample stride cs, sample index modulo cmod: the two
+// CFG halves of an inpainting step read one copy; the three guidance groups of an edit step each have their own). The taps
+// accumulate in OIHW order from the bias, as conv3x3_cin4_kernel does, so zero weights on channels 4..CIN-1 give its result bit
+// for bit. Weights [CIN*9][Cout] fill 101 KB (CIN 9) / 90 KB (CIN 8) of shared memory and every CTA stages all of them: PIX
+// output pixels per CTA amortise that staging.
+template <int CIN, int PIX>
 __global__ void __launch_bounds__(256)
-conv3x3_cin9_kernel(const float* __restrict__ x, long long xs, const float* __restrict__ cond, long long cs, int cmod, int H, int W,
-                    const float* __restrict__ w, const float* __restrict__ b, int Cout, float* __restrict__ y,
-                    __half* __restrict__ y_hi, __half* __restrict__ y_lo) {
+conv3x3_cin_cond_kernel(const float* __restrict__ x, long long xs, const float* __restrict__ cond, long long cs, int cmod, int H,
+                        int W, const float* __restrict__ w, const float* __restrict__ b, int Cout, float* __restrict__ y,
+                        __half* __restrict__ y_hi, __half* __restrict__ y_lo) {
+  constexpr int K = CIN * 9;
   pdl_enter();
   extern __shared__ float sm[];
-  float* s_w = sm;                  // [81][Cout]
-  float* s_in = sm + 81 * Cout;     // [PIX][81]
+  float* s_w = sm;                  // [K][Cout]
+  float* s_in = sm + K * Cout;      // [PIX][K]
   const int n = blockIdx.y;
   const int HW = H * W;
   const int p0 = blockIdx.x * PIX;
-  for (int i = threadIdx.x; i < 81 * Cout; i += blockDim.x) {
+  for (int i = threadIdx.x; i < K * Cout; i += blockDim.x) {
     const int k = i / Cout, co = i % Cout;  // k = ci*9 + tap (OIHW inner order)
-    s_w[i] = w[(size_t)co * 81 + k];
+    s_w[i] = w[(size_t)co * K + k];
   }
   const float* xn = x + (size_t)n * xs;
   const float* cn = cond + (size_t)(n % cmod) * cs - (size_t)4 * HW;  // channel ci >= 4 at cn + ci*HW
-  for (int i = threadIdx.x; i < PIX * 81; i += blockDim.x) {
-    const int pl = i / 81, k = i % 81;
+  for (int i = threadIdx.x; i < PIX * K; i += blockDim.x) {
+    const int pl = i / K, k = i % K;
     const int ci = k / 9, tap = k % 9;
     const int p = p0 + pl;
     float v = 0.f;
@@ -785,7 +788,7 @@ conv3x3_cin9_kernel(const float* __restrict__ x, long long xs, const float* __re
     if (p >= HW) continue;
     float acc = b ? b[co] : 0.f;
 #pragma unroll 9
-    for (int k = 0; k < 81; ++k) acc += s_in[pl * 81 + k] * s_w[k * Cout + co];
+    for (int k = 0; k < K; ++k) acc += s_in[pl * K + k] * s_w[k * Cout + co];
     const size_t o = ((size_t)n * HW + p) * Cout + co;
     y[o] = acc;
     if (y_hi) {
@@ -795,17 +798,24 @@ conv3x3_cin9_kernel(const float* __restrict__ x, long long xs, const float* __re
     }
   }
 }
-void conv3x3_cin9_launch(const float* x, long long x_stride, const float* cond, long long cond_stride, int cond_mod, int n, int H,
-                         int W, const float* w, const float* b, int Cout, float* y, Half2Ptr y16, cudaStream_t st) {
-  constexpr int PIX = kConvCin9Pix;
-  const size_t smem = (size_t)(81 * Cout + PIX * 81) * sizeof(float);
+template <int CIN>
+static void conv3x3_cin_cond_go(const float* x, long long x_stride, const float* cond, long long cond_stride, int cond_mod, int n,
+                                int H, int W, const float* w, const float* b, int Cout, float* y, Half2Ptr y16, cudaStream_t st) {
+  constexpr int PIX = kConvCinCondPix;
+  const size_t smem = (size_t)(CIN * 9 * Cout + PIX * CIN * 9) * sizeof(float);
   static DeviceOnce once;
   if (once.first())
-    SDB_CUDA(cudaFuncSetAttribute(conv3x3_cin9_kernel<PIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SDB_CUDA(cudaFuncSetAttribute(conv3x3_cin_cond_kernel<CIN, PIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   dim3 grid(ceil_div(H * W, PIX), n);
-  launch_k(conv3x3_cin9_kernel<PIX>, grid, dim3(256), smem, st, x, x_stride, cond, cond_stride, cond_mod, H, W, w, b, Cout, y,
-           y16.hi, y16.lo);
+  launch_k(conv3x3_cin_cond_kernel<CIN, PIX>, grid, dim3(256), smem, st, x, x_stride, cond, cond_stride, cond_mod, H, W, w, b,
+           Cout, y, y16.hi, y16.lo);
   SDB_CUDA(cudaGetLastError());
+}
+void conv3x3_cin_cond_launch(int cin, const float* x, long long x_stride, const float* cond, long long cond_stride, int cond_mod,
+                             int n, int H, int W, const float* w, const float* b, int Cout, float* y, Half2Ptr y16, cudaStream_t st) {
+  SDB_CHECK(cin == 8 || cin == 9, "conv3x3_cin_cond_launch: cin must be 8 or 9");
+  (cin == 8 ? conv3x3_cin_cond_go<8> : conv3x3_cin_cond_go<9>)(x, x_stride, cond, cond_stride, cond_mod, n, H, W, w, b, Cout, y,
+                                                              y16, st);
 }
 
 // ============================================================ conv 3x3, Cout <= 8, fused GroupNorm + SiLU (fp32, CUDA cores)
@@ -1202,11 +1212,14 @@ __host__ __device__ void step_noise_keys(uint64_t seed, int t, uint32_t* k0, uin
 // expression sample_latent has always used; its kernel keeps the argument list and the instructions it had.
 // PER_SAMPLE (a batch of different requests, DESIGN §7 f7): the scale and the eta noise key of sample i / (4 plane) come from
 // s.scales / s.noise_seeds, and z is drawn at the index within the sample. The arithmetic is the same expression.
-template <int KIND, bool BLEND, bool PER_SAMPLE = false>
+// GROUPS = 3 (InstructPix2Pix, DESIGN §7 f10): eu = e_U, ec = e_I and ec + count = e_T, and the guidance is
+// pred = e_U + s_T (e_T - e_I) + s_I (e_I - e_U) with scale = s_T, scale_i = s_I, left to right with _rn intrinsics; the UNet input
+// batch holds the latent three times.
+template <int KIND, bool BLEND, bool PER_SAMPLE = false, int GROUPS = 2>
 __device__ __forceinline__ void cfg_step(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
                                          long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
                                          float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
-                                         const float* __restrict__ w, int plane, const SamplerStep& s) {
+                                         const float* __restrict__ w, int plane, const SamplerStep& s, float scale_i = 0.f) {
   pdl_enter();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) {
     const float u = eu[i], c = ec[i];
@@ -1221,7 +1234,11 @@ __device__ __forceinline__ void cfg_step(const float* __restrict__ eu, const flo
         step_noise_keys(s.noise_seeds[smp], s.t, &k0, &k1);
       }
     }
-    const float pred = u + (c - u) * sc;                  // stablediffusion/mod.rs:190-191
+    float pred;
+    if constexpr (GROUPS == 3)
+      pred = __fadd_rn(__fadd_rn(u, __fmul_rn(sc, __fsub_rn(ec[i + count], c))), __fmul_rn(scale_i, __fsub_rn(c, u)));
+    else
+      pred = u + (c - u) * sc;                            // stablediffusion/mod.rs:190-191
     const float x = lat[i];
     const float x0 = (x - pred * sqrt_1m_at) / sqrt_at;   // :152
     float nl;
@@ -1243,6 +1260,7 @@ __device__ __forceinline__ void cfg_step(const float* __restrict__ eu, const flo
     }
     lat[i] = nl;
     lat[i + count] = nl;  // the UNet input batch holds the latent twice (uncond half | cond half)
+    if constexpr (GROUPS == 3) lat[i + 2 * count] = nl;
   }
 }
 template <bool BLEND>
@@ -1283,6 +1301,31 @@ void cfg_sampler_launch(int kind, const SamplerStep& s, const float* eps_u, cons
   } else {
     w ? go(cfg_sampler_kernel<STEP_DPMPP_2M, true, false>) : go(cfg_sampler_kernel<STEP_DPMPP_2M, false, false>);
   }
+  SDB_CUDA(cudaGetLastError());
+}
+template <int KIND>
+__global__ void cfg3_sampler_kernel(const float* __restrict__ eps, float* __restrict__ lat, long long count, float scale_t,
+                                    float scale_i, float sqrt_1m_at, float sqrt_at, float sqrt_aprev, float dir_coef,
+                                    const SamplerStep s) {
+  cfg_step<KIND, false, false, 3>(eps, eps + count, lat, count, scale_t, sqrt_1m_at, sqrt_at, sqrt_aprev, dir_coef, nullptr,
+                                  nullptr, nullptr, 0, s, scale_i);
+}
+void cfg3_sampler_launch(int kind, const SamplerStep& s, const float* eps, float* latent, long long count, float text_scale,
+                         float image_scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef,
+                         cudaStream_t st) {
+  SDB_CHECK(kind == STEP_DDIM || kind == STEP_DDIM_ETA || kind == STEP_DPMPP_2M, "cfg3_sampler_launch: kind");
+  int grid = (int)((count + 255) / 256);
+  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
+  auto go = [&](auto kernel) {
+    launch_k(kernel, dim3(grid), dim3(256), 0, st, eps, latent, count, text_scale, image_scale, sqrt_one_minus_at, sqrt_at,
+             sqrt_aprev, dir_coef, s);
+  };
+  if (kind == STEP_DDIM)
+    go(cfg3_sampler_kernel<STEP_DDIM>);
+  else if (kind == STEP_DDIM_ETA)
+    go(cfg3_sampler_kernel<STEP_DDIM_ETA>);
+  else
+    go(cfg3_sampler_kernel<STEP_DPMPP_2M>);
   SDB_CUDA(cudaGetLastError());
 }
 void cfg_ddim_launch(const float* eps_u, const float* eps_c, float* latent, long long count, float scale,
@@ -1468,8 +1511,10 @@ __global__ void stage_cfg_context_kernel(const float* __restrict__ cond, int L, 
   }
 }
 void stage_cfg_context_launch(const float* cond, int L, const float* uncond, long long ustride, const int* lens, int n, int Lpad,
-                              float* out, cudaStream_t st) {
-  const long long total = 2ll * n * Lpad * 768;
+                              float* out, cudaStream_t st, int groups) {
+  // groups - 1 unconditional groups (rows b < (groups - 1) n) read uncond[b * ustride], then one prompt group
+  const long long total = (long long)groups * n * Lpad * 768;
+  n *= groups - 1;
   int grid = (int)((total + 255) / 256);
   if (grid > g_num_sms * 16) grid = g_num_sms * 16;
   launch_k(stage_cfg_context_kernel, dim3(grid), dim3(256), 0, st, cond, L, uncond, ustride, lens, n, Lpad, total, out);

@@ -68,11 +68,12 @@ void nhwc_to_nchw_launch(const float* x, int n, int C, int H, int W, float* y, c
 // pre: optional 1x1 4->4 conv (post_quant_conv) with scalar input scale applied to the input first.
 void conv3x3_cin4_launch(const float* x_nchw, int n, int H, int W, const float* w, const float* b, int Cout,
                          const float* pre_w, const float* pre_b, float pre_scale, float* y, Half2Ptr y16, cudaStream_t st);
-// the 9-channel inpainting UNet's conv_in (DESIGN §7 f9): channels 0-3 from x (sample stride x_stride), 4-8 from cond (sample stride
-// cond_stride, sample index modulo cond_mod); kConvCin9Pix output pixels per CTA
-constexpr int kConvCin9Pix = 32;
-void conv3x3_cin9_launch(const float* x, long long x_stride, const float* cond, long long cond_stride, int cond_mod, int n, int H,
-                         int W, const float* w, const float* b, int Cout, float* y, Half2Ptr y16, cudaStream_t st);
+// conv_in of a conditioned UNet, cin 9 (inpainting, DESIGN §7 f9) or 8 (InstructPix2Pix, f10): channels 0-3 from x (sample
+// stride x_stride), 4..cin-1 from cond (sample stride cond_stride, sample index modulo cond_mod); kConvCinCondPix output pixels
+// per CTA
+constexpr int kConvCinCondPix = 32;
+void conv3x3_cin_cond_launch(int cin, const float* x, long long x_stride, const float* cond, long long cond_stride, int cond_mod,
+                             int n, int H, int W, const float* w, const float* b, int Cout, float* y, Half2Ptr y16, cudaStream_t st);
 // 3x3 pad 1, Cout <= 4, input NHWC fp32 with fused GroupNorm+SiLU; output NCHW fp32 [n,Cout,H,W];
 // weights repacked [Cout][9][C] fp32.
 void conv3x3_small_cout_launch(const float* x, int n, int H, int W, int C, const double* sums, const float* gamma,
@@ -122,6 +123,12 @@ struct SamplerStep {   // per-step scalars, computed on the host in double and p
 void cfg_sampler_launch(int kind, const SamplerStep& s, const float* eps_u, const float* eps_c, float* latent, long long count,
                         float scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
                         const float* z0, const float* eps0, const float* w, int plane);
+// The three-way guidance + update of an InstructPix2Pix step (DESIGN §7 f10), one launch of any kind: eps [3][count] holds the
+// groups e_U | e_I | e_T, pred = e_U + text_scale (e_T - e_I) + image_scale (e_I - e_U), and the result goes to all three copies
+// of the latent in latent [3][count]. The update is cfg_sampler_launch's for the kind (STEP_DDIM: cfg_ddim_launch's).
+void cfg3_sampler_launch(int kind, const SamplerStep& s, const float* eps, float* latent, long long count, float text_scale,
+                         float image_scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef,
+                         cudaStream_t st);
 // ---- img2img staging: u8 HWC RGB [nb][Hp][Wp][3] -> encoder input [nb][4][Hp][Wp], v / 127.5 - 1, fourth plane zero
 void u8_to_enc_input_launch(const uint8_t* rgb, int nb, int Hp, int Wp, float* out, cudaStream_t st);
 // 9-channel inpainting: the masked image's encoder input [nb,4,Hp,Wp] and the latent mask into channel 0 of cond [nb,5,Hp/8,Wp/8]
@@ -152,9 +159,10 @@ void randn_seeds_launch(float* x, int n, long long per, const uint64_t* seeds, c
 // The CFG context of a sampling call: out [2n][Lpad][768], samples [0, n) the unconditional rows, [n, 2n) the prompt rows.
 // Row r of out sample b is copied when r < lens[b] (device [2n]: uncond lengths, then cond lengths) and zero otherwise, so the
 // caller's pad rows are never read. cond [n][L][768]; uncond [n][Lu][768] with ustride = Lu * 768, or [Lu][768] with ustride 0
-// (one negative broadcast over the batch).
+// (one negative broadcast over the batch). groups = 3 (InstructPix2Pix, DESIGN §7 f10): out [3n][Lpad][768], samples [0, 2n) the
+// negative, [2n, 3n) the prompt rows; ustride must be 0 then.
 void stage_cfg_context_launch(const float* cond, int L, const float* uncond, long long ustride, const int* lens, int n, int Lpad,
-                              float* out, cudaStream_t st);
+                              float* out, cudaStream_t st, int groups = 2);
 
 // ---- row softmax for the 1-head VAE attention: P = softmax(S*scale) rows -> fp16 hi(/lo)
 void softmax_rows_launch(const float* S, long long rows, int cols, float scale, Half2Ptr out, cudaStream_t st);

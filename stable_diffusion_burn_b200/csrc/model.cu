@@ -954,7 +954,7 @@ struct UNetIO {
   float* out;          // [nb,4,H,W] NCHW
   int H, W;
   const float* emb_all = nullptr;  // [1000][emb_total] rows precomputed per timestep value (sample_latent), or null
-  // 9-channel conv_in (DESIGN §7 f9): input channels 4-8 of sample i at cond + (i % cond_mod) * cond_stride
+  // 9- / 8-channel conv_in (DESIGN §7 f9, f10): input channels 4.. of sample i at cond + (i % cond_mod) * cond_stride
   long long x_stride = 0;
   const float* cond = nullptr;
   long long cond_stride = 0;
@@ -1000,9 +1000,9 @@ static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
       case BK_CONV: {
         o = f.act16(H, W, b.cout);
         KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * H * W * 9.0 * b.cin * b.cout);
-        if (b.cin == 9)
-          conv3x3_cin9_launch(io.x, io.x_stride, io.cond, io.cond_stride, io.cond_mod, f.nb, H, W, mptr(c, b.conv.wi), b.conv.bias,
-                              b.cout, o.p, o.raw16, c.stream);
+        if (b.cin != 4)
+          conv3x3_cin_cond_launch(b.cin, io.x, io.x_stride, io.cond, io.cond_stride, io.cond_mod, f.nb, H, W, mptr(c, b.conv.wi),
+                                  b.conv.bias, b.cout, o.p, o.raw16, c.stream);
         else
           conv3x3_cin4_launch(io.x, f.nb, H, W, mptr(c, b.conv.wi), b.conv.bias, b.cout, nullptr, nullptr, 1.f, o.p, o.raw16,
                               c.stream);
@@ -1296,8 +1296,8 @@ struct StreamJoin {  // run on c.stream ordered after / before the caller's stre
 }  // namespace
 
 // UNet pass over nb samples with per-sample context lengths. d_ctx_padded [nb][Lpad][768].
-// A 9-channel UNet reads d_x [nb,4,H,W] and d_cond [nb/2,5,H,W] (both CFG halves of a step share it), or with d_cond null
-// d_x [nb,9,H,W].
+// A 9-channel UNet reads d_x [nb,4,H,W] and d_cond [nb/2,5,H,W] (both CFG halves of a step share it), an 8-channel one d_x
+// [nb,4,H,W] and d_cond [nb,4,H,W] (each guidance group has its own); with d_cond null either reads d_x [nb,cin,H,W].
 static void unet_pass(Ctx& c, int nb, const float* d_x, const int* d_t, const float* d_ctx_padded, int Lpad, int* d_kvlen,
                       int H, int W, float* d_out, const CtxState* shared_cs, const float* emb_all = nullptr,
                       const float* d_cond = nullptr) {
@@ -1312,11 +1312,12 @@ static void unet_pass(Ctx& c, int nb, const float* d_x, const int* d_t, const fl
   UNetIO io{d_x, d_t, d_out, H, W};
   io.emb_all = emb_all;
   const long long hw = (long long)H * W;
-  if (c.unet_cin == 9) {
+  const int cin = c.unet_cin;
+  if (cin != 4) {
     if (d_cond)
-      io.x_stride = 4 * hw, io.cond = d_cond, io.cond_stride = 5 * hw, io.cond_mod = nb / 2;
+      io.x_stride = 4 * hw, io.cond = d_cond, io.cond_stride = (cin - 4) * hw, io.cond_mod = cin == 9 ? nb / 2 : nb;
     else
-      io.x_stride = 9 * hw, io.cond = d_x + 4 * hw, io.cond_stride = 9 * hw, io.cond_mod = nb;
+      io.x_stride = cin * hw, io.cond = d_x + 4 * hw, io.cond_stride = cin * hw, io.cond_mod = nb;
   }
   unet_forward(f, io, *cs);
   c.work.off = mark;
@@ -1431,11 +1432,19 @@ void model_latent_to_image_host(Ctx& c, const float* latent, int n, int H, int W
   SDB_CUDA(cudaStreamSynchronize(c.stream));
 }
 
+// an 8-channel InstructPix2Pix UNet (sdb_create_pix2pix) reads an image latent and runs three-way guidance: only sdb_edit_image
+// (and the single-pass sdb_unet_forward) drive it
+static void check_not_pix2pix(const Ctx& c, const char* what) {
+  SDB_CHECK(c.unet_cin != 8, std::string(what) + ": this context runs an 8-channel InstructPix2Pix UNet (sdb_create_pix2pix), "
+                                                 "which needs an input image and image guidance; call sdb_edit_image");
+}
+
 // a 9-channel UNet (sdb_create_inpaint) reads a mask and a masked-image latent that text-to-image does not have
 static void check_txt2img(const Ctx& c) {
-  SDB_CHECK(c.unet_cin == 4,
+  SDB_CHECK(c.unet_cin != 9,
             "sample: this context runs a 9-channel inpainting UNet (sdb_create_inpaint), which needs a mask and an image; for "
             "text-to-image call sdb_img2img with an all-255 mask at strength 1");
+  check_not_pix2pix(c, "sample");
 }
 
 static void check_sample_args(int n, int L, int Lu, int n_steps, int H, int W) {
@@ -1478,6 +1487,12 @@ struct Batch {
   const uint64_t* d_noise_seed = nullptr;  // device [n]: eta noise seeds of the per-sample step
 };
 
+// InstructPix2Pix (DESIGN §7 f10): what the sampler loop adds for three-way guidance
+struct EditIn {
+  const float* cond = nullptr;  // [3n,4,H,W]: 0 | c_I | c_I, one block per guidance group, read by the 8-channel conv_in
+  double image_scale = 0.0;     // s_I; the Batch's scale is s_T
+};
+
 Batch uniform_batch(const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale) {
   Batch b;
   b.n = n, b.cond = d_context, b.L = L, b.uncond = d_uncond, b.Lu = Lu, b.scale = scale;
@@ -1489,34 +1504,38 @@ Batch uniform_batch(const float* d_context, int n, int L, const float* d_uncond,
 // sample_latent + latent_to_image (stablediffusion/mod.rs:51-160) from schedule index `first` on. The conditional and
 // unconditional UNet evaluations of a step (forward_diffuser :162-192) run as ONE batch-2n pass: weights stream from HBM once.
 // ii == null: txt2img from d_init_latent. Otherwise the start latent and (with a mask) the per-step blend come from ii; a
-// 9-channel UNet reads ii->cond instead of blending. Runs on c.stream; the caller joins the streams.
+// 9-channel UNet reads ii->cond instead of blending. ei (an InstructPix2Pix edit, DESIGN §7 f10; ii null): the step's pass is
+// batch-3n, groups e_U | e_I | e_T (negative without the image, negative with it, prompt with it), and ei->cond holds each
+// group's image channels. Runs on c.stream; the caller joins the streams.
 static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const float* d_init_latent, const Img2ImgIn* ii, int H,
-                        int W, float* d_latent_out, uint8_t* d_rgb) {
+                        int W, float* d_latent_out, uint8_t* d_rgb, const EditIn* ei = nullptr) {
   Model& m = M(c);
   c.work.reset();
   const int n = b.n;
-  const int nb = 2 * n;
+  const int groups = ei ? 3 : 2;
+  const int nb = groups * n;
   // padded to the longest row count any sample reads, not to the caller's strides: the step graph is keyed on Lpad
   int lmax = 1;
   for (int i = 0; i < n; ++i) lmax = std::max(lmax, std::max(b.len[i], b.ulen[i]));
   const int Lpad = round_up(lmax, 32);
   const size_t le = (size_t)n * 4 * H * W;
-  // batch layout: samples [0,n) = unconditional context, [n,2n) = prompt context
+  // batch layout: samples [0,n) = unconditional context, [n,2n) = prompt context; an edit: [0,2n) negative, [2n,3n) prompt
   float* ctxp = c.work.get<float>((size_t)nb * Lpad * 768);
-  float* xb = c.work.get<float>(2 * le);
-  float* eps = c.work.get<float>(2 * le);
+  float* xb = c.work.get<float>(groups * le);
+  float* eps = c.work.get<float>(groups * le);
   int* d_t = c.work.get<int>(1024);
   int* d_len = c.work.get<int>(nb);
   std::vector<int> lens(nb);
-  for (int i = 0; i < nb; ++i) lens[i] = i < n ? b.ulen[i] : b.len[i - n];
+  const int nu = (groups - 1) * n;  // samples that read the negative
+  for (int i = 0; i < nb; ++i) lens[i] = i < nu ? b.ulen[i % n] : b.len[i - nu];
   SDB_CUDA(cudaMemcpyAsync(d_len, lens.data(), nb * 4, cudaMemcpyHostToDevice, c.stream));
   {
     KernelScope ks(c, KC_ELEMENTWISE);
-    stage_cfg_context_launch(b.cond, b.L, b.uncond, b.ustride, d_len, n, Lpad, ctxp, c.stream);
+    stage_cfg_context_launch(b.cond, b.L, b.uncond, b.ustride, d_len, n, Lpad, ctxp, c.stream, groups);
   }
   if (!ii) {
-    SDB_CUDA(cudaMemcpyAsync(xb, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
-    SDB_CUDA(cudaMemcpyAsync(xb + le, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
+    for (int g = 0; g < groups; ++g)
+      SDB_CUDA(cudaMemcpyAsync(xb + g * le, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
   } else {
     KernelScope ks(c, KC_ELEMENTWISE);
     img2img_prep_launch(ii->z0, ii->eps, xb, (long long)le, ii->sa, ii->sb, ii->mask, ii->w, H, W, c.stream);
@@ -1553,7 +1572,8 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const fl
   const long long key = ((long long)nb << 48) ^ ((long long)H << 36) ^ ((long long)W << 24) ^ ((long long)Lpad << 8) ^
                         (long long)(c.opt_precision & 3);
   const bool use_graph = c.opt_graphs && !c.profiling;
-  const float* cond = ii ? ii->cond : nullptr;  // an io slot that can grow and move between calls: part of the graph match
+  // an io slot that can grow and move between calls: part of the graph match
+  const float* cond = ii ? ii->cond : (ei ? ei->cond : nullptr);
   int* d_tcur = c.work.get<int>(1);
   const size_t work_mark = c.work.off;
   cudaGraphExec_t exec = nullptr;
@@ -1638,7 +1658,10 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const fl
       }
       s.hist = hist;
     }
-    if (kind == STEP_DDIM && !b.d_scale) {
+    if (ei) {
+      cfg3_sampler_launch(kind, s, eps, xb, (long long)le, (float)b.scale, (float)ei->image_scale, (float)std::sqrt(1.0 - a_t),
+                          (float)std::sqrt(a_t), (float)std::sqrt(a_prev), (float)dir, c.stream);
+    } else if (kind == STEP_DDIM && !b.d_scale) {
       cfg_ddim_launch(eps, eps + le, xb, (long long)le, (float)b.scale, (float)std::sqrt(1.0 - a_t), (float)std::sqrt(a_t),
                       (float)std::sqrt(a_prev), (float)dir, c.stream, blend ? ii->z0 : nullptr, blend ? ii->eps : nullptr,
                       blend ? ii->w : nullptr, H * W);
@@ -1700,6 +1723,7 @@ static int img2img_first(double strength, int n_steps) {
 
 static void check_img2img_args(const Ctx& c, int n, int L, int Lu, int n_steps, int H, int W, const void* image, const void* mask,
                                const void* context, const void* uncond, const void* latent_out, const void* rgb) {
+  check_not_pix2pix(c, "img2img");
   check_sample_args(n, L, Lu, n_steps, H, W);
   SDB_CHECK(image && context && uncond, "img2img: null image, context or uncond");
   SDB_CHECK(mask || c.unet_cin == 4, "img2img: the mask is NULL; a 9-channel inpainting UNet (sdb_create_inpaint) needs one");
@@ -1710,7 +1734,7 @@ static void check_img2img_args(const Ctx& c, int n, int L, int Lu, int n_steps, 
 // z0 and the latent mask live in io slots, not in the work arena: the arena prefix up to the loop's work_mark is laid out
 // exactly as txt2img lays it out, so no cached step graph can see img2img data where it expects its own temporaries.
 // A 9-channel UNet (DESIGN §7 f9) gets no blend: inpaint_prep writes the masked image's encoder input and the latent mask, and
-// a second encoder pass (the same chunks) writes z_m, so the conditioning tensor [n,5,H,W] (io slot kIoInpaintCond) holds
+// a second encoder pass (the same chunks) writes z_m, so the conditioning tensor [n,5,H,W] (io slot kIoUNetCond) holds
 // m_lat | z_m for conv_in.
 // Runs on c.stream; the caller has checked the arguments and joined the streams.
 static void img2img_run(Ctx& c, const Batch& b, const uint8_t* d_image, const uint8_t* d_mask, double strength, int n_steps,
@@ -1726,7 +1750,7 @@ static void img2img_run(Ctx& c, const Batch& b, const uint8_t* d_image, const ui
   const size_t le = (size_t)n * 4 * H * W;
   ii.z0 = (float*)c.io(kIoImg2ImgZ0, le * 4);
   if (ii.mask) ii.w = (float*)c.io(kIoImg2ImgW, (size_t)n * H * W * 4);
-  float* cond = inpaint ? (float*)c.io(kIoInpaintCond, (size_t)n * 5 * H * W * 4) : nullptr;
+  float* cond = inpaint ? (float*)c.io(kIoUNetCond, (size_t)n * 5 * H * W * 4) : nullptr;
   c.work.reset();
   const int Hp = 8 * H, Wp = 8 * W;
   const size_t plane = (size_t)Hp * Wp;
@@ -1794,6 +1818,89 @@ void model_img2img_host(Ctx& c, const uint8_t* image, const uint8_t* mask, doubl
   else
     randn_launch(d_n, (long long)le, seed, c.stream);  // the latent txt2img would start from for this seed
   model_img2img_dev(c, d_i, d_m, strength, d_c, n, L, d_u, Lu, scale, n_steps, d_n, H, W, d_lo, d_r, c.stream);
+  if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
+  if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+// ================================================================================ InstructPix2Pix (DESIGN §7 f10)
+static void check_edit_args(const Ctx& c, int n, int L, int Lu, double text_scale, double image_scale, int n_steps, int H, int W,
+                            const void* image, const void* context, const void* uncond, const void* latent_out, const void* rgb) {
+  char msg[240];
+  snprintf(msg, sizeof(msg),
+           "edit_image: this context's UNet takes %d input channels; InstructPix2Pix needs the 8-channel UNet of a context from "
+           "sdb_create_pix2pix",
+           c.unet_cin);
+  SDB_CHECK(c.unet_cin == 8, msg);
+  check_sample_args(n, L, Lu, n_steps, H, W);
+  SDB_CHECK(image && context && uncond, "edit_image: null image, context or uncond");
+  SDB_CHECK(latent_out || rgb, "edit_image: request the latent, the image or both");
+  snprintf(msg, sizeof(msg), "edit_image: text_scale = %.17g is not finite", text_scale);
+  SDB_CHECK(std::isfinite(text_scale), msg);
+  snprintf(msg, sizeof(msg), "edit_image: image_scale = %.17g is not finite", image_scale);
+  SDB_CHECK(std::isfinite(image_scale), msg);
+}
+
+// The encoder (chunks of 4 images, as model_encode_dev) writes c_I, unscaled, into group 1 of the conditioning tensor
+// [3n,4,H,W] (io slot kIoUNetCond, outside the work arena like img2img's z0); group 2 is a copy and group 0 zero. Then the
+// sampler loop from t = 999 over the full schedule with three guidance groups.
+// Runs on c.stream; the caller has checked the arguments and joined the streams.
+static void edit_run(Ctx& c, const Batch& b, double image_scale, const uint8_t* d_image, int n_steps, const float* d_init_latent,
+                     int H, int W, float* d_latent_out, uint8_t* d_rgb) {
+  const int n = b.n;
+  const size_t le = (size_t)n * 4 * H * W;
+  float* cond = (float*)c.io(kIoUNetCond, 3 * le * 4);
+  c.work.reset();
+  const int Hp = 8 * H, Wp = 8 * W;
+  const size_t plane = (size_t)Hp * Wp;
+  SDB_CUDA(cudaMemsetAsync(cond, 0, le * 4, c.stream));
+  for (int i0 = 0; i0 < n; i0 += 4) {
+    const int nb = std::min(4, n - i0);
+    const size_t mark = c.work.off;
+    float* img4 = c.work.get<float>((size_t)nb * 4 * plane);
+    {
+      KernelScope ks(c, KC_ELEMENTWISE);
+      u8_to_enc_input_launch(d_image + (size_t)i0 * 3 * plane, nb, Hp, Wp, img4, c.stream);
+    }
+    Fwd f(c, nb);
+    vae_encode(f, img4, Hp, Wp, cond + le + (size_t)i0 * 4 * H * W);
+    c.work.off = mark;
+  }
+  SDB_CUDA(cudaMemcpyAsync(cond + 2 * le, cond + le, le * 4, cudaMemcpyDeviceToDevice, c.stream));
+  EditIn ei;
+  ei.cond = cond, ei.image_scale = image_scale;
+  sample_loop(c, b, n_steps, 0, d_init_latent, nullptr, H, W, d_latent_out, d_rgb, &ei);
+}
+
+void model_edit_dev(Ctx& c, const uint8_t* d_image, const float* d_context, int n, int L, const float* d_uncond, int Lu,
+                    double text_scale, double image_scale, int n_steps, const float* d_init_latent, int H, int W,
+                    float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
+  check_edit_args(c, n, L, Lu, text_scale, image_scale, n_steps, H, W, d_image, d_context, d_uncond, d_latent_out, d_rgb);
+  SDB_CHECK(d_init_latent, "edit_image: the device entry needs the start latent");
+  StreamJoin join(c, caller);
+  edit_run(c, uniform_batch(d_context, n, L, d_uncond, Lu, text_scale), image_scale, d_image, n_steps, d_init_latent, H, W,
+           d_latent_out, d_rgb);
+}
+
+void model_edit_host(Ctx& c, const uint8_t* image, const float* context, int n, int L, const float* uncond, int Lu,
+                     double text_scale, double image_scale, int n_steps, const float* init_latent, uint64_t seed, int H, int W,
+                     float* latent_out, uint8_t* rgb) {
+  check_edit_args(c, n, L, Lu, text_scale, image_scale, n_steps, H, W, image, context, uncond, latent_out, rgb);
+  const size_t le = (size_t)n * 4 * H * W, ce = (size_t)n * L * 768, ue = (size_t)Lu * 768, re = (size_t)n * 3 * 64 * H * W;
+  float* d_c = (float*)c.io(0, ce * 4);
+  float* d_u = (float*)c.io(1, ue * 4);
+  float* d_l = (float*)c.io(2, le * 4);
+  float* d_lo = latent_out ? (float*)c.io(3, le * 4) : nullptr;
+  uint8_t* d_r = rgb ? (uint8_t*)c.io(4, re) : nullptr;
+  uint8_t* d_i = (uint8_t*)c.io(5, re);
+  SDB_CUDA(cudaMemcpyAsync(d_c, context, ce * 4, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(d_u, uncond, ue * 4, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(d_i, image, re, cudaMemcpyHostToDevice, c.stream));
+  if (init_latent)
+    SDB_CUDA(cudaMemcpyAsync(d_l, init_latent, le * 4, cudaMemcpyHostToDevice, c.stream));
+  else
+    randn_launch(d_l, (long long)le, seed, c.stream);  // the latent sdb_sample_image starts from for this seed
+  model_edit_dev(c, d_i, d_c, n, L, d_u, Lu, text_scale, image_scale, n_steps, d_l, H, W, d_lo, d_r, c.stream);
   if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
   if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
@@ -1949,6 +2056,7 @@ void model_img2img_batch_host(Ctx& c, const sdb_batch* sb, const uint8_t* image,
 // same pass sample_latent replays as a CUDA graph), then pred = u + (c - u) * scale. d_u / d_c may be null.
 void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const float* d_context, int n, int L, const float* d_uncond,
                                 int Lu, double scale, int H, int W, float* d_pred, float* d_u, float* d_c, cudaStream_t caller) {
+  check_not_pix2pix(c, "forward_diffuser (two-way guidance)");
   SDB_CHECK(n >= 1 && L >= 1 && Lu >= 1 && t >= 0 && t < 1000, "forward_diffuser arguments");
   SDB_CHECK(H % 8 == 0 && W % 8 == 0 && ((H / 8) * (W / 8)) % 8 == 0, "unsupported latent size");
   StreamJoin join(c, caller);

@@ -6,7 +6,8 @@
 namespace sdb {
 
 void model_create(Ctx& c);   // builds the tensor registry, allocates arenas
-// rejects a unet/input_blocks/conv/weight of [320,C,3,3] with C != c.unet_cin, naming both shapes and the create entry to use
+// rejects a unet/input_blocks/conv/weight of [320,C,3,3] with C != c.unet_cin (4, 8 or 9), naming both shapes and the create
+// entry to use
 void check_conv_in_shape(const Ctx& c, const std::string& what, int ndim, const int64_t* dims);
 void model_destroy(Ctx& c);
 void model_init_synthetic(Ctx& c, uint32_t seed);
@@ -50,6 +51,13 @@ void model_img2img_batch_dev(Ctx& c, const sdb_batch* b, const uint8_t* d_image,
                              cudaStream_t caller);
 void model_img2img_batch_host(Ctx& c, const sdb_batch* b, const uint8_t* image, const uint8_t* mask, double strength,
                               int n_steps, const float* noise, int H, int W, float* latent_out, uint8_t* rgb);
+// InstructPix2Pix (DESIGN §7 f10) on an 8-channel context: three-way guidance from t = 999, the image latent unscaled
+void model_edit_dev(Ctx& c, const uint8_t* d_image, const float* d_context, int n, int L, const float* d_uncond, int Lu,
+                    double text_scale, double image_scale, int n_steps, const float* d_init_latent, int H, int W,
+                    float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller);
+void model_edit_host(Ctx& c, const uint8_t* image, const float* context, int n, int L, const float* uncond, int Lu,
+                     double text_scale, double image_scale, int n_steps, const float* init_latent, uint64_t seed, int H, int W,
+                     float* latent_out, uint8_t* rgb);
 void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const float* d_context, int n, int L, const float* d_uncond,
                                 int Lu, double scale, int H, int W, float* d_pred, float* d_u, float* d_c, cudaStream_t caller);
 void model_forward_diffuser_host(Ctx& c, const float* latent, int t, const float* context, int n, int L, const float* uncond,

@@ -166,10 +166,12 @@ void model_create(Ctx& c) {
   int level = 0;
   for (int i = 0; i < 12; ++i) {
     BlockSpec s = kInBlocks[i];
-    if (i == 0) s.cin = c.unet_cin;  // 9 for an inpainting UNet (sdb_create_inpaint): latent | mask | masked-image latent
+    // 9 for an inpainting UNet (sdb_create_inpaint): latent | mask | masked-image latent; 8 for InstructPix2Pix
+    // (sdb_create_pix2pix): latent | image latent
+    if (i == 0) s.cin = c.unet_cin;
     build_block(b, m->in_blocks[i], std::string("unet/input_blocks/") + s.field, s);
     m->in_blocks[i].level = level;
-    if (i == 0) c.tensors[m->in_blocks[0].conv.bi].fan_in = 4 * 9;  // only the weight of a 9-channel conv_in differs
+    if (i == 0) c.tensors[m->in_blocks[0].conv.bi].fan_in = 4 * 9;  // only the weight of a wider conv_in differs
     if (kInBlocks[i].kind == BK_DOWN) level++;  // following blocks run one level lower (the down conv itself reads level-1 input)
   }
   b.resblock(m->mid_res1, "unet/middle_block/res1", 1280, 1280);
@@ -277,13 +279,13 @@ void model_create(Ctx& c) {
 
 void check_conv_in_shape(const Ctx& c, const std::string& what, int ndim, const int64_t* dims) {
   if (ndim != 4 || dims[1] == c.unet_cin) return;  // other mismatches get the generic shape message
-  const bool nine = dims[1] == 9;
+  const char* use = dims[1] == 9   ? "a 9-channel inpainting UNet loads into a context from sdb_create_inpaint"
+                    : dims[1] == 8 ? "an 8-channel InstructPix2Pix UNet loads into a context from sdb_create_pix2pix"
+                                   : "a 4-channel UNet loads into a context from sdb_create";
   char msg[400];
   snprintf(msg, sizeof(msg),
            "%s: unet/input_blocks/conv/weight is [%lld,%lld,%lld,%lld] but this context's conv_in is [320,%d,3,3]; %s",
-           what.c_str(), (long long)dims[0], (long long)dims[1], (long long)dims[2], (long long)dims[3], c.unet_cin,
-           nine ? "a 9-channel inpainting UNet loads into a context from sdb_create_inpaint"
-                : "a 4-channel UNet loads into a context from sdb_create");
+           what.c_str(), (long long)dims[0], (long long)dims[1], (long long)dims[2], (long long)dims[3], c.unet_cin, use);
   throw Error(msg);
 }
 

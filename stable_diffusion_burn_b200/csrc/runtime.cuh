@@ -120,7 +120,9 @@ constexpr int kIoImg2ImgZ0 = 8;  // encoded image latent z0 [n,4,H,W]
 constexpr int kIoImg2ImgW = 9;   // latent mask w [n,H,W]
 constexpr int kIoSamplerHist = 10;  // DPM-Solver++(2M): x0 of the previous step [n,4,H,W]
 constexpr int kIoBatchTab = 11;     // per-sample tables of a batch call: seeds, noise seeds [n] u64, guidance scales [n] f32
-constexpr int kIoInpaintCond = 12;  // 9-channel inpainting: the UNet's extra input channels [n,5,H,W] = latent mask | z_m
+// a conditioned UNet's extra input channels: [n,5,H,W] = latent mask | z_m (9-channel inpainting) or [3n,4,H,W] = 0 | c_I | c_I
+// (8-channel InstructPix2Pix, one per guidance group); a context is only ever one of the two kinds
+constexpr int kIoUNetCond = 12;
 
 struct Ctx {
   int device = 0;
@@ -150,7 +152,8 @@ struct Ctx {
   int sampler_kind = 0;
   double sampler_eta = 0.0;
   uint64_t sampler_noise_seed = 0;
-  // input channels of the UNet's conv_in: 4 (sdb_create) or 9 (sdb_create_inpaint: latent | mask | masked-image latent)
+  // input channels of the UNet's conv_in: 4 (sdb_create), 9 (sdb_create_inpaint: latent | mask | masked-image latent) or 8
+  // (sdb_create_pix2pix: latent | image latent)
   int unet_cin = 4;
   // profiling
   bool profiling = false;
@@ -160,7 +163,7 @@ struct Ctx {
   double cls_issued[KC_COUNT] = {0};  // tensor-core FLOPs actually issued (x passes for split-fp16 products)
   int64_t cls_launches[KC_COUNT] = {0};
   // grow-only device staging for the host-buffer entry points (no cudaMalloc/cudaFree per call: each is a device-wide sync).
-  // Slots 0..6: host-entry staging; kIoImg2Img*, kIoSamplerHist, kIoBatchTab, kIoInpaintCond: buffers the sampling entries
+  // Slots 0..6: host-entry staging; kIoImg2Img*, kIoSamplerHist, kIoBatchTab, kIoUNetCond: buffers the sampling entries
   // keep outside the work arena.
   struct IoBuf {
     void* p = nullptr;

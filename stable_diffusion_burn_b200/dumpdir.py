@@ -68,14 +68,14 @@ def conv_stride(name: str) -> int:
 
 
 def save_dump_dir(root: str, params: dict, eps: float | dict = 1e-5) -> None:
-    """Writes `params` (registry name -> array, incl. "alpha_cumulative_products") as the reference's dump-dir; a 9-channel
-    conv_in writes the inpainting registry (DESIGN.md §7 f9)."""
-    inpaint = CONV_IN in params and np.shape(params[CONV_IN])[1] == 9
+    """Writes `params` (registry name -> array, incl. "alpha_cumulative_products") as the reference's dump-dir; a 9- or
+    8-channel conv_in writes the inpainting (DESIGN.md §7 f9) or InstructPix2Pix (f10) registry."""
+    width = np.shape(params[CONV_IN])[1] if CONV_IN in params else 4
     eps_of = (lambda d: eps.get(d, 1e-5)) if isinstance(eps, dict) else (lambda d: eps)
     os.makedirs(root, exist_ok=True)
     save_scalar(1000, "n_steps", root)
     save_tensor(params[SCHEDULE_NAME], SCHEDULE_FILE, root)
-    for name, shape, kind, _ in topology.all_params(inpaint):
+    for name, shape, kind, _ in topology.conv_in_width_params(width):
         if name not in params:
             continue  # optional tensor left out on purpose (bias / GroupNorm affine)
         d, leaf = name.rsplit("/", 1)
@@ -120,13 +120,13 @@ def save_dump_dir(root: str, params: dict, eps: float | dict = 1e-5) -> None:
 
 
 def load_dump_dir(root: str) -> dict:
-    """numpy reader (for the oracle): registry name -> array, optional tensors filled like the reference does. A 9-channel
-    conv_in reads the inpainting registry."""
+    """numpy reader (for the oracle): registry name -> array, optional tensors filled like the reference does. A 9- or
+    8-channel conv_in reads the inpainting or InstructPix2Pix registry."""
     out = {SCHEDULE_NAME: read_tensor(os.path.join(root, SCHEDULE_FILE + ".npy"))}
     group = {d for d, _, g in _norm_dirs() if g}
     conv_in = os.path.join(root, CONV_IN + ".npy")
-    inpaint = os.path.exists(conv_in) and read_tensor(conv_in).shape[1] == 9
-    for name, shape, kind, _ in topology.all_params(inpaint):
+    width = read_tensor(conv_in).shape[1] if os.path.exists(conv_in) else 4
+    for name, shape, kind, _ in topology.conv_in_width_params(width):
         f = os.path.join(root, name + ".npy")
         if os.path.exists(f):
             a = read_tensor(f)

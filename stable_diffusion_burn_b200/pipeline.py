@@ -25,8 +25,8 @@ class UNet:
         self._c = ctx
 
     def forward(self, x: np.ndarray, timesteps, context: np.ndarray) -> np.ndarray:
-        """x [n,4,H,W] (an inpainting UNet: [n,9,H,W] = latent | mask | masked-image latent); timesteps Int[1] (one t for
-        the batch); context [n,L,768] -> [n,4,H,W]."""
+        """x [n,4,H,W] (an inpainting UNet: [n,9,H,W] = latent | mask | masked-image latent; an InstructPix2Pix UNet:
+        [n,8,H,W] = latent | image latent); timesteps Int[1] (one t for the batch); context [n,L,768] -> [n,4,H,W]."""
         ts = np.asarray(timesteps).reshape(-1)
         if ts.size != 1:
             raise ValueError("timesteps must hold exactly one value (reference: Tensor<B,1,Int> of length 1)")
@@ -61,10 +61,12 @@ class CLIP:
 
 class StableDiffusion:
     """Owns the device context; `diffusion`, `autoencoder` and `clip` mirror the reference's fields. inpaint=True holds an
-    inpainting checkpoint (a 9-channel UNet, DESIGN.md §7 f9): img2img then needs a mask, and the txt2img calls fail."""
+    inpainting checkpoint (a 9-channel UNet, DESIGN.md §7 f9): img2img then needs a mask, and the txt2img calls fail.
+    pix2pix=True holds an InstructPix2Pix checkpoint (an 8-channel UNet, f10): edit_image is then the sampling call, and the
+    txt2img, img2img and batch calls fail."""
 
-    def __init__(self, device: int = 0, inpaint: bool = False):
-        self.ctx = Context(device, inpaint=inpaint)
+    def __init__(self, device: int = 0, inpaint: bool = False, pix2pix: bool = False):
+        self.ctx = Context(device, inpaint=inpaint, pix2pix=pix2pix)
         self.diffusion = UNet(self.ctx)
         self.autoencoder = Autoencoder(self.ctx)
         self.clip = CLIP(self.ctx)
@@ -168,6 +170,19 @@ class StableDiffusion:
         with self._sampler(sampler, eta, noise_seed):
             rgb = self.ctx.img2img(image, context, unconditional_context, unconditional_guidance_scale, n_steps, strength,
                                    mask=mask, noise=noise, seed=seed)
+        return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
+
+    def edit_image(self, image, context, unconditional_context, guidance_scale: float = 7.5, image_guidance_scale: float = 1.5,
+                   n_steps: int = 100, init_latent=None, seed: int = 0, sampler: str = "ddim", eta: float = 0.0,
+                   noise_seed: int = 0):
+        """InstructPix2Pix editing (pix2pix=True; DESIGN.md §7 f10): image u8 [n, height, width, 3] HWC RGB, the format
+        sample_image returns; context [n, L, 768] the instructions; unconditional_context [Lu, 768]. Every step runs the UNet on
+        (no image, negative), (image, negative) and (image, instruction) and combines them with guidance_scale (text) and
+        image_guidance_scale, the defaults of the original pipeline. -> list of n flat uint8 arrays of height*width*3, like
+        sample_image."""
+        with self._sampler(sampler, eta, noise_seed):
+            rgb = self.ctx.edit_image(image, context, unconditional_context, guidance_scale, image_guidance_scale, n_steps,
+                                      init_latent=init_latent, seed=seed)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
 
     # ---- batches of different requests (an extension, DESIGN.md §7 f7): one UNet pass per step for all of them

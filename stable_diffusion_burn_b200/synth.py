@@ -98,10 +98,11 @@ def alpha_cumulative_products() -> np.ndarray:
     return np.cumprod(1.0 - betas).astype(np.float32)
 
 
-def make_params(seed: int = 0, which=None, inpaint=False) -> dict:
-    """name -> np.float32 array for every tensor on the path (≈3.6 GB fp32 in total). inpaint: the 9-channel registry, whose
-    tensors other than unet/input_blocks/conv/weight equal the 4-channel ones (the stream is keyed by name)."""
-    plist = topology.all_params(inpaint) if which is None else which
+def make_params(seed: int = 0, which=None, inpaint=False, pix2pix=False) -> dict:
+    """name -> np.float32 array for every tensor on the path (≈3.6 GB fp32 in total). inpaint: the 9-channel registry, pix2pix:
+    the 8-channel one; their tensors other than unet/input_blocks/conv/weight equal the 4-channel ones (the stream is keyed by
+    name)."""
+    plist = topology.all_params(inpaint, pix2pix) if which is None else which
     out = {n: make_tensor(n, s, k, f, seed) for (n, s, k, f) in plist}
     out["alpha_cumulative_products"] = alpha_cumulative_products()
     return out

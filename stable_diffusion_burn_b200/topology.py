@@ -107,16 +107,20 @@ def _unet_block(out, name, kind, cin, cout):
         raise ValueError(kind)
 
 
-def unet_params(prefix="unet", in_channels=4):
-    """in_channels: 4 (SD-v1) or 9 (an inpainting UNet: conv_in reads latent | mask | masked-image latent, DESIGN.md §7 f9)."""
+def unet_params(prefix="unet", in_channels=4, pix2pix=False):
+    """in_channels: 4 (SD-v1) or 9 (an inpainting UNet: conv_in reads latent | mask | masked-image latent, DESIGN.md §7 f9).
+    pix2pix=True (with in_channels 4): the InstructPix2Pix UNet, whose conv_in reads latent | image latent, 8 channels (f10)."""
     if in_channels not in (4, 9):
-        raise ValueError(f"in_channels must be 4 or 9, got {in_channels}")
+        raise ValueError(f"in_channels must be 4 or 9, got {in_channels} (the 8-channel InstructPix2Pix UNet is pix2pix=True)")
+    if pix2pix and in_channels != 4:
+        raise ValueError("pix2pix=True widens the 4-channel conv_in to 8 channels; in_channels must be 4")
+    conv_in = 8 if pix2pix else in_channels
     out = []
     _lin(out, f"{prefix}/lin1_time_embed", 320, EMB_DIM)
     _lin(out, f"{prefix}/lin2_time_embed", EMB_DIM, EMB_DIM)
     for i, (f, kind, cin, cout) in enumerate(UNET_INPUT_BLOCKS):
-        _unet_block(out, f"{prefix}/input_blocks/{f}", kind, in_channels if i == 0 else cin, cout)
-    # conv_in's bias keeps the 4-channel fan-in: only the weight of a 9-channel registry differs (its synthetic stream too)
+        _unet_block(out, f"{prefix}/input_blocks/{f}", kind, conv_in if i == 0 else cin, cout)
+    # conv_in's bias keeps the 4-channel fan-in: only the weight of a wider registry differs (its synthetic stream too)
     b = next(i for i, e in enumerate(out) if e[0] == f"{prefix}/input_blocks/conv/bias")
     out[b] = out[b][:3] + (4 * 9,)
     # middle: ResTransformerRes(1280,1280,1280,768,8) unet/mod.rs:58, 328-351
@@ -215,9 +219,20 @@ def clip_params(prefix="clip"):
     return out
 
 
-def all_params(inpaint=False):
-    """The registry in sdb_create's order; inpaint=True: sdb_create_inpaint's (a 9-channel unet/input_blocks/conv)."""
-    return unet_params(in_channels=9 if inpaint else 4) + vae_decoder_params() + clip_params() + vae_encoder_params()
+def all_params(inpaint=False, pix2pix=False):
+    """The registry in sdb_create's order; inpaint=True: sdb_create_inpaint's (a 9-channel unet/input_blocks/conv);
+    pix2pix=True: sdb_create_pix2pix's (an 8-channel one)."""
+    if inpaint and pix2pix:
+        raise ValueError("a registry is either the inpainting (inpaint=True) or the InstructPix2Pix (pix2pix=True) one")
+    return (unet_params(in_channels=9 if inpaint else 4, pix2pix=pix2pix) + vae_decoder_params() + clip_params() +
+            vae_encoder_params())
+
+
+def conv_in_width_params(width):
+    """all_params of the registry whose unet/input_blocks/conv/weight has `width` input channels (4, 8 or 9)."""
+    if width not in (4, 8, 9):
+        raise ValueError(f"no registry has a {width}-channel conv_in (4, 8 or 9)")
+    return all_params(inpaint=width == 9, pix2pix=width == 8)
 
 
 if __name__ == "__main__":
