@@ -210,6 +210,60 @@ def batch_struct(b, context_ptr=None, uncond_ptr=None):
                     p(b["seed"], C.c_uint64), p(b["noise_seed"], C.c_uint64))
 
 
+def _check_outputs(latent, rgb):
+    if not (latent or rgb):
+        raise ValueError("request the latent, the image or both")
+
+
+def _outputs(n, H, W, latent, rgb):
+    """the requested outputs: the latent [n,4,H,W] and / or the u8 image [n,8H,8W,3], None for the other"""
+    return (np.empty((n, 4, H, W), np.float32) if latent else None,
+            np.empty((n, 8 * H, 8 * W, 3), np.uint8) if rgb else None)
+
+
+def _result(lat, out):
+    """a tuple (latent, rgb) when both were requested, else the one that was"""
+    if lat is not None and out is not None:
+        return lat, out
+    return out if lat is None else lat
+
+
+def _u8ptr(a):
+    return None if a is None else a.ctypes.data_as(_u8p)
+
+
+def _fptr(a):
+    return None if a is None else ptr(a)
+
+
+def _image(image, n=None):
+    """u8 [n, 8H, 8W, 3] (n checked when given) -> (the contiguous image, H, W) of the latent"""
+    image = np.ascontiguousarray(image, dtype=np.uint8)
+    if (image.ndim != 4 or (n is not None and image.shape[0] != n) or image.shape[3] != 3 or image.shape[1] % 8
+            or image.shape[2] % 8):
+        raise ValueError("image must be u8 [n, 8H, 8W, 3]")
+    return image, image.shape[1] // 8, image.shape[2] // 8
+
+
+def _mask(mask, image):
+    if mask is None:
+        return None
+    mask = np.ascontiguousarray(mask, dtype=np.uint8)
+    if mask.shape != image.shape[:3]:
+        raise ValueError("mask must be u8 [n, 8H, 8W]")
+    return mask
+
+
+def _latent(a, shape, what):
+    """None, or `a` as f32 of `shape` [n, 4, H, W]"""
+    if a is None:
+        return None
+    a = f32(a)
+    if a.shape != shape:
+        raise ValueError(f"{what} must be [n, 4, H, W]")
+    return a
+
+
 class Context:
     """Owns one sdb_ctx (one CUDA device). inpaint=True: a 9-channel inpainting UNet (sdb_create_inpaint, DESIGN.md §7 f9);
     pix2pix=True: an 8-channel InstructPix2Pix UNet (sdb_create_pix2pix, f10)."""
@@ -432,68 +486,42 @@ class Context:
         (255 = regenerate, 0 = keep) or None; noise [n,4,H,W] or None (the seeded stream sample_image starts from). On an
         inpainting context the mask is required and binary (>= 128 regenerates) and conditions the UNet instead of a blend.
         -> the latent [n,4,H,W] and / or the u8 image [n,8H,8W,3]: a tuple (latent, rgb) when both are requested."""
-        if not (latent or rgb):
-            raise ValueError("request the latent, the image or both")
-        image = np.ascontiguousarray(image, dtype=np.uint8)
-        if image.ndim != 4 or image.shape[3] != 3 or image.shape[1] % 8 or image.shape[2] % 8:
-            raise ValueError("image must be u8 [n, 8H, 8W, 3]")
-        n, Hp, Wp, _ = image.shape
-        H, W = Hp // 8, Wp // 8
+        _check_outputs(latent, rgb)
+        image, H, W = _image(image)
+        n = image.shape[0]
         context = f32(context); uncond = f32(uncond)
-        if mask is not None:
-            mask = np.ascontiguousarray(mask, dtype=np.uint8)
-            if mask.shape != (n, Hp, Wp):
-                raise ValueError("mask must be u8 [n, 8H, 8W]")
-        if noise is not None:
-            noise = f32(noise)
-            if noise.shape != (n, 4, H, W):
-                raise ValueError("noise must be [n, 4, H, W]")
-        lat = np.empty((n, 4, H, W), np.float32) if latent else None
-        out = np.empty((n, Hp, Wp, 3), np.uint8) if rgb else None
-        self.check(self.lib.sdb_img2img(self.h, image.ctypes.data_as(_u8p), None if mask is None else mask.ctypes.data_as(_u8p),
-                                        float(strength), ptr(context), n, context.shape[1], ptr(uncond), uncond.shape[0],
-                                        float(scale), int(n_steps), None if noise is None else ptr(noise), int(seed), H, W,
-                                        None if lat is None else ptr(lat), None if out is None else out.ctypes.data_as(_u8p)))
-        if latent and rgb:
-            return lat, out
-        return lat if latent else out
+        mask = _mask(mask, image)
+        noise = _latent(noise, (n, 4, H, W), "noise")
+        lat, out = _outputs(n, H, W, latent, rgb)
+        self.check(self.lib.sdb_img2img(self.h, _u8ptr(image), _u8ptr(mask), float(strength), ptr(context), n, context.shape[1],
+                                        ptr(uncond), uncond.shape[0], float(scale), int(n_steps), _fptr(noise), int(seed), H, W,
+                                        _fptr(lat), _u8ptr(out)))
+        return _result(lat, out)
 
     def edit_image(self, image, context, uncond, text_scale, image_scale, n_steps, init_latent=None, seed=0, latent=False,
                    rgb=True):
         """InstructPix2Pix image editing on an 8-channel context (include/sdb200.h: sdb_edit_image). image u8 [n,8H,8W,3];
         context [n,L,768]; uncond [Lu,768]; init_latent [n,4,H,W] or None (the seeded stream sample_image starts from).
         -> the latent [n,4,H,W] and / or the u8 image [n,8H,8W,3]: a tuple (latent, rgb) when both are requested."""
-        if not (latent or rgb):
-            raise ValueError("request the latent, the image or both")
-        image = np.ascontiguousarray(image, dtype=np.uint8)
-        if image.ndim != 4 or image.shape[3] != 3 or image.shape[1] % 8 or image.shape[2] % 8:
-            raise ValueError("image must be u8 [n, 8H, 8W, 3]")
-        n, Hp, Wp, _ = image.shape
-        H, W = Hp // 8, Wp // 8
+        _check_outputs(latent, rgb)
+        image, H, W = _image(image)
+        n = image.shape[0]
         context = f32(context); uncond = f32(uncond)
         if context.ndim != 3 or context.shape[0] != n:
             raise ValueError("context must be [n, L, 768], one prompt per image")
-        if init_latent is not None:
-            init_latent = f32(init_latent)
-            if init_latent.shape != (n, 4, H, W):
-                raise ValueError("init_latent must be [n, 4, H, W]")
-        lat = np.empty((n, 4, H, W), np.float32) if latent else None
-        out = np.empty((n, Hp, Wp, 3), np.uint8) if rgb else None
-        self.check(self.lib.sdb_edit_image(self.h, image.ctypes.data_as(_u8p), ptr(context), n, context.shape[1], ptr(uncond),
-                                           uncond.shape[0], float(text_scale), float(image_scale), int(n_steps),
-                                           None if init_latent is None else ptr(init_latent), int(seed), H, W,
-                                           None if lat is None else ptr(lat), None if out is None else out.ctypes.data_as(_u8p)))
-        if latent and rgb:
-            return lat, out
-        return lat if latent else out
+        init_latent = _latent(init_latent, (n, 4, H, W), "init_latent")
+        lat, out = _outputs(n, H, W, latent, rgb)
+        self.check(self.lib.sdb_edit_image(self.h, _u8ptr(image), ptr(context), n, context.shape[1], ptr(uncond), uncond.shape[0],
+                                           float(text_scale), float(image_scale), int(n_steps), _fptr(init_latent), int(seed), H, W,
+                                           _fptr(lat), _u8ptr(out)))
+        return _result(lat, out)
 
     def sample_batch(self, contexts, unconds, scales, n_steps, seeds=None, noise_seeds=None, init_latent=None, H=64, W=64,
                      latent=False, rgb=True):
         """n different requests in one call (include/sdb200.h: sdb_sample_batch; pack_batch for the arguments). init_latent
         [n,4,H,W] or None (each request's latent from its seed). -> the latent [n,4,H,W] and / or the u8 image [n,8H,8W,3]: a
         tuple (latent, rgb) when both are requested."""
-        if not (latent or rgb):
-            raise ValueError("request the latent, the image or both")
+        _check_outputs(latent, rgb)
         b = pack_batch(contexts, unconds, scales, seeds, noise_seeds)
         n = b["context"].shape[0]
         if init_latent is not None:
@@ -501,46 +529,26 @@ class Context:
             if init_latent.ndim != 4 or init_latent.shape[:2] != (n, 4):
                 raise ValueError("init_latent must be [n, 4, H, W]")
             H, W = init_latent.shape[2:]
-        lat = np.empty((n, 4, H, W), np.float32) if latent else None
-        out = np.empty((n, 8 * H, 8 * W, 3), np.uint8) if rgb else None
-        self.check(self.lib.sdb_sample_batch(self.h, C.byref(batch_struct(b)), int(n_steps),
-                                             None if init_latent is None else ptr(init_latent), H, W,
-                                             None if lat is None else ptr(lat), None if out is None else out.ctypes.data_as(_u8p)))
-        if latent and rgb:
-            return lat, out
-        return lat if latent else out
+        lat, out = _outputs(n, H, W, latent, rgb)
+        self.check(self.lib.sdb_sample_batch(self.h, C.byref(batch_struct(b)), int(n_steps), _fptr(init_latent), H, W, _fptr(lat),
+                                             _u8ptr(out)))
+        return _result(lat, out)
 
     def img2img_batch(self, image, contexts, unconds, scales, n_steps, strength, mask=None, noise=None, seeds=None,
                       noise_seeds=None, latent=False, rgb=True):
         """n different requests of image-to-image / inpainting in one call (include/sdb200.h: sdb_img2img_batch). image u8
         [n,8H,8W,3]; mask u8 [n,8H,8W] or None (required on an inpainting context); noise [n,4,H,W] or None (each request's
         noise from its seed)."""
-        if not (latent or rgb):
-            raise ValueError("request the latent, the image or both")
+        _check_outputs(latent, rgb)
         b = pack_batch(contexts, unconds, scales, seeds, noise_seeds)
         n = b["context"].shape[0]
-        image = np.ascontiguousarray(image, dtype=np.uint8)
-        if image.ndim != 4 or image.shape[0] != n or image.shape[3] != 3 or image.shape[1] % 8 or image.shape[2] % 8:
-            raise ValueError("image must be u8 [n, 8H, 8W, 3]")
-        Hp, Wp = image.shape[1:3]
-        H, W = Hp // 8, Wp // 8
-        if mask is not None:
-            mask = np.ascontiguousarray(mask, dtype=np.uint8)
-            if mask.shape != (n, Hp, Wp):
-                raise ValueError("mask must be u8 [n, 8H, 8W]")
-        if noise is not None:
-            noise = f32(noise)
-            if noise.shape != (n, 4, H, W):
-                raise ValueError("noise must be [n, 4, H, W]")
-        lat = np.empty((n, 4, H, W), np.float32) if latent else None
-        out = np.empty((n, Hp, Wp, 3), np.uint8) if rgb else None
-        self.check(self.lib.sdb_img2img_batch(self.h, C.byref(batch_struct(b)), image.ctypes.data_as(_u8p),
-                                              None if mask is None else mask.ctypes.data_as(_u8p), float(strength), int(n_steps),
-                                              None if noise is None else ptr(noise), H, W, None if lat is None else ptr(lat),
-                                              None if out is None else out.ctypes.data_as(_u8p)))
-        if latent and rgb:
-            return lat, out
-        return lat if latent else out
+        image, H, W = _image(image, n)
+        mask = _mask(mask, image)
+        noise = _latent(noise, (n, 4, H, W), "noise")
+        lat, out = _outputs(n, H, W, latent, rgb)
+        self.check(self.lib.sdb_img2img_batch(self.h, C.byref(batch_struct(b)), _u8ptr(image), _u8ptr(mask), float(strength),
+                                              int(n_steps), _fptr(noise), H, W, _fptr(lat), _u8ptr(out)))
+        return _result(lat, out)
 
     # ---- profiling
     def profile(self, on=True):

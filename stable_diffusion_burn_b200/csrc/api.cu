@@ -322,12 +322,29 @@ int sdb_decode_latent_dev(sdb_ctx* ctx, const float* d_latent, int n, int H, int
   API_END
 }
 
+// the request of a single-prompt sampling entry: n prompts of L rows, one negative of Lu rows broadcast over them, one scale
+static SampleRequest uniform_request(int kind, const float* context, int n, int L, const float* uncond, int Lu, double scale,
+                                     int n_steps, int H, int W) {
+  SampleRequest r;
+  r.kind = kind, r.context = context, r.n = n, r.L = L, r.uncond = uncond, r.Lu = Lu, r.scale = scale;
+  r.n_steps = n_steps, r.H = H, r.W = W;
+  return r;
+}
+
+static SampleRequest batch_request(int kind, const sdb_batch* batch, int n_steps, int H, int W) {
+  SampleRequest r;
+  r.kind = kind, r.batched = true, r.batch = batch, r.n_steps = n_steps, r.H = H, r.W = W;
+  return r;
+}
+
 int sdb_sample_latent(sdb_ctx* ctx, const float* context, int n, int L, const float* uncond, int Lu,
                       double guidance_scale, int n_steps, const float* init_latent, uint64_t seed, int H, int W,
                       float* latent_out) {
   API_BEGIN(ctx)
   need_final(c);
-  model_sample_host(c, context, n, L, uncond, Lu, guidance_scale, n_steps, init_latent, seed, H, W, latent_out, nullptr);
+  SampleRequest r = uniform_request(SAMPLE_TXT2IMG, context, n, L, uncond, Lu, guidance_scale, n_steps, H, W);
+  r.start = init_latent, r.seed = seed, r.latent_out = latent_out;
+  model_sample_host(c, r);
   API_END
 }
 
@@ -342,7 +359,9 @@ int sdb_sample_image(sdb_ctx* ctx, const float* context, int n, int L, const flo
                      int n_steps, const float* init_latent, uint64_t seed, int H, int W, uint8_t* rgb) {
   API_BEGIN(ctx)
   need_final(c);
-  model_sample_host(c, context, n, L, uncond, Lu, guidance_scale, n_steps, init_latent, seed, H, W, nullptr, rgb);
+  SampleRequest r = uniform_request(SAMPLE_TXT2IMG, context, n, L, uncond, Lu, guidance_scale, n_steps, H, W);
+  r.start = init_latent, r.seed = seed, r.rgb = rgb;
+  model_sample_host(c, r);
   API_END
 }
 
@@ -351,8 +370,9 @@ int sdb_sample_image_dev(sdb_ctx* ctx, const float* d_context, int n, int L, con
                          void* stream) {
   API_BEGIN(ctx)
   need_final(c);
-  model_sample_dev(c, d_context, n, L, d_uncond, Lu, guidance_scale, n_steps, d_init_latent, H, W, nullptr, d_rgb,
-                   (cudaStream_t)stream);
+  SampleRequest r = uniform_request(SAMPLE_TXT2IMG, d_context, n, L, d_uncond, Lu, guidance_scale, n_steps, H, W);
+  r.start = d_init_latent, r.rgb = d_rgb;
+  model_sample_dev(c, r, (cudaStream_t)stream);
   API_END
 }
 
@@ -361,8 +381,9 @@ int sdb_img2img(sdb_ctx* ctx, const uint8_t* image, const uint8_t* mask, double 
                 float* latent_out, uint8_t* rgb_out) {
   API_BEGIN(ctx)
   need_final(c);
-  model_img2img_host(c, image, mask, strength, context, n, L, uncond, Lu, guidance_scale, n_steps, noise, seed, H, W, latent_out,
-                     rgb_out);
+  SampleRequest r = uniform_request(SAMPLE_IMG2IMG, context, n, L, uncond, Lu, guidance_scale, n_steps, H, W);
+  r.image = image, r.mask = mask, r.strength = strength, r.start = noise, r.seed = seed, r.latent_out = latent_out, r.rgb = rgb_out;
+  model_sample_host(c, r);
   API_END
 }
 
@@ -371,8 +392,9 @@ int sdb_img2img_dev(sdb_ctx* ctx, const uint8_t* d_image, const uint8_t* d_mask,
                     float* d_latent_out, uint8_t* d_rgb_out, void* stream) {
   API_BEGIN(ctx)
   need_final(c);
-  model_img2img_dev(c, d_image, d_mask, strength, d_context, n, L, d_uncond, Lu, guidance_scale, n_steps, d_noise, H, W,
-                    d_latent_out, d_rgb_out, (cudaStream_t)stream);
+  SampleRequest r = uniform_request(SAMPLE_IMG2IMG, d_context, n, L, d_uncond, Lu, guidance_scale, n_steps, H, W);
+  r.image = d_image, r.mask = d_mask, r.strength = strength, r.start = d_noise, r.latent_out = d_latent_out, r.rgb = d_rgb_out;
+  model_sample_dev(c, r, (cudaStream_t)stream);
   API_END
 }
 
@@ -381,8 +403,9 @@ int sdb_edit_image(sdb_ctx* ctx, const uint8_t* image, const float* context, int
                    float* latent_out, uint8_t* rgb_out) {
   API_BEGIN(ctx)
   need_final(c);
-  model_edit_host(c, image, context, n, L, uncond, Lu, text_scale, image_scale, n_steps, init_latent, seed, H, W, latent_out,
-                  rgb_out);
+  SampleRequest r = uniform_request(SAMPLE_EDIT, context, n, L, uncond, Lu, text_scale, n_steps, H, W);
+  r.image = image, r.image_scale = image_scale, r.start = init_latent, r.seed = seed, r.latent_out = latent_out, r.rgb = rgb_out;
+  model_sample_host(c, r);
   API_END
 }
 
@@ -391,8 +414,9 @@ int sdb_edit_image_dev(sdb_ctx* ctx, const uint8_t* d_image, const float* d_cont
                        float* d_latent_out, uint8_t* d_rgb_out, void* stream) {
   API_BEGIN(ctx)
   need_final(c);
-  model_edit_dev(c, d_image, d_context, n, L, d_uncond, Lu, text_scale, image_scale, n_steps, d_init_latent, H, W, d_latent_out,
-                 d_rgb_out, (cudaStream_t)stream);
+  SampleRequest r = uniform_request(SAMPLE_EDIT, d_context, n, L, d_uncond, Lu, text_scale, n_steps, H, W);
+  r.image = d_image, r.image_scale = image_scale, r.start = d_init_latent, r.latent_out = d_latent_out, r.rgb = d_rgb_out;
+  model_sample_dev(c, r, (cudaStream_t)stream);
   API_END
 }
 
@@ -400,7 +424,9 @@ int sdb_sample_batch(sdb_ctx* ctx, const sdb_batch* batch, int n_steps, const fl
                      uint8_t* rgb_out) {
   API_BEGIN(ctx)
   need_final(c);
-  model_sample_batch_host(c, batch, n_steps, init_latent, H, W, latent_out, rgb_out);
+  SampleRequest r = batch_request(SAMPLE_TXT2IMG, batch, n_steps, H, W);
+  r.start = init_latent, r.latent_out = latent_out, r.rgb = rgb_out;
+  model_sample_host(c, r);
   API_END
 }
 
@@ -408,7 +434,9 @@ int sdb_sample_batch_dev(sdb_ctx* ctx, const sdb_batch* batch, int n_steps, cons
                          float* d_latent_out, uint8_t* d_rgb_out, void* stream) {
   API_BEGIN(ctx)
   need_final(c);
-  model_sample_batch_dev(c, batch, n_steps, d_init_latent, H, W, d_latent_out, d_rgb_out, (cudaStream_t)stream);
+  SampleRequest r = batch_request(SAMPLE_TXT2IMG, batch, n_steps, H, W);
+  r.start = d_init_latent, r.latent_out = d_latent_out, r.rgb = d_rgb_out;
+  model_sample_dev(c, r, (cudaStream_t)stream);
   API_END
 }
 
@@ -416,7 +444,9 @@ int sdb_img2img_batch(sdb_ctx* ctx, const sdb_batch* batch, const uint8_t* image
                       int n_steps, const float* noise, int H, int W, float* latent_out, uint8_t* rgb_out) {
   API_BEGIN(ctx)
   need_final(c);
-  model_img2img_batch_host(c, batch, image, mask, strength, n_steps, noise, H, W, latent_out, rgb_out);
+  SampleRequest r = batch_request(SAMPLE_IMG2IMG, batch, n_steps, H, W);
+  r.image = image, r.mask = mask, r.strength = strength, r.start = noise, r.latent_out = latent_out, r.rgb = rgb_out;
+  model_sample_host(c, r);
   API_END
 }
 
@@ -424,8 +454,9 @@ int sdb_img2img_batch_dev(sdb_ctx* ctx, const sdb_batch* batch, const uint8_t* d
                           int n_steps, const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb_out, void* stream) {
   API_BEGIN(ctx)
   need_final(c);
-  model_img2img_batch_dev(c, batch, d_image, d_mask, strength, n_steps, d_noise, H, W, d_latent_out, d_rgb_out,
-                          (cudaStream_t)stream);
+  SampleRequest r = batch_request(SAMPLE_IMG2IMG, batch, n_steps, H, W);
+  r.image = d_image, r.mask = d_mask, r.strength = strength, r.start = d_noise, r.latent_out = d_latent_out, r.rgb = d_rgb_out;
+  model_sample_dev(c, r, (cudaStream_t)stream);
   API_END
 }
 

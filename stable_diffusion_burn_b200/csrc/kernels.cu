@@ -1209,7 +1209,7 @@ __host__ __device__ void step_noise_keys(uint64_t seed, int t, uint32_t* k0, uin
 // x = w nl + (1 - w) (sqrt(a_prev) z0 + sqrt(1 - a_prev) eps), w = mask[sample][pixel % plane]. nl is the same expression in
 // both instantiations, so an all-ones mask reproduces the unmasked step bit for bit. The blend and the new samplers' updates
 // are written with _rn intrinsics (no FMA contraction) so that a test can restate them exactly in float32. STEP_DDIM is the
-// expression sample_latent has always used; its kernel keeps the argument list and the instructions it had.
+// expression sample_latent has always used; its instantiations keep the instructions they had.
 // PER_SAMPLE (a batch of different requests, DESIGN §7 f7): the scale and the eta noise key of sample i / (4 plane) come from
 // s.scales / s.noise_seeds, and z is drawn at the index within the sample. The arithmetic is the same expression.
 // GROUPS = 3 (InstructPix2Pix, DESIGN §7 f10): eu = e_U, ec = e_I and ec + count = e_T, and the guidance is
@@ -1263,82 +1263,44 @@ __device__ __forceinline__ void cfg_step(const float* __restrict__ eu, const flo
     if constexpr (GROUPS == 3) lat[i + 2 * count] = nl;
   }
 }
-template <bool BLEND>
-__global__ void cfg_ddim_kernel(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
-                                long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
-                                float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
-                                const float* __restrict__ w, int plane) {
-  cfg_step<STEP_DDIM, BLEND>(eu, ec, lat, count, scale, sqrt_1m_at, sqrt_at, sqrt_aprev, dir_coef, z0, e0, w, plane, SamplerStep{});
+// GROUPS = 3 reads e_I and e_T from one eps [3][count] at eu; the two-group kinds take ec from the launcher
+template <int KIND, bool BLEND, bool PER_SAMPLE, int GROUPS>
+__global__ void cfg_step_kernel(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
+                                long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev, float dir_coef,
+                                float scale_i, const float* __restrict__ z0, const float* __restrict__ e0,
+                                const float* __restrict__ w, int plane, const SamplerStep s) {
+  cfg_step<KIND, BLEND, PER_SAMPLE, GROUPS>(eu, GROUPS == 3 ? eu + count : ec, lat, count, scale, sqrt_1m_at, sqrt_at, sqrt_aprev,
+                                            dir_coef, z0, e0, w, plane, s, scale_i);
 }
-template <int KIND, bool BLEND, bool PER_SAMPLE>
-__global__ void cfg_sampler_kernel(const float* __restrict__ eu, const float* __restrict__ ec, float* __restrict__ lat,
-                                   long long count, float scale, float sqrt_1m_at, float sqrt_at, float sqrt_aprev,
-                                   float dir_coef, const float* __restrict__ z0, const float* __restrict__ e0,
-                                   const float* __restrict__ w, int plane, const SamplerStep s) {
-  cfg_step<KIND, BLEND, PER_SAMPLE>(eu, ec, lat, count, scale, sqrt_1m_at, sqrt_at, sqrt_aprev, dir_coef, z0, e0, w, plane, s);
-}
-void cfg_sampler_launch(int kind, const SamplerStep& s, const float* eps_u, const float* eps_c, float* latent, long long count,
-                        float scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
-                        const float* z0, const float* eps0, const float* w, int plane) {
-  const bool per_sample = s.scales != nullptr;
-  SDB_CHECK(kind == STEP_DDIM_ETA || kind == STEP_DPMPP_2M || (kind == STEP_DDIM && per_sample), "cfg_sampler_launch: kind");
-  SDB_CHECK(!per_sample || (plane > 0 && (kind != STEP_DDIM_ETA || s.noise_seeds)), "cfg_sampler_launch: per-sample inputs");
-  int grid = (int)((count + 255) / 256);
-  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
-  auto go = [&](auto kernel) {
-    launch_k(kernel, dim3(grid), dim3(256), 0, st, eps_u, eps_c, latent, count, scale, sqrt_one_minus_at, sqrt_at, sqrt_aprev,
-             dir_coef, z0, eps0, w, plane, s);
-  };
-  if (per_sample) {
-    if (kind == STEP_DDIM)
-      w ? go(cfg_sampler_kernel<STEP_DDIM, true, true>) : go(cfg_sampler_kernel<STEP_DDIM, false, true>);
-    else if (kind == STEP_DDIM_ETA)
-      w ? go(cfg_sampler_kernel<STEP_DDIM_ETA, true, true>) : go(cfg_sampler_kernel<STEP_DDIM_ETA, false, true>);
-    else
-      w ? go(cfg_sampler_kernel<STEP_DPMPP_2M, true, true>) : go(cfg_sampler_kernel<STEP_DPMPP_2M, false, true>);
-  } else if (kind == STEP_DDIM_ETA) {
-    w ? go(cfg_sampler_kernel<STEP_DDIM_ETA, true, false>) : go(cfg_sampler_kernel<STEP_DDIM_ETA, false, false>);
-  } else {
-    w ? go(cfg_sampler_kernel<STEP_DPMPP_2M, true, false>) : go(cfg_sampler_kernel<STEP_DPMPP_2M, false, false>);
-  }
-  SDB_CUDA(cudaGetLastError());
-}
+// the five instantiations of one kind: three groups (no blend, uniform), or two groups with or without blend and per-sample inputs
 template <int KIND>
-__global__ void cfg3_sampler_kernel(const float* __restrict__ eps, float* __restrict__ lat, long long count, float scale_t,
-                                    float scale_i, float sqrt_1m_at, float sqrt_at, float sqrt_aprev, float dir_coef,
-                                    const SamplerStep s) {
-  cfg_step<KIND, false, false, 3>(eps, eps + count, lat, count, scale_t, sqrt_1m_at, sqrt_at, sqrt_aprev, dir_coef, nullptr,
-                                  nullptr, nullptr, 0, s, scale_i);
-}
-void cfg3_sampler_launch(int kind, const SamplerStep& s, const float* eps, float* latent, long long count, float text_scale,
-                         float image_scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef,
-                         cudaStream_t st) {
-  SDB_CHECK(kind == STEP_DDIM || kind == STEP_DDIM_ETA || kind == STEP_DPMPP_2M, "cfg3_sampler_launch: kind");
-  int grid = (int)((count + 255) / 256);
-  if (grid > g_num_sms * 8) grid = g_num_sms * 8;
+static void cfg_step_go(const CfgStepArgs& a, dim3 grid, cudaStream_t st) {
+  const bool blend = a.w != nullptr, per_sample = a.s.scales != nullptr;
   auto go = [&](auto kernel) {
-    launch_k(kernel, dim3(grid), dim3(256), 0, st, eps, latent, count, text_scale, image_scale, sqrt_one_minus_at, sqrt_at,
-             sqrt_aprev, dir_coef, s);
+    launch_k(kernel, grid, dim3(256), 0, st, a.eu, a.ec, a.lat, a.count, a.scale, a.sqrt_1m_at, a.sqrt_at, a.sqrt_aprev, a.dir_coef,
+             a.scale_i, a.z0, a.e0, a.w, a.plane, a.s);
   };
-  if (kind == STEP_DDIM)
-    go(cfg3_sampler_kernel<STEP_DDIM>);
-  else if (kind == STEP_DDIM_ETA)
-    go(cfg3_sampler_kernel<STEP_DDIM_ETA>);
+  if (a.groups == 3)
+    go(cfg_step_kernel<KIND, false, false, 3>);
+  else if (per_sample)
+    blend ? go(cfg_step_kernel<KIND, true, true, 2>) : go(cfg_step_kernel<KIND, false, true, 2>);
   else
-    go(cfg3_sampler_kernel<STEP_DPMPP_2M>);
-  SDB_CUDA(cudaGetLastError());
+    blend ? go(cfg_step_kernel<KIND, true, false, 2>) : go(cfg_step_kernel<KIND, false, false, 2>);
 }
-void cfg_ddim_launch(const float* eps_u, const float* eps_c, float* latent, long long count, float scale,
-                     float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
-                     const float* z0, const float* eps0, const float* w, int plane) {
-  int grid = (int)((count + 255) / 256);
+void cfg_step_launch(const CfgStepArgs& a, cudaStream_t st) {
+  const bool blend = a.w != nullptr, per_sample = a.s.scales != nullptr;
+  SDB_CHECK(a.groups == 2 || (a.groups == 3 && !blend && !per_sample), "cfg_step_launch: groups");
+  SDB_CHECK(!per_sample || (a.plane > 0 && (a.kind != STEP_DDIM_ETA || a.s.noise_seeds)), "cfg_step_launch: per-sample inputs");
+  int grid = (int)((a.count + 255) / 256);
   if (grid > g_num_sms * 8) grid = g_num_sms * 8;
-  if (w)
-    launch_k(cfg_ddim_kernel<true>, dim3(grid), dim3(256), 0, st, eps_u, eps_c, latent, count, scale, sqrt_one_minus_at, sqrt_at,
-             sqrt_aprev, dir_coef, z0, eps0, w, plane);
+  if (a.kind == STEP_DDIM)
+    cfg_step_go<STEP_DDIM>(a, dim3(grid), st);
+  else if (a.kind == STEP_DDIM_ETA)
+    cfg_step_go<STEP_DDIM_ETA>(a, dim3(grid), st);
+  else if (a.kind == STEP_DPMPP_2M)
+    cfg_step_go<STEP_DPMPP_2M>(a, dim3(grid), st);
   else
-    launch_k(cfg_ddim_kernel<false>, dim3(grid), dim3(256), 0, st, eps_u, eps_c, latent, count, scale, sqrt_one_minus_at, sqrt_at,
-             sqrt_aprev, dir_coef, (const float*)nullptr, (const float*)nullptr, (const float*)nullptr, 0);
+    SDB_CHECK(false, "cfg_step_launch: kind");
   SDB_CUDA(cudaGetLastError());
 }
 

@@ -96,14 +96,8 @@ void gemv_launch(const float* x, const float* W, const float* b, int K, int N, f
 void embed_tokens_launch(const int* tok, const float* E, const float* Pos, int n, int L, int Lp, int D, int vocab, float* x,
                          cudaStream_t st);
 
-// ---- sampler elementwise (reference stablediffusion/mod.rs:152-156, 190-191)
-// pred = u + (c-u)*scale ; x0 = (lat - pred*sqrt(1-a_t))/sqrt(a_t) ; lat' = x0*sqrt(a_prev) + pred*sqrt(1-a_prev)
-// latent holds 2*count floats: the update is written to both halves (uncond | cond inputs of the next step)
-// w != null (masked img2img): lat' = w lat' + (1 - w) (sqrt(a_prev) z0 + sqrt(1 - a_prev) eps0), w [n][plane] per latent cell
-void cfg_ddim_launch(const float* eps_u, const float* eps_c, float* latent, long long count, float scale,
-                     float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
-                     const float* z0 = nullptr, const float* eps0 = nullptr, const float* w = nullptr, int plane = 0);
-// The other updates of the same fused step (DESIGN §7 f6), one launch per step like cfg_ddim_launch, which is STEP_DDIM.
+// ---- the sampler's fused guidance + update step (reference stablediffusion/mod.rs:152-156, 190-191; DESIGN §7 f5, f6, f7, f10)
+// pred = u + (c-u)*scale ; x0 = (lat - pred*sqrt(1-a_t))/sqrt(a_t) ; lat' = x0*sqrt(a_prev) + pred*sqrt(1-a_prev) (STEP_DDIM)
 enum : int { STEP_DDIM = 0, STEP_DDIM_ETA = 1, STEP_DPMPP_2M = 2 };
 struct SamplerStep {   // per-step scalars, computed on the host in double and passed as f32
   float* hist = nullptr;      // STEP_DPMPP_2M: x0 of the previous step [count]; read when `second`, always overwritten
@@ -112,7 +106,7 @@ struct SamplerStep {   // per-step scalars, computed on the host in double and p
   int second = 0;
   float s = 0.f;              // STEP_DDIM_ETA: x' = sqrt(a_prev) x0 + dir_coef pred + s z
   uint32_t k0 = 0, k1 = 0;    // STEP_DDIM_ETA: key of z (step_noise_keys)
-  float ka = 0.f, kb = 0.f;   // blend: known = ka z0 + kb eps0 (sqrt(a_prev), sqrt(1 - a_prev))
+  float ka = 0.f, kb = 0.f;   // blend of the kinds other than STEP_DDIM: known = ka z0 + kb eps0 (sqrt(a_prev), sqrt(1 - a_prev))
   // per-sample inputs of a batch of different requests (DESIGN §7 f7). scales != null selects the per-sample instantiations:
   // sample s = i / (4 plane) takes scales[s] instead of `scale`, and STEP_DDIM_ETA draws z at the index within the sample,
   // keyed by step_noise_keys(noise_seeds[s], t) instead of (k0, k1). Any kind, STEP_DDIM included, may run per sample.
@@ -120,15 +114,27 @@ struct SamplerStep {   // per-step scalars, computed on the host in double and p
   const uint64_t* noise_seeds = nullptr;  // device [n]
   int t = 0;                             // timestep value of the step
 };
-void cfg_sampler_launch(int kind, const SamplerStep& s, const float* eps_u, const float* eps_c, float* latent, long long count,
-                        float scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef, cudaStream_t st,
-                        const float* z0, const float* eps0, const float* w, int plane);
-// The three-way guidance + update of an InstructPix2Pix step (DESIGN §7 f10), one launch of any kind: eps [3][count] holds the
-// groups e_U | e_I | e_T, pred = e_U + text_scale (e_T - e_I) + image_scale (e_I - e_U), and the result goes to all three copies
-// of the latent in latent [3][count]. The update is cfg_sampler_launch's for the kind (STEP_DDIM: cfg_ddim_launch's).
-void cfg3_sampler_launch(int kind, const SamplerStep& s, const float* eps, float* latent, long long count, float text_scale,
-                         float image_scale, float sqrt_one_minus_at, float sqrt_at, float sqrt_aprev, float dir_coef,
-                         cudaStream_t st);
+// One launch per step. groups = 2: eu / ec [count] the unconditional / prompt predictions, the update goes to both halves of
+// lat [2][count]. groups = 3 (InstructPix2Pix): eu = eps [3][count] holds e_U | e_I | e_T (ec unused),
+// pred = e_U + scale (e_T - e_I) + scale_i (e_I - e_U), and the update goes to all three copies in lat [3][count].
+// w != null (masked img2img, two groups): lat' = w lat' + (1 - w) (sqrt(a_prev) z0 + sqrt(1 - a_prev) e0), w [n][plane].
+struct CfgStepArgs {
+  const float* eu = nullptr;
+  const float* ec = nullptr;
+  float* lat = nullptr;
+  long long count = 0;
+  float scale = 0.f;
+  float sqrt_1m_at = 0.f, sqrt_at = 0.f, sqrt_aprev = 0.f, dir_coef = 0.f;
+  const float* z0 = nullptr;
+  const float* e0 = nullptr;
+  const float* w = nullptr;
+  int plane = 0;        // H * W of the latent
+  SamplerStep s;
+  float scale_i = 0.f;  // groups = 3: the image guidance scale
+  int kind = STEP_DDIM;
+  int groups = 2;
+};
+void cfg_step_launch(const CfgStepArgs& a, cudaStream_t st);
 // ---- img2img staging: u8 HWC RGB [nb][Hp][Wp][3] -> encoder input [nb][4][Hp][Wp], v / 127.5 - 1, fourth plane zero
 void u8_to_enc_input_launch(const uint8_t* rgb, int nb, int Hp, int Wp, float* out, cudaStream_t st);
 // 9-channel inpainting: the masked image's encoder input [nb,4,Hp,Wp] and the latent mask into channel 0 of cond [nb,5,Hp/8,Wp/8]

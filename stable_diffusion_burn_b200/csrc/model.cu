@@ -1439,21 +1439,6 @@ static void check_not_pix2pix(const Ctx& c, const char* what) {
                                                  "which needs an input image and image guidance; call sdb_edit_image");
 }
 
-// a 9-channel UNet (sdb_create_inpaint) reads a mask and a masked-image latent that text-to-image does not have
-static void check_txt2img(const Ctx& c) {
-  SDB_CHECK(c.unet_cin != 9,
-            "sample: this context runs a 9-channel inpainting UNet (sdb_create_inpaint), which needs a mask and an image; for "
-            "text-to-image call sdb_img2img with an all-255 mask at strength 1");
-  check_not_pix2pix(c, "sample");
-}
-
-static void check_sample_args(int n, int L, int Lu, int n_steps, int H, int W) {
-  SDB_CHECK(n >= 1 && L >= 1 && Lu >= 1, "sample arguments");
-  SDB_CHECK(n_steps >= 1 && n_steps <= 1000, "n_steps must be in [1,1000] (step_by(0) panics in the reference)");
-  SDB_CHECK(H % 8 == 0 && W % 8 == 0, "latent size must be a multiple of 8");
-  SDB_CHECK(((H / 8) * (W / 8)) % 8 == 0, "unsupported latent size: (H/8)*(W/8) must be a multiple of 8");
-}
-
 // timesteps (stablediffusion/mod.rs:111,123): (0..1000).rev().step_by(1000 / n_steps)
 static std::vector<int> ddim_timesteps(int n_steps) {
   std::vector<int> ts;
@@ -1461,16 +1446,85 @@ static std::vector<int> ddim_timesteps(int n_steps) {
   return ts;
 }
 
-namespace {
-struct Img2ImgIn {  // what the sampler loop needs to start part way down the schedule from an encoded image
-  float* z0 = nullptr;          // [n,4,H,W] encoder output; scaled by 0.18215 in place by the preparation kernel
-  const float* eps = nullptr;   // [n,4,H,W] the noise
-  const uint8_t* mask = nullptr;  // [n,8H,8W] or null
-  float* w = nullptr;           // [n,H,W] latent mask (written when mask is set)
-  float sa = 0.f, sb = 0.f;     // sqrt(abar[t0]), sqrt(1 - abar[t0])
-  const float* cond = nullptr;  // 9-channel UNet (DESIGN §7 f9): [n,5,H,W] latent mask | z_m, read by conv_in; no blend then
-};
+// The schedule index img2img starts from (DESIGN §7 f5): k = floor(strength * N) of the N timesteps run, the last k of them.
+static int img2img_first(double strength, int n_steps) {
+  SDB_CHECK(std::isfinite(strength) && strength > 0.0 && strength <= 1.0, "img2img: strength must be finite and in (0, 1]");
+  const int N = (int)ddim_timesteps(n_steps).size();
+  const int k = (int)std::floor(strength * (double)N);
+  char msg[160];
+  snprintf(msg, sizeof(msg), "img2img: strength %.17g runs none of the %d timesteps; the smallest valid strength is 1/%d = %.17g",
+           strength, N, N, 1.0 / N);
+  SDB_CHECK(k >= 1, msg);
+  return N - k;
+}
 
+// Rejects a request before anything is staged. The context kind comes first, so a call on the wrong context names the right
+// entry whatever its pointers are; then the batch descriptor (naming the field, the sample and the value), the shape and step
+// arguments, the pointers, the strength and the scales. host: a NULL start is drawn from the seed(s). Returns the schedule index
+// the call starts from.
+static int sample_n(const SampleRequest& r) { return r.batch ? r.batch->n : r.n; }
+
+static int check_request(const Ctx& c, const SampleRequest& r, bool host) {
+  const bool txt2img = r.kind == SAMPLE_TXT2IMG, img2img = r.kind == SAMPLE_IMG2IMG, edit = r.kind == SAMPLE_EDIT;
+  char msg[240];
+  if (edit) {
+    snprintf(msg, sizeof(msg),
+             "edit_image: this context's UNet takes %d input channels; InstructPix2Pix needs the 8-channel UNet of a context from "
+             "sdb_create_pix2pix",
+             c.unet_cin);
+    SDB_CHECK(c.unet_cin == 8, msg);
+  } else {
+    // a 9-channel UNet (sdb_create_inpaint) reads a mask and a masked-image latent that text-to-image does not have
+    SDB_CHECK(!txt2img || c.unet_cin != 9,
+              "sample: this context runs a 9-channel inpainting UNet (sdb_create_inpaint), which needs a mask and an image; for "
+              "text-to-image call sdb_img2img with an all-255 mask at strength 1");
+    check_not_pix2pix(c, txt2img ? "sample" : "img2img");
+  }
+  const sdb_batch* b = r.batch;
+  if (r.batched) {
+    SDB_CHECK(b, "batch: null descriptor");
+    snprintf(msg, sizeof(msg), "batch: n = %d must be >= 1", b->n);
+    SDB_CHECK(b->n >= 1, msg);
+    snprintf(msg, sizeof(msg), "batch: the row strides L = %d and Lu = %d must be >= 1", b->L, b->Lu);
+    SDB_CHECK(b->L >= 1 && b->Lu >= 1, msg);
+    SDB_CHECK(b->context, "batch: context is NULL");
+    SDB_CHECK(b->uncond, "batch: uncond is NULL");
+    SDB_CHECK(b->guidance_scale, "batch: guidance_scale is NULL");
+    SDB_CHECK(b->seed || r.start, "batch: seed is NULL and no init latent / noise is given");
+    for (int i = 0; i < b->n; ++i) {
+      const int l = b->context_len ? b->context_len[i] : b->L, lu = b->uncond_len ? b->uncond_len[i] : b->Lu;
+      snprintf(msg, sizeof(msg), "batch: context_len[%d] = %d is outside [1, L = %d]", i, l, b->L);
+      SDB_CHECK(l >= 1 && l <= b->L, msg);
+      snprintf(msg, sizeof(msg), "batch: uncond_len[%d] = %d is outside [1, Lu = %d]", i, lu, b->Lu);
+      SDB_CHECK(lu >= 1 && lu <= b->Lu, msg);
+      snprintf(msg, sizeof(msg), "batch: guidance_scale[%d] = %.17g is not finite", i, b->guidance_scale[i]);
+      SDB_CHECK(std::isfinite(b->guidance_scale[i]), msg);
+    }
+  }
+  const int L = b ? b->L : r.L, Lu = b ? b->Lu : r.Lu;
+  SDB_CHECK(sample_n(r) >= 1 && L >= 1 && Lu >= 1, "sample arguments");
+  SDB_CHECK(r.n_steps >= 1 && r.n_steps <= 1000, "n_steps must be in [1,1000] (step_by(0) panics in the reference)");
+  SDB_CHECK(r.H % 8 == 0 && r.W % 8 == 0, "latent size must be a multiple of 8");
+  SDB_CHECK(((r.H / 8) * (r.W / 8)) % 8 == 0, "unsupported latent size: (H/8)*(W/8) must be a multiple of 8");
+  const std::string what = img2img ? "img2img" : (edit ? "edit_image" : (b ? "sample_batch" : "sample"));
+  if (!txt2img) {
+    SDB_CHECK(r.image && (b ? b->context : r.context) && (b ? b->uncond : r.uncond), what + ": null image, context or uncond");
+    SDB_CHECK(edit || r.mask || c.unet_cin == 4,
+              "img2img: the mask is NULL; a 9-channel inpainting UNet (sdb_create_inpaint) needs one");
+  }
+  if (!txt2img || b) SDB_CHECK(r.latent_out || r.rgb, what + ": request the latent, the image or both");
+  if (!txt2img && !host && !b) SDB_CHECK(r.start, what + (img2img ? ": the device entry needs the noise latent"
+                                                                  : ": the device entry needs the start latent"));
+  if (edit) {
+    snprintf(msg, sizeof(msg), "edit_image: text_scale = %.17g is not finite", r.scale);
+    SDB_CHECK(std::isfinite(r.scale), msg);
+    snprintf(msg, sizeof(msg), "edit_image: image_scale = %.17g is not finite", r.image_scale);
+    SDB_CHECK(std::isfinite(r.image_scale), msg);
+  }
+  return img2img ? img2img_first(r.strength, r.n_steps) : 0;
+}
+
+namespace {
 // The n requests of a sampling call (DESIGN §7 f7). The single-request entries describe a uniform batch: every sample reads the L
 // prompt rows and the one broadcast negative, under one scale, and eta noise runs over the call's flat latent. The batch entries
 // give each sample its own prompt length, negative, scale and noise seed.
@@ -1487,32 +1541,129 @@ struct Batch {
   const uint64_t* d_noise_seed = nullptr;  // device [n]: eta noise seeds of the per-sample step
 };
 
-// InstructPix2Pix (DESIGN §7 f10): what the sampler loop adds for three-way guidance
-struct EditIn {
-  const float* cond = nullptr;  // [3n,4,H,W]: 0 | c_I | c_I, one block per guidance group, read by the 8-channel conv_in
-  double image_scale = 0.0;     // s_I; the Batch's scale is s_T
+struct BatchTab {  // the per-sample tables of a batch call on the device (io slot kIoBatchTab)
+  const uint64_t* seed = nullptr;
+  const uint64_t* noise_seed = nullptr;
+  const float* scale = nullptr;
 };
 
-Batch uniform_batch(const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale) {
-  Batch b;
-  b.n = n, b.cond = d_context, b.L = L, b.uncond = d_uncond, b.Lu = Lu, b.scale = scale;
-  b.len.assign(n, L), b.ulen.assign(n, Lu);
-  return b;
-}
+// What the sampler loop starts from and conditions on, resolved from a request by sample_run
+struct StepCond {
+  int groups = 2;                 // 3: InstructPix2Pix (DESIGN §7 f10), groups e_U | e_I | e_T
+  const float* start = nullptr;   // txt2img, edit: [n,4,H,W] copied into every group
+  float* z0 = nullptr;            // img2img (start from img2img_prep): [n,4,H,W] encoder output, scaled by 0.18215 in place
+  const float* eps = nullptr;     // img2img: [n,4,H,W] the noise
+  const uint8_t* mask = nullptr;  // masked img2img: [n,8H,8W]
+  float* w = nullptr;             // masked img2img: [n,H,W] latent mask, written by img2img_prep; selects the blend
+  float sa = 0.f, sb = 0.f;       // img2img: sqrt(abar[t0]), sqrt(1 - abar[t0])
+  // the UNet's extra input channels (io slot kIoUNetCond) or null: [n,5,H,W] latent mask | z_m (9-channel inpainting, DESIGN §7
+  // f9), [3n,4,H,W] 0 | c_I | c_I (InstructPix2Pix, one block per guidance group)
+  const float* cond = nullptr;
+  double image_scale = 0.0;       // s_I of an edit; the Batch's scale is s_T
+};
 }  // namespace
 
-// sample_latent + latent_to_image (stablediffusion/mod.rs:51-160) from schedule index `first` on. The conditional and
-// unconditional UNet evaluations of a step (forward_diffuser :162-192) run as ONE batch-2n pass: weights stream from HBM once.
-// ii == null: txt2img from d_init_latent. Otherwise the start latent and (with a mask) the per-step blend come from ii; a
-// 9-channel UNet reads ii->cond instead of blending. ei (an InstructPix2Pix edit, DESIGN §7 f10; ii null): the step's pass is
-// batch-3n, groups e_U | e_I | e_T (negative without the image, negative with it, prompt with it), and ei->cond holds each
-// group's image channels. Runs on c.stream; the caller joins the streams.
-static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const float* d_init_latent, const Img2ImgIn* ii, int H,
-                        int W, float* d_latent_out, uint8_t* d_rgb, const EditIn* ei = nullptr) {
+// u8 HWC images [n][8H][8W][3] (or, d_image null, encoder inputs [n][4][8H][8W] already staged) -> the encoder in chunks of 4 (the
+// work arena bound of decode_chunked) -> sample i's latent at dst + i * stride, times scale (stride 0: [n,4,H,W], unscaled)
+static void encode_images(Ctx& c, const uint8_t* d_image, const float* d_enc_in, int n, int H, int W, float* dst,
+                          long long stride = 0, float scale = 1.f) {
+  const int Hp = 8 * H, Wp = 8 * W;
+  const size_t plane = (size_t)Hp * Wp;
+  for (int i0 = 0; i0 < n; i0 += 4) {
+    const int nb = std::min(4, n - i0);
+    const size_t mark = c.work.off;
+    const float* in = d_enc_in + (size_t)i0 * 4 * plane;
+    if (d_image) {
+      float* img4 = c.work.get<float>((size_t)nb * 4 * plane);
+      KernelScope ks(c, KC_ELEMENTWISE);
+      u8_to_enc_input_launch(d_image + (size_t)i0 * 3 * plane, nb, Hp, Wp, img4, c.stream);
+      in = img4;
+    }
+    Fwd f(c, nb);
+    vae_encode(f, in, Hp, Wp, dst + i0 * (stride ? stride : 4ll * H * W), stride, scale);
+    c.work.off = mark;
+  }
+}
+
+// The fused step's per-step scalars for timestep t (DESIGN §7 f6): computed in double, rounded once to f32. h_prev: DPM++'s h of
+// the previous step this call ran; has_prev: the step has one (second order).
+static void step_scalars(const Ctx& c, const std::vector<float>& alphas, int kind, int t, int step, bool has_prev, double& h_prev,
+                         CfgStepArgs& a) {
+  // alphas are read as f32 and widened to f64 (stablediffusion/mod.rs:124-140)
+  const double a_t = (double)alphas[t];
+  const double a_prev = (t >= step) ? (double)alphas[t - step] : 1.0;
+  double dir = std::sqrt(1.0 - a_prev);
+  SamplerStep& s = a.s;
+  if (kind != STEP_DDIM) {
+    s.ka = (float)std::sqrt(a_prev), s.kb = (float)dir;
+    if (kind == STEP_DDIM_ETA) {  // Song et al. 2021 eq. 16; s = 0 on the final step (a_prev = 1)
+      const double sig = c.sampler_eta * std::sqrt((1.0 - a_prev) / (1.0 - a_t)) * std::sqrt(1.0 - a_t / a_prev);
+      dir = std::sqrt(std::max(0.0, 1.0 - a_prev - sig * sig));
+      s.s = (float)sig;
+      step_noise_keys(c.sampler_noise_seed, t, &s.k0, &s.k1);
+    } else if (t < step) {  // DPM++ final step: sigma' = 0, h = inf: first order, x' = x0
+      s.cx = 0.f, s.cd = 1.f;
+    } else {  // DPM-Solver++(2M) (Lu et al. 2022), data prediction, lambda = ln(alpha / sigma)
+      const double lam = std::log(std::sqrt(a_t) / std::sqrt(1.0 - a_t));
+      const double lam_next = std::log(std::sqrt(a_prev) / std::sqrt(1.0 - a_prev));
+      const double h = lam_next - lam;
+      s.cx = (float)(std::sqrt(1.0 - a_prev) / std::sqrt(1.0 - a_t));
+      s.cd = (float)(-std::sqrt(a_prev) * std::expm1(-h));
+      if (has_prev) {  // second order: the first step a call runs has no history
+        const double c2 = 1.0 / (2.0 * (h_prev / h));
+        s.second = 1, s.c1 = (float)(1.0 + c2), s.c2 = (float)c2;
+      }
+      h_prev = h;
+    }
+  }
+  s.t = t;
+  a.sqrt_1m_at = (float)std::sqrt(1.0 - a_t), a.sqrt_at = (float)std::sqrt(a_t), a.sqrt_aprev = (float)std::sqrt(a_prev);
+  a.dir_coef = (float)dir;
+}
+
+// The cached CUDA graph of the step's UNet pass (`pass`), captured on first use. A graph bakes in the addresses of xb, eps, the
+// context K/V, the step's temporaries (work_mark on) and cond, an io slot that can grow and move between calls, so those are
+// matched beside the shape key; txt2img, img2img and batch calls of one shape share their graphs.
+template <class Pass>
+static Model::GraphEntry step_graph(Ctx& c, Model::GraphEntry want, int* d_tcur, const int* d_t, const Pass& pass) {
+  Model& m = M(c);
+  for (const Model::GraphEntry& g : m.graphs)
+    if (g.key == want.key && g.xb == want.xb && g.eps == want.eps && g.kv == want.kv && g.work_mark == want.work_mark &&
+        g.cond == want.cond)
+      return g;
+  // warm-up pass outside capture (sets kernel attributes), then capture
+  SDB_CUDA(cudaMemcpyAsync(d_tcur, d_t, 4, cudaMemcpyDeviceToDevice, c.stream));
+  pass();
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  const int64_t before = c.launches;
+  cudaGraph_t graph;
+  SDB_CUDA(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
+  try {
+    pass();
+  } catch (...) {
+    cudaGraph_t g2;
+    cudaStreamEndCapture(c.stream, &g2);
+    throw;
+  }
+  SDB_CUDA(cudaStreamEndCapture(c.stream, &graph));
+  want.launches = c.launches - before;
+  c.launches = before;
+  SDB_CUDA(cudaGraphInstantiate(&want.exec, graph, 0));
+  cudaGraphDestroy(graph);
+  m.graphs.push_back(want);
+  return want;
+}
+
+// sample_latent + latent_to_image (stablediffusion/mod.rs:51-160) from schedule index `first` on. The guidance groups of a step
+// (forward_diffuser :162-192) run as ONE batch-(groups n) UNet pass: weights stream from HBM once. Two groups: unconditional |
+// prompt. Three (an edit): negative without the image, negative with it, prompt with it, and k.cond holds each group's image
+// channels. Runs on c.stream; the caller joins the streams.
+static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const StepCond& k, int H, int W, float* d_latent_out,
+                        uint8_t* d_rgb) {
   Model& m = M(c);
   c.work.reset();
   const int n = b.n;
-  const int groups = ei ? 3 : 2;
+  const int groups = k.groups;
   const int nb = groups * n;
   // padded to the longest row count any sample reads, not to the caller's strides: the step graph is keyed on Lpad
   int lmax = 1;
@@ -1533,12 +1684,12 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const fl
     KernelScope ks(c, KC_ELEMENTWISE);
     stage_cfg_context_launch(b.cond, b.L, b.uncond, b.ustride, d_len, n, Lpad, ctxp, c.stream, groups);
   }
-  if (!ii) {
-    for (int g = 0; g < groups; ++g)
-      SDB_CUDA(cudaMemcpyAsync(xb + g * le, d_init_latent, le * 4, cudaMemcpyDeviceToDevice, c.stream));
-  } else {
+  if (k.z0) {
     KernelScope ks(c, KC_ELEMENTWISE);
-    img2img_prep_launch(ii->z0, ii->eps, xb, (long long)le, ii->sa, ii->sb, ii->mask, ii->w, H, W, c.stream);
+    img2img_prep_launch(k.z0, k.eps, xb, (long long)le, k.sa, k.sb, k.mask, k.w, H, W, c.stream);
+  } else {
+    for (int g = 0; g < groups; ++g)
+      SDB_CUDA(cudaMemcpyAsync(xb + g * le, k.start, le * 4, cudaMemcpyDeviceToDevice, c.stream));
   }
   const int step = 1000 / n_steps;
   std::vector<int> ts = ddim_timesteps(n_steps);
@@ -1568,375 +1719,43 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const fl
   CtxState cs;
   prepare_context(f, ctxp, Lpad, d_len, cs);  // context K/V: once per image, not once per step
 
-  // one CUDA graph of the UNet step per (nb,H,W,Lpad); replayed with a different timestep slot each step
-  const long long key = ((long long)nb << 48) ^ ((long long)H << 36) ^ ((long long)W << 24) ^ ((long long)Lpad << 8) ^
-                        (long long)(c.opt_precision & 3);
-  const bool use_graph = c.opt_graphs && !c.profiling;
-  // an io slot that can grow and move between calls: part of the graph match
-  const float* cond = ii ? ii->cond : (ei ? ei->cond : nullptr);
   int* d_tcur = c.work.get<int>(1);
-  const size_t work_mark = c.work.off;
-  cudaGraphExec_t exec = nullptr;
-  int64_t graph_launches = 0;
-  if (use_graph) {
-    for (auto& g : m.graphs)
-      if (g.key == key && g.io[0] == (void*)xb && g.io[1] == (void*)eps && g.io[2] == (void*)cs.kv[0].kv &&
-          g.io[4] == (void*)(uintptr_t)work_mark &&  // the step's own temporaries start at work_mark
-          g.io[5] == (const void*)cond)
-        exec = g.exec, graph_launches = (int64_t)(intptr_t)g.io[3];
-    if (!exec) {
-      // warm-up pass outside capture (sets kernel attributes), then capture
-      SDB_CUDA(cudaMemcpyAsync(d_tcur, d_t, 4, cudaMemcpyDeviceToDevice, c.stream));
-      unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all, cond);
-      SDB_CUDA(cudaStreamSynchronize(c.stream));
-      const int64_t before = c.launches;
-      cudaGraph_t graph;
-      SDB_CUDA(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
-      try {
-        unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all, cond);
-      } catch (...) {
-        cudaGraph_t g2;
-        cudaStreamEndCapture(c.stream, &g2);
-        throw;
-      }
-      SDB_CUDA(cudaStreamEndCapture(c.stream, &graph));
-      graph_launches = c.launches - before;
-      c.launches = before;
-      SDB_CUDA(cudaGraphInstantiate(&exec, graph, 0));
-      cudaGraphDestroy(graph);
-      Model::GraphEntry ge;
-      ge.key = key, ge.exec = exec;
-      memset(ge.io, 0, sizeof(ge.io));
-      ge.io[0] = xb, ge.io[1] = eps, ge.io[2] = cs.kv[0].kv, ge.io[3] = (void*)(intptr_t)graph_launches;
-      ge.io[4] = (void*)(uintptr_t)work_mark;
-      ge.io[5] = (void*)cond;
-      m.graphs.push_back(ge);
-    }
-  }
-  // the sampler (DESIGN §7 f6): DDIM with eta = 0 is sample_latent's own step and keeps its kernel
+  auto pass = [&] { unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all, k.cond); };
+  // one CUDA graph of the UNet step per (nb,H,W,Lpad); replayed with a different timestep slot each step
+  Model::GraphEntry graph;
+  graph.key = ((long long)nb << 48) ^ ((long long)H << 36) ^ ((long long)W << 24) ^ ((long long)Lpad << 8) ^
+              (long long)(c.opt_precision & 3);
+  graph.xb = xb, graph.eps = eps, graph.kv = cs.kv[0].kv, graph.work_mark = c.work.off, graph.cond = k.cond;
+  if (c.opt_graphs && !c.profiling) graph = step_graph(c, graph, d_tcur, d_t, pass);
+  // the sampler (DESIGN §7 f6): DDIM with eta = 0 is sample_latent's own step
   const bool dpm = c.sampler_kind == SDB_SAMPLER_DPMPP_2M;
-  const int kind = dpm ? STEP_DPMPP_2M : (c.sampler_eta != 0.0 ? STEP_DDIM_ETA : STEP_DDIM);
-  float* hist = dpm ? (float*)c.io(kIoSamplerHist, le * 4) : nullptr;
+  CfgStepArgs call;
+  call.kind = dpm ? STEP_DPMPP_2M : (c.sampler_eta != 0.0 ? STEP_DDIM_ETA : STEP_DDIM);
+  call.groups = groups;
+  call.eu = eps, call.ec = eps + le, call.lat = xb, call.count = (long long)le, call.plane = H * W;
+  call.scale = (float)b.scale, call.scale_i = (float)k.image_scale;
+  if (k.w) call.z0 = k.z0, call.e0 = k.eps, call.w = k.w;
+  call.s.hist = dpm ? (float*)c.io(kIoSamplerHist, le * 4) : nullptr;
+  call.s.scales = b.d_scale, call.s.noise_seeds = b.d_noise_seed;  // per-sample step (batch entries) when set
   double h_prev = 0.0;  // DPM++: h of the previous step this call ran (none before the first)
   for (size_t i = 0; i < ts.size(); ++i) {
-    const int t = ts[i];
-    // alphas are read as f32 and widened to f64 (stablediffusion/mod.rs:124-140)
-    const double a_t = (double)m.alphas_host[t];
-    const double a_prev = (t >= step) ? (double)m.alphas_host[t - step] : 1.0;
     SDB_CUDA(cudaMemcpyAsync(d_tcur, d_t + i, 4, cudaMemcpyDeviceToDevice, c.stream));
-    if (exec) {
-      SDB_CUDA(cudaGraphLaunch(exec, c.stream));
-      c.launches += graph_launches;
+    if (graph.exec) {
+      SDB_CUDA(cudaGraphLaunch(graph.exec, c.stream));
+      c.launches += graph.launches;
     } else {
-      c.work.off = work_mark;
-      unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all, cond);
+      c.work.off = graph.work_mark;
+      pass();
     }
     KernelScope ks(c, KC_ELEMENTWISE);
-    const bool blend = ii && ii->mask && !ii->cond;
-    double dir = std::sqrt(1.0 - a_prev);
-    SamplerStep s;
-    if (kind != STEP_DDIM) {
-      s.ka = (float)std::sqrt(a_prev), s.kb = (float)dir;
-      if (kind == STEP_DDIM_ETA) {  // Song et al. 2021 eq. 16; s = 0 on the final step (a_prev = 1)
-        const double sig = c.sampler_eta * std::sqrt((1.0 - a_prev) / (1.0 - a_t)) * std::sqrt(1.0 - a_t / a_prev);
-        dir = std::sqrt(std::max(0.0, 1.0 - a_prev - sig * sig));
-        s.s = (float)sig;
-        step_noise_keys(c.sampler_noise_seed, t, &s.k0, &s.k1);
-      } else if (t < step) {  // DPM++ final step: sigma' = 0, h = inf: first order, x' = x0
-        s.cx = 0.f, s.cd = 1.f;
-      } else {  // DPM-Solver++(2M) (Lu et al. 2022), data prediction, lambda = ln(alpha / sigma)
-        const double lam = std::log(std::sqrt(a_t) / std::sqrt(1.0 - a_t));
-        const double lam_next = std::log(std::sqrt(a_prev) / std::sqrt(1.0 - a_prev));
-        const double h = lam_next - lam;
-        s.cx = (float)(std::sqrt(1.0 - a_prev) / std::sqrt(1.0 - a_t));
-        s.cd = (float)(-std::sqrt(a_prev) * std::expm1(-h));
-        if (i > 0) {  // second order: the first step a call runs has no history
-          const double c2 = 1.0 / (2.0 * (h_prev / h));
-          s.second = 1, s.c1 = (float)(1.0 + c2), s.c2 = (float)c2;
-        }
-        h_prev = h;
-      }
-      s.hist = hist;
-    }
-    if (ei) {
-      cfg3_sampler_launch(kind, s, eps, xb, (long long)le, (float)b.scale, (float)ei->image_scale, (float)std::sqrt(1.0 - a_t),
-                          (float)std::sqrt(a_t), (float)std::sqrt(a_prev), (float)dir, c.stream);
-    } else if (kind == STEP_DDIM && !b.d_scale) {
-      cfg_ddim_launch(eps, eps + le, xb, (long long)le, (float)b.scale, (float)std::sqrt(1.0 - a_t), (float)std::sqrt(a_t),
-                      (float)std::sqrt(a_prev), (float)dir, c.stream, blend ? ii->z0 : nullptr, blend ? ii->eps : nullptr,
-                      blend ? ii->w : nullptr, H * W);
-    } else {
-      s.scales = b.d_scale, s.noise_seeds = b.d_noise_seed, s.t = t;  // per-sample step (batch entries) when set
-      cfg_sampler_launch(kind, s, eps, eps + le, xb, (long long)le, (float)b.scale, (float)std::sqrt(1.0 - a_t),
-                         (float)std::sqrt(a_t), (float)std::sqrt(a_prev), (float)dir, c.stream, blend ? ii->z0 : nullptr,
-                         blend ? ii->eps : nullptr, blend ? ii->w : nullptr, H * W);
-    }
+    CfgStepArgs a = call;
+    step_scalars(c, m.alphas_host, a.kind, ts[i], step, i > 0, h_prev, a);
+    cfg_step_launch(a, c.stream);
   }
-  c.work.off = work_mark;
+  c.work.off = graph.work_mark;
   if (d_latent_out) SDB_CUDA(cudaMemcpyAsync(d_latent_out, xb, le * 4, cudaMemcpyDeviceToDevice, c.stream));
   if (d_rgb) latent_to_image_dev(c, xb, n, H, W, d_rgb);
 }
-
-void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale,
-                      int n_steps, const float* d_init_latent, int H, int W, float* d_latent_out, uint8_t* d_rgb,
-                      cudaStream_t caller) {
-  check_txt2img(c);
-  check_sample_args(n, L, Lu, n_steps, H, W);
-  StreamJoin join(c, caller);
-  sample_loop(c, uniform_batch(d_context, n, L, d_uncond, Lu, scale), n_steps, 0, d_init_latent, nullptr, H, W, d_latent_out,
-              d_rgb);
-}
-
-void model_sample_host(Ctx& c, const float* context, int n, int L, const float* uncond, int Lu, double scale, int n_steps,
-                       const float* init_latent, uint64_t seed, int H, int W, float* latent_out, uint8_t* rgb) {
-  check_txt2img(c);
-  const size_t le = (size_t)n * 4 * H * W, ce = (size_t)n * L * 768, ue = (size_t)Lu * 768, re = (size_t)n * 3 * 64 * H * W;
-  float* d_c = (float*)c.io(0, ce * 4);
-  float* d_u = (float*)c.io(1, ue * 4);
-  float* d_l = (float*)c.io(2, le * 4);
-  float* d_lo = latent_out ? (float*)c.io(3, le * 4) : nullptr;
-  uint8_t* d_r = rgb ? (uint8_t*)c.io(4, re) : nullptr;
-  SDB_CUDA(cudaMemcpyAsync(d_c, context, ce * 4, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_u, uncond, ue * 4, cudaMemcpyHostToDevice, c.stream));
-  if (init_latent)
-    SDB_CUDA(cudaMemcpyAsync(d_l, init_latent, le * 4, cudaMemcpyHostToDevice, c.stream));
-  else
-    randn_launch(d_l, (long long)le, seed, c.stream);
-  model_sample_dev(c, d_c, n, L, d_u, Lu, scale, n_steps, d_l, H, W, d_lo, d_r, c.stream);
-  if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
-  if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-}
-
-// ================================================================================ image-to-image / inpainting (DESIGN §7 f5)
-// The schedule index img2img starts from: k = floor(strength * N) of the N timesteps run, the last k of them.
-static int img2img_first(double strength, int n_steps) {
-  SDB_CHECK(std::isfinite(strength) && strength > 0.0 && strength <= 1.0, "img2img: strength must be finite and in (0, 1]");
-  const int N = (int)ddim_timesteps(n_steps).size();
-  const int k = (int)std::floor(strength * (double)N);
-  char msg[160];
-  snprintf(msg, sizeof(msg), "img2img: strength %.17g runs none of the %d timesteps; the smallest valid strength is 1/%d = %.17g",
-           strength, N, N, 1.0 / N);
-  SDB_CHECK(k >= 1, msg);
-  return N - k;
-}
-
-static void check_img2img_args(const Ctx& c, int n, int L, int Lu, int n_steps, int H, int W, const void* image, const void* mask,
-                               const void* context, const void* uncond, const void* latent_out, const void* rgb) {
-  check_not_pix2pix(c, "img2img");
-  check_sample_args(n, L, Lu, n_steps, H, W);
-  SDB_CHECK(image && context && uncond, "img2img: null image, context or uncond");
-  SDB_CHECK(mask || c.unet_cin == 4, "img2img: the mask is NULL; a 9-channel inpainting UNet (sdb_create_inpaint) needs one");
-  SDB_CHECK(latent_out || rgb, "img2img: request the latent, the image or both");
-}
-
-// Encoder (chunks of 4 images, as model_encode_dev) -> z0 in an io slot -> sampler loop from t0 = ts[N - k] -> decode.
-// z0 and the latent mask live in io slots, not in the work arena: the arena prefix up to the loop's work_mark is laid out
-// exactly as txt2img lays it out, so no cached step graph can see img2img data where it expects its own temporaries.
-// A 9-channel UNet (DESIGN §7 f9) gets no blend: inpaint_prep writes the masked image's encoder input and the latent mask, and
-// a second encoder pass (the same chunks) writes z_m, so the conditioning tensor [n,5,H,W] (io slot kIoUNetCond) holds
-// m_lat | z_m for conv_in.
-// Runs on c.stream; the caller has checked the arguments and joined the streams.
-static void img2img_run(Ctx& c, const Batch& b, const uint8_t* d_image, const uint8_t* d_mask, double strength, int n_steps,
-                        const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb) {
-  Model& m = M(c);
-  const int n = b.n;
-  const int first = img2img_first(strength, n_steps);
-  const double abar = (double)m.alphas_host[ddim_timesteps(n_steps)[first]];  // read as f32, widened (mod.rs:124-140)
-  Img2ImgIn ii;
-  ii.sa = (float)std::sqrt(abar), ii.sb = (float)std::sqrt(1.0 - abar);
-  const bool inpaint = c.unet_cin == 9;
-  ii.eps = d_noise, ii.mask = inpaint ? nullptr : d_mask;
-  const size_t le = (size_t)n * 4 * H * W;
-  ii.z0 = (float*)c.io(kIoImg2ImgZ0, le * 4);
-  if (ii.mask) ii.w = (float*)c.io(kIoImg2ImgW, (size_t)n * H * W * 4);
-  float* cond = inpaint ? (float*)c.io(kIoUNetCond, (size_t)n * 5 * H * W * 4) : nullptr;
-  c.work.reset();
-  const int Hp = 8 * H, Wp = 8 * W;
-  const size_t plane = (size_t)Hp * Wp;
-  for (int i0 = 0; i0 < n; i0 += 4) {
-    const int nb = std::min(4, n - i0);
-    const size_t mark = c.work.off;
-    float* img4 = c.work.get<float>((size_t)nb * 4 * plane);
-    {
-      KernelScope ks(c, KC_ELEMENTWISE);
-      u8_to_enc_input_launch(d_image + (size_t)i0 * 3 * plane, nb, Hp, Wp, img4, c.stream);
-    }
-    Fwd f(c, nb);
-    vae_encode(f, img4, Hp, Wp, ii.z0 + (size_t)i0 * 4 * H * W);
-    c.work.off = mark;
-  }
-  if (inpaint) {
-    float* enc_in = c.work.get<float>((size_t)n * 4 * plane);
-    {
-      KernelScope ks(c, KC_ELEMENTWISE);
-      inpaint_prep_launch(d_image, d_mask, n, Hp, Wp, enc_in, cond, c.stream);
-    }
-    for (int i0 = 0; i0 < n; i0 += 4) {
-      const int nb = std::min(4, n - i0);
-      const size_t mark = c.work.off;
-      Fwd f(c, nb);
-      vae_encode(f, enc_in + (size_t)i0 * 4 * plane, Hp, Wp, cond + ((size_t)i0 * 5 + 1) * H * W, 5ll * H * W, 0.18215f);
-      c.work.off = mark;
-    }
-    ii.cond = cond;
-  }
-  sample_loop(c, b, n_steps, first, nullptr, &ii, H, W, d_latent_out, d_rgb);
-}
-
-void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
-                       int L, const float* d_uncond, int Lu, double scale, int n_steps, const float* d_noise, int H, int W,
-                       float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
-  check_img2img_args(c, n, L, Lu, n_steps, H, W, d_image, d_mask, d_context, d_uncond, d_latent_out, d_rgb);
-  SDB_CHECK(d_noise, "img2img: the device entry needs the noise latent");
-  img2img_first(strength, n_steps);
-  StreamJoin join(c, caller);
-  img2img_run(c, uniform_batch(d_context, n, L, d_uncond, Lu, scale), d_image, d_mask, strength, n_steps, d_noise, H, W,
-              d_latent_out, d_rgb);
-}
-
-void model_img2img_host(Ctx& c, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
-                        const float* uncond, int Lu, double scale, int n_steps, const float* noise, uint64_t seed, int H, int W,
-                        float* latent_out, uint8_t* rgb) {
-  check_img2img_args(c, n, L, Lu, n_steps, H, W, image, mask, context, uncond, latent_out, rgb);
-  img2img_first(strength, n_steps);  // reject before staging anything
-  const size_t le = (size_t)n * 4 * H * W, ce = (size_t)n * L * 768, ue = (size_t)Lu * 768, re = (size_t)n * 3 * 64 * H * W,
-               me = (size_t)n * 64 * H * W;
-  float* d_c = (float*)c.io(0, ce * 4);
-  float* d_u = (float*)c.io(1, ue * 4);
-  float* d_n = (float*)c.io(2, le * 4);
-  float* d_lo = latent_out ? (float*)c.io(3, le * 4) : nullptr;
-  uint8_t* d_r = rgb ? (uint8_t*)c.io(4, re) : nullptr;
-  uint8_t* d_i = (uint8_t*)c.io(5, re);
-  uint8_t* d_m = mask ? (uint8_t*)c.io(6, me) : nullptr;
-  SDB_CUDA(cudaMemcpyAsync(d_c, context, ce * 4, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_u, uncond, ue * 4, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_i, image, re, cudaMemcpyHostToDevice, c.stream));
-  if (mask) SDB_CUDA(cudaMemcpyAsync(d_m, mask, me, cudaMemcpyHostToDevice, c.stream));
-  if (noise)
-    SDB_CUDA(cudaMemcpyAsync(d_n, noise, le * 4, cudaMemcpyHostToDevice, c.stream));
-  else
-    randn_launch(d_n, (long long)le, seed, c.stream);  // the latent txt2img would start from for this seed
-  model_img2img_dev(c, d_i, d_m, strength, d_c, n, L, d_u, Lu, scale, n_steps, d_n, H, W, d_lo, d_r, c.stream);
-  if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
-  if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-}
-
-// ================================================================================ InstructPix2Pix (DESIGN §7 f10)
-static void check_edit_args(const Ctx& c, int n, int L, int Lu, double text_scale, double image_scale, int n_steps, int H, int W,
-                            const void* image, const void* context, const void* uncond, const void* latent_out, const void* rgb) {
-  char msg[240];
-  snprintf(msg, sizeof(msg),
-           "edit_image: this context's UNet takes %d input channels; InstructPix2Pix needs the 8-channel UNet of a context from "
-           "sdb_create_pix2pix",
-           c.unet_cin);
-  SDB_CHECK(c.unet_cin == 8, msg);
-  check_sample_args(n, L, Lu, n_steps, H, W);
-  SDB_CHECK(image && context && uncond, "edit_image: null image, context or uncond");
-  SDB_CHECK(latent_out || rgb, "edit_image: request the latent, the image or both");
-  snprintf(msg, sizeof(msg), "edit_image: text_scale = %.17g is not finite", text_scale);
-  SDB_CHECK(std::isfinite(text_scale), msg);
-  snprintf(msg, sizeof(msg), "edit_image: image_scale = %.17g is not finite", image_scale);
-  SDB_CHECK(std::isfinite(image_scale), msg);
-}
-
-// The encoder (chunks of 4 images, as model_encode_dev) writes c_I, unscaled, into group 1 of the conditioning tensor
-// [3n,4,H,W] (io slot kIoUNetCond, outside the work arena like img2img's z0); group 2 is a copy and group 0 zero. Then the
-// sampler loop from t = 999 over the full schedule with three guidance groups.
-// Runs on c.stream; the caller has checked the arguments and joined the streams.
-static void edit_run(Ctx& c, const Batch& b, double image_scale, const uint8_t* d_image, int n_steps, const float* d_init_latent,
-                     int H, int W, float* d_latent_out, uint8_t* d_rgb) {
-  const int n = b.n;
-  const size_t le = (size_t)n * 4 * H * W;
-  float* cond = (float*)c.io(kIoUNetCond, 3 * le * 4);
-  c.work.reset();
-  const int Hp = 8 * H, Wp = 8 * W;
-  const size_t plane = (size_t)Hp * Wp;
-  SDB_CUDA(cudaMemsetAsync(cond, 0, le * 4, c.stream));
-  for (int i0 = 0; i0 < n; i0 += 4) {
-    const int nb = std::min(4, n - i0);
-    const size_t mark = c.work.off;
-    float* img4 = c.work.get<float>((size_t)nb * 4 * plane);
-    {
-      KernelScope ks(c, KC_ELEMENTWISE);
-      u8_to_enc_input_launch(d_image + (size_t)i0 * 3 * plane, nb, Hp, Wp, img4, c.stream);
-    }
-    Fwd f(c, nb);
-    vae_encode(f, img4, Hp, Wp, cond + le + (size_t)i0 * 4 * H * W);
-    c.work.off = mark;
-  }
-  SDB_CUDA(cudaMemcpyAsync(cond + 2 * le, cond + le, le * 4, cudaMemcpyDeviceToDevice, c.stream));
-  EditIn ei;
-  ei.cond = cond, ei.image_scale = image_scale;
-  sample_loop(c, b, n_steps, 0, d_init_latent, nullptr, H, W, d_latent_out, d_rgb, &ei);
-}
-
-void model_edit_dev(Ctx& c, const uint8_t* d_image, const float* d_context, int n, int L, const float* d_uncond, int Lu,
-                    double text_scale, double image_scale, int n_steps, const float* d_init_latent, int H, int W,
-                    float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
-  check_edit_args(c, n, L, Lu, text_scale, image_scale, n_steps, H, W, d_image, d_context, d_uncond, d_latent_out, d_rgb);
-  SDB_CHECK(d_init_latent, "edit_image: the device entry needs the start latent");
-  StreamJoin join(c, caller);
-  edit_run(c, uniform_batch(d_context, n, L, d_uncond, Lu, text_scale), image_scale, d_image, n_steps, d_init_latent, H, W,
-           d_latent_out, d_rgb);
-}
-
-void model_edit_host(Ctx& c, const uint8_t* image, const float* context, int n, int L, const float* uncond, int Lu,
-                     double text_scale, double image_scale, int n_steps, const float* init_latent, uint64_t seed, int H, int W,
-                     float* latent_out, uint8_t* rgb) {
-  check_edit_args(c, n, L, Lu, text_scale, image_scale, n_steps, H, W, image, context, uncond, latent_out, rgb);
-  const size_t le = (size_t)n * 4 * H * W, ce = (size_t)n * L * 768, ue = (size_t)Lu * 768, re = (size_t)n * 3 * 64 * H * W;
-  float* d_c = (float*)c.io(0, ce * 4);
-  float* d_u = (float*)c.io(1, ue * 4);
-  float* d_l = (float*)c.io(2, le * 4);
-  float* d_lo = latent_out ? (float*)c.io(3, le * 4) : nullptr;
-  uint8_t* d_r = rgb ? (uint8_t*)c.io(4, re) : nullptr;
-  uint8_t* d_i = (uint8_t*)c.io(5, re);
-  SDB_CUDA(cudaMemcpyAsync(d_c, context, ce * 4, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_u, uncond, ue * 4, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_i, image, re, cudaMemcpyHostToDevice, c.stream));
-  if (init_latent)
-    SDB_CUDA(cudaMemcpyAsync(d_l, init_latent, le * 4, cudaMemcpyHostToDevice, c.stream));
-  else
-    randn_launch(d_l, (long long)le, seed, c.stream);  // the latent sdb_sample_image starts from for this seed
-  model_edit_dev(c, d_i, d_c, n, L, d_u, Lu, text_scale, image_scale, n_steps, d_l, H, W, d_lo, d_r, c.stream);
-  if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
-  if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-}
-
-// ================================================================================ batches of different requests (DESIGN §7 f7)
-// Rejects a malformed descriptor before anything is staged, naming the field, the sample and the value.
-static void check_batch(const sdb_batch* b, bool need_seed) {
-  SDB_CHECK(b, "batch: null descriptor");
-  char msg[200];
-  snprintf(msg, sizeof(msg), "batch: n = %d must be >= 1", b->n);
-  SDB_CHECK(b->n >= 1, msg);
-  snprintf(msg, sizeof(msg), "batch: the row strides L = %d and Lu = %d must be >= 1", b->L, b->Lu);
-  SDB_CHECK(b->L >= 1 && b->Lu >= 1, msg);
-  SDB_CHECK(b->context, "batch: context is NULL");
-  SDB_CHECK(b->uncond, "batch: uncond is NULL");
-  SDB_CHECK(b->guidance_scale, "batch: guidance_scale is NULL");
-  SDB_CHECK(b->seed || !need_seed, "batch: seed is NULL and no init latent / noise is given");
-  for (int i = 0; i < b->n; ++i) {
-    const int l = b->context_len ? b->context_len[i] : b->L, lu = b->uncond_len ? b->uncond_len[i] : b->Lu;
-    snprintf(msg, sizeof(msg), "batch: context_len[%d] = %d is outside [1, L = %d]", i, l, b->L);
-    SDB_CHECK(l >= 1 && l <= b->L, msg);
-    snprintf(msg, sizeof(msg), "batch: uncond_len[%d] = %d is outside [1, Lu = %d]", i, lu, b->Lu);
-    SDB_CHECK(lu >= 1 && lu <= b->Lu, msg);
-    snprintf(msg, sizeof(msg), "batch: guidance_scale[%d] = %.17g is not finite", i, b->guidance_scale[i]);
-    SDB_CHECK(std::isfinite(b->guidance_scale[i]), msg);
-  }
-}
-
-namespace {
-struct BatchTab {  // the per-sample tables of a batch call on the device (io slot kIoBatchTab)
-  const uint64_t* seed;
-  const uint64_t* noise_seed;
-  const float* scale;
-};
-}  // namespace
 
 // Scales are cast to float as the single-request entries cast theirs; a NULL noise_seed array means the context's noise seed
 // (sdb_set_sampler) for every sample.
@@ -1956,9 +1775,15 @@ static BatchTab upload_batch_tab(Ctx& c, const sdb_batch& b) {
   return {(const uint64_t*)d, (const uint64_t*)d + n, (const float*)(d + (size_t)n * 16)};
 }
 
-// the Batch of a descriptor whose context and uncond are device pointers
-static Batch batch_of(const sdb_batch& sb, const BatchTab& tab) {
+// The Batch of a request whose context and uncond are device pointers
+static Batch batch_of(const SampleRequest& r, const BatchTab& tab) {
   Batch b;
+  if (!r.batch) {  // uniform
+    b.n = r.n, b.cond = r.context, b.L = r.L, b.uncond = r.uncond, b.Lu = r.Lu, b.scale = r.scale;
+    b.len.assign(r.n, r.L), b.ulen.assign(r.n, r.Lu);
+    return b;
+  }
+  const sdb_batch& sb = *r.batch;
   b.n = sb.n, b.cond = sb.context, b.L = sb.L, b.uncond = sb.uncond, b.Lu = sb.Lu, b.ustride = (long long)sb.Lu * 768;
   for (int i = 0; i < sb.n; ++i) {
     b.len.push_back(sb.context_len ? sb.context_len[i] : sb.L);
@@ -1968,92 +1793,111 @@ static Batch batch_of(const sdb_batch& sb, const BatchTab& tab) {
   return b;
 }
 
-// [n,4,H,W] in io slot 2: sample i is the latent the single-request entries draw for seed[i] at n = 1
-static float* seeded_latent(Ctx& c, int n, int H, int W, const uint64_t* d_seed) {
-  float* d = (float*)c.io(2, (size_t)n * 4 * H * W * 4);
-  KernelScope ks(c, KC_ELEMENTWISE);
-  randn_seeds_launch(d, n, 4ll * H * W, d_seed, c.stream);
-  return d;
+// One checked request with device pointers, on c.stream. A batch's NULL start is drawn per sample into io slot kIoStart: sample i is
+// the latent the single-request entries draw for seed[i] at n = 1.
+// img2img: the encoder writes z0 into an io slot, then the sampler loop runs from t0 = ts[first]. z0 and the latent mask live in
+// io slots, not in the work arena: the arena prefix up to the loop's work_mark is laid out exactly as txt2img lays it out, so no
+// cached step graph can see img2img data where it expects its own temporaries. A 9-channel UNet (DESIGN §7 f9) gets no blend:
+// inpaint_prep writes the masked image's encoder input and the latent mask, and a second encoder pass writes z_m, so the
+// conditioning tensor [n,5,H,W] (io slot kIoUNetCond) holds m_lat | z_m for conv_in.
+// edit: the encoder writes c_I, unscaled, into group 1 of the conditioning tensor [3n,4,H,W] (io slot kIoUNetCond); group 2 is a
+// copy and group 0 zero. Then the sampler loop from t = 999 over the full schedule with three guidance groups.
+static void sample_run(Ctx& c, const SampleRequest& r, int first) {
+  Model& m = M(c);
+  BatchTab tab;
+  if (r.batch) tab = upload_batch_tab(c, *r.batch);
+  const Batch b = batch_of(r, tab);
+  const int n = b.n, H = r.H, W = r.W;
+  const size_t le = (size_t)n * 4 * H * W;
+  const float* start = r.start;
+  if (!start && r.batch) {
+    float* d = (float*)c.io(kIoStart, le * 4);
+    KernelScope ks(c, KC_ELEMENTWISE);
+    randn_seeds_launch(d, n, 4ll * H * W, tab.seed, c.stream);
+    start = d;
+  }
+  StepCond k;
+  if (r.kind == SAMPLE_IMG2IMG) {
+    const double abar = (double)m.alphas_host[ddim_timesteps(r.n_steps)[first]];  // read as f32, widened (mod.rs:124-140)
+    k.sa = (float)std::sqrt(abar), k.sb = (float)std::sqrt(1.0 - abar);
+    const bool inpaint = c.unet_cin == 9;
+    k.eps = start, k.mask = inpaint ? nullptr : r.mask;
+    k.z0 = (float*)c.io(kIoImg2ImgZ0, le * 4);
+    if (k.mask) k.w = (float*)c.io(kIoImg2ImgW, (size_t)n * H * W * 4);
+    float* cond = inpaint ? (float*)c.io(kIoUNetCond, (size_t)n * 5 * H * W * 4) : nullptr;
+    c.work.reset();
+    encode_images(c, r.image, nullptr, n, H, W, k.z0);
+    if (inpaint) {
+      float* enc_in = c.work.get<float>((size_t)n * 4 * 64 * H * W);
+      {
+        KernelScope ks(c, KC_ELEMENTWISE);
+        inpaint_prep_launch(r.image, r.mask, n, 8 * H, 8 * W, enc_in, cond, c.stream);
+      }
+      encode_images(c, nullptr, enc_in, n, H, W, cond + (size_t)H * W, 5ll * H * W, 0.18215f);
+      k.cond = cond;
+    }
+  } else if (r.kind == SAMPLE_EDIT) {
+    float* cond = (float*)c.io(kIoUNetCond, 3 * le * 4);
+    c.work.reset();
+    SDB_CUDA(cudaMemsetAsync(cond, 0, le * 4, c.stream));
+    encode_images(c, r.image, nullptr, n, H, W, cond + le);
+    SDB_CUDA(cudaMemcpyAsync(cond + 2 * le, cond + le, le * 4, cudaMemcpyDeviceToDevice, c.stream));
+    k.groups = 3, k.start = start, k.cond = cond, k.image_scale = r.image_scale;
+  } else {
+    k.start = start;
+  }
+  sample_loop(c, b, r.n_steps, first, k, H, W, r.latent_out, r.rgb);
 }
 
-// copies a host descriptor's context and uncond to io slots 0 / 1 and points the device descriptor at them
-static sdb_batch stage_batch_host(Ctx& c, const sdb_batch& sb) {
-  sdb_batch db = sb;
-  const size_t ce = (size_t)sb.n * sb.L * 768, ue = (size_t)sb.n * sb.Lu * 768;
-  float* d_c = (float*)c.io(0, ce * 4);
-  float* d_u = (float*)c.io(1, ue * 4);
-  SDB_CUDA(cudaMemcpyAsync(d_c, sb.context, ce * 4, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_u, sb.uncond, ue * 4, cudaMemcpyHostToDevice, c.stream));
-  db.context = d_c, db.uncond = d_u;
-  return db;
-}
-
-void model_sample_batch_dev(Ctx& c, const sdb_batch* sb, int n_steps, const float* d_init_latent, int H, int W,
-                            float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller) {
-  check_txt2img(c);
-  check_batch(sb, !d_init_latent);
-  check_sample_args(sb->n, sb->L, sb->Lu, n_steps, H, W);
-  SDB_CHECK(d_latent_out || d_rgb, "sample_batch: request the latent, the image or both");
+void model_sample_dev(Ctx& c, const SampleRequest& r, cudaStream_t caller) {
+  const int first = check_request(c, r, false);
   StreamJoin join(c, caller);
-  const BatchTab tab = upload_batch_tab(c, *sb);
-  if (!d_init_latent) d_init_latent = seeded_latent(c, sb->n, H, W, tab.seed);
-  sample_loop(c, batch_of(*sb, tab), n_steps, 0, d_init_latent, nullptr, H, W, d_latent_out, d_rgb);
+  sample_run(c, r, first);
 }
 
-void model_sample_batch_host(Ctx& c, const sdb_batch* sb, int n_steps, const float* init_latent, int H, int W, float* latent_out,
-                             uint8_t* rgb) {
-  check_txt2img(c);
-  check_batch(sb, !init_latent);
-  check_sample_args(sb->n, sb->L, sb->Lu, n_steps, H, W);
-  SDB_CHECK(latent_out || rgb, "sample_batch: request the latent, the image or both");
-  const size_t le = (size_t)sb->n * 4 * H * W, re = (size_t)sb->n * 3 * 64 * H * W;
-  const sdb_batch db = stage_batch_host(c, *sb);
-  float* d_l = init_latent ? (float*)c.io(2, le * 4) : nullptr;
-  float* d_lo = latent_out ? (float*)c.io(3, le * 4) : nullptr;
-  uint8_t* d_r = rgb ? (uint8_t*)c.io(4, re) : nullptr;
-  if (init_latent) SDB_CUDA(cudaMemcpyAsync(d_l, init_latent, le * 4, cudaMemcpyHostToDevice, c.stream));
-  model_sample_batch_dev(c, &db, n_steps, d_l, H, W, d_lo, d_r, c.stream);
-  if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
-  if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-}
-
-void model_img2img_batch_dev(Ctx& c, const sdb_batch* sb, const uint8_t* d_image, const uint8_t* d_mask, double strength,
-                             int n_steps, const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb,
-                             cudaStream_t caller) {
-  check_batch(sb, !d_noise);
-  check_img2img_args(c, sb->n, sb->L, sb->Lu, n_steps, H, W, d_image, d_mask, sb->context, sb->uncond, d_latent_out, d_rgb);
-  img2img_first(strength, n_steps);
-  StreamJoin join(c, caller);
-  const BatchTab tab = upload_batch_tab(c, *sb);
-  if (!d_noise) d_noise = seeded_latent(c, sb->n, H, W, tab.seed);
-  img2img_run(c, batch_of(*sb, tab), d_image, d_mask, strength, n_steps, d_noise, H, W, d_latent_out, d_rgb);
-}
-
-void model_img2img_batch_host(Ctx& c, const sdb_batch* sb, const uint8_t* image, const uint8_t* mask, double strength,
-                              int n_steps, const float* noise, int H, int W, float* latent_out, uint8_t* rgb) {
-  check_batch(sb, !noise);
-  check_img2img_args(c, sb->n, sb->L, sb->Lu, n_steps, H, W, image, mask, sb->context, sb->uncond, latent_out, rgb);
-  img2img_first(strength, n_steps);  // reject before staging anything
-  const int n = sb->n;
-  const size_t le = (size_t)n * 4 * H * W, re = (size_t)n * 3 * 64 * H * W, me = (size_t)n * 64 * H * W;
-  const sdb_batch db = stage_batch_host(c, *sb);
-  float* d_n = noise ? (float*)c.io(2, le * 4) : nullptr;
-  float* d_lo = latent_out ? (float*)c.io(3, le * 4) : nullptr;
-  uint8_t* d_r = rgb ? (uint8_t*)c.io(4, re) : nullptr;
-  uint8_t* d_i = (uint8_t*)c.io(5, re);
-  uint8_t* d_m = mask ? (uint8_t*)c.io(6, me) : nullptr;
-  SDB_CUDA(cudaMemcpyAsync(d_i, image, re, cudaMemcpyHostToDevice, c.stream));
-  if (mask) SDB_CUDA(cudaMemcpyAsync(d_m, mask, me, cudaMemcpyHostToDevice, c.stream));
-  if (noise) SDB_CUDA(cudaMemcpyAsync(d_n, noise, le * 4, cudaMemcpyHostToDevice, c.stream));
-  model_img2img_batch_dev(c, &db, d_i, d_m, strength, n_steps, d_n, H, W, d_lo, d_r, c.stream);
-  if (latent_out) SDB_CUDA(cudaMemcpyAsync(latent_out, d_lo, le * 4, cudaMemcpyDeviceToHost, c.stream));
-  if (rgb) SDB_CUDA(cudaMemcpyAsync(rgb, d_r, re, cudaMemcpyDeviceToHost, c.stream));
+// Copies a host request's inputs into the staging io slots, runs it on c.stream, copies the requested outputs back and
+// synchronises. A NULL start of a single request is the latent randn_launch draws for its seed (uncounted, as txt2img has always
+// drawn it); a batch draws its own per-sample seeds in sample_run.
+void model_sample_host(Ctx& c, const SampleRequest& r) {
+  const int first = check_request(c, r, true);
+  const int n = sample_n(r);
+  const size_t le = (size_t)n * 4 * r.H * r.W, re = (size_t)n * 3 * 64 * r.H * r.W, me = (size_t)n * 64 * r.H * r.W;
+  auto upload = [&](int slot, const void* host, size_t bytes) {
+    void* d = c.io(slot, bytes);
+    SDB_CUDA(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, c.stream));
+    return d;
+  };
+  SampleRequest d = r;
+  sdb_batch db;
+  if (r.batch) {
+    db = *r.batch;
+    db.context = (const float*)upload(kIoContext, db.context, (size_t)n * db.L * 768 * 4);
+    db.uncond = (const float*)upload(kIoUncond, db.uncond, (size_t)n * db.Lu * 768 * 4);
+    d.batch = &db;
+  } else {
+    d.context = (const float*)upload(kIoContext, r.context, (size_t)n * r.L * 768 * 4);
+    d.uncond = (const float*)upload(kIoUncond, r.uncond, (size_t)r.Lu * 768 * 4);
+  }
+  if (r.image) d.image = (const uint8_t*)upload(kIoImage, r.image, re);
+  if (r.mask) d.mask = (const uint8_t*)upload(kIoMask, r.mask, me);
+  if (r.start) {
+    d.start = (const float*)upload(kIoStart, r.start, le * 4);
+  } else if (!r.batch) {
+    float* s = (float*)c.io(kIoStart, le * 4);
+    randn_launch(s, (long long)le, r.seed, c.stream);
+    d.start = s;
+  }
+  d.latent_out = r.latent_out ? (float*)c.io(kIoLatentOut, le * 4) : nullptr;
+  d.rgb = r.rgb ? (uint8_t*)c.io(kIoRgb, re) : nullptr;
+  sample_run(c, d, first);
+  if (r.latent_out) SDB_CUDA(cudaMemcpyAsync(r.latent_out, d.latent_out, le * 4, cudaMemcpyDeviceToHost, c.stream));
+  if (r.rgb) SDB_CUDA(cudaMemcpyAsync(r.rgb, d.rgb, re, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
 }
 
 // forward_diffuser (stablediffusion/mod.rs:162-192): the two UNet evaluations of one guidance step as ONE batch-2n pass (the
-// same pass sample_latent replays as a CUDA graph), then pred = u + (c - u) * scale. d_u / d_c may be null.
+// same pass sample_latent replays as a CUDA graph, its context staged by the same kernel), then pred = u + (c - u) * scale.
+// d_u / d_c may be null.
 void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const float* d_context, int n, int L, const float* d_uncond,
                                 int Lu, double scale, int H, int W, float* d_pred, float* d_u, float* d_c, cudaStream_t caller) {
   check_not_pix2pix(c, "forward_diffuser (two-way guidance)");
@@ -2069,17 +1913,16 @@ void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const floa
   float* eps = c.work.get<float>(2 * le);
   int* d_t = c.work.get<int>(1);
   int* d_len = c.work.get<int>(nb);
-  SDB_CUDA(cudaMemsetAsync(ctxp, 0, (size_t)nb * Lpad * 768 * 4, c.stream));
-  for (int i = 0; i < n; ++i)
-    SDB_CUDA(cudaMemcpyAsync(ctxp + (size_t)i * Lpad * 768, d_uncond, (size_t)Lu * 768 * 4, cudaMemcpyDeviceToDevice, c.stream));
-  SDB_CUDA(cudaMemcpy2DAsync(ctxp + (size_t)n * Lpad * 768, (size_t)Lpad * 768 * 4, d_context, (size_t)L * 768 * 4,
-                             (size_t)L * 768 * 4, n, cudaMemcpyDeviceToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(xb, d_latent, li * 4, cudaMemcpyDeviceToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(xb + li, d_latent, li * 4, cudaMemcpyDeviceToDevice, c.stream));
   std::vector<int> lens(nb);
   for (int i = 0; i < nb; ++i) lens[i] = i < n ? Lu : L;
   SDB_CUDA(cudaMemcpyAsync(d_t, &t, 4, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaMemcpyAsync(d_len, lens.data(), nb * 4, cudaMemcpyHostToDevice, c.stream));
+  {
+    KernelScope ks(c, KC_ELEMENTWISE);
+    stage_cfg_context_launch(d_context, L, d_uncond, 0, d_len, n, Lpad, ctxp, c.stream);
+  }
+  SDB_CUDA(cudaMemcpyAsync(xb, d_latent, li * 4, cudaMemcpyDeviceToDevice, c.stream));
+  SDB_CUDA(cudaMemcpyAsync(xb + li, d_latent, li * 4, cudaMemcpyDeviceToDevice, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
   unet_pass(c, nb, xb, d_t, ctxp, Lpad, d_len, H, W, eps, nullptr);
   if (d_u) SDB_CUDA(cudaMemcpyAsync(d_u, eps, le * 4, cudaMemcpyDeviceToDevice, c.stream));

@@ -29,35 +29,33 @@ void model_decode_dev(Ctx& c, const float* d_latent, int n, int H, int W, float*
 void model_encode_host(Ctx& c, const float* img, int n, int H, int W, float* latent);
 void model_encode_dev(Ctx& c, const float* d_img, int n, int H, int W, float* d_latent, cudaStream_t caller);
 void model_latent_to_image_host(Ctx& c, const float* latent, int n, int H, int W, uint8_t* rgb);
-void model_sample_host(Ctx& c, const float* context, int n, int L, const float* uncond, int Lu, double scale, int n_steps,
-                       const float* init_latent, uint64_t seed, int H, int W, float* latent_out, uint8_t* rgb);
-void model_sample_dev(Ctx& c, const float* d_context, int n, int L, const float* d_uncond, int Lu, double scale,
-                      int n_steps, const float* d_init_latent, int H, int W, float* d_latent_out, uint8_t* d_rgb,
-                      cudaStream_t caller);
-// image-to-image / masked inpainting (DESIGN §7 f5): image u8 [n,8H,8W,3], mask u8 [n,8H,8W] or null, noise [n,4,H,W]
-void model_img2img_dev(Ctx& c, const uint8_t* d_image, const uint8_t* d_mask, double strength, const float* d_context, int n,
-                       int L, const float* d_uncond, int Lu, double scale, int n_steps, const float* d_noise, int H, int W,
-                       float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller);
-void model_img2img_host(Ctx& c, const uint8_t* image, const uint8_t* mask, double strength, const float* context, int n, int L,
-                        const float* uncond, int Lu, double scale, int n_steps, const float* noise, uint64_t seed, int H, int W,
-                        float* latent_out, uint8_t* rgb);
-// batches of different requests (DESIGN §7 f7): sdb_batch with device (dev) or host (host) context / uncond
-void model_sample_batch_dev(Ctx& c, const sdb_batch* b, int n_steps, const float* d_init_latent, int H, int W,
-                            float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller);
-void model_sample_batch_host(Ctx& c, const sdb_batch* b, int n_steps, const float* init_latent, int H, int W, float* latent_out,
-                             uint8_t* rgb);
-void model_img2img_batch_dev(Ctx& c, const sdb_batch* b, const uint8_t* d_image, const uint8_t* d_mask, double strength,
-                             int n_steps, const float* d_noise, int H, int W, float* d_latent_out, uint8_t* d_rgb,
-                             cudaStream_t caller);
-void model_img2img_batch_host(Ctx& c, const sdb_batch* b, const uint8_t* image, const uint8_t* mask, double strength,
-                              int n_steps, const float* noise, int H, int W, float* latent_out, uint8_t* rgb);
-// InstructPix2Pix (DESIGN §7 f10) on an 8-channel context: three-way guidance from t = 999, the image latent unscaled
-void model_edit_dev(Ctx& c, const uint8_t* d_image, const float* d_context, int n, int L, const float* d_uncond, int Lu,
-                    double text_scale, double image_scale, int n_steps, const float* d_init_latent, int H, int W,
-                    float* d_latent_out, uint8_t* d_rgb, cudaStream_t caller);
-void model_edit_host(Ctx& c, const uint8_t* image, const float* context, int n, int L, const float* uncond, int Lu,
-                     double text_scale, double image_scale, int n_steps, const float* init_latent, uint64_t seed, int H, int W,
-                     float* latent_out, uint8_t* rgb);
+// One sampling call of any kind: text-to-image, image-to-image / masked inpainting / 9-channel inpainting (DESIGN §7 f5, f9),
+// batches of different requests (f7) and InstructPix2Pix edits (f10). The sdb_* sampling entries fill it from their arguments;
+// pointers are host pointers for model_sample_host and device pointers for model_sample_dev.
+enum : int { SAMPLE_TXT2IMG = 0, SAMPLE_IMG2IMG = 1, SAMPLE_EDIT = 2 };
+struct SampleRequest {
+  int kind = SAMPLE_TXT2IMG;  // SAMPLE_IMG2IMG: plain, masked or 9-channel inpainting, as the context's UNet and the mask select
+  // the prompts: a batch entry's descriptor (batched; may be null, which the checks reject), or n prompts of L rows [n][L][768],
+  // one negative of Lu rows [Lu][768] broadcast over the batch and one guidance scale (an edit's text scale)
+  bool batched = false;
+  const sdb_batch* batch = nullptr;
+  const float* context = nullptr;
+  const float* uncond = nullptr;
+  int n = 0, L = 0, Lu = 0;
+  double scale = 0.0;
+  const uint8_t* image = nullptr;  // img2img, edit: u8 [n,8H,8W,3]
+  const uint8_t* mask = nullptr;   // img2img: u8 [n,8H,8W] or null
+  double strength = 1.0;           // img2img
+  double image_scale = 0.0;        // edit
+  // [n,4,H,W]: the init latent (txt2img, edit) or the noise (img2img). Null: drawn from seed (host entries) or a batch's seeds
+  const float* start = nullptr;
+  uint64_t seed = 0;
+  int n_steps = 0, H = 0, W = 0;   // latent height and width
+  float* latent_out = nullptr;     // [n,4,H,W] or null
+  uint8_t* rgb = nullptr;          // u8 [n,8H,8W,3] or null
+};
+void model_sample_dev(Ctx& c, const SampleRequest& r, cudaStream_t caller);
+void model_sample_host(Ctx& c, const SampleRequest& r);
 void model_forward_diffuser_dev(Ctx& c, const float* d_latent, int t, const float* d_context, int n, int L, const float* d_uncond,
                                 int Lu, double scale, int H, int W, float* d_pred, float* d_u, float* d_c, cudaStream_t caller);
 void model_forward_diffuser_host(Ctx& c, const float* latent, int t, const float* context, int n, int L, const float* uncond,

@@ -181,11 +181,16 @@ struct Model {
   // sampler
   int alphas_i = -1;
   std::vector<float> alphas_host;
-  // graphs (keyed by shape)
+  // captured UNet step passes of the sampler loop (model.cu: step_graph), keyed by shape and matched on the addresses they bake in
   struct GraphEntry {
-    long long key;
-    cudaGraphExec_t exec;
-    void* io[8];
+    long long key = 0;
+    cudaGraphExec_t exec = nullptr;
+    int64_t launches = 0;         // kernel launches one replay stands for
+    const float* xb = nullptr;    // the step's UNet input and output
+    const float* eps = nullptr;
+    const void* kv = nullptr;     // the context K/V of the first transformer
+    size_t work_mark = 0;         // the step's own temporaries start here in the work arena
+    const float* cond = nullptr;  // the UNet's extra input channels (io slot kIoUNetCond) or null
   };
   std::vector<GraphEntry> graphs;
   // packing units in finalize order: the UNet blocks, then the time-embedding table (unit_emb), then the CLIP blocks

@@ -116,6 +116,14 @@ struct MetaCheck {
   bool must_be_absent = false;  // e.g. a bias file on a bias-less Linear
 };
 
+// host-buffer inputs and outputs of a sampling call (model_sample_host)
+constexpr int kIoContext = 0;    // prompt rows
+constexpr int kIoUncond = 1;     // negative rows: [Lu] broadcast or [n][Lu]
+constexpr int kIoStart = 2;      // the start latent (init latent or img2img noise), given or drawn from the seed(s)
+constexpr int kIoLatentOut = 3;
+constexpr int kIoRgb = 4;
+constexpr int kIoImage = 5;      // u8 [n,8H,8W,3]
+constexpr int kIoMask = 6;       // u8 [n,8H,8W]
 constexpr int kIoImg2ImgZ0 = 8;  // encoded image latent z0 [n,4,H,W]
 constexpr int kIoImg2ImgW = 9;   // latent mask w [n,H,W]
 constexpr int kIoSamplerHist = 10;  // DPM-Solver++(2M): x0 of the previous step [n,4,H,W]

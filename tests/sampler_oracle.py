@@ -1,7 +1,7 @@
 """CPU oracle of the samplers (DESIGN.md §7 f6): stochastic DDIM (eta) and DPM-Solver++(2M) — TEST INFRASTRUCTURE ONLY.
 
 The reference samples with DDIM at eta = 0 (oracle/sd_oracle.py: sample_latent). The per-step coefficients below are computed in
-double exactly as the library's host loop computes them (csrc/model.cu: sample_loop) and rounded once to float32; the new
+double exactly as the library's host loop computes them (csrc/model.cu: step_scalars) and rounded once to float32; the new
 updates are evaluated in numpy float32, one rounding per operation, which is what the fused step's __f*_rn intrinsics compute.
 The solvers take an explicit list of schedule values, so the same step functions drive the full model (sampler_latent) and
 the closed-form Gaussian problem the convergence-order test integrates (gaussian_*).

@@ -2,9 +2,9 @@
 (sdb_sample_image_dev, cfg 7.5) on a 4-channel context against an edit (sdb_edit_image_dev, text 7.5 / image 1.5) on an
 8-channel one, one context per process, three alternated CUDA-event timed runs of each after warm-up. Then, in processes of
 their own, per-launch device times from torch.profiler: the UNet's conv_in with 4 and 8 input channels at a 64x64 latent (nb = 3
-and 12, sdb_unet_forward_dev), and the fused guidance + update step of each call (two-way cfg_ddim_kernel, three-way
-cfg3_sampler_kernel) at n = 1 and 4, graphs off so every launch is traced. The card, power limit and SM clock are read in the
-same call.
+and 12, sdb_unet_forward_dev), and the fused guidance + update step of each call (cfg_step_kernel, two-way <0, false, false, 2>,
+three-way <0, false, false, 3>) at n = 1 and 4, graphs off so every launch is traced. The card, power limit and SM clock are read
+in the same call.
 Usage: python tools/pix2pix_time.py            (the driver; each measurement runs as  python tools/pix2pix_time.py <mode> <cin> <n>)"""
 import ctypes as C
 import os
@@ -69,7 +69,7 @@ def step(cin, n):
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         run()
         torch.cuda.synchronize()
-    name = "cfg3_sampler_kernel" if cin == 8 else "cfg_ddim_kernel"
+    name = f"cfg_step_kernel<0, false, false, {3 if cin == 8 else 2}>"
     us = [e.device_time for e in prof.events() if name in e.name and e.device_time > 0]
     print(f"RESULT {np.mean(us):.3f} {len(us)}")
     c.close()
@@ -126,7 +126,7 @@ def main():
             us, k = sub("conv_in", cin, nb)
             print(f"conv_in cin={cin} 64x64 nb={nb}: {us:.2f} us per launch ({int(k)} launches)", flush=True)
     for n in (1, 4):
-        for cin, what in ((4, "two-way cfg_ddim_kernel"), (8, "three-way cfg3_sampler_kernel")):
+        for cin, what in ((4, "two-way cfg_step_kernel"), (8, "three-way cfg_step_kernel")):
             us, k = sub("step", cin, n)
             print(f"step n={n} {what}: {us:.2f} us per launch ({int(k)} launches)", flush=True)
     card()
