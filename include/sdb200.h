@@ -365,6 +365,40 @@ int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n
 int sdb_test_spatial_transformer(sdb_ctx* ctx, int index, const float* x, int n, int c, int H, int W, const float* context,
                                  int lmax, const int32_t* lens, int flags, float* out, float* out16, float* out_norm, float* taps_y,
                                  float* taps_ln, int32_t* trace);
+/* One stage of the autoencoder, or one of the two CUDA-core convs the UNet shares with it, run on the weights
+ * sdb_finalize_weights packed with the model's own launch code. Needs finalized weights. stage (x [n][c][H][W] NCHW, c as listed):
+ *   SDB_VAE_DEC_IN     decoder conv_in with post_quant_conv and the pre-scale `scale` folded in; x = latent (c 4) -> out 512 ch
+ *   SDB_VAE_DEC_ATTN,  decoder / encoder mid attention (c 512; H * W a multiple of 64, at most 9216); tap = the attention output
+ *   SDB_VAE_ENC_ATTN   before proj_out (fp16 hi + lo), out_norm = SiLU(GroupNorm(out; mid/block_2/norm1)) from proj_out's partials
+ *   SDB_VAE_DEC_OUT,   norm_out + SiLU + conv_out, fused (c 128 -> 3, 320 -> 4, 512 -> 8); for SDB_VAE_ENC_OUT, tap receives
+ *   SDB_VAE_UNET_OUT,  quant_conv + the slice [0, 4): [n][4][H][W], or with flags & 2 strided and scaled as the inpainting tensor
+ *   SDB_VAE_ENC_OUT    [n][5][H][W] is filled (channels 1-4, times `scale`); values the slice does not write are kept from entry
+ *   SDB_VAE_ENC_IN     encoder conv_in on the zero-padded 3 -> 4 channel weights (c 4) -> 128 ch
+ *   SDB_VAE_UNET_IN    the UNet's conv_in (c 4) -> 320 ch with out16 = its fp16 hi + lo copy; on a 9- / 8-channel context cond
+ *                      [n][cin-4][H][W] holds the extra channels, read as the sampler stages them (sample s reads cond[s % m])
+ *   SDB_VAE_ENC_DOWN0..2  encoder/blocks/i/downsampler (c 128 / 256 / 512, H and W even) -> [n][c][H/2][W/2]; out_norm =
+ *                      SiLU(GroupNorm(out; blocks/i+1/res1/norm1)) from the conv's partials
+ * flags: 1 = x is staged with GroupNorm partials, as a ResnetBlock leaves it (a 3-pass identity conv: the stage sees hi + lo of x);
+ * else the fp32 tensor without statistics. out16 / tap / out_norm may be NULL where a stage has none. trace (256 ints): [0]
+ * GroupNorm stagings, [1..4] their path (1-3 as sdb_test_resblock; 4 sums by the statistics kernel, 5 sums from producer partials,
+ * 6 after the 64:1 pre-fold), [5] GEMMs, 12 ints each from [6] (as sdb_test_spatial_transformer), [200] small-Cout conv launches,
+ * [201..203] its rows per tile, channels per round and channel groups, [204] softmax launches, [205] their values per thread,
+ * [206] m of SDB_VAE_UNET_IN's cond (0 without cond). */
+enum {
+  SDB_VAE_DEC_IN = 0,
+  SDB_VAE_DEC_ATTN = 1,
+  SDB_VAE_ENC_ATTN = 2,
+  SDB_VAE_DEC_OUT = 3,
+  SDB_VAE_UNET_OUT = 4,
+  SDB_VAE_ENC_OUT = 5,
+  SDB_VAE_ENC_IN = 6,
+  SDB_VAE_UNET_IN = 7,
+  SDB_VAE_ENC_DOWN0 = 8,
+  SDB_VAE_ENC_DOWN1 = 9,
+  SDB_VAE_ENC_DOWN2 = 10
+};
+int sdb_test_vae_stage(sdb_ctx* ctx, int stage, const float* x, const float* cond, int n, int c, int H, int W, float scale,
+                       int flags, float* out, float* out16, float* tap, float* out_norm, int32_t* trace);
 /* The first `count` values of stochastic DDIM's noise z at timestep t (0 <= t < 1000) for noise_seed, as the fused sampler step
  * draws them (see sdb_set_sampler). Host buffer out [count]. */
 int sdb_test_step_noise(sdb_ctx* ctx, uint64_t noise_seed, int t, int64_t count, float* out);

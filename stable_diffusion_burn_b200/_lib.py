@@ -113,6 +113,8 @@ SIGNATURES = [
     ("sdb_test_spatial_transformer", C.c_int, [_ctx, C.c_int, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, C.c_int,
                                                C.POINTER(C.c_int32), C.c_int, _f32p, _f32p, _f32p, _f32p, _f32p,
                                                C.POINTER(C.c_int32)]),
+    ("sdb_test_vae_stage", C.c_int, [_ctx, C.c_int, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
+                                     _f32p, _f32p, _f32p, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_step_noise", C.c_int, [_ctx, C.c_uint64, C.c_int, C.c_int64, _f32p]),
     ("sdb_test_groupnorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_test_layernorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, _f32p]),
@@ -706,6 +708,51 @@ class Context:
                 for i in range(min(int(t[126]), 4))]
         tr = {"gn": [paths.get(int(v), int(v)) for v in t[1:1 + min(int(t[0]), 4)]], "gemms": gemms, "attn": attn}
         return dict(out=out, out16=out16, out_norm=outn, y=y, ln=ln, trace=tr)
+
+    # sdb_test_vae_stage stages (include/sdb200.h: SDB_VAE_*): name -> (stage, input channels, output channels)
+    VAE_STAGES = {"dec_in": (0, 4, 512), "dec_attn": (1, 512, 512), "enc_attn": (2, 512, 512), "dec_out": (3, 128, 3),
+                  "unet_out": (4, 320, 4), "enc_out": (5, 512, 8), "enc_in": (6, 4, 128), "unet_in": (7, 4, 320),
+                  "enc_down0": (8, 128, 128), "enc_down1": (9, 256, 256), "enc_down2": (10, 512, 512)}
+    _GN_PATHS = {1: "fused", 2: "apply", 3: "apply+fold", 4: "sums:stats", 5: "sums:partials", 6: "sums:fold"}
+
+    def test_vae_stage(self, stage, x, cond=None, scale=1.0, stats=True, quant=None):
+        """One autoencoder stage (or the UNet's conv_in / out conv) on the finalized weights, by name of VAE_STAGES. x
+        [n, c, H, W]; cond [n, cin - 4, H, W] for "unet_in" on a 9- / 8-channel context; scale: the decoder conv_in's pre-scale, or
+        the strided quant slice's scale; stats: x carries producer GroupNorm partials; quant ("enc_out" only): None for the plain
+        quant slice, or an [n, 5, H, W] array the strided + scaled slice writes channels 1-4 of (the rest is kept).
+        -> dict: out [n, cout, Ho, Wo]; out16 (its fp16 hi + lo copy, "unet_in"); tap (the attention output before proj_out, or
+        the quant slice's output); out_norm (the next ResnetBlock's norm1 operand); trace ({"gn", "gemms", "conv", "softmax",
+        "cond_mod"})."""
+        sid, cin, cout = self.VAE_STAGES[stage]
+        x = f32(x)
+        n, c, H, W = x.shape
+        down = stage.startswith("enc_down")
+        Ho, Wo = (H // 2, W // 2) if down else (H, W)
+        out = np.empty((n, cout, Ho, Wo), np.float32)
+        out16 = np.zeros((n, cout, Ho, Wo), np.float32) if stage == "unet_in" else None
+        out_norm = np.zeros((n, cout, Ho, Wo), np.float32) if (down or stage.endswith("attn")) else None
+        tap = None
+        if stage.endswith("attn"):
+            tap = np.zeros((n, 512, H, W), np.float32)
+        elif stage == "enc_out":
+            tap = np.zeros((n, 4, H, W), np.float32) if quant is None else f32(quant).copy()
+            assert quant is None or tap.shape == (n, 5, H, W)
+        cnd = f32(cond) if cond is not None else None
+        t = np.zeros(256, np.int32)
+        p = lambda a: None if a is None else ptr(a)
+        flags = (1 if stats else 0) | (2 if quant is not None else 0)
+        self.check(self.lib.sdb_test_vae_stage(self.h, sid, ptr(x), p(cnd), n, c, H, W, float(scale), flags, ptr(out), p(out16),
+                                               p(tap), p(out_norm), t.ctypes.data_as(C.POINTER(C.c_int32))))
+        keys = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1", "passes")
+        gemms = []
+        for i in range(min(int(t[5]), 16)):
+            g = dict(zip(keys, (int(v) for v in t[6 + 12 * i:17 + 12 * i])))
+            g["epi"] = {r for b, r in enumerate(self._EPI_ROLES) if int(t[17 + 12 * i]) >> b & 1}
+            gemms.append(g)
+        tr = {"gn": [self._GN_PATHS.get(int(v), int(v)) for v in t[1:1 + min(int(t[0]), 4)]], "gemms": gemms,
+              "conv": [tuple(int(v) for v in t[201:204])] * int(t[200]), "softmax": [int(t[205])] * int(t[204]),
+              "cond_mod": int(t[206])}
+        return dict(out=out, out16=out16, tap=tap, out_norm=out_norm, trace=tr)
 
     def test_groupnorm(self, x, gamma, beta, silu=False):
         x = f32(x); n, c, H, W = x.shape

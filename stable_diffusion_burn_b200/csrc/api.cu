@@ -997,6 +997,15 @@ int sdb_test_spatial_transformer(sdb_ctx* ctx, int index, const float* x, int n,
   API_END
 }
 
+int sdb_test_vae_stage(sdb_ctx* ctx, int stage, const float* x, const float* cond, int n, int ch, int H, int W, float scale, int flags,
+                       float* out, float* out16, float* tap, float* out_norm, int32_t* trace) {
+  API_BEGIN(ctx)
+  need_final(c);
+  c.work.reset();
+  model_test_vae_stage(c, stage, x, cond, n, ch, H, W, scale, flags, out, out16, tap, out_norm, trace);
+  API_END
+}
+
 int sdb_test_step_noise(sdb_ctx* ctx, uint64_t noise_seed, int t, int64_t count, float* out) {
   API_BEGIN(ctx)
   SDB_CHECK(out && count >= 1, "step_noise: null output or count < 1");

@@ -914,9 +914,9 @@ conv3x3_small_cout_kernel(const float* __restrict__ x, int H, int W, int C, cons
     for (int o = 0; o < COUT; ++o) y[((size_t)n * COUT + o) * HW + (size_t)h * W + w] = acc[o] + b[o];
   }
 }
-void conv3x3_small_cout_launch(const float* x, int n, int H, int W, int C, const double* sums, const float* gamma,
-                               const float* beta, float eps, const float* w_packed, const float* b, int Cout,
-                               float* y_nchw, cudaStream_t st) {
+SmallCoutVariant conv3x3_small_cout_launch(const float* x, int n, int H, int W, int C, const double* sums, const float* gamma,
+                                           const float* beta, float eps, const float* w_packed, const float* b, int Cout,
+                                           float* y_nchw, cudaStream_t st) {
   SDB_CHECK(C % 16 == 0, "conv3x3_small_cout: channels must be a multiple of 16");
   // too few 8-row tiles to fill the machine -> 2-row tiles, 32 channels per round and group, the channel chunks split over
   // KS = 5 or 4 groups of two warps (10 / 8 warps per CTA; 320 = 10 x 32 and 512 = 16 x 32 channels)
@@ -954,6 +954,7 @@ void conv3x3_small_cout_launch(const float* x, int n, int H, int W, int C, const
 #undef SDB_SMALL_CONV
 #undef SDB_SMALL_KS
   SDB_CUDA(cudaGetLastError());
+  return {th, ck, ksplit};
 }
 
 // quant_conv (1x1, 8 -> 8) followed by the slice [0..4) of Autoencoder::encode_image (autoencoder/mod.rs:60-66): NCHW in/out
@@ -1674,15 +1675,17 @@ softmax_rows_kernel(const float* __restrict__ S, int cols, float scale_log2, __h
     if (i < cols) split_store1(v[k] * inv, hi, lo, row * cols + i);
   }
 }
-void softmax_rows_launch(const float* S, long long rows, int cols, float scale, Half2Ptr out, cudaStream_t st) {
+int softmax_rows_launch(const float* S, long long rows, int cols, float scale, Half2Ptr out, cudaStream_t st) {
   const float sl2 = scale * 1.4426950408889634f;
+  int per;
   if (cols <= 4096)
-    softmax_rows_kernel<16><<<(unsigned)rows, 256, 0, st>>>(S, cols, sl2, out.hi, out.lo);
-  else if (cols <= 9216)
-    softmax_rows_kernel<36><<<(unsigned)rows, 256, 0, st>>>(S, cols, sl2, out.hi, out.lo);
+    softmax_rows_kernel<16><<<(unsigned)rows, 256, 0, st>>>(S, cols, sl2, out.hi, out.lo), per = 16;
+  else if (cols <= kSoftmaxRowsMax)
+    softmax_rows_kernel<36><<<(unsigned)rows, 256, 0, st>>>(S, cols, sl2, out.hi, out.lo), per = 36;
   else
     throw Error("softmax_rows: row too long");
   SDB_CUDA(cudaGetLastError());
+  return per;
 }
 
 // ============================================================ synthetic weights

@@ -75,10 +75,13 @@ constexpr int kConvCinCondPix = 32;
 void conv3x3_cin_cond_launch(int cin, const float* x, long long x_stride, const float* cond, long long cond_stride, int cond_mod,
                              int n, int H, int W, const float* w, const float* b, int Cout, float* y, Half2Ptr y16, cudaStream_t st);
 // 3x3 pad 1, Cout <= 4, input NHWC fp32 with fused GroupNorm+SiLU; output NCHW fp32 [n,Cout,H,W];
-// weights repacked [Cout][9][C] fp32.
-void conv3x3_small_cout_launch(const float* x, int n, int H, int W, int C, const double* sums, const float* gamma,
-                               const float* beta, float eps, const float* w_packed, const float* b, int Cout,
-                               float* y_nchw, cudaStream_t st);
+// weights repacked [Cout][9][C] fp32. Returns the variant it launched: rows per CTA tile, channels per round, channel groups.
+struct SmallCoutVariant {
+  int th, ck, ks;
+};
+SmallCoutVariant conv3x3_small_cout_launch(const float* x, int n, int H, int W, int C, const double* sums, const float* gamma,
+                                           const float* beta, float eps, const float* w_packed, const float* b, int Cout,
+                                           float* y_nchw, cudaStream_t st);
 
 // ---- time embedding (reference unet/mod.rs:19-30, 115-118, 718-722)
 // emb = lin2(silu(lin1([cos|sin](t*f)))) ; then for every ResBlock r: e_r = lin_embed_r(silu(emb))
@@ -170,8 +173,10 @@ void randn_seeds_launch(float* x, int n, long long per, const uint64_t* seeds, c
 void stage_cfg_context_launch(const float* cond, int L, const float* uncond, long long ustride, const int* lens, int n, int Lpad,
                               float* out, cudaStream_t st, int groups = 2);
 
-// ---- row softmax for the 1-head VAE attention: P = softmax(S*scale) rows -> fp16 hi(/lo)
-void softmax_rows_launch(const float* S, long long rows, int cols, float scale, Half2Ptr out, cudaStream_t st);
+// ---- row softmax for the 1-head VAE attention: P = softmax(S*scale) rows -> fp16 hi(/lo); cols <= kSoftmaxRowsMax. Returns the
+// values per thread (PER) of the instance it launched.
+constexpr int kSoftmaxRowsMax = 9216;
+int softmax_rows_launch(const float* S, long long rows, int cols, float scale, Half2Ptr out, cudaStream_t st);
 
 // ---- weight packing (master fp32 -> kernel layouts)
 // conv OIHW [Cout][Cin][k][k] -> [Cout][k*k*Cin] with K index = tap*Cin + c ; fp16 hi (+lo)

@@ -633,6 +633,7 @@ struct Fwd {
       const int nbk = x.C / x.gn.bucket;
       const float* part = x.gn.buf;
       int cap = x.gn.cap, slots = x.gn.slots;
+      if (c.trace_on) c.gn_trace.push_back(slots > 128 ? GN_PATH_SUMS_FOLD : GN_PATH_SUMS_PARTIALS);
       if (slots > 128) {
         const int s2 = gn_fold_slots(slots);
         float* folded = c.work.get<float>((size_t)nb * s2 * nbk * 2);
@@ -644,6 +645,7 @@ struct Fwd {
       gn_sums_from_partials_launch(part, cap, slots, nbk, x.C, x.gn.bucket, nb, sums, c.stream);
       return sums;
     }
+    if (c.trace_on) c.gn_trace.push_back(GN_PATH_SUMS_STATS);
     float* part = c.work.get<float>(gn_stats_partial_floats(nb, HW));
     KernelScope ks(c, KC_GN_STATS, 0, (double)nb * HW * x.C * 4.0);
     gn_stats_launch(x.p, x.C, nullptr, 0, nb, HW, sums, part, tk, c.stream);
@@ -961,6 +963,45 @@ struct UNetIO {
   int cond_mod = 1;
 };
 
+// The conditioned UNets' extra input channels (unet_pass): a 9-channel UNet reads d_x [nb,4,H,W] and d_cond [nb/2,5,H,W] (both
+// CFG halves of a step share it), an 8-channel one d_x [nb,4,H,W] and d_cond [nb,4,H,W] (each guidance group has its own); with
+// d_cond null either reads d_x [nb,cin,H,W].
+static void unet_cond_io(const Ctx& c, int nb, const float* d_x, const float* d_cond, UNetIO& io) {
+  const long long hw = (long long)io.H * io.W;
+  const int cin = c.unet_cin;
+  if (cin != 4) {
+    if (d_cond)
+      io.x_stride = 4 * hw, io.cond = d_cond, io.cond_stride = (cin - 4) * hw, io.cond_mod = cin == 9 ? nb / 2 : nb;
+    else
+      io.x_stride = cin * hw, io.cond = d_x + 4 * hw, io.cond_stride = cin * hw, io.cond_mod = nb;
+  }
+}
+
+// conv_in (unet/mod.rs:124-127, first input block): 3x3 Cin 4 / 8 / 9 -> 320 on CUDA cores, with the fp16 copy the first
+// ResBlock's skip reads
+static void unet_conv_in(Fwd& f, const UNetBlockW& b, const UNetIO& io, const Act& o) {
+  Ctx& c = f.c;
+  KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * io.H * io.W * 9.0 * b.cin * b.cout);
+  if (b.cin != 4)
+    conv3x3_cin_cond_launch(b.cin, io.x, io.x_stride, io.cond, io.cond_stride, io.cond_mod, f.nb, io.H, io.W, mptr(c, b.conv.wi),
+                            b.conv.bias, b.cout, o.p, o.raw16, c.stream);
+  else
+    conv3x3_cin4_launch(io.x, f.nb, io.H, io.W, mptr(c, b.conv.wi), b.conv.bias, b.cout, nullptr, nullptr, 1.f, o.p, o.raw16,
+                        c.stream);
+}
+
+// GroupNorm + SiLU + 3x3 conv to cout <= 8 channels, fused, fp32 on CUDA cores, NCHW result y [nb,cout,H,W]: the UNet's out
+// (unet/mod.rs:138-140, 320 -> 4), the decoder's norm_out + conv_out (autoencoder/mod.rs:215-216, 128 -> 3) and the encoder's
+// (512 -> 8)
+static void norm_conv_out(Fwd& f, const Act& x, const NormW& norm, const ConvW& conv, int cout, float* y) {
+  Ctx& c = f.c;
+  double* sums = f.stats(x);
+  KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * x.H * x.W * 9.0 * x.C * cout);
+  const SmallCoutVariant v = conv3x3_small_cout_launch(x.p, f.nb, x.H, x.W, x.C, sums, norm.gamma, norm.beta, norm.eps,
+                                                       conv.w_small, conv.bias, cout, y, c.stream);
+  if (c.trace_on) c.conv_trace.insert(c.conv_trace.end(), {v.th, v.ck, v.ks});
+}
+
 static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
   Ctx& c = f.c;
   Model& m = f.m;
@@ -997,17 +1038,10 @@ static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
   auto do_block = [&](UNetBlockW& b, const Act& x0, const Act* x1) -> Act {
     Act o;
     switch (b.kind) {
-      case BK_CONV: {
+      case BK_CONV:
         o = f.act16(H, W, b.cout);
-        KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * H * W * 9.0 * b.cin * b.cout);
-        if (b.cin != 4)
-          conv3x3_cin_cond_launch(b.cin, io.x, io.x_stride, io.cond, io.cond_stride, io.cond_mod, f.nb, H, W, mptr(c, b.conv.wi),
-                                  b.conv.bias, b.cout, o.p, o.raw16, c.stream);
-        else
-          conv3x3_cin4_launch(io.x, f.nb, H, W, mptr(c, b.conv.wi), b.conv.bias, b.cout, nullptr, nullptr, 1.f, o.p, o.raw16,
-                              c.stream);
+        unet_conv_in(f, b, io, o);
         break;
-      }
       case BK_DOWN: {  // unet/mod.rs:412-427: 3x3 stride 2 pad 1
         o = f.act16(H / 2, W / 2, b.cout);
         const size_t mk = c.work.off;
@@ -1076,13 +1110,8 @@ static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
     saved.pop_back();
     x = do_block(b, x, &skip);
   }
-  // out: GroupNorm + SiLU + conv 320 -> 4 (:138-140), fused, fp32 on CUDA cores, NCHW result
-  {
-    double* sums = f.stats(x);
-    KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * H * W * 9.0 * 320 * 4);
-    conv3x3_small_cout_launch(x.p, f.nb, H, W, 320, sums, m.norm_out.gamma, m.norm_out.beta, m.norm_out.eps, m.conv_out.w_small,
-                              m.conv_out.bias, 4, io.out, c.stream);
-  }
+  // out: GroupNorm + SiLU + conv 320 -> 4 (:138-140)
+  norm_conv_out(f, x, m.norm_out, m.conv_out, 4, io.out);
   c.work.off = mark0;
 }
 
@@ -1094,7 +1123,9 @@ static void run_resnet(Fwd& f, ResnetW& r, const Act& x, Act& out) {
 
 // reference autoencoder/mod.rs:562-608: 1 head, d = C = 512, N = H*W tokens. S is materialised per image
 // (64 MB at 64x64) because the op runs once per image; q/k/v/proj are the same wgmma GEMMs.
-static void run_vae_attention(Fwd& f, VaeAttnW& a, const Act& x, Act& out) {
+// o_tap (sdb_test_vae_stage): caller-allocated hi + lo storage [nb*HW][C] that receives the attention output before proj_out; its lo
+// is cleared when the policy keeps no lo half
+static void run_vae_attention(Fwd& f, VaeAttnW& a, const Act& x, Act& out, Half2Ptr* o_tap = nullptr) {
   Ctx& c = f.c;
   const size_t mark = c.work.off;
   const int P = a.passes;
@@ -1104,7 +1135,13 @@ static void run_vae_attention(Fwd& f, VaeAttnW& a, const Act& x, Act& out) {
   ActOp h = f.gn_operand(x, nullptr, a.norm, false, lo);
   const int Mp = round_up((int)Mt, 32);
   Half2Ptr q16 = f.half2((size_t)Mt * C, lo), k16 = f.half2((size_t)Mt * C, lo), vT = f.half2((size_t)C * Mp, lo);
-  Half2Ptr o16 = f.half2((size_t)Mt * C, lo);
+  Half2Ptr o16;
+  if (o_tap) {
+    if (!lo) o_tap->lo = nullptr;
+    o16 = *o_tap;
+  } else {
+    o16 = f.half2((size_t)Mt * C, lo);
+  }
   {
     Epilogue ep;
     ep.out_f16 = q16, ep.bias = a.q.bias;
@@ -1138,7 +1175,8 @@ static void run_vae_attention(Fwd& f, VaeAttnW& a, const Act& x, Act& out) {
     }
     {
       KernelScope ks(c, KC_ELEMENTWISE, 0, (double)HW * HW * 6.0);
-      softmax_rows_launch(S, HW, HW, scale, p16, c.stream);
+      const int per = softmax_rows_launch(S, HW, HW, scale, p16, c.stream);
+      if (c.trace_on) c.softmax_trace.push_back(per);
     }
     WeightOp vs;
     vs.p.hi = vT.hi + (size_t)s * HW, vs.p.lo = vT.lo ? vT.lo + (size_t)s * HW : nullptr;
@@ -1156,6 +1194,16 @@ static void run_vae_attention(Fwd& f, VaeAttnW& a, const Act& x, Act& out) {
   c.work.off = mark;
 }
 
+// decoder conv_in 4 -> 512 with post_quant_conv (1x1, 4->4) and the latent's pre-scale folded into its input gather
+// (autoencoder/mod.rs:68-71, 205): latent [nb,4,H,W] NCHW -> x
+static void vae_dec_conv_in(Fwd& f, const float* d_latent, float pre_scale, const Act& x) {
+  Ctx& c = f.c;
+  Model& m = f.m;
+  KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * x.H * x.W * 36.0 * 512);
+  conv3x3_cin4_launch(d_latent, f.nb, x.H, x.W, mptr(c, m.vae_conv_in.wi), m.vae_conv_in.bias, 512, mptr(c, m.post_quant.wi),
+                      m.post_quant.bias, pre_scale, x.p, Half2Ptr{}, c.stream);
+}
+
 // latent [nb,4,H,W] NCHW (already divided by 0.18215 when called from latent_to_image) -> img [nb,3,8H,8W] NCHW
 static void vae_decode(Fwd& f, const float* d_latent, int H, int W, float pre_scale, float* d_img) {
   Ctx& c = f.c;
@@ -1163,13 +1211,8 @@ static void vae_decode(Fwd& f, const float* d_latent, int H, int W, float pre_sc
   const size_t mark0 = c.work.off;
   f.gn_slot = 0;
   f.init_sums(40);
-  // post_quant_conv (1x1, 4->4) folded into conv_in's input gather (autoencoder/mod.rs:68-71, 205)
   Act x = f.act(H, W, 512);
-  {
-    KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * H * W * 36.0 * 512);
-    conv3x3_cin4_launch(d_latent, f.nb, H, W, mptr(c, m.vae_conv_in.wi), m.vae_conv_in.bias, 512, mptr(c, m.post_quant.wi),
-                        m.post_quant.bias, pre_scale, x.p, Half2Ptr{}, c.stream);
-  }
+  vae_dec_conv_in(f, d_latent, pre_scale, x);
   // Mid (autoencoder/mod.rs:456-463)
   {
     Act a = f.act(H, W, 512), b = f.act(H, W, 512), d = f.act(H, W, 512);
@@ -1201,12 +1244,7 @@ static void vae_decode(Fwd& f, const float* d_latent, int H, int W, float pre_sc
     }
   }
   // norm_out + SiLU + conv_out 128 -> 3 (autoencoder/mod.rs:215-216)
-  {
-    double* sums = f.stats(x);
-    KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * H * W * 9.0 * 128 * 3);
-    conv3x3_small_cout_launch(x.p, f.nb, H, W, 128, sums, m.vae_norm_out.gamma, m.vae_norm_out.beta, m.vae_norm_out.eps,
-                              m.vae_conv_out.w_small, m.vae_conv_out.bias, 3, d_img, c.stream);
-  }
+  norm_conv_out(f, x, m.vae_norm_out, m.vae_conv_out, 3, d_img);
   c.work.off = mark0;
 }
 
@@ -1214,6 +1252,39 @@ static void vae_decode(Fwd& f, const float* d_latent, int H, int W, float pre_sc
 // Autoencoder::encode_image (autoencoder/mod.rs:60-66): Encoder::forward (:133-145) -> quant_conv -> channels [0,4).
 // d_img4: the image with a zero fourth plane [nb][4][H][W]; d_latent [nb][4][H/8][W/8], or with out_stride > 0 sample i at
 // d_latent + i * out_stride, scaled by out_scale (the inpainting conditioning tensor).
+// conv_in 3 -> 128 (:138) on the Cin = 4 kernel: d_img4 [nb,4,H,W] with weights padded by a zero fourth input channel
+static void vae_enc_conv_in(Fwd& f, const float* d_img4, const Act& x) {
+  Ctx& c = f.c;
+  EncoderW& e = f.m.enc;
+  KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * x.H * x.W * 27.0 * 128);
+  conv3x3_cin4_launch(d_img4, f.nb, x.H, x.W, e.conv_in_w4, e.conv_in.bias, 128, nullptr, nullptr, 1.f, x.p, Half2Ptr{}, c.stream);
+}
+
+// an EncoderBlock's downsampler (:255-265): 3x3 stride 2, padded bottom/right only, with the GroupNorm partials the next
+// ResnetBlock's norm1 reads. x [nb,H,W,C] -> o [nb,H/2,W/2,C] (o allocated by the caller)
+static void vae_enc_down(Fwd& f, const ConvW& down, const Act& x, Act& o) {
+  Ctx& c = f.c;
+  SDB_CHECK(x.H % 2 == 0 && x.W % 2 == 0, "encode_image: image height and width must be multiples of 8");
+  const size_t mk = c.work.off;
+  ActOp a = f.raw_operand(x, nullptr, PREP_PHASE2, true);
+  Epilogue ep;
+  ep.out_f32 = o.p, ep.bias = down.bias, ep.gn = &o.gn;
+  run_gemm(c, G_CONV3_S2_PAD01, a, nullptr, down.packed, down.passes, ep);
+  c.work.off = mk;
+}
+
+// quant_conv 8 -> 8 and the slice [0,4) (:60-66): y8 [nb,8,HW] -> d_latent [nb,4,HW], or with out_stride > 0 sample i at
+// d_latent + i * out_stride, scaled by out_scale
+static void vae_enc_quant(Fwd& f, const float* y8, int HW, float* d_latent, long long out_stride, float out_scale) {
+  Ctx& c = f.c;
+  EncoderW& e = f.m.enc;
+  KernelScope ks(c, KC_ELEMENTWISE);
+  if (out_stride)
+    quant_conv_slice_scaled_launch(y8, mptr(c, e.quant.wi), e.quant.bias, f.nb, HW, out_stride, out_scale, d_latent, c.stream);
+  else
+    quant_conv_slice_launch(y8, mptr(c, e.quant.wi), e.quant.bias, f.nb, HW, d_latent, c.stream);
+}
+
 static void vae_encode(Fwd& f, const float* d_img4, int H, int W, float* d_latent, long long out_stride = 0, float out_scale = 1.f) {
   Ctx& c = f.c;
   EncoderW& e = f.m.enc;
@@ -1221,10 +1292,7 @@ static void vae_encode(Fwd& f, const float* d_img4, int H, int W, float* d_laten
   f.gn_slot = 0;
   f.init_sums(40);
   Act x = f.act(H, W, 128);
-  {
-    KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * H * W * 27.0 * 128);
-    conv3x3_cin4_launch(d_img4, f.nb, H, W, e.conv_in_w4, e.conv_in.bias, 128, nullptr, nullptr, 1.f, x.p, Half2Ptr{}, c.stream);
-  }
+  vae_enc_conv_in(f, d_img4, x);
   // EncoderBlocks (:255-265): two ResnetBlocks, then the stride-2 conv padded bottom/right only
   for (int i = 0; i < 4; ++i) {
     EncoderBlockW& eb = e.blocks[i];
@@ -1236,12 +1304,7 @@ static void vae_encode(Fwd& f, const float* d_img4, int H, int W, float* d_laten
     if (eb.has_down) {
       SDB_CHECK(H % 2 == 0 && W % 2 == 0, "encode_image: image height and width must be multiples of 8");
       Act o = f.act(H / 2, W / 2, eb.down.cout);
-      const size_t mk = c.work.off;
-      ActOp a = f.raw_operand(x, nullptr, PREP_PHASE2, true);
-      Epilogue ep;
-      ep.out_f32 = o.p, ep.bias = eb.down.bias, ep.gn = &o.gn;
-      run_gemm(c, G_CONV3_S2_PAD01, a, nullptr, eb.down.packed, eb.down.passes, ep);
-      c.work.off = mk;
+      vae_enc_down(f, eb.down, x, o);
       x = o;
       H /= 2, W /= 2;
     }
@@ -1256,19 +1319,8 @@ static void vae_encode(Fwd& f, const float* d_img4, int H, int W, float* d_laten
   }
   // norm_out + SiLU + conv_out 512 -> 8 (fp32 CUDA cores, NCHW), then quant_conv 8 -> 8 and the slice [0,4)
   float* y8 = c.work.get<float>((size_t)f.nb * 8 * H * W);
-  {
-    double* sums = f.stats(x);
-    KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * H * W * 9.0 * 512 * 8);
-    conv3x3_small_cout_launch(x.p, f.nb, H, W, 512, sums, e.norm_out.gamma, e.norm_out.beta, e.norm_out.eps, e.conv_out.w_small,
-                              e.conv_out.bias, 8, y8, c.stream);
-  }
-  {
-    KernelScope ks(c, KC_ELEMENTWISE);
-    if (out_stride)
-      quant_conv_slice_scaled_launch(y8, mptr(c, e.quant.wi), e.quant.bias, f.nb, H * W, out_stride, out_scale, d_latent, c.stream);
-    else
-      quant_conv_slice_launch(y8, mptr(c, e.quant.wi), e.quant.bias, f.nb, H * W, d_latent, c.stream);
-  }
+  norm_conv_out(f, x, e.norm_out, e.conv_out, 8, y8);
+  vae_enc_quant(f, y8, H * W, d_latent, out_stride, out_scale);
   c.work.off = mark0;
 }
 
@@ -1295,9 +1347,7 @@ struct StreamJoin {  // run on c.stream ordered after / before the caller's stre
 };
 }  // namespace
 
-// UNet pass over nb samples with per-sample context lengths. d_ctx_padded [nb][Lpad][768].
-// A 9-channel UNet reads d_x [nb,4,H,W] and d_cond [nb/2,5,H,W] (both CFG halves of a step share it), an 8-channel one d_x
-// [nb,4,H,W] and d_cond [nb,4,H,W] (each guidance group has its own); with d_cond null either reads d_x [nb,cin,H,W].
+// UNet pass over nb samples with per-sample context lengths. d_ctx_padded [nb][Lpad][768]. d_x / d_cond: see unet_cond_io.
 static void unet_pass(Ctx& c, int nb, const float* d_x, const int* d_t, const float* d_ctx_padded, int Lpad, int* d_kvlen,
                       int H, int W, float* d_out, const CtxState* shared_cs, const float* emb_all = nullptr,
                       const float* d_cond = nullptr) {
@@ -1311,14 +1361,7 @@ static void unet_pass(Ctx& c, int nb, const float* d_x, const int* d_t, const fl
   }
   UNetIO io{d_x, d_t, d_out, H, W};
   io.emb_all = emb_all;
-  const long long hw = (long long)H * W;
-  const int cin = c.unet_cin;
-  if (cin != 4) {
-    if (d_cond)
-      io.x_stride = 4 * hw, io.cond = d_cond, io.cond_stride = (cin - 4) * hw, io.cond_mod = cin == 9 ? nb / 2 : nb;
-    else
-      io.x_stride = cin * hw, io.cond = d_x + 4 * hw, io.cond_stride = cin * hw, io.cond_mod = nb;
-  }
+  unet_cond_io(c, nb, d_x, d_cond, io);
   unet_forward(f, io, *cs);
   c.work.off = mark;
 }
@@ -1357,6 +1400,22 @@ void model_unet_forward_host(Ctx& c, const float* x, int t, const float* context
   SDB_CUDA(cudaStreamSynchronize(c.stream));
 }
 
+// The autoencoder's mid attention (run_vae_attention) takes the latent's H * W positions as one row of S and of P: the row
+// softmax holds at most kSoftmaxRowsMax = 9216 = 96 x 96 of them (a 768 x 768 px image); the S GEMM has N = HW (a multiple of 32)
+// and the P.V GEMM reads P [HW][HW] as an operand of HW channels (a multiple of 64). Every entry that decodes or encodes refuses
+// other latents here, before it launches anything.
+static void check_vae_latent(int H, int W, const std::string& what) {
+  char msg[320];
+  snprintf(msg, sizeof(msg), "%s: unsupported latent size %dx%d: the autoencoder's attention needs H*W a multiple of 64",
+           what.c_str(), H, W);
+  SDB_CHECK(H >= 1 && W >= 1 && ((long long)H * W) % 64 == 0, msg);
+  snprintf(msg, sizeof(msg),
+           "%s: a %dx%d latent (%dx%d px) is too large for the autoencoder's attention, which takes at most %d latent positions "
+           "(H*W): the largest supported image is 768x768 px (a 96x96 latent)",
+           what.c_str(), H, W, 8 * H, 8 * W, kSoftmaxRowsMax);
+  SDB_CHECK((long long)H * W <= kSoftmaxRowsMax, msg);
+}
+
 static void decode_chunked(Ctx& c, const float* d_latent, int n, int H, int W, float pre_scale, float* d_img) {
   // bounded working set: at most 4 images of 128-channel 8Hx8W activations at a time
   const int chunk = 4;
@@ -1368,6 +1427,7 @@ static void decode_chunked(Ctx& c, const float* d_latent, int n, int H, int W, f
 }
 
 void model_decode_dev(Ctx& c, const float* d_latent, int n, int H, int W, float* d_img, cudaStream_t caller) {
+  check_vae_latent(H, W, "decode_latent");
   StreamJoin join(c, caller);
   c.work.reset();
   decode_chunked(c, d_latent, n, H, W, 1.0f, d_img);
@@ -1386,6 +1446,7 @@ void model_decode_host(Ctx& c, const float* latent, int n, int H, int W, float* 
 void model_encode_dev(Ctx& c, const float* d_img, int n, int H, int W, float* d_latent, cudaStream_t caller) {
   SDB_CHECK(n >= 1 && H >= 64 && W >= 64 && H % 8 == 0 && W % 8 == 0 && ((H / 8) * (W / 8)) % 8 == 0,
             "encode_image: height and width must be multiples of 8, at least 64, with (H/8)*(W/8) a multiple of 8");
+  check_vae_latent(H / 8, W / 8, "encode_image");
   StreamJoin join(c, caller);
   c.work.reset();
   const size_t plane = (size_t)H * W;
@@ -1414,6 +1475,7 @@ void model_encode_host(Ctx& c, const float* img, int n, int H, int W, float* lat
 
 // latent_to_image (stablediffusion/mod.rs:69-100)
 static void latent_to_image_dev(Ctx& c, const float* d_latent, int n, int H, int W, uint8_t* d_rgb) {
+  check_vae_latent(H, W, "latent_to_image");
   float* d_img = c.work.get<float>((size_t)n * 3 * 64 * H * W);
   // `latent * (1.0 / 0.18215)`: the scalar is rounded to f32 before the multiply, as burn's mul_scalar does
   decode_chunked(c, d_latent, n, H, W, (float)(1.0 / 0.18215), d_img);
@@ -1507,6 +1569,8 @@ static int check_request(const Ctx& c, const SampleRequest& r, bool host) {
   SDB_CHECK(r.H % 8 == 0 && r.W % 8 == 0, "latent size must be a multiple of 8");
   SDB_CHECK(((r.H / 8) * (r.W / 8)) % 8 == 0, "unsupported latent size: (H/8)*(W/8) must be a multiple of 8");
   const std::string what = img2img ? "img2img" : (edit ? "edit_image" : (b ? "sample_batch" : "sample"));
+  // the autoencoder runs when the request encodes an image or asks for RGB: refuse a latent it cannot take before any UNet step
+  if (!txt2img || r.rgb) check_vae_latent(r.H, r.W, what);
   if (!txt2img) {
     SDB_CHECK(r.image && (b ? b->context : r.context) && (b ? b->uncond : r.uncond), what + ": null image, context or uncond");
     SDB_CHECK(edit || r.mask || c.unet_cin == 4,
@@ -2155,7 +2219,10 @@ void model_test_attention(Ctx& c, const float* q, const float* k, const float* v
 namespace {
 struct TraceScope {  // records the GEMM choices and GroupNorm paths of everything queued while it lives
   Ctx& c;
-  explicit TraceScope(Ctx& c_) : c(c_) { c.gemm_trace.clear(), c.attn_trace.clear(), c.gn_trace.clear(), c.trace_on = true; }
+  explicit TraceScope(Ctx& c_) : c(c_) {
+    c.gemm_trace.clear(), c.attn_trace.clear(), c.gn_trace.clear(), c.conv_trace.clear(), c.softmax_trace.clear();
+    c.trace_on = true;
+  }
   ~TraceScope() { c.trace_on = false; }
 };
 }  // namespace
@@ -2390,6 +2457,132 @@ void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, in
       taps_ln[(i * Mt + r) * 2] = sm, taps_ln[(i * Mt + r) * 2 + 1] = sq;
     }
   }
+}
+
+// ================================================================================ autoencoder stage test entry
+// NCHW host output of an NHWC fp32 activation
+static void fetch_act(Ctx& c, const Act& a, float* out) {
+  float* d = c.work.get<float>(a.count());
+  nhwc_to_nchw_launch(a.p, a.n, a.C, a.H, a.W, d, c.stream);
+  SDB_CUDA(cudaMemcpyAsync(out, d, a.count() * 4, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, int n, int Cx, int H, int W, float scale, int flags,
+                          float* out, float* out16, float* tap, float* out_norm, int32_t* trace) {
+  Model& m = M(c);
+  EncoderW& e = m.enc;
+  SDB_CHECK(stage >= SDB_VAE_DEC_IN && stage <= SDB_VAE_ENC_DOWN2, "test_vae_stage: stage is one of SDB_VAE_*");
+  SDB_CHECK(n >= 1 && H >= 1 && W >= 1 && x && out && trace, "test_vae_stage: arguments");
+  SDB_CHECK((flags & ~3) == 0 && (!(flags & 2) || stage == SDB_VAE_ENC_OUT),
+            "test_vae_stage: flags are 1 (x with producer GroupNorm partials) | 2 (SDB_VAE_ENC_OUT: strided, scaled quant slice)");
+  const bool attn = stage == SDB_VAE_DEC_ATTN || stage == SDB_VAE_ENC_ATTN;
+  const bool down = stage >= SDB_VAE_ENC_DOWN0;
+  const int di = stage - SDB_VAE_ENC_DOWN0;
+  int cin = 4, cout = 0;
+  switch (stage) {
+    case SDB_VAE_DEC_IN: cout = 512; break;
+    case SDB_VAE_DEC_ATTN: case SDB_VAE_ENC_ATTN: cin = cout = 512; break;
+    case SDB_VAE_DEC_OUT: cin = 128, cout = 3; break;
+    case SDB_VAE_UNET_OUT: cin = 320, cout = 4; break;
+    case SDB_VAE_ENC_OUT: cin = 512, cout = 8; break;
+    case SDB_VAE_ENC_IN: cout = 128; break;
+    case SDB_VAE_UNET_IN: cout = 320; break;
+    default: cin = cout = e.blocks[di].down.cout; break;
+  }
+  SDB_CHECK(Cx == cin, "test_vae_stage: x must have " + std::to_string(cin) + " channels for this stage");
+  if (attn) check_vae_latent(H, W, "test_vae_stage");
+  if (down) SDB_CHECK(H % 2 == 0 && W % 2 == 0, "test_vae_stage: the downsampler needs even H and W");
+  const bool cond_ctx = stage == SDB_VAE_UNET_IN && c.unet_cin != 4;
+  SDB_CHECK(cond_ctx == (cond != nullptr), "test_vae_stage: cond [n][cin-4][H][W] is given exactly for SDB_VAE_UNET_IN on a 9- or "
+                                           "8-channel context");
+  SDB_CHECK(!cond_ctx || c.unet_cin != 9 || n % 2 == 0, "test_vae_stage: a 9-channel conv_in runs on the two CFG halves: n even");
+  SDB_CHECK(stage != SDB_VAE_ENC_OUT || tap, "test_vae_stage: SDB_VAE_ENC_OUT needs tap for the quant slice");
+  const int HW = H * W;
+  Fwd f(c, n);
+  f.init_sums(4);
+  float* d_x = (cin == 4) ? upload(c, x, (size_t)n * 4 * HW) : nullptr;
+  const float* d_cond = cond_ctx ? upload(c, cond, (size_t)n * (c.unet_cin - 4) * HW) : nullptr;
+  Act a;
+  if (cin != 4) a = stage_activation(f, x, cin, H, W, flags & 1);
+  // the UNet's conv_in output carries the fp16 copy the first ResBlock's skip reads
+  Act o = stage == SDB_VAE_UNET_IN ? f.act16(H, W, cout) : f.act(down ? H / 2 : H, down ? W / 2 : W, cout);
+  Half2Ptr otap;
+  float* y = nullptr;   // NCHW outputs of the small-Cout conv and the quant slice
+  float* q = nullptr;
+  const size_t qcount = (size_t)n * ((flags & 2) ? 5 : 4) * HW;
+  ActOp g;
+  int cond_mod = 0;
+  std::fill(trace, trace + kVaeTraceInts, 0);
+  {
+    TraceScope ts(c);
+    switch (stage) {
+      case SDB_VAE_DEC_IN:
+        vae_dec_conv_in(f, d_x, scale, o);
+        break;
+      case SDB_VAE_DEC_ATTN:
+      case SDB_VAE_ENC_ATTN: {
+        otap = f.half2((size_t)n * HW * 512, true);
+        const bool dec = stage == SDB_VAE_DEC_ATTN;
+        run_vae_attention(f, dec ? m.mid_attn : e.mid_attn, a, o, &otap);
+        g = f.gn_operand(o, nullptr, dec ? m.mid_block2.norm1 : e.mid_block2.norm1, true, true);  // the next ResnetBlock's norm1
+        break;
+      }
+      case SDB_VAE_DEC_OUT:
+      case SDB_VAE_UNET_OUT:
+      case SDB_VAE_ENC_OUT:
+        y = c.work.get<float>((size_t)n * cout * HW);
+        if (stage == SDB_VAE_DEC_OUT) norm_conv_out(f, a, m.vae_norm_out, m.vae_conv_out, 3, y);
+        if (stage == SDB_VAE_UNET_OUT) norm_conv_out(f, a, m.norm_out, m.conv_out, 4, y);
+        if (stage == SDB_VAE_ENC_OUT) {
+          norm_conv_out(f, a, e.norm_out, e.conv_out, 8, y);
+          // strided + scaled: as encode_images writes the masked-image latent into channels 1-4 of the inpainting tensor [n,5,H,W]
+          q = upload(c, tap, qcount);
+          if (flags & 2)
+            vae_enc_quant(f, y, HW, q + HW, 5ll * HW, scale);
+          else
+            vae_enc_quant(f, y, HW, q, 0, 1.f);
+        }
+        break;
+      case SDB_VAE_ENC_IN:
+        vae_enc_conv_in(f, d_x, o);
+        break;
+      case SDB_VAE_UNET_IN: {
+        UNetIO io{d_x, nullptr, nullptr, H, W};
+        unet_cond_io(c, n, d_x, d_cond, io);
+        cond_mod = io.cond ? io.cond_mod : 0;
+        unet_conv_in(f, m.in_blocks[0], io, o);
+        break;
+      }
+      default:
+        vae_enc_down(f, e.blocks[di].down, a, o);
+        g = f.gn_operand(o, nullptr, e.blocks[di + 1].res[0].norm1, true, true);  // the next block's first ResnetBlock
+        break;
+    }
+    trace[0] = (int)c.gn_trace.size();
+    for (size_t i = 0; i < c.gn_trace.size() && i < 4; ++i) trace[1 + i] = c.gn_trace[i];
+    trace[5] = (int)c.gemm_trace.size();
+    for (size_t i = 0; i < c.gemm_trace.size() && i < 16; ++i) {
+      const Ctx::GemmRecord& r = c.gemm_trace[i];
+      const int v[12] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels, r.passes, r.epi};
+      std::copy(v, v + 12, trace + 6 + 12 * i);
+    }
+    trace[200] = (int)c.conv_trace.size() / 3;
+    std::copy(c.conv_trace.begin(), c.conv_trace.begin() + std::min<size_t>(c.conv_trace.size(), 3), trace + 201);
+    trace[204] = (int)c.softmax_trace.size();
+    if (!c.softmax_trace.empty()) trace[205] = c.softmax_trace.back();
+    trace[206] = cond_mod;
+  }
+  if (y) {
+    SDB_CUDA(cudaMemcpyAsync(out, y, (size_t)n * cout * HW * 4, cudaMemcpyDeviceToHost, c.stream));
+    if (q) SDB_CUDA(cudaMemcpyAsync(tap, q, qcount * 4, cudaMemcpyDeviceToHost, c.stream));
+    SDB_CUDA(cudaStreamSynchronize(c.stream));
+    return;
+  }
+  fetch_act(c, o, out);
+  if (out16) fetch_half2(c, o.raw16, n, cout, o.H, o.W, out16);
+  if (tap && attn) fetch_half2(c, otap, n, 512, H, W, tap);
+  if (out_norm && g.p.hi) fetch_half2(c, g.p, n, cout, o.H, o.W, out_norm);
 }
 
 }  // namespace sdb

@@ -81,5 +81,9 @@ constexpr int kStTraceInts = 160;
 void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, int C, int H, int W, const float* context, int Lmax,
                                     const int32_t* lens, int flags, float* out, float* out16, float* out_norm, float* taps_y,
                                     float* taps_ln, int32_t* trace);
+// autoencoder stage test entry (sdb200.h: sdb_test_vae_stage); trace = kVaeTraceInts ints
+constexpr int kVaeTraceInts = 256;
+void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, int n, int C, int H, int W, float scale, int flags,
+                          float* out, float* out16, float* tap, float* out_norm, int32_t* trace);
 
 }  // namespace sdb

@@ -37,8 +37,16 @@ struct TensorInfo {
 };
 
 // which GroupNorm kernel staged an operand: statistics and apply in one launch, apply from producer partials, or apply after
-// the 64:1 pre-fold of more than 128 partial slots
-enum GnPath : int { GN_PATH_FUSED = 1, GN_PATH_APPLY = 2, GN_PATH_APPLY_FOLD = 3 };
+// the 64:1 pre-fold of more than 128 partial slots; and where the fused GroupNorm + small-Cout convs got their [n][32][2] sums
+// (Fwd::stats): the statistics kernel over the tensor, the producer's partials, or those partials after the pre-fold
+enum GnPath : int {
+  GN_PATH_FUSED = 1,
+  GN_PATH_APPLY = 2,
+  GN_PATH_APPLY_FOLD = 3,
+  GN_PATH_SUMS_STATS = 4,
+  GN_PATH_SUMS_PARTIALS = 5,
+  GN_PATH_SUMS_FOLD = 6
+};
 // epilogue roles of a recorded GEMM (Ctx::GemmRecord::epi): LayerNorm statistics out, LayerNorm-consuming correction, GEGLU,
 // fp16-pair residual, fp32 residual, GroupNorm partials out
 enum EpiRole : int { EPI_ROLE_LNS = 1, EPI_ROLE_LNC = 2, EPI_ROLE_GEGLU = 4, EPI_ROLE_RES16 = 8, EPI_ROLE_RES32 = 16, EPI_ROLE_GN = 32 };
@@ -197,6 +205,8 @@ struct Ctx {
   std::vector<GemmRecord> gemm_trace;
   std::vector<AttnRecord> attn_trace;
   std::vector<int> gn_trace;  // GN_PATH_*
+  std::vector<int> conv_trace;     // fused GroupNorm + small-Cout convs: TH, CK, KS of each launch (sdb_test_vae_stage)
+  std::vector<int> softmax_trace;  // VAE attention row softmax: PER of each launch
 
   float* master_ptr(const std::string& name);
   const TensorInfo& info(const std::string& name);
