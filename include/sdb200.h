@@ -399,6 +399,16 @@ enum {
 };
 int sdb_test_vae_stage(sdb_ctx* ctx, int stage, const float* x, const float* cond, int n, int c, int H, int W, float scale,
                        int flags, float* out, float* out16, float* tap, float* out_norm, int32_t* trace);
+/* One block of the CLIP text encoder (clip/mod.rs:109-115), index 0..11, or with index 12 its final LayerNorm, run on the weights
+ * sdb_finalize_weights packed with the encoder's own launch code. Needs finalized weights. x [n][L][768] (1 <= L <= 77) is the
+ * residual stream entering the block, staged at the encoder's per-sample row pitch round_up(L, 8) as the embedding leaves it;
+ * flags: 1 = the pad rows hold large finite junk instead of zeros. out [n][L][768] = the block output (index 12: the final
+ * LayerNorm). taps (NULL, or unused for index 12) = 11 planes of [n][L][768] floats: LN1 (fp16 hi + lo), q, k (fp16), V (read
+ * back from V^T, fp16), the attention output (hi + lo), x after the attention, LN2 (hi + lo), then QuickGELU(fc1) (hi + lo) as
+ * [n][L][3072]. trace (80 ints): [0] GEMMs, 13 ints each from [1]: the 12 of sdb_test_spatial_transformer, then the epilogue
+ * activation (1 QuickGELU); [70] attention launches, [71..76] dpad, Nq, Nk, split q / k, per-sample lengths, causal. */
+int sdb_test_clip_block(sdb_ctx* ctx, int index, const float* x, int n, int L, int flags, float* out, float* taps,
+                        int32_t* trace);
 /* The first `count` values of stochastic DDIM's noise z at timestep t (0 <= t < 1000) for noise_seed, as the fused sampler step
  * draws them (see sdb_set_sampler). Host buffer out [count]. */
 int sdb_test_step_noise(sdb_ctx* ctx, uint64_t noise_seed, int t, int64_t count, float* out);

@@ -115,6 +115,7 @@ SIGNATURES = [
                                                C.POINTER(C.c_int32)]),
     ("sdb_test_vae_stage", C.c_int, [_ctx, C.c_int, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
                                      _f32p, _f32p, _f32p, _f32p, C.POINTER(C.c_int32)]),
+    ("sdb_test_clip_block", C.c_int, [_ctx, C.c_int, _f32p, C.c_int, C.c_int, C.c_int, _f32p, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_step_noise", C.c_int, [_ctx, C.c_uint64, C.c_int, C.c_int64, _f32p]),
     ("sdb_test_groupnorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_test_layernorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, _f32p]),
@@ -753,6 +754,36 @@ class Context:
               "conv": [tuple(int(v) for v in t[201:204])] * int(t[200]), "softmax": [int(t[205])] * int(t[204]),
               "cond_mod": int(t[206])}
         return dict(out=out, out16=out16, tap=tap, out_norm=out_norm, trace=tr)
+
+    CLIP_TAPS = ("ln1", "q", "k", "v", "o", "x_attn", "ln2", "h")
+
+    def test_clip_block(self, index, x, junk=False, taps=True):
+        """CLIP block `index` (0..11), or the final LayerNorm (12), on the finalized weights. x [n, L, 768] is the residual
+        stream entering it; junk: the pad rows of the row pitch hold large finite values instead of zeros. -> dict: out
+        [n, L, 768]; the taps of CLIP_TAPS ([n, L, 768], h [n, L, 3072]) unless taps is False or index is 12; trace ({"gemms":
+        [...], "attn": [...]})."""
+        x = f32(x)
+        n, L, D = x.shape
+        assert D == 768
+        out = np.empty((n, L, 768), np.float32)
+        tp = np.zeros((11, n, L, 768), np.float32) if taps and index < 12 else None
+        t = np.zeros(80, np.int32)
+        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
+        self.check(self.lib.sdb_test_clip_block(self.h, int(index), ptr(x), n, L, 1 if junk else 0, ptr(out),
+                                                None if tp is None else ptr(tp), i32(t)))
+        keys = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1", "passes")
+        gemms = []
+        for i in range(min(int(t[0]), 5)):
+            g = dict(zip(keys, (int(v) for v in t[1 + 13 * i:12 + 13 * i])))
+            g["epi"] = {r for b, r in enumerate(self._EPI_ROLES) if int(t[12 + 13 * i]) >> b & 1}
+            g["act"] = int(t[13 + 13 * i])
+            gemms.append(g)
+        attn = [dict(zip(("dpad", "Nq", "Nk", "qk3", "kvlen", "causal"), (int(v) for v in t[71:77])))] * min(int(t[70]), 1)
+        res = dict(out=out, trace={"gemms": gemms, "attn": attn})
+        if tp is not None:
+            res.update({k: tp[i] for i, k in enumerate(self.CLIP_TAPS[:7])})
+            res["h"] = tp[7:].reshape(n, L, 3072)
+        return res
 
     def test_groupnorm(self, x, gamma, beta, silu=False):
         x = f32(x); n, c, H, W = x.shape

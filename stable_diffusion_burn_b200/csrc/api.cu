@@ -1006,6 +1006,14 @@ int sdb_test_vae_stage(sdb_ctx* ctx, int stage, const float* x, const float* con
   API_END
 }
 
+int sdb_test_clip_block(sdb_ctx* ctx, int index, const float* x, int n, int L, int flags, float* out, float* taps, int32_t* trace) {
+  API_BEGIN(ctx)
+  need_final(c);
+  c.work.reset();
+  model_test_clip_block(c, index, x, n, L, flags, out, taps, trace);
+  API_END
+}
+
 int sdb_test_step_noise(sdb_ctx* ctx, uint64_t noise_seed, int t, int64_t count, float* out) {
   API_BEGIN(ctx)
   SDB_CHECK(out && count >= 1, "step_noise: null output or count < 1");

@@ -2015,75 +2015,117 @@ void model_forward_diffuser_host(Ctx& c, const float* latent, int t, const float
 }
 
 // ================================================================================ CLIP text encoder
-// reference src/model/clip/mod.rs:56-75 (CLIP::forward), :109-115 (block), :158-180 (attention with the causal mask of
-// src/backend.rs:130-139), :204-227 (MLP with QuickGELU). tokens [n][L] int32 -> out [n][L][768]. SURVEY §8f row f1.
+// The encoder's working set for n samples of L tokens. Rows are laid out at the per-sample pitch Lp = round_up(L, 8), which keeps
+// every TMA tile origin 16-byte aligned; the rows l >= L of a sample are padding.
+struct ClipBufs {
+  int n = 0, L = 0, Lp = 0, Mr = 0, Mp = 0;
+  float* x = nullptr;  // residual stream [Mr][768] fp32, updated in place by each block
+  Half2Ptr l16, o16, h16;  // LayerNorm output, attention output [Mr][768], QuickGELU(fc1) [Mr][3072]: fp16 hi + lo
+  __half* qk = nullptr;  // q | k [Mr][1536], single fp16 values
+  __half* vT = nullptr;  // V^T [768][Mp], sample s at columns s*Lp; the GEMM that writes it is Mp = round_up(Mr, 32) wide
+};
+static ClipBufs clip_bufs(Fwd& f, int n, int L) {
+  Ctx& c = f.c;
+  const int D = 768;
+  ClipBufs b;
+  b.n = n, b.L = L, b.Lp = round_up(L, 8), b.Mr = n * b.Lp, b.Mp = round_up(b.Mr, 32);
+  b.x = c.work.get<float>((size_t)b.Mr * D);
+  b.l16 = f.half2((size_t)b.Mr * D, true), b.o16 = f.half2((size_t)b.Mr * D, true), b.h16 = f.half2((size_t)b.Mr * 4 * D, true);
+  b.qk = c.work.get<__half>((size_t)b.Mr * 2 * D);
+  b.vT = c.work.get<__half>((size_t)D * b.Mp);
+  // pad rows (l >= L) never reach a real row (causal mask, row-wise ops) but must stay finite: 0 * NaN would poison P.V
+  SDB_CUDA(cudaMemsetAsync(b.o16.hi, 0, (size_t)b.Mr * D * 2, c.stream));
+  SDB_CUDA(cudaMemsetAsync(b.o16.lo, 0, (size_t)b.Mr * D * 2, c.stream));
+  return b;
+}
+
+static void clip_layernorm(Ctx& c, const ClipBufs& b, const NormW& nw, Half2Ptr o, float* o32) {
+  KernelScope ks(c, KC_LAYERNORM);
+  layernorm_launch(b.x, b.Mr, 768, nw.gamma, nw.beta, nw.eps, o, o32, c.stream);
+}
+
+// device copies of one block's intermediate state (sdb_test_clip_block), taken in stream order before the next step rewrites the
+// buffer: LN1 and LN2 (hi + lo), q | k, V^T, the attention output (hi + lo), x after the attention, QuickGELU(fc1) (hi + lo)
+struct ClipTaps {
+  Half2Ptr ln1, ln2, o, h;
+  __half* qk = nullptr;
+  __half* vT = nullptr;
+  float* x_attn = nullptr;
+};
+
+// reference src/model/clip/mod.rs:109-115 (block), :158-180 (attention with the causal mask of src/backend.rs:130-139), :204-227
+// (MLP with QuickGELU)
+static void run_clip_block(Fwd& f, const ClipBlockW& cb, const ClipBufs& b, const ClipTaps* taps = nullptr) {
+  Ctx& c = f.c;
+  const int D = 768, heads = 12, Mr = b.Mr;
+  auto copy = [&](void* dst, const void* src, size_t bytes) {
+    SDB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, c.stream));
+  };
+  auto tap16 = [&](Half2Ptr dst, Half2Ptr src, size_t count) { copy(dst.hi, src.hi, count * 2), copy(dst.lo, src.lo, count * 2); };
+  clip_layernorm(c, b, cb.attn_ln, b.l16, nullptr);
+  if (taps) tap16(taps->ln1, b.l16, (size_t)Mr * D);
+  {
+    Epilogue ep;
+    ep.out_f16.hi = b.qk, ep.bias = cb.bias_qk;
+    run_gemm(c, G_LINEAR, f.rows_operand(b.l16, Mr, D), nullptr, cb.w_qk, 3, ep);
+  }
+  {
+    WeightOp tok;
+    tok.p = b.l16, tok.N = b.Mp, tok.rows = Mr, tok.K = D;
+    Epilogue ep;
+    ep.out_f16.hi = b.vT;
+    run_gemm(c, G_LINEAR, f.rows_operand(cb.value.packed.p, D, D), nullptr, tok, 3, ep);
+  }
+  if (taps) copy(taps->qk, b.qk, (size_t)Mr * 2 * D * 2), copy(taps->vT, b.vT, (size_t)D * b.Mp * 2);
+  {
+    AttnOp at;
+    at.q = b.qk, at.ldq = 2 * D, at.q_col0 = 0, at.q_rows = b.Lp;
+    at.k = b.qk, at.ldk = 2 * D, at.k_col0 = D, at.k_rows = b.Lp;
+    at.vT = b.vT, at.ldv = b.Mp;
+    at.nb = b.n, at.heads = heads, at.d = 64, at.dpad = 64, at.Nq = b.L, at.Nk = b.L;
+    at.causal = 1;
+    at.out = b.o16, at.ldo = D;
+    run_attention(c, at);
+  }
+  if (taps) tap16(taps->o, b.o16, (size_t)Mr * D);
+  {
+    Epilogue ep;
+    ep.out_f32 = b.x, ep.residual = b.x, ep.bias = cb.bias_out;
+    run_gemm(c, G_LINEAR, f.rows_operand(b.o16, Mr, D), nullptr, cb.out.packed, 3, ep);
+  }
+  if (taps) copy(taps->x_attn, b.x, (size_t)Mr * D * 4);
+  clip_layernorm(c, b, cb.mlp_ln, b.l16, nullptr);
+  if (taps) tap16(taps->ln2, b.l16, (size_t)Mr * D);
+  {
+    Epilogue ep;
+    ep.out_f16 = b.h16, ep.bias = cb.fc1.bias, ep.act = 1;
+    run_gemm(c, G_LINEAR, f.rows_operand(b.l16, Mr, D), nullptr, cb.fc1.packed, 3, ep);
+  }
+  if (taps) tap16(taps->h, b.h16, (size_t)Mr * 4 * D);
+  {
+    Epilogue ep;
+    ep.out_f32 = b.x, ep.residual = b.x, ep.bias = cb.fc2.bias;
+    run_gemm(c, G_LINEAR, f.rows_operand(b.h16, Mr, 4 * D), nullptr, cb.fc2.packed, 3, ep);
+  }
+}
+
+// reference src/model/clip/mod.rs:56-75 (CLIP::forward). tokens [n][L] int32 -> out [n][L][768]. SURVEY §8f row f1.
 void model_clip_forward_dev(Ctx& c, const int* d_tok, int n, int L, float* d_out, cudaStream_t caller) {
   Model& m = M(c);
   SDB_CHECK(n >= 1 && L >= 1 && L <= 77, "clip_forward: 1 <= L <= 77 (position table), n >= 1");
   StreamJoin join(c, caller);
   c.work.reset();
   Fwd f(c, n);
-  const int D = 768, heads = 12;
-  const int Lp = round_up(L, 8);           // per-sample row pitch: keeps every TMA tile origin 16-byte aligned
-  const int Mr = n * Lp, Mp = round_up(Mr, 32);
-  float* x = c.work.get<float>((size_t)Mr * D);
-  float* y = c.work.get<float>((size_t)Mr * D);
-  Half2Ptr l16 = f.half2((size_t)Mr * D, true), o16 = f.half2((size_t)Mr * D, true), h16 = f.half2((size_t)Mr * 4 * D, true);
-  __half* qk = c.work.get<__half>((size_t)Mr * 2 * D);
-  __half* vT = c.work.get<__half>((size_t)D * Mp);
-  // pad rows (l >= L) never reach a real row (causal mask, row-wise ops) but must stay finite: 0 * NaN would poison P.V
-  SDB_CUDA(cudaMemsetAsync(o16.hi, 0, (size_t)Mr * D * 2, c.stream));
-  SDB_CUDA(cudaMemsetAsync(o16.lo, 0, (size_t)Mr * D * 2, c.stream));
+  const int D = 768;
+  const ClipBufs b = clip_bufs(f, n, L);
+  const int Lp = b.Lp;
+  float* y = c.work.get<float>((size_t)b.Mr * D);
   {
     KernelScope ks(c, KC_ELEMENTWISE);
-    embed_tokens_launch(d_tok, mptr(c, m.clip.tok_i), mptr(c, m.clip.pos_i), n, L, Lp, D, 49408, x, c.stream);
+    embed_tokens_launch(d_tok, mptr(c, m.clip.tok_i), mptr(c, m.clip.pos_i), n, L, Lp, D, 49408, b.x, c.stream);
   }
-  auto ln = [&](const NormW& nw, Half2Ptr o, float* o32) {
-    KernelScope ks(c, KC_LAYERNORM);
-    layernorm_launch(x, Mr, D, nw.gamma, nw.beta, nw.eps, o, o32, c.stream);
-  };
-  for (ClipBlockW& cb : m.clip.blocks) {
-    ln(cb.attn_ln, l16, nullptr);
-    {
-      Epilogue ep;
-      ep.out_f16.hi = qk, ep.bias = cb.bias_qk;
-      run_gemm(c, G_LINEAR, f.rows_operand(l16, Mr, D), nullptr, cb.w_qk, 3, ep);
-    }
-    {
-      WeightOp tok;
-      tok.p = l16, tok.N = Mp, tok.rows = Mr, tok.K = D;
-      Epilogue ep;
-      ep.out_f16.hi = vT;
-      run_gemm(c, G_LINEAR, f.rows_operand(cb.value.packed.p, D, D), nullptr, tok, 3, ep);
-    }
-    {
-      AttnOp at;
-      at.q = qk, at.ldq = 2 * D, at.q_col0 = 0, at.q_rows = Lp;
-      at.k = qk, at.ldk = 2 * D, at.k_col0 = D, at.k_rows = Lp;
-      at.vT = vT, at.ldv = Mp;
-      at.nb = n, at.heads = heads, at.d = 64, at.dpad = 64, at.Nq = L, at.Nk = L;
-      at.causal = 1;
-      at.out = o16, at.ldo = D;
-      run_attention(c, at);
-    }
-    {
-      Epilogue ep;
-      ep.out_f32 = x, ep.residual = x, ep.bias = cb.bias_out;
-      run_gemm(c, G_LINEAR, f.rows_operand(o16, Mr, D), nullptr, cb.out.packed, 3, ep);
-    }
-    ln(cb.mlp_ln, l16, nullptr);
-    {
-      Epilogue ep;
-      ep.out_f16 = h16, ep.bias = cb.fc1.bias, ep.act = 1;
-      run_gemm(c, G_LINEAR, f.rows_operand(l16, Mr, D), nullptr, cb.fc1.packed, 3, ep);
-    }
-    {
-      Epilogue ep;
-      ep.out_f32 = x, ep.residual = x, ep.bias = cb.fc2.bias;
-      run_gemm(c, G_LINEAR, f.rows_operand(h16, Mr, 4 * D), nullptr, cb.fc2.packed, 3, ep);
-    }
-  }
-  ln(m.clip.ln_final, Half2Ptr{}, y);
+  for (const ClipBlockW& cb : m.clip.blocks) run_clip_block(f, cb, b);
+  clip_layernorm(c, b, m.clip.ln_final, Half2Ptr{}, y);
   SDB_CUDA(cudaMemcpy2DAsync(d_out, (size_t)L * D * 4, y, (size_t)Lp * D * 4, (size_t)L * D * 4, n, cudaMemcpyDeviceToDevice,
                              c.stream));
 }
@@ -2583,6 +2625,99 @@ void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, 
   if (out16) fetch_half2(c, o.raw16, n, cout, o.H, o.W, out16);
   if (tap && attn) fetch_half2(c, otap, n, 512, H, W, tap);
   if (out_norm && g.p.hi) fetch_half2(c, g.p, n, cout, o.H, o.W, out_norm);
+}
+
+// ================================================================================ CLIP block test entry
+void model_test_clip_block(Ctx& c, int index, const float* x, int n, int L, int flags, float* out, float* taps, int32_t* trace) {
+  Model& m = M(c);
+  const int nblk = (int)m.clip.blocks.size();
+  SDB_CHECK(index >= 0 && index <= nblk, "test_clip_block: index is a block 0..11, or 12 for the final LayerNorm");
+  SDB_CHECK(n >= 1 && L >= 1 && L <= 77 && x && out && trace, "test_clip_block: arguments (1 <= L <= 77)");
+  SDB_CHECK((flags & ~1) == 0, "test_clip_block: flags are 1 (pad rows hold large finite junk instead of zeros)");
+  const int D = 768;
+  Fwd f(c, n);
+  const ClipBufs b = clip_bufs(f, n, L);
+  const int Lp = b.Lp, Mr = b.Mr;
+  // x [n][L][768] staged at the row pitch Lp, as embed_tokens_launch leaves the embedding: pad rows zero, or junk that must never
+  // reach a real row
+  std::vector<float> hx((size_t)Mr * D, 0.f);
+  for (int s = 0; s < n; ++s)
+    for (int l = 0; l < Lp; ++l)
+      for (int j = 0; j < D; ++j) {
+        const size_t r = (size_t)s * Lp + l;
+        if (l < L)
+          hx[r * D + j] = x[((size_t)s * L + l) * D + j];
+        else if (flags & 1)
+          hx[r * D + j] = 2.0e4f * (float)((r * 7919 + (size_t)j * 104729) % 2001) / 1000.f - 2.0e4f;
+      }
+  SDB_CUDA(cudaMemcpyAsync(b.x, hx.data(), hx.size() * 4, cudaMemcpyHostToDevice, c.stream));
+  ClipTaps tp;
+  if (taps && index < nblk) {
+    tp.ln1 = f.half2((size_t)Mr * D, true), tp.ln2 = f.half2((size_t)Mr * D, true), tp.o = f.half2((size_t)Mr * D, true);
+    tp.h = f.half2((size_t)Mr * 4 * D, true);
+    tp.qk = c.work.get<__half>((size_t)Mr * 2 * D);
+    tp.vT = c.work.get<__half>((size_t)D * b.Mp);
+    tp.x_attn = c.work.get<float>((size_t)Mr * D);
+  }
+  float* y = index < nblk ? b.x : c.work.get<float>((size_t)Mr * D);
+  std::fill(trace, trace + kClipTraceInts, 0);
+  {
+    TraceScope ts(c);
+    if (index < nblk)
+      run_clip_block(f, m.clip.blocks[index], b, tp.qk ? &tp : nullptr);
+    else
+      clip_layernorm(c, b, m.clip.ln_final, Half2Ptr{}, y);
+    trace[0] = (int)c.gemm_trace.size();
+    for (size_t i = 0; i < c.gemm_trace.size() && i < 5; ++i) {
+      const Ctx::GemmRecord& r = c.gemm_trace[i];
+      const int v[13] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels, r.passes, r.epi,
+                         r.act};
+      std::copy(v, v + 13, trace + 1 + 13 * i);
+    }
+    trace[70] = (int)c.attn_trace.size();
+    if (!c.attn_trace.empty()) {
+      const Ctx::AttnRecord& r = c.attn_trace[0];
+      const int v[6] = {r.dpad, r.Nq, r.Nk, r.qk3, r.kvlen, r.causal};
+      std::copy(v, v + 6, trace + 71);
+    }
+  }
+  // real rows only, [n][L][width]
+  auto real_rows = [&](const std::vector<float>& src, int width, int col0, int pitch, float* dst) {
+    for (int s = 0; s < n; ++s)
+      for (int l = 0; l < L; ++l)
+        std::copy(&src[((size_t)s * Lp + l) * pitch + col0], &src[((size_t)s * Lp + l) * pitch + col0] + width,
+                  dst + ((size_t)s * L + l) * width);
+  };
+  auto fetch32 = [&](const float* d, size_t count) {
+    std::vector<float> h(count);
+    SDB_CUDA(cudaMemcpyAsync(h.data(), d, count * 4, cudaMemcpyDeviceToHost, c.stream));
+    SDB_CUDA(cudaStreamSynchronize(c.stream));
+    return h;
+  };
+  auto fetch16 = [&](const __half* hi, const __half* lo, size_t count) {
+    std::vector<__half> h(count), l(lo ? count : 0);
+    SDB_CUDA(cudaMemcpyAsync(h.data(), hi, count * 2, cudaMemcpyDeviceToHost, c.stream));
+    if (lo) SDB_CUDA(cudaMemcpyAsync(l.data(), lo, count * 2, cudaMemcpyDeviceToHost, c.stream));
+    SDB_CUDA(cudaStreamSynchronize(c.stream));
+    std::vector<float> v(count);
+    for (size_t i = 0; i < count; ++i) v[i] = __half2float(h[i]) + (lo ? __half2float(l[i]) : 0.f);
+    return v;
+  };
+  real_rows(fetch32(y, (size_t)Mr * D), D, 0, D, out);
+  if (!tp.qk) return;
+  const size_t tc = (size_t)n * L * D;  // one [n][L][768] tap
+  real_rows(fetch16(tp.ln1.hi, tp.ln1.lo, (size_t)Mr * D), D, 0, D, taps);
+  const std::vector<float> qk = fetch16(tp.qk, nullptr, (size_t)Mr * 2 * D);
+  real_rows(qk, D, 0, 2 * D, taps + tc);
+  real_rows(qk, D, D, 2 * D, taps + 2 * tc);
+  const std::vector<float> vT = fetch16(tp.vT, nullptr, (size_t)D * b.Mp);
+  for (int s = 0; s < n; ++s)
+    for (int l = 0; l < L; ++l)
+      for (int j = 0; j < D; ++j) taps[3 * tc + ((size_t)s * L + l) * D + j] = vT[(size_t)j * b.Mp + (size_t)s * Lp + l];
+  real_rows(fetch16(tp.o.hi, tp.o.lo, (size_t)Mr * D), D, 0, D, taps + 4 * tc);
+  real_rows(fetch32(tp.x_attn, (size_t)Mr * D), D, 0, D, taps + 5 * tc);
+  real_rows(fetch16(tp.ln2.hi, tp.ln2.lo, (size_t)Mr * D), D, 0, D, taps + 6 * tc);
+  real_rows(fetch16(tp.h.hi, tp.h.lo, (size_t)Mr * 4 * D), 4 * D, 0, 4 * D, taps + 7 * tc);
 }
 
 }  // namespace sdb

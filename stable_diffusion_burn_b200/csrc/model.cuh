@@ -85,5 +85,8 @@ void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, in
 constexpr int kVaeTraceInts = 256;
 void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, int n, int C, int H, int W, float scale, int flags,
                           float* out, float* out16, float* tap, float* out_norm, int32_t* trace);
+// CLIP block test entry (sdb200.h: sdb_test_clip_block); trace = kClipTraceInts ints
+constexpr int kClipTraceInts = 80;
+void model_test_clip_block(Ctx& c, int index, const float* x, int n, int L, int flags, float* out, float* taps, int32_t* trace);
 
 }  // namespace sdb

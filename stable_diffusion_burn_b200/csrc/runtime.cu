@@ -185,6 +185,9 @@ void run_attention(Ctx& c, const AttnOp& a) {
   // the causal mask is applied inside the first key tile only (CLIP: L <= 77); longer causal sequences are not supported
   SDB_CHECK(!a.causal || a.Nk <= 128, "causal attention supports at most 128 keys");
   SDB_CHECK(a.Nk >= 1 && a.Nq >= 1, "attention needs at least one query and one key");
+  // V^T: sample s starts at column s * k_rows, the inner coordinate of its TMA boxes, which must be 16-byte aligned (an unaligned
+  // one faults the kernel instead of failing here)
+  SDB_CHECK(a.v_mn || a.k_rows % 8 == 0, "attention with V transposed: the per-sample key rows must be a multiple of 8");
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.nb = a.nb, p.heads = a.heads, p.d = a.d, p.dpad = a.dpad, p.Nq = a.Nq, p.Nk = a.Nk;
@@ -218,7 +221,7 @@ void run_attention(Ctx& c, const AttnOp& a) {
     memset(dbg_buf, 0, 256 * sizeof(long long));
     p.dbg = dbg_buf;
   }
-  if (c.trace_on) c.attn_trace.push_back({a.dpad, a.Nq, a.Nk, p.qk3, a.kvlen ? 1 : 0});
+  if (c.trace_on) c.attn_trace.push_back({a.dpad, a.Nq, a.Nk, p.qk3, a.kvlen ? 1 : 0, a.causal});
   {
     KernelScope ks(c, KC_ATTN, flops, 0);
     attention_launch(am, p, c.stream);
@@ -401,7 +404,7 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
   if (c.trace_on) {
     const int epi = (ep.ln_out ? EPI_ROLE_LNS : 0) | (ep.ln_in ? EPI_ROLE_LNC : 0) | (ep.geglu ? EPI_ROLE_GEGLU : 0) |
                     (ep.residual16.hi ? EPI_ROLE_RES16 : 0) | (ep.residual ? EPI_ROLE_RES32 : 0) | (gn ? EPI_ROLE_GN : 0);
-    c.gemm_trace.push_back({kind_in, w.N, BN, split, p.TN, p.TH, p.TW, p.xkc * 64, gn ? gn->slots : 0, a1in ? a1.C : 0, passes, epi});
+    c.gemm_trace.push_back({kind_in, w.N, BN, split, p.TN, p.TH, p.TW, p.xkc * 64, gn ? gn->slots : 0, a1in ? a1.C : 0, passes, epi, ep.act});
   }
   p.gn_part = gn ? gn->buf : nullptr;
   p.gn_cap = gn ? gn->cap : 0, p.gn_bucket = gn ? gn->bucket : 1;

@@ -194,12 +194,12 @@ struct Ctx {
   std::string dbg_label;
   // launch record for the test entries (sdb_test_resblock, sdb_test_spatial_transformer): what run_gemm chose per GEMM, what
   // run_attention launched and which GroupNorm path Fwd::gn_operand took, so a test can assert it reached the path it is meant
-  // to cover. epi: EPI_ROLE_* bits of the epilogue (gn only when the statistics were really written)
+  // to cover. epi: EPI_ROLE_* bits of the epilogue (gn only when the statistics were really written); act: Epilogue::act
   struct GemmRecord {
-    int kind, N, BN, split, TN, TH, TW, xk_channels, gn_slots, a1_channels, passes, epi;
+    int kind, N, BN, split, TN, TH, TW, xk_channels, gn_slots, a1_channels, passes, epi, act;
   };
   struct AttnRecord {
-    int dpad, Nq, Nk, qk3, kvlen;
+    int dpad, Nq, Nk, qk3, kvlen, causal;
   };
   bool trace_on = false;
   std::vector<GemmRecord> gemm_trace;
