@@ -271,12 +271,11 @@ int sdb_sample_image_dev(sdb_ctx* ctx, const float* d_context, int n, int L, con
                          int H, int W, uint8_t* d_rgb, void* stream);
 
 /* ---- configuration / instrumentation ------------------------------------------------------- */
-/* key/value knobs: "precision" = 1|2|3 tensor-core passes per product (0 = the per-layer policy, see DESIGN.md),
- * "graphs" = 0|1 (CUDA-graph replay of the UNet step), "splitk" = 0|1. A/B switches of measured design choices (defaults are the
- * measured-faster settings; results do not change beyond rounding, the first two not at all): "emb_hoist" (time-embedding rows of
- * all timesteps once per sample call), "attn_regsplit" (setmaxnreg build of the attention kernel), "attn_split" (fp16 hi + lo
- * q / k on the 3-pass levels), "prefetch_w", "raw16", "skip_merge", "gn_epilogue", "mlp_passes",
- * "splitk_min_iters", "splitk_chunk", "gn_apply_ctas", "gn_min_pix". Unknown keys are an error. */
+/* Run configurations: "precision" = 1|2|3 tensor-core passes per product (0 = the per-layer policy, DESIGN.md), "graphs" = 0|1
+ * (CUDA-graph replay of the UNet step), "splitk" = 0|1, "emb_hoist" = 0|1 (0: per-step time-embedding GEMVs, as sdb_unet_forward
+ * runs them). Test hooks (default 1; 0 selects a path production takes elsewhere): "raw16" (prep_operand staging, as for the
+ * stride-2 convs), "skip_merge" (the 1x1 skip conv as its own GEMM, as in the VAE encoder), "gn_epilogue" (the fused GroupNorm,
+ * as behind the Cin = 4 convs), "attn_split" (fp16 q / k at d = 40 / 80; no production call takes it). Unknown keys: error. */
 int sdb_set_option(sdb_ctx* ctx, const char* key, int value);
 /* Per-kernel-class timing: when enabled, every launch is bracketed by CUDA events on the
  * context's stream (graphs are bypassed). */

@@ -119,7 +119,7 @@ static int create(int device, int unet_cin, sdb_ctx** out) {
     h->c.device = device;
     h->c.unet_cin = unet_cin;
     h->c.debug_sync = getenv("SDB_DEBUG_SYNC") && atoi(getenv("SDB_DEBUG_SYNC")) != 0;
-    if (getenv("SDB_PDL")) g_pdl_enabled = atoi(getenv("SDB_PDL")) != 0, g_pdl_late = atoi(getenv("SDB_PDL")) == 2;
+    if (getenv("SDB_PDL")) g_pdl_enabled = atoi(getenv("SDB_PDL")) != 0;
     SDB_CUDA(cudaStreamCreateWithFlags(&h->c.stream, cudaStreamNonBlocking));
     model_create(h->c);
     *out = h;
@@ -566,28 +566,14 @@ int sdb_set_option(sdb_ctx* ctx, const char* key, int value) {
     c.opt_splitk = value;
   else if (k == "raw16")
     c.opt_raw16 = value;
-  else if (k == "splitk_min_iters")
-    c.opt_splitk_min_iters = value;
-  else if (k == "splitk_chunk")
-    c.opt_splitk_chunk = value < 1 ? 1 : value;
   else if (k == "attn_split")
     c.opt_attn_split = value;
-  else if (k == "attn_regsplit")
-    g_attn_regsplit = value;
   else if (k == "emb_hoist")
     c.opt_emb_hoist = value;
-  else if (k == "prefetch_w")
-    c.opt_prefetch_w = value;
-  else if (k == "mlp_passes")
-    c.opt_mlp_passes = value;
   else if (k == "gn_epilogue")
     c.opt_gn_epilogue = value;
   else if (k == "skip_merge")
     c.opt_skip_merge = value;
-  else if (k == "gn_apply_ctas")
-    g_gn_apply_ctas = value < 1 ? 1 : value;
-  else if (k == "gn_min_pix")
-    g_gn_min_pix = value < 1 ? 1 : value;
   else
     throw Error("unknown option: " + k);
   model_invalidate_graphs(c);

@@ -51,9 +51,7 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// RS = true (register split): setmaxnreg moves registers from the producer warpgroup (down to 40 per thread) to the two softmax
-// warpgroups (up to 232). Without it ptxas budgets 65536 / 384 = 168 registers per thread for every role.
-template <int DPAD, bool VMN, bool QK3, bool RS>
+template <int DPAD, bool VMN, bool QK3>
 __global__ void __launch_bounds__(384, 1)
 attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ CUtensorMap mk,
                  const __grid_constant__ CUtensorMap mv, const __grid_constant__ CUtensorMap mq_lo,
@@ -103,9 +101,7 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
   const int kvlen = p.kvlen ? max(1, min(p.kvlen[s], p.Nk)) : p.Nk;
   const int T = (kvlen + 127) / 128;
 
-  // (setmaxnreg sits INSIDE the role branches: ptxas budgets the code after a join with the smaller of the two limits)
   if (warp < 4) {
-    if (RS) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     // ======================================================================= TMA producers
     // warp 0 loads Q and the K tiles, warp 1 the V tiles: the consumers free a K stage a whole softmax before the V stage of the
     // same tile, so the next K load must not queue behind the wait for that V stage
@@ -150,7 +146,6 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
       }
     }
   } else {
-    if (RS) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     // ======================================================================= softmax warpgroups + epilogue
     // accumulator layout of m64nN (see Wgmma in common.cuh): this thread holds rows rw + 8 hh (hh = 0, 1) of the warpgroup's
     // 64, columns 8 (i / 4) + 2 (lane % 4) + i % 2 of element i, with hh = (i / 2) % 2
@@ -372,23 +367,14 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
   __syncthreads();
 }
 
-// option "attn_regsplit": launches use the register-split variant (see attention_kernel). Same arithmetic in the same order:
-// bit-identical to the variant without it.
-int g_attn_regsplit = 0;
-
-template <int DPAD, bool VMN, bool QK3, bool RS>
-static void launch_attn3(const AttnMaps& m, const AttnParams& p, cudaStream_t st) {
+template <int DPAD, bool VMN, bool QK3>
+static void launch_attn2(const AttnMaps& m, const AttnParams& p, cudaStream_t st) {
   constexpr int smem = AttnCfg<DPAD, VMN, QK3>::SMEM;
   static DeviceOnce once;
   if (once.first())
-    SDB_CUDA(cudaFuncSetAttribute(attention_kernel<DPAD, VMN, QK3, RS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    SDB_CUDA(cudaFuncSetAttribute(attention_kernel<DPAD, VMN, QK3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   dim3 grid((p.Nq + 127) / 128, p.heads, p.nb);
-  launch_k(attention_kernel<DPAD, VMN, QK3, RS>, grid, dim3(384), (size_t)smem, st, m.q, m.k, m.v, m.q_lo, m.k_lo, p);
-}
-template <int DPAD, bool VMN, bool QK3>
-static void launch_attn2(const AttnMaps& m, const AttnParams& p, cudaStream_t st) {
-  if (g_attn_regsplit) return launch_attn3<DPAD, VMN, QK3, true>(m, p, st);
-  launch_attn3<DPAD, VMN, QK3, false>(m, p, st);
+  launch_k(attention_kernel<DPAD, VMN, QK3>, grid, dim3(384), (size_t)smem, st, m.q, m.k, m.v, m.q_lo, m.k_lo, p);
 }
 template <int DPAD>
 static void launch_attn(const AttnMaps& m, const AttnParams& p, cudaStream_t st) {

@@ -27,6 +27,5 @@ struct AttnMaps {
 };
 void attention_launch(const AttnMaps& m, const AttnParams& p, cudaStream_t st);
 bool attention_supports_qk3(int dpad);
-extern int g_attn_regsplit;  // 1: launches run the register-split (setmaxnreg) variant
 
 }  // namespace sdb

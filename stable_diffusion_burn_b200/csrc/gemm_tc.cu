@@ -140,7 +140,6 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   const int lane = threadIdx.x & 31;
   long long* const dbg = (p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) ? p.dbg : nullptr;
   if (dbg && threadIdx.x == 0) dbg[0] = clock64();
-  if (!p.pdl_late) pdl_trigger();  // the next kernel of the stream may begin its own prologue
 
   // ---- tile coordinates
   int mt = blockIdx.x;
@@ -178,8 +177,8 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   if (dbg && threadIdx.x == 0) dbg[1] = clock64();
   // Programmatic dependent launch: everything above overlapped the previous kernel's tail. From here on each role waits for the
   // previous kernel (griddepcontrol.wait) only where it first touches data that kernel may have written:
-  //   producer : WEIGHTS are immutable, so the weight tiles of the first STAGES k-chunks (and an L2 prefetch of the rest of this
-  //              CTA's weight strip when the launch is weight-bound) are issued BEFORE the wait; activation tiles after it
+  //   producer : WEIGHTS are immutable, so the weight tiles of the first STAGES k-chunks are issued BEFORE the wait; activation
+  //              tiles after it
   //   consumers: wait before the epilogue's first read of residual / time-embedding rows; all of this kernel's stores follow it
   if (warp == 0) {
     // ===================================================== TMA producer (one elected lane: see elect_one in common.cuh)
@@ -215,14 +214,6 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       for (int i = 0; i < npre; ++i) {
         mbar_expect_tx(&full_bar[i], L::BYTES);
         load_b(it_begin + i, i);
-      }
-      if (p.prefetch_w) {
-        for (int it = it_begin + npre; it < it_end; ++it) {
-          const CUtensorMap* bm = it < main_iters ? maps.b : maps.bx;
-          const int bk = (it < main_iters ? it : it - main_iters) * BK;
-          tma_prefetch_l2_2d(&bm[0], bk, b_row0);
-          if (PASSES >= 3) tma_prefetch_l2_2d(&bm[1], bk, b_row0);
-        }
       }
       pdl_wait();
       for (int i = 0; i < npre; ++i) load_a(it_begin + i, i);
@@ -386,7 +377,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     const bool pre_issued = plain;
     if (pre_issued) issue_addends(col0 + half * 32 + cq);
 
-    if (p.pdl_late) pdl_trigger();
+    pdl_trigger();  // the epilogue starts: the next kernel of the stream may begin its own prologue
     if (dbg && threadIdx.x == 128) dbg[5] = clock64();
     constexpr uint32_t TROW = AccLayout<BN>::PITCH;
     const uint32_t arow = smem_u32(smem) + q * 32 * TROW;  // row 32 q of the accumulator image

@@ -40,9 +40,6 @@ struct GemmParams {
   int geglu;               // 1: columns are (x|gate) interleaved per tile, output width N/2
   long long* dbg;          // SDB_GEMM_DBG: 8 clock64 stamps of CTA (0,0,0) (entry, prologue done, first TMA issued, first
                            // operands landed, last MMA issued, accumulator ready, epilogue stores done, exit)
-  int prefetch_w;          // 1: the producer prefetches the rest of its weight strip into L2 before griddepcontrol.wait (launches
-                           // with few M tiles, where the weights stream from HBM and nothing else hides their latency)
-  int pdl_late;            // 1: release the dependent launch when the epilogue starts instead of at kernel entry
   int act;                 // 1: QuickGELU x*sigmoid(1.702x) on the result (CLIP MLP, clip/mod.rs:224-226)
   // GroupNorm statistics of the OUTPUT tensor, produced here so that the consuming GroupNorm needs neither a statistics pass over
   // the tensor nor a grid rendezvous: per (image, slot, channel bucket) partial (sum, sum of squares) of the final fp32 values,

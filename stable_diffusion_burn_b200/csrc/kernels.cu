@@ -494,16 +494,15 @@ void gn_sums_from_partials_launch(const float* part, int cap, int slots, int nbk
   SDB_CUDA(cudaGetLastError());
 }
 
-int g_gn_apply_ctas = 0;  // 0: four CTAs per SM of the device
 void gn_apply_launch(const GnSrc& s0, const GnSrc& s1, int bucket, int n, int H, int W, int silu, const float* gamma,
                      const float* beta, float eps, Half2Ptr out, cudaStream_t st) {
   const int C = s0.C + s1.C, HW = H * W;
   SDB_CHECK(C % 64 == 0 && s0.C % 8 == 0 && C <= 2560 && bucket > 0 && s0.C % bucket == 0 && s1.C % bucket == 0 &&
                 (C / 32) % bucket == 0 && C / bucket <= 256,
             "GroupNorm apply: channel / bucket geometry");
-  // no co-residency constraint any more; every CTA repeats the fold of its image's partials (8-24 KB from L2), so the grid is
-  // kept to g_gn_apply_ctas CTAs (4 per SM by default), at least one pixel each
-  const int ctas = g_gn_apply_ctas > 0 ? g_gn_apply_ctas : 4 * g_num_sms;
+  // every CTA repeats the fold of its image's partials (8-24 KB from L2), so the grid is kept small, at least one pixel per CTA
+  constexpr int kGnApplyCtasPerSm = 4;
+  const int ctas = kGnApplyCtasPerSm * g_num_sms;
   int pix = (int)((((long long)HW * n) + ctas - 1) / ctas);
   if (pix < 1) pix = 1;
   dim3 grid(ceil_div(HW, pix), n);
@@ -512,10 +511,10 @@ void gn_apply_launch(const GnSrc& s0, const GnSrc& s1, int bucket, int n, int H,
   SDB_CUDA(cudaGetLastError());
 }
 
-int g_gn_min_pix = 1;  // pixels per CTA floor: small feature maps are latency-bound, so they get many small CTAs
 static int gn_fused_pix(int n, int HW) {
+  constexpr int kGnFusedMinPix = 1;  // pixels per CTA floor: small feature maps are latency-bound, so they get many small CTAs
   int pix = (int)((((long long)HW * n) + 295) / 296);  // <= 296 CTAs (2 per SM): short fold, always co-resident
-  return pix < g_gn_min_pix ? g_gn_min_pix : pix;
+  return pix < kGnFusedMinPix ? kGnFusedMinPix : pix;
 }
 size_t gn_fused_partial_floats(int n, int HW) { return (size_t)n * ceil_div(HW, gn_fused_pix(n, HW)) * 64; }
 

@@ -19,8 +19,6 @@ void gn_stats_launch(const float* x0, int C0, const float* x1, int C1, int n, in
                      unsigned int* tickets, cudaStream_t st);
 // One-launch GroupNorm(+SiLU) -> fp16 hi(/lo) operand: statistics and apply fused through an in-kernel grid wait.
 // tickets: [n] zeroed counters; partials: gn_fused_partial_floats(n,HW) floats of scratch.
-extern int g_gn_min_pix;
-extern int g_gn_apply_ctas;
 size_t gn_fused_partial_floats(int n, int HW);
 void gn_fused_launch(const float* x0, int C0, const float* x1, int C1, int n, int H, int W, int silu, const float* gamma,
                      const float* beta, float eps, Half2Ptr out, float* partials, unsigned int* tickets, cudaStream_t st);

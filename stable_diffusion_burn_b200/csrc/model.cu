@@ -898,18 +898,17 @@ static void run_spatial_transformer(Fwd& f, SpatialTransformerW& s, const CtxSta
   }
   tap(2, st3);
   // ---- GEGLU MLP: x += lin(x_a * gelu(gate)), LN3 folded into the GEGLU projection
-  const int Pm = c.opt_mlp_passes ? c.opt_mlp_passes : P;  // pass policy of the MLP pair (DESIGN.md "precision")
-  Half2Ptr g16 = f.half2((size_t)Mt * 4 * C, Pm >= 2 || c.opt_precision >= 2);
+  Half2Ptr g16 = f.half2((size_t)Mt * 4 * C, lo);
   {
     Epilogue ep;
     ep.geglu = 1, ep.out_f16 = g16;
     ln_consume(ep, st3, s.ln3, s.u_geglu_hi, s.u_geglu_full, s.v_geglu);
-    run_gemm(c, G_LINEAR, f.rows_operand(y16, Mt, C), nullptr, s.w_geglu, Pm, ep);
+    run_gemm(c, G_LINEAR, f.rows_operand(y16, Mt, C), nullptr, s.w_geglu, P, ep);
   }
   {
     Epilogue ep;
     ep.out_f16 = y16, ep.residual16 = y16, ep.bias = s.ff.bias;
-    run_gemm(c, G_LINEAR, f.rows_operand(g16, Mt, 4 * C), nullptr, s.ff.packed, Pm, ep);
+    run_gemm(c, G_LINEAR, f.rows_operand(g16, Mt, 4 * C), nullptr, s.ff.packed, P, ep);
   }
   tap(3, nullptr);
   // ---- proj_out + residual with the block input

@@ -13,9 +13,7 @@ namespace sdb {
 
 // Programmatic dependent launch: with every kernel releasing its dependents at entry, early CTAs of the next kernel sit on the
 // SMs while the GEMM still runs; the GEMMs therefore release them when their epilogue starts and load their first weight tiles
-// ahead of griddepcontrol.wait.
-// SDB_PDL=0 disables, 1 = release at entry everywhere, 2 (default) = late release in the GEMMs.
-int g_pdl_late = 1;
+// ahead of griddepcontrol.wait. SDB_PDL=0 disables PDL (a debugging aid).
 bool g_pdl_enabled = true;
 int g_num_sms = 132;
 
@@ -357,14 +355,15 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
 
 
   // split-K when the grid cannot fill the machine and the K loop is long
+  constexpr int kSplitKMinIters = 32;  // shortest K loop (in 64-wide k-chunks) that is split
+  constexpr int kSplitKChunk = 8;      // k-chunks every split keeps, so the rendezvous + fold stays small against its mainloop
   const int iters = p.num_taps * p.kc + p.xkc;
   int split = 1;
   if (c.opt_splitk && kind != G_CONV3_UP2 && !ep.geglu && !ep.ln_out && !ep.ln_in) {
     const int ctas = m_tiles * n_tiles;
-    if (ctas <= g_num_sms / 2 && iters >= c.opt_splitk_min_iters) {
-      // floor: ctas*split must stay within ONE wave of the SMs (one CTA per SM: a 2-wave grid costs 2x);
-      // every split keeps >= 16 k-chunks so the rendezvous + fold stays small against its mainloop
-      split = std::min(std::min(g_num_sms / ctas, iters / c.opt_splitk_chunk), 16);
+    if (ctas <= g_num_sms / 2 && iters >= kSplitKMinIters) {
+      // floor: ctas*split must stay within ONE wave of the SMs (one CTA per SM: a 2-wave grid costs 2x)
+      split = std::min(std::min(g_num_sms / ctas, iters / kSplitKChunk), 16);
       if (split < 1) split = 1;
     }
   }
@@ -425,8 +424,6 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
   p.residual = ep.residual;
   p.geglu = ep.geglu;
   p.act = ep.act;
-  p.pdl_late = g_pdl_late;
-  p.prefetch_w = (g_pdl_enabled && c.opt_prefetch_w && m_tiles <= 4) ? 1 : 0;
   const int nout = ep.geglu ? w.N / 2 : w.N;
   p.ldc = ep.ldc ? ep.ldc : nout;
   p.ldc16 = ep.ldc16 ? ep.ldc16 : nout;

@@ -156,13 +156,10 @@ struct Ctx {
   int opt_precision = 0;  // 0 = per-layer policy, 1/2/3 = force
   int opt_graphs = 1;
   int opt_splitk = 1;
-  int opt_splitk_min_iters = 32, opt_splitk_chunk = 8;  // split-K: shortest K loop that is split, k-chunks kept per split
   int opt_skip_merge = 1; // ResBlock skip 1x1 conv folded into conv_out's K loop (needs raw16)
   int opt_raw16 = 1;      // epilogues also write the fp16 hi/lo copy a later raw-operand consumer needs (no staging launch)
-  int opt_mlp_passes = 0;   // 0: the transformer MLP (GEGLU + ff) follows its level's pass policy; 1: single fp16 pass everywhere
   int opt_attn_split = 1;   // fused attention on the 3-pass levels takes q / k as fp16 hi + lo pairs (fp32-class logits)
   int opt_emb_hoist = 1;    // sample_latent computes the time-embedding rows of every timestep once per call (not once per step)
-  int opt_prefetch_w = 0;   // 1: weight-bound GEMMs (<= 4 M tiles) prefetch their weight strip into L2 ahead of griddepcontrol.wait.
   int opt_gn_epilogue = 1;  // GroupNorm statistics produced by the GEMM epilogue that writes the tensor (no stats pass, no rendezvous)
   // sampler of the sampling entries (sdb_set_sampler, DESIGN §7 f6): SDB_SAMPLER_DDIM with eta, or SDB_SAMPLER_DPMPP_2M
   int sampler_kind = 0;

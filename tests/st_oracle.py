@@ -28,14 +28,13 @@ HEADS = 8
 
 @dataclass(frozen=True)
 class Rounding:
-    passes: int = 3      # passes of the block's GEMMs (proj_in, q|k|v, out projections, cross q, proj_out)
-    mlp_passes: int = 3  # passes of the GEGLU projection and ff
+    passes: int = 3      # passes of the block's GEMMs (all but the context K / V)
     qk_split: bool = True  # attention logits from hi + lo q / k (else fp16 q / k)
     attention: bool = False  # fp16 P and V (and q / k unless qk_split)
 
     @staticmethod
-    def of(passes, mlp_passes, qk_split):
-        return Rounding(passes, mlp_passes, qk_split, True)
+    def of(passes, qk_split):
+        return Rounding(passes, qk_split, True)
 
 
 EXACT = Rounding()
@@ -86,7 +85,7 @@ def spatial_transformer(W, name, x, context, lens, r: Rounding = EXACT, eps=1e-5
     n, c, h, w = x.shape
     act = lambda a, p: _round(a, "fp16") if p == 1 else a
     wgt = lambda a, p: _round(a, "fp16") if p <= 2 else a
-    P, Pm = r.passes, r.mlp_passes
+    P = r.passes
 
     def ln_fold(y, ln, wmat, bias, p):
         """LayerNorm(y) @ wmat + bias with gamma folded into the weights and the normalisation applied after the product"""
@@ -112,8 +111,8 @@ def spatial_transformer(W, name, x, context, lens, r: Rounding = EXACT, eps=1e-5
     o = _attention(q, k, v, lens, r.attention, r.qk_split).reshape(n * h * w, c)
     y2 = lin(o, f"{t}/attn2/out", P, y1)
     # GEGLU MLP
-    hg = ln_fold(y2, "norm3", W[f"{t}/mlp/geglu/proj/weight"], W[f"{t}/mlp/geglu/proj/bias"], Pm)
-    y3 = lin(hg[:, :4 * c] * gelu_erf(hg[:, 4 * c:]), f"{t}/mlp/lin", Pm, y2)
+    hg = ln_fold(y2, "norm3", W[f"{t}/mlp/geglu/proj/weight"], W[f"{t}/mlp/geglu/proj/bias"], P)
+    y3 = lin(hg[:, :4 * c] * gelu_erf(hg[:, 4 * c:]), f"{t}/mlp/lin", P, y2)
     # proj_out + the block input
     po = act(y3, P) @ wgt(W[f"{name}/proj_out/weight"].reshape(c, c), P).T + W[f"{name}/proj_out/bias"]
     out = x + po.reshape(n, h, w, c).permute(0, 3, 1, 2)

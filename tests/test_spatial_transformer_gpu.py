@@ -55,7 +55,6 @@ TOL = {
     (3, "default"): dict(y=(7.1e-6, 2.4e-4, 3.8e-4, 4.2e-4), add=(4.8e-4, 7.0e-4, 5.3e-4, 4.2e-4), out=(3.3e-4, 5.1e-4)),
     (3, "gn_epilogue=0"): dict(y=(7.1e-6, 2.4e-4, 3.8e-4, 4.3e-4), add=(4.8e-4, 7.0e-4, 5.3e-4, 4.3e-4), out=(3.3e-4, 5.1e-4)),
     (3, "attn_split=0"): dict(y=(7.1e-6, 2.7e-4, 5.3e-4, 5.9e-4), add=(5.2e-4, 1.0e-3, 7.4e-4, 5.9e-4), out=(4.6e-4, 8.0e-4)),
-    (3, "mlp_passes=1"): dict(y=(7.1e-6, 2.4e-4, 3.8e-4, 7.3e-4), add=(4.8e-4, 7.0e-4, 1.3e-3, 7.3e-4), out=(5.8e-4, 7.2e-4)),
     (3, "precision=3"): dict(y=(1.4e-5, 3.6e-4, 6.8e-4, 7.4e-4), add=(6.5e-4, 1.4e-3, 9.5e-4, 7.4e-4), out=(6.1e-4, 1.0e-3)),
     (3, "r=4"): dict(y=(8.8e-7, 5.7e-5, 1.1e-4, 1.4e-4), add=(4.1e-4, 6.7e-4, 5.2e-4, 1.4e-4), out=(1.4e-4, 2.6e-4)),
     (3, "r=16"): dict(y=(2.8e-7, 1.7e-5, 3.3e-5, 4.2e-5), add=(5.0e-4, 7.0e-4, 5.7e-4, 4.3e-5), out=(4.2e-5, 9.3e-5)),
@@ -66,7 +65,7 @@ TOL = {
     (1, "r=16"): dict(y=(8.2e-7, 6.6e-5, 2.8e-4, 6.2e-4), add=(1.5e-3, 7.5e-3, 1.2e-2, 1.0e-3), out=(1.0e-3, 1.6e-3)),
 }
 TOL_LN = 7e-7  # LayerNorm row sums against fp64 sums of the y they describe
-OPTION_DEFAULTS = {"precision": 0, "attn_split": 1, "mlp_passes": 0, "gn_epilogue": 1}
+OPTION_DEFAULTS = {"precision": 0, "attn_split": 1, "gn_epilogue": 1}
 
 
 def rel(a, b):
@@ -115,13 +114,12 @@ def case_inputs(name):
 
 
 def effective(idx, opts):
-    """(passes of the block GEMMs, passes of the MLP pair, split q / k) the options select on block `idx`"""
+    """(passes of the block GEMMs, split q / k) the options select on block `idx`"""
     level_p = BLOCKS[idx][2]
     prec = opts.get("precision", 0)
     P = prec or level_p
-    Pm = prec or opts.get("mlp_passes", 0) or level_p
     qk = (level_p >= 2 or prec >= 2) and opts.get("attn_split", 1) == 1 and DPAD[BLOCKS[idx][1]] in (48, 80)
-    return P, Pm, qk
+    return P, qk
 
 
 _REF = {}
@@ -142,7 +140,7 @@ def expect_trace(name, tr, opts):
     idx, h, w, n, lens, _ = CASES[name]
     c = BLOCKS[idx][1]
     hw, dpad = h * w, DPAD[c]
-    P, Pm, qk = effective(idx, opts)
+    P, qk = effective(idx, opts)
     gn_epi = opts.get("gn_epilogue", 1)
     # proj_out's GroupNorm partials over flattened token rows: whole 128-row tiles of one image, or 2 / 4 images per tile
     slots = (hw // 128 if hw % 128 == 0 else (1 if 128 % hw == 0 and hw >= 32 else 0)) if gn_epi else 0
@@ -151,7 +149,7 @@ def expect_trace(name, tr, opts):
     roles = [{"lns"}, {"lnc"}, {"res16", "lns"}, {"lnc"}, {"res16", "lns"}, {"lnc", "geglu"}, {"res16"},
              {"res32"} | ({"gn"} if slots else set())]
     assert [x["epi"] for x in g] == roles, [x["epi"] for x in g]
-    assert [x["passes"] for x in g] == [P] * 5 + [Pm] * 2 + [P]
+    assert [x["passes"] for x in g] == [P] * 8
     assert [x["N"] for x in g] == [c, 3 * 8 * dpad, c, 8 * dpad, c, 8 * c, c, c]
     assert g[7]["gn_slots"] == slots, (g[7]["gn_slots"], slots)
     lpad = -(-max(lens) // 32) * 32
@@ -176,11 +174,11 @@ class Options:
 def check(ctx, W, name, variant, r_key=0, **opts):
     idx, h, w, n, lens, act16 = CASES[name]
     c = BLOCKS[idx][1]
-    P, Pm, qk = effective(idx, opts)
+    P, qk = effective(idx, opts)
     x, ctxt, lens = case_inputs(name)
     with Options(ctx, **opts):
         res = ctx.test_spatial_transformer(idx, x, ctxt, lens, act16=act16)
-    ref, ys = reference(W, name, r_key, x, ctxt, lens, S.Rounding.of(P, Pm, qk))
+    ref, ys = reference(W, name, r_key, x, ctxt, lens, S.Rounding.of(P, qk))
     out = res["out"]
     e = rel(out, ref)
     emax = float(np.abs(out - ref).max() / np.abs(ref).max())
@@ -200,7 +198,7 @@ def check(ctx, W, name, variant, r_key=0, **opts):
                                                                                 W[f"{BLOCKS[idx][0]}/norm/bias"]))
     refn = F.silu(F.group_norm(torch.from_numpy(out.astype(np.float64)), 32, gamma, beta, 1e-5)).numpy()
     en = rel(res["out_norm"], refn)
-    print(f"st {name} [{variant}] P={P} Pm={Pm} qk3={int(qk)} |mu|/sd {mus:.2f}: out rel L2 {e:.3e} max {emax:.3e} | "
+    print(f"st {name} [{variant}] P={P} qk3={int(qk)} |mu|/sd {mus:.2f}: out rel L2 {e:.3e} max {emax:.3e} | "
           f"y proj_in {ey[0]:.3e} attn1 {ey[1]:.3e} attn2 {ey[2]:.3e} mlp {ey[3]:.3e} | added attn1 {ed[0]:.3e} "
           f"attn2 {ed[1]:.3e} mlp {ed[2]:.3e} proj_out {ed[3]:.3e} | LN sums {max(eln):.2e} | GN(out) {en:.2e}")
     tol = TOL[(P, variant)]
@@ -230,11 +228,6 @@ def test_spatial_transformer_default(ctx, blocks, name):
 def test_spatial_transformer_single_fp16_qk(ctx, blocks, name):
     """levels 0-1 with the attention on single fp16 q / k (the 1 x 1 logits product)"""
     check(ctx, blocks[CASES[name][0]], name, "attn_split=0", attn_split=0)
-
-
-@pytest.mark.parametrize("name", L01)
-def test_spatial_transformer_mlp_single_pass(ctx, blocks, name):
-    check(ctx, blocks[CASES[name][0]], name, "mlp_passes=1", mlp_passes=1)
 
 
 @pytest.mark.parametrize("name", L2MID)

@@ -68,7 +68,7 @@ def test_reference_rounding_matches_oracle_emulation():
         O.set_emulation("fp16", "awAWq")
         O.set_emulation_fn(lambda blk, name, role: None if name and "/attn2/key" in name or name and "/attn2/value" in name else "fp16")
         O._EMU["ln_fused"] = True
-        ref, _, ora = run_both(a, x, ctx, (6, 6), S.Rounding.of(1, 1, False))
+        ref, _, ora = run_both(a, x, ctx, (6, 6), S.Rounding.of(1, False))
     finally:
         O._EMU.clear()
         O._EMU.update(saved)
