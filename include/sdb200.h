@@ -290,34 +290,41 @@ int sdb_profile_get_issued(sdb_ctx* ctx, int cls, double* issued_flops);
 /* Number of kernel launches issued by this context since creation (sdb_profile_reset zeroes it). */
 int64_t sdb_launch_count(sdb_ctx* ctx);
 
-/* ---- unit-test entry points for single kernels (device pointers) ----------------------------- */
+/* ---- unit-test entry points for single kernels (host pointers) ------------------------------- */
+/* The GEMM test entries below (sdb_test_linear, sdb_test_gemm_ex, sdb_test_conv2d, sdb_test_ln_fold, sdb_test_conv_groupnorm)
+ * take a trailing `trace`: NULL, or SDB_GEMM_TRACE_INTS ints that receive what each GEMM of the call launched, so a test can
+ * assert which kernel instance it reached. [0] GEMMs, then 14 ints each from [1] (at most 4 GEMMs): the 13 of
+ * sdb_test_clip_block (kind, N, BN, split-K, TN, TH, TW, extra-K channels, GroupNorm slots written, second-source channels,
+ * passes, epilogue roles, activation), then the pipeline stages of the kernel instance. */
+#define SDB_GEMM_TRACE_INTS 64
 /* C[M,N] (fp32) = A[M,K] (fp32, rounded to the operand format) x B[K,N] (fp32 [in,out]) + bias.
  * Exercises the wgmma GEMM exactly as the Linear layers use it. */
 int sdb_test_linear(sdb_ctx* ctx, const float* a, const float* w, const float* bias, int M, int K, int N,
-                    int passes, float* c);
+                    int passes, float* c, int32_t* trace);
 /* The GEMM's other epilogues and K-loop forms, each reachable in isolation: out = A[M,K] x W[K,N] (+ bias) (+ residual[M,N])
  * (+ XA[M,XK] x XW[XK,N], the "extra K" operands the ResBlock skip conv rides on). flags: 1 = GEGLU (W = [K][x | gate], out
- * [M, N/2] = (x + b_x) * gelu_erf(gate + b_g), unet/mod.rs:578-592); 4 = read the result back from the fp16 hi + lo outputs.
- * Split-K is chosen by the library's own policy (small M x N grid, K >= 2048). */
+ * [M, N/2] = (x + b_x) * gelu_erf(gate + b_g), unet/mod.rs:578-592); 4 = read the result back from the fp16 hi + lo outputs;
+ * 8 (with 4) = return the two fp16 planes separately: out = [2][M][N (or N/2)], hi then lo, each value converted to float.
+ * Split-K is chosen by the library's own policy (small M x N grid, long K). */
 int sdb_test_gemm_ex(sdb_ctx* ctx, const float* a, const float* w, const float* bias, const float* residual, int M, int K,
-                     int N, int passes, int flags, const float* xa, const float* xw, int XK, float* out);
+                     int N, int passes, int flags, const float* xa, const float* xw, int XK, float* out, int32_t* trace);
 /* conv2d NCHW fp32 in/out through the implicit-GEMM path (3x3 pad 1 stride 1|2, or 1x1). */
 int sdb_test_conv2d(sdb_ctx* ctx, const float* x, const float* w, const float* bias, int n, int cin, int H,
-                    int W, int cout, int ksize, int stride, int upsample, int passes, float* y);
+                    int W, int cout, int ksize, int stride, int upsample, int passes, float* y, int32_t* trace);
 /* The LayerNorm-free TransformerBlock chain in isolation (unet/mod.rs:521-527): y = a w0 + b0 (+ a2 w0 + b0 accumulated in place
  * on the fp16 hi/lo residual pair; a2 may be NULL) with row statistics from the producing epilogue, then
  * out = LayerNorm(y; gamma, beta) w1 + b1 with the LayerNorm folded into the consuming GEMM (gamma in the weights, rank-1
  * correction in the epilogue); geglu = 1: w1 = [C][x | gate], out [M, N/2] = x * gelu(gate). C a multiple of 160. */
 int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float* w0, const float* b0, const float* gamma,
                      const float* beta, const float* w1, const float* b1, int M, int K0, int C, int N, int passes, int geglu,
-                     float* out);
+                     float* out, int32_t* trace);
 /* conv (3x3 pad 1 or 1x1) whose epilogue also leaves the GroupNorm statistics of its output, followed by the apply-only
  * GroupNorm(+SiLU) that consumes them (the ResBlock's conv_in -> norm_out -> SiLU chain, unet/mod.rs:716-725). stride 2 (3x3)
  * is the UNet downsample conv, upsample = 1 (3x3) the folded nearest-2x + conv of the upsample blocks. NCHW fp32 in/out;
  * *slots = partial-statistics slots per image the GEMM wrote (> 0). */
 int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const float* bias, const float* gamma,
                             const float* beta, int n, int cin, int H, int W, int cout, int ksize, int stride, int upsample,
-                            int passes, int silu, float* y, int* slots);
+                            int passes, int silu, float* y, int* slots, int32_t* trace);
 /* GroupNorm(32 groups)+optional SiLU, NCHW fp32 in/out. */
 int sdb_test_groupnorm(sdb_ctx* ctx, const float* x, const float* gamma, const float* beta, int n, int c,
                        int H, int W, int silu, float* y);

@@ -59,7 +59,7 @@ SIGNATURES = [
     ("sdb_forward_diffuser_dev", C.c_int, [_ctx, C.c_void_p, C.c_int32, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                            C.c_double, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     ("sdb_test_gemm_ex", C.c_int, [_ctx, _f32p, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, _f32p,
-                                   C.c_int, _f32p]),
+                                   C.c_int, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_read_dump_tensor", C.c_int64, [C.c_char_p, C.c_int, C.POINTER(C.c_int64), _f32p, C.c_int64]),
     ("sdb_encode_image", C.c_int, [_ctx, _f32p, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_encode_image_dev", C.c_int, [_ctx, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
@@ -98,13 +98,14 @@ SIGNATURES = [
                                   C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     ("sdb_profile_get_issued", C.c_int, [_ctx, C.c_int, C.POINTER(C.c_double)]),
     ("sdb_launch_count", C.c_int64, [_ctx]),
-    ("sdb_test_linear", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
+    ("sdb_test_linear", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_conv2d", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                  C.c_int, C.c_int, C.c_int, _f32p]),
+                                  C.c_int, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_ln_fold", C.c_int, [_ctx, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int,
-                                   C.c_int, C.c_int, _f32p]),
+                                   C.c_int, C.c_int, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_conv_groupnorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                          C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int)]),
+                                          C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int),
+                                          C.POINTER(C.c_int32)]),
     ("sdb_test_resblock", C.c_int, [_ctx, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                     _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p,
                                     C.c_int, C.c_int, _f32p, _f32p, _f32p, C.POINTER(C.c_int32)]),
@@ -574,29 +575,58 @@ class Context:
         return int(self.lib.sdb_launch_count(self.h))
 
     # ---- single-kernel test entries
-    def test_linear(self, a, w, bias=None, passes=1):
+    # The GEMM entries take trace=True to also return what each of their GEMMs launched (include/sdb200.h: SDB_GEMM_TRACE_INTS):
+    # a list of dicts with the keys below, "epi" as the set of _EPI_ROLES names.
+    GEMM_TRACE_INTS = 64
+    _GEMM_TRACE_KEYS = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1", "passes", "epi", "act", "stages")
+
+    @staticmethod
+    def _trace_buf(trace):
+        if not trace:
+            return None, None
+        t = np.zeros(Context.GEMM_TRACE_INTS, np.int32)
+        return t, t.ctypes.data_as(C.POINTER(C.c_int32))
+
+    @classmethod
+    def _decode_gemm_trace(cls, t):
+        gemms = []
+        for i in range(int(t[0])):
+            g = dict(zip(cls._GEMM_TRACE_KEYS, (int(v) for v in t[1 + 14 * i:15 + 14 * i])))
+            g["epi"] = {r for b, r in enumerate(cls._EPI_ROLES) if g["epi"] >> b & 1}
+            gemms.append(g)
+        return gemms
+
+    def test_linear(self, a, w, bias=None, passes=1, trace=False):
         a = f32(a); w = f32(w)
         M, K = a.shape; N = w.shape[1]
         out = np.empty((M, N), np.float32)
         b = f32(bias) if bias is not None else None
-        self.check(self.lib.sdb_test_linear(self.h, ptr(a), ptr(w), ptr(b) if b is not None else None, M, K, N, passes, ptr(out)))
-        return out
+        t, tp = self._trace_buf(trace)
+        self.check(self.lib.sdb_test_linear(self.h, ptr(a), ptr(w), ptr(b) if b is not None else None, M, K, N, passes, ptr(out),
+                                            tp))
+        return (out, self._decode_gemm_trace(t)) if trace else out
 
-    def test_gemm_ex(self, a, w, bias=None, residual=None, passes=1, geglu=False, from_f16=False, xa=None, xw=None):
+    def test_gemm_ex(self, a, w, bias=None, residual=None, passes=1, geglu=False, from_f16=False, xa=None, xw=None,
+                     planes=False, trace=False):
+        """planes: return the fp16 outputs as the pair (hi, lo) of float arrays instead of hi + lo (implies from_f16)."""
         a = f32(a); w = f32(w)
         M, K = a.shape; N = w.shape[1]
-        out = np.empty((M, N // 2 if geglu else N), np.float32)
+        shape = (M, N // 2 if geglu else N)
+        out = np.empty((2, *shape) if planes else shape, np.float32)
         opt = lambda v: (None, None) if v is None else (f32(v), ptr(f32(v)))
         keep = [opt(bias), opt(residual), opt(xa), opt(xw)]
         for i, (arr, _) in enumerate(keep):  # keep the contiguous copies alive across the call
             if arr is not None:
                 keep[i] = (arr, ptr(arr))
         XK = 0 if xa is None else keep[2][0].shape[1]
-        self.check(self.lib.sdb_test_gemm_ex(self.h, ptr(a), ptr(w), keep[0][1], keep[1][1], M, K, N, passes,
-                                             (1 if geglu else 0) | (4 if from_f16 else 0), keep[2][1], keep[3][1], XK, ptr(out)))
-        return out
+        flags = (1 if geglu else 0) | (4 if (from_f16 or planes) else 0) | (8 if planes else 0)
+        t, tp = self._trace_buf(trace)
+        self.check(self.lib.sdb_test_gemm_ex(self.h, ptr(a), ptr(w), keep[0][1], keep[1][1], M, K, N, passes, flags, keep[2][1],
+                                             keep[3][1], XK, ptr(out), tp))
+        res = (out[0], out[1]) if planes else out
+        return (res, self._decode_gemm_trace(t)) if trace else res
 
-    def test_conv2d(self, x, w, bias=None, stride=1, upsample=0, passes=1):
+    def test_conv2d(self, x, w, bias=None, stride=1, upsample=0, passes=1, trace=False):
         x = f32(x); w = f32(w)
         n, cin, H, W = x.shape
         cout, _, k, _ = w.shape
@@ -604,22 +634,24 @@ class Context:
         Wo = 2 * W if upsample else (W // 2 if stride == 2 else W)
         y = np.empty((n, cout, Ho, Wo), np.float32)
         b = f32(bias) if bias is not None else None
+        t, tp = self._trace_buf(trace)
         self.check(self.lib.sdb_test_conv2d(self.h, ptr(x), ptr(w), ptr(b) if b is not None else None, n, cin, H, W, cout,
-                                            k, stride, upsample, passes, ptr(y)))
-        return y
+                                            k, stride, upsample, passes, ptr(y), tp))
+        return (y, self._decode_gemm_trace(t)) if trace else y
 
-    def test_ln_fold(self, a, w0, b0, gamma, beta, w1, b1=None, a2=None, passes=3, geglu=False):
+    def test_ln_fold(self, a, w0, b0, gamma, beta, w1, b1=None, a2=None, passes=3, geglu=False, trace=False):
         a, w0, b0, gamma, beta, w1 = (f32(v) for v in (a, w0, b0, gamma, beta, w1))
         b1 = f32(b1) if b1 is not None else None
         a2 = f32(a2) if a2 is not None else None
         M, K0 = a.shape; Cc = w0.shape[1]; N = w1.shape[1]
         out = np.empty((M, N // 2 if geglu else N), np.float32)
+        t, tp = self._trace_buf(trace)
         self.check(self.lib.sdb_test_ln_fold(self.h, ptr(a), ptr(a2) if a2 is not None else None, ptr(w0), ptr(b0), ptr(gamma),
                                              ptr(beta), ptr(w1), ptr(b1) if b1 is not None else None, M, K0, Cc, N, passes,
-                                             1 if geglu else 0, ptr(out)))
-        return out
+                                             1 if geglu else 0, ptr(out), tp))
+        return (out, self._decode_gemm_trace(t)) if trace else out
 
-    def test_conv_groupnorm(self, x, w, bias, gamma, beta, passes=3, silu=False, stride=1, upsample=0):
+    def test_conv_groupnorm(self, x, w, bias, gamma, beta, passes=3, silu=False, stride=1, upsample=0, trace=False):
         x = f32(x); w = f32(w); bias = f32(bias); gamma = f32(gamma); beta = f32(beta)
         n, cin, H, W = x.shape
         cout, _, k, _ = w.shape
@@ -627,9 +659,10 @@ class Context:
         Wo = 2 * W if upsample else (W // 2 if stride == 2 else W)
         y = np.empty((n, cout, Ho, Wo), np.float32)
         slots = C.c_int()
+        t, tp = self._trace_buf(trace)
         self.check(self.lib.sdb_test_conv_groupnorm(self.h, ptr(x), ptr(w), ptr(bias), ptr(gamma), ptr(beta), n, cin, H, W, cout, k,
-                                                    stride, upsample, passes, 1 if silu else 0, ptr(y), C.byref(slots)))
-        return y, slots.value
+                                                    stride, upsample, passes, 1 if silu else 0, ptr(y), C.byref(slots), tp))
+        return (y, slots.value, self._decode_gemm_trace(t)) if trace else (y, slots.value)
 
     @staticmethod
     def _decode_trace(t):

@@ -615,10 +615,37 @@ int64_t sdb_launch_count(sdb_ctx* ctx) { return ctx ? ctx->c.launches : -1; }
 
 // ------------------------------------------------------------------------------ single-kernel test entries
 // (host pointers; each call stages through the context's work arena)
+
+// The GEMM launch record of one test call (trace = NULL or SDB_GEMM_TRACE_INTS ints, include/sdb200.h): [0] GEMMs, then per GEMM
+// the 13 ints of Ctx::GemmRecord and the stage count of the kernel instance run_gemm chose.
+struct GemmTraceScope {
+  static constexpr int kPer = 14, kMax = (SDB_GEMM_TRACE_INTS - 1) / kPer;
+  Ctx& c;
+  int32_t* out;
+  GemmTraceScope(Ctx& c, int32_t* out) : c(c), out(out) {
+    c.gemm_trace.clear();
+    c.trace_on = out != nullptr;
+  }
+  ~GemmTraceScope() { c.trace_on = false; }
+  void write() const {
+    if (!out) return;
+    SDB_CHECK((int)c.gemm_trace.size() <= kMax, "GEMM trace: too many GEMMs for the trace");
+    std::fill(out, out + SDB_GEMM_TRACE_INTS, 0);
+    out[0] = (int)c.gemm_trace.size();
+    for (size_t i = 0; i < c.gemm_trace.size(); ++i) {
+      const Ctx::GemmRecord& r = c.gemm_trace[i];
+      const int v[kPer] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels, r.passes, r.epi,
+                           r.act, gemm_tc_stages(r.BN, r.passes)};
+      std::copy(v, v + kPer, out + 1 + kPer * i);
+    }
+  }
+};
+
 int sdb_test_linear(sdb_ctx* ctx, const float* a, const float* w, const float* bias, int M, int K, int N, int passes,
-                    float* out) {
+                    float* out, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
+  GemmTraceScope ts(c, trace);
   float* d_a = c.work.get<float>((size_t)M * K);
   float* d_w = c.work.get<float>((size_t)K * N);
   float* d_b = bias ? c.work.get<float>(N) : nullptr;
@@ -642,14 +669,17 @@ int sdb_test_linear(sdb_ctx* ctx, const float* a, const float* w, const float* b
   run_gemm(c, G_LINEAR, A, nullptr, Wp, passes, ep);
   SDB_CUDA(cudaMemcpyAsync(out, d_c, sizeof(float) * M * N, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
+  ts.write();
   API_END
 }
 
 int sdb_test_gemm_ex(sdb_ctx* ctx, const float* a, const float* w, const float* bias, const float* residual, int M, int K, int N,
-                     int passes, int flags, const float* xa, const float* xw, int XK, float* out) {
+                     int passes, int flags, const float* xa, const float* xw, int XK, float* out, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  const bool geglu = flags & 1, from_f16 = flags & 4;
+  GemmTraceScope ts(c, trace);
+  const bool geglu = flags & 1, from_f16 = flags & 4, planes = flags & 8;
+  SDB_CHECK(!planes || from_f16, "gemm_ex test: the separate fp16 planes (flag 8) need the fp16 outputs (flag 4)");
   SDB_CHECK(!geglu || (N % 128 == 0 && !residual && !xa), "GEGLU test: N (= 2 * hidden) must be a multiple of 128, no residual / extra K");
   const int Nout = geglu ? N / 2 : N;
   auto up = [&](const float* h, size_t cnt) {
@@ -701,18 +731,23 @@ int sdb_test_gemm_ex(sdb_ctx* ctx, const float* a, const float* w, const float* 
     SDB_CUDA(cudaMemcpyAsync(hi.data(), o16.hi, hi.size() * 2, cudaMemcpyDeviceToHost, c.stream));
     SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, lo.size() * 2, cudaMemcpyDeviceToHost, c.stream));
     SDB_CUDA(cudaStreamSynchronize(c.stream));
-    for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
+    if (planes)
+      for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]), out[hi.size() + i] = __half2float(lo[i]);
+    else
+      for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
   } else {
     SDB_CUDA(cudaMemcpyAsync(out, d_c, sizeof(float) * M * Nout, cudaMemcpyDeviceToHost, c.stream));
     SDB_CUDA(cudaStreamSynchronize(c.stream));
   }
+  ts.write();
   API_END
 }
 
 int sdb_test_conv2d(sdb_ctx* ctx, const float* x, const float* w, const float* bias, int n, int cin, int H, int W,
-                    int cout, int ksize, int stride, int upsample, int passes, float* y) {
+                    int cout, int ksize, int stride, int upsample, int passes, float* y, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
+  GemmTraceScope ts(c, trace);
   SDB_CHECK(ksize == 1 || ksize == 3, "ksize");
   SDB_CHECK(stride == 1 || (stride == 2 && ksize == 3 && !upsample), "stride");
   const int Hin = H, Win = W;
@@ -767,14 +802,16 @@ int sdb_test_conv2d(sdb_ctx* ctx, const float* x, const float* w, const float* b
   nhwc_to_nchw_launch(d_yh, n, cout, Ho, Wo, d_y, c.stream);
   SDB_CUDA(cudaMemcpyAsync(y, d_y, sizeof(float) * yout, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
+  ts.write();
   API_END
 }
 
 int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float* w0, const float* b0, const float* gamma,
                      const float* beta, const float* w1, const float* b1, int M, int K0, int C, int N, int passes, int geglu,
-                     float* out) {
+                     float* out, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
+  GemmTraceScope ts(c, trace);
   SDB_CHECK(C % 160 == 0 && K0 % 64 == 0 && (!geglu || (N % 128 == 0 && b1)), "ln_fold test shapes");
   auto up = [&](const float* h, size_t cnt) {
     float* d = c.work.get<float>(cnt);
@@ -832,14 +869,16 @@ int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float*
   SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, lo.size() * 2, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
   for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
+  ts.write();
   API_END
 }
 
 int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const float* bias, const float* gamma, const float* beta,
                             int n, int cin, int H, int W, int cout, int ksize, int stride, int upsample, int passes, int silu,
-                            float* y, int* used_epilogue_stats) {
+                            float* y, int* used_epilogue_stats, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
+  GemmTraceScope ts(c, trace);
   SDB_CHECK(ksize == 1 || ksize == 3, "ksize");
   SDB_CHECK((stride == 1 && (upsample == 0 || (upsample == 1 && ksize == 3))) || (stride == 2 && ksize == 3 && !upsample),
             "stride / upsample");
@@ -899,6 +938,7 @@ int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const 
   nhwc_to_nchw_launch(d_yh, n, cout, Ho, Wo, d_y, c.stream);
   SDB_CUDA(cudaMemcpyAsync(y, d_y, sizeof(float) * yout, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
+  ts.write();
   API_END
 }
 

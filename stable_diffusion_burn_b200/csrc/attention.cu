@@ -356,10 +356,9 @@ attention_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__
         const int col = 8 * (i >> 2) + cl;
         if (col < p.d) {
           const float f0 = o[i] * inv_l[hh], f1 = o[i + 1] * inv_l[hh];
-          const __half2 hi = __floats2half2_rn(f0, f1);
-          const float2 hf = __half22float2(hi);
-          *reinterpret_cast<__half2*>(p.out_hi + orow + col) = hi;
-          if (p.out_lo) *reinterpret_cast<__half2*>(p.out_lo + orow + col) = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
+          const HalfPair2 sp = split_f16x2(f0, f1);
+          *reinterpret_cast<__half2*>(p.out_hi + orow + col) = sp.hi;
+          if (p.out_lo) *reinterpret_cast<__half2*>(p.out_lo + orow + col) = sp.lo;
         }
       }
     }

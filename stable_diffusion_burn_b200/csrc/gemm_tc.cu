@@ -8,7 +8,7 @@
 //   warpgroup 0    : TMA producer (warp 0: cp.async.bulk.tensor 5-D activation boxes + 2-D weight boxes; warps 1-3 idle)
 //   warpgroups 1-2 : consumers. Each issues wgmma m64nBNk16 (fp16 x fp16 -> fp32 in registers) for 64 of the 128 rows, then
 //                    both write the accumulator to shared memory as a row-major fp32 image and run the epilogue from it
-//                    (bias / time-embedding row / residual / GEGLU / statistics -> global)
+//                    (bias / residual / GEGLU / statistics -> global)
 // Multi-pass products (PASSES = 2, 3) add the low-order fp16 halves of the operands
 // (A_lo*B_hi, A_hi*B_lo) into the same accumulator for fp32-class accuracy.
 #include "gemm_tc.cuh"
@@ -50,11 +50,11 @@ __device__ __noinline__ void epilogue_store(float4 f, unsigned int o32, unsigned
   }
   if (out_f32) *reinterpret_cast<float4*>(out_f32 + o32) = f;
   if (out_f16) {
-    __half2 h[2] = {f2h2_sat(f.x, f.y), f2h2_sat(f.z, f.w)};
+    const HalfPair2 s0 = split_f16x2(f.x, f.y), s1 = split_f16x2(f.z, f.w);
+    __half2 h[2] = {s0.hi, s1.hi};
     *reinterpret_cast<uint2*>(out_f16 + o16) = *reinterpret_cast<uint2*>(h);
     if (out_f16_lo) {
-      const float2 f0 = __half22float2(h[0]), f1 = __half22float2(h[1]);
-      __half2 l[2] = {__floats2half2_rn(f.x - f0.x, f.y - f0.y), __floats2half2_rn(f.z - f1.x, f.w - f1.y)};
+      __half2 l[2] = {s0.lo, s1.lo};
       *reinterpret_cast<uint2*>(out_f16_lo + o16) = *reinterpret_cast<uint2*>(l);
     }
   }
@@ -179,7 +179,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   // previous kernel (griddepcontrol.wait) only where it first touches data that kernel may have written:
   //   producer : WEIGHTS are immutable, so the weight tiles of the first STAGES k-chunks are issued BEFORE the wait; activation
   //              tiles after it
-  //   consumers: wait before the epilogue's first read of residual / time-embedding rows; all of this kernel's stores follow it
+  //   consumers: wait before the epilogue's first read of residual rows; all of this kernel's stores follow it
   if (warp == 0) {
     // ===================================================== TMA producer (one elected lane: see elect_one in common.cuh)
     if (elect_one()) {
@@ -234,7 +234,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     }
   } else if (warp >= 4) {
     // ===================================================== consumers: wgmma mainloop, then the epilogue
-    pdl_wait();  // residual / time-embedding rows below may come from the previous kernel; every store of this kernel follows
+    pdl_wait();  // residual rows below may come from the previous kernel; every store of this kernel follows
     const int wg = (warp - 4) >> 2;  // rows [64 wg, 64 wg + 64) of the tile
     {
       float acc[BN / 2];
@@ -297,15 +297,13 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     const int m = row_ok ? ((pn * p.OH + phh * p.os + p.oa + up_a) * p.OW + pw * p.os + p.ob + up_b) : -1;
 
     // ---- work that needs no accumulator, done while the main loop runs: the element offsets of the 8 rows this lane
-    // serves in every column chunk (rr = 4 i + sub), the bias of each chunk, and the first chunk's addends (residual or
-    // time-embedding row; run_gemm guarantees at most one of them). The epilogue is a chain of L2 round trips: everything
-    // issued here is off that chain.
+    // serves in every column chunk (rr = 4 i + sub), the bias of each chunk, and the first chunk's residual addends. The
+    // epilogue is a chain of L2 round trips: everything issued here is off that chain.
     const int sub = lane >> 3;          // row within a group of 4
     const int cq = (lane & 7) * 4;      // 4-column group inside the 32-column chunk
     constexpr int NCHUNK = (BN + CSTEP - 1) / CSTEP;
     int mr8[8], ao[8];
     float4 bvs[NCHUNK], ad[8];
-    const float* ad_ptr = p.residual ? p.residual : p.rowbias;
     const bool res_pair = p.res_hi != nullptr;  // the residual lives as an fp16 hi + lo pair (row stride ldc16)
     const bool plain = p.split_k == 1 && !kGEGLU;
     // EPI_LNC: mean / rstd of this lane's own accumulator row, from the partial row sums the producer of A left
@@ -326,14 +324,12 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       }
     }
     {
-      const bool use_res = p.residual != nullptr;
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int rr = i * 4 + sub;
         const int mr = __shfl_sync(0xffffffffu, m, rr);
-        const int pnr = __shfl_sync(0xffffffffu, pn, rr);
         mr8[i] = mr;
-        ao[i] = res_pair ? mr * p.ldc16 : (use_res ? mr * p.ldc : pnr * p.N);
+        ao[i] = res_pair ? mr * p.ldc16 : mr * p.ldc;
         ad[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         if constexpr (kLNC) mu8[i] = __shfl_sync(0xffffffffu, ln_mu, rr), rs8[i] = __shfl_sync(0xffffffffu, ln_rs, rr);
       }
@@ -353,7 +349,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       }
     }
     auto issue_addends = [&](int col) {
-      if constexpr (kLNC) return;  // a LayerNorm-consuming GEMM has neither residual nor row bias (run_gemm checks): no registers for them
+      if constexpr (kLNC) return;  // a LayerNorm-consuming GEMM has no residual (run_gemm checks): no registers for them
       if (col >= p.N) return;
       if (res_pair) {
 #pragma unroll
@@ -367,10 +363,10 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
           }
         return;
       }
-      if (ad_ptr == nullptr) return;
+      if (p.residual == nullptr) return;
 #pragma unroll
       for (int i = 0; i < 8; ++i)
-        if (mr8[i] >= 0) ad[i] = *reinterpret_cast<const float4*>(ad_ptr + (unsigned)(ao[i] + col));
+        if (mr8[i] >= 0) ad[i] = *reinterpret_cast<const float4*>(p.residual + (unsigned)(ao[i] + col));
     };
     // the residual may be produced by the previous kernel (always complete: stream order) or be this launch's own
     // output buffer written by an EARLIER launch (in-place accumulate): both are safe to read before the MMAs finish
@@ -447,9 +443,8 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
           if (qw < p.W && qh < p.H && qn < p.nimg && col < p.N) {
             const int mr = (qn * p.OH + qh * p.os + p.oa) * p.OW + qw * p.os + p.ob;
             // the addends first, then the partials four at a time: independent loads in flight together, summed in z order
-            float4 bv = make_float4(0.f, 0.f, 0.f, 0.f), rb = bv, rs = bv;
+            float4 bv = make_float4(0.f, 0.f, 0.f, 0.f), rs = bv;
             if (p.bias) bv = *reinterpret_cast<const float4*>(p.bias + col);
-            if (p.rowbias) rb = *reinterpret_cast<const float4*>(p.rowbias + (size_t)qn * p.N + col);
             if (p.residual) rs = *reinterpret_cast<const float4*>(p.residual + (size_t)mr * p.ldc + col);
             if (p.res_hi) {
               const uint2 h = *reinterpret_cast<const uint2*>(p.res_hi + (size_t)mr * p.ldc16 + col);
@@ -478,8 +473,8 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
               const float4 v = __ldcg(reinterpret_cast<const float4*>(wp + (size_t)z * zs));
               acc.x += v.x, acc.y += v.y, acc.z += v.z, acc.w += v.w;
             }
-            acc.x += bv.x + rb.x + rs.x, acc.y += bv.y + rb.y + rs.y;
-            acc.z += bv.z + rb.z + rs.z, acc.w += bv.w + rb.w + rs.w;
+            acc.x += bv.x + rs.x, acc.y += bv.y + rs.y;
+            acc.z += bv.z + rs.z, acc.w += bv.w + rs.w;
             if constexpr (kGN) {
               gsum.x += acc.x, gsum.y += acc.y, gsum.z += acc.z, gsum.w += acc.w;
               gsq.x = fmaf(acc.x, acc.x, gsq.x), gsq.y = fmaf(acc.y, acc.y, gsq.y), gsq.z = fmaf(acc.z, acc.z, gsq.z), gsq.w = fmaf(acc.w, acc.w, gsq.w);
@@ -685,7 +680,7 @@ static void launch_epi(const GemmMaps& maps, const GemmParams& p, cudaStream_t s
   dim3 grid(p.tiles_n * p.tiles_h * p.tiles_w, (p.N + BN - 1) / BN, p.up2 ? 4 : p.split_k);
   launch_k(gemm_tc_kernel<BN, PASSES, STAGES, EPI>, grid, dim3(128 + 32 * EW), (size_t)smem, stream, maps, p);
 }
-// the statistics-producing epilogues exist for the tile widths their tensors use (run_gemm checks with gemm_tc_supports_epi)
+// the statistics-producing epilogues exist for the tile widths their tensors use (run_gemm picks those widths for them)
 template <int BN, int PASSES, int STAGES>
 static void launch_inst(const GemmMaps& maps, const GemmParams& p, cudaStream_t stream) {
   SDB_CHECK((p.gn_part != nullptr) + (p.ln_out != nullptr) + (p.ln_in != nullptr) <= 1, "one statistics role per launch");
@@ -709,13 +704,25 @@ static void launch_inst(const GemmMaps& maps, const GemmParams& p, cudaStream_t 
   SDB_CHECK(!p.gn_part && !p.ln_out && !p.ln_in, "this statistics epilogue is not built for this tile width");
   launch_epi<BN, PASSES, STAGES, EPI_PLAIN>(maps, p, stream);
 }
-bool gemm_tc_supports(int BN, int epi) {
-  return epi == EPI_PLAIN || (epi == EPI_GN && BN >= 128) || (epi == EPI_LNS && BN == 160) || (epi == EPI_LNC && (BN == 128 || BN == 160));
-}
 
 template <int BN, int PASSES>
 static void launch_bn(const GemmMaps& maps, const GemmParams& p, cudaStream_t stream) {
   launch_inst<BN, PASSES, pick_stages<BN, PASSES>()>(maps, p, stream);
+}
+
+int gemm_tc_stages(int BN, int passes) {
+  SDB_CHECK(passes >= 1 && passes <= 3, "passes");
+  constexpr int t[4][3] = {{pick_stages<64, 1>(), pick_stages<64, 2>(), pick_stages<64, 3>()},
+                           {pick_stages<128, 1>(), pick_stages<128, 2>(), pick_stages<128, 3>()},
+                           {pick_stages<160, 1>(), pick_stages<160, 2>(), pick_stages<160, 3>()},
+                           {pick_stages<256, 1>(), pick_stages<256, 2>(), pick_stages<256, 3>()}};
+  switch (BN) {
+    case 64: return t[0][passes - 1];
+    case 128: return t[1][passes - 1];
+    case 160: return t[2][passes - 1];
+    case 256: return t[3][passes - 1];
+    default: throw Error("unsupported BN");
+  }
 }
 
 void gemm_tc_launch(const GemmMaps& maps, const GemmParams& p, int BN, int passes, cudaStream_t stream) {

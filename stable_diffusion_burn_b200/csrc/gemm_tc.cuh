@@ -33,7 +33,6 @@ struct GemmParams {
   __half* out_f16;         // [M][ldc16] or null (hi part)
   __half* out_f16_lo;      // residual part for multi-pass consumers, or null
   const float* bias;       // [N] or null
-  const float* rowbias;    // [nimg][N] or null (time embedding row per image)
   const float* residual;   // [M][ldc] or null
   int ldc;                 // row stride of out_f32 / residual (elements)
   int ldc16;               // row stride of out_f16
@@ -66,12 +65,8 @@ struct GemmParams {
   int OH, OW, os, oa, ob;
 };
 
-struct GemmLaunch {
-  int BN, passes, stages;
-};
-
 void gemm_tc_launch(const GemmMaps& maps, const GemmParams& p, int BN, int passes, cudaStream_t stream);
-bool gemm_tc_supports(int BN, int epi);  // epi: 0 plain, 1 GroupNorm statistics, 2 LayerNorm row statistics, 3 LayerNorm consume
-int gemm_tc_smem_bytes(int BN, int passes, int stages);
+// pipeline stages of the (BN, passes) kernel instance: the depth of its shared-memory operand ring
+int gemm_tc_stages(int BN, int passes);
 
 }  // namespace sdb

@@ -11,19 +11,20 @@ namespace sdb {
 static inline int ceil_div(long long a, long long b) { return int((a + b - 1) / b); }
 
 __device__ __forceinline__ void split_store8(const float (&f)[8], __half* hi, __half* lo) {
-  __half2 h[4];
+  __half2 h[4], l[4];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) h[j] = f2h2_sat(f[2 * j], f[2 * j + 1]);
-  *reinterpret_cast<uint4*>(hi) = *reinterpret_cast<uint4*>(h);
-  if (lo) {
-    __half2 l[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float2 hf = __half22float2(h[j]);
-      l[j] = __floats2half2_rn(f[2 * j] - hf.x, f[2 * j + 1] - hf.y);
-    }
-    *reinterpret_cast<uint4*>(lo) = *reinterpret_cast<uint4*>(l);
+  for (int j = 0; j < 4; ++j) {
+    const HalfPair2 s = split_f16x2(f[2 * j], f[2 * j + 1]);
+    h[j] = s.hi, l[j] = s.lo;
   }
+  *reinterpret_cast<uint4*>(hi) = *reinterpret_cast<uint4*>(h);
+  if (lo) *reinterpret_cast<uint4*>(lo) = *reinterpret_cast<uint4*>(l);
+}
+
+__device__ __forceinline__ void split_store1(float f, __half* hi, __half* lo, size_t o) {
+  const HalfPair2 s = split_f16x2(f, 0.f);
+  hi[o] = __low2half(s.hi);
+  if (lo) lo[o] = __low2half(s.lo);
 }
 
 // ============================================================ GroupNorm statistics
@@ -724,11 +725,7 @@ conv3x3_cin4_kernel(const float* __restrict__ x, int H, int W, const float* __re
     for (int k = 0; k < 36; ++k) acc += s_in[pl * 36 + k] * s_w[k * Cout + co];
     const size_t o = ((size_t)n * HW + p) * Cout + co;
     y[o] = acc;
-    if (y_hi) {  // fp16 hi/lo copy for a consumer that takes this tensor as a raw GEMM operand
-      const __half h = __float2half_rn(acc);
-      y_hi[o] = h;
-      if (y_lo) y_lo[o] = __float2half_rn(acc - __half2float(h));
-    }
+    if (y_hi) split_store1(acc, y_hi, y_lo, o);  // fp16 hi/lo copy for a consumer that takes this tensor as a raw GEMM operand
   }
 }
 void conv3x3_cin4_launch(const float* x_nchw, int n, int H, int W, const float* w, const float* b, int Cout,
@@ -790,11 +787,7 @@ conv3x3_cin_cond_kernel(const float* __restrict__ x, long long xs, const float* 
     for (int k = 0; k < K; ++k) acc += s_in[pl * K + k] * s_w[k * Cout + co];
     const size_t o = ((size_t)n * HW + p) * Cout + co;
     y[o] = acc;
-    if (y_hi) {
-      const __half h = __float2half_rn(acc);
-      y_hi[o] = h;
-      if (y_lo) y_lo[o] = __float2half_rn(acc - __half2float(h));
-    }
+    if (y_hi) split_store1(acc, y_hi, y_lo, o);
   }
 }
 template <int CIN>
@@ -1489,11 +1482,6 @@ void step_noise_launch(float* x, long long count, uint64_t seed, int t, cudaStre
 }
 
 // ============================================================ weight packing
-__device__ __forceinline__ void split_store1(float f, __half* hi, __half* lo, size_t o) {
-  const __half h = __float2half_rn(f);
-  hi[o] = h;
-  if (lo) lo[o] = __float2half_rn(f - __half2float(h));
-}
 __global__ void pack_conv_kernel(const float* __restrict__ w, int Cout, int Cin, int kk, __half* hi, __half* lo) {
   const long long total = (long long)Cout * kk * Cin;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {

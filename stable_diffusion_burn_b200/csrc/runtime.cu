@@ -412,22 +412,20 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
   p.ln_in = ep.ln_in, p.ln_in_slots = ep.ln_in_slots, p.ln_C = ep.ln_C, p.ln_eps = ep.ln_eps;
   p.ln_u = passes >= 3 ? ep.ln_u_full : ep.ln_u_hi;
   SDB_CHECK(!ep.ln_in || (p.ln_u && ep.ln_in_slots > 0 && ep.ln_C == w.K && kind == G_LINEAR), "LayerNorm-consuming GEMM: arguments");
-  SDB_CHECK(!ep.ln_in || (!ep.residual && !ep.rowbias && !ep.residual16.hi), "LayerNorm-consuming GEMM: no residual / row bias");
+  SDB_CHECK(!ep.ln_in || (!ep.residual && !ep.residual16.hi), "LayerNorm-consuming GEMM: no residual");
   SDB_CHECK(!ep.ln_out || kind == G_LINEAR, "LayerNorm statistics: rows must be tokens");
   p.res_hi = ep.residual16.hi, p.res_lo = ep.residual16.lo;
-  SDB_CHECK(!ep.residual16.hi || (ep.residual16.lo && !ep.residual && !ep.rowbias), "fp16-pair residual: needs both halves, excludes the fp32 residual / row bias");
+  SDB_CHECK(!ep.residual16.hi || (ep.residual16.lo && !ep.residual), "fp16-pair residual: needs both halves, excludes the fp32 residual");
   p.out_f32 = ep.out_f32;
   p.out_f16 = ep.out_f16.hi;
   p.out_f16_lo = ep.out_f16.lo;
   p.bias = ep.bias;
-  p.rowbias = ep.rowbias;
   p.residual = ep.residual;
   p.geglu = ep.geglu;
   p.act = ep.act;
   const int nout = ep.geglu ? w.N / 2 : w.N;
   p.ldc = ep.ldc ? ep.ldc : nout;
   p.ldc16 = ep.ldc16 ? ep.ldc16 : nout;
-  SDB_CHECK(!(ep.rowbias && ep.residual), "epilogue takes a time-embedding row or a residual, not both");
   p.os = (kind == G_CONV3_UP2) ? 2 : 1;
   p.OH = a0.H * p.os, p.OW = a0.W * p.os;
   SDB_CHECK((double)a0.n * p.OH * p.OW * (double)std::max(p.ldc, p.ldc16) < 2147483648.0,

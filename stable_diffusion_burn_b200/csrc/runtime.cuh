@@ -108,7 +108,6 @@ struct Epilogue {
   float* out_f32 = nullptr;
   Half2Ptr out_f16;
   const float* bias = nullptr;
-  const float* rowbias = nullptr;
   const float* residual = nullptr;
   int geglu = 0;
   int act = 0;    // 1 = QuickGELU

@@ -5,6 +5,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import gemm_ref as G
+
 pytestmark = pytest.mark.gpu
 
 # tolerance per number of tensor-core passes (relative L2): 1 pass = fp16 operand rounding,
@@ -147,23 +149,63 @@ def test_layernorm(ctx, rows, c):
     assert rel(out, ref.numpy()) < 5e-6
 
 
-@pytest.mark.parametrize("scale", [1.0e3, 3.0e4, 1.0e5])
+@pytest.mark.parametrize("scale", [1.0e3, 3.0e4, 1.0e5, 3.0e5, 1.0e6])
 def test_raw_operand_fp16_range(ctx, scale):
     """Raw (un-normalised) GEMM operands — skip 1x1 convs, upsample / downsample convs, the VAE's nin_shortcut — are staged as
     fp16 hi + lo pairs. The hi half saturates at 65504 and the lo half carries the excess, so the multi-pass product stays finite
-    and accurate for |x| < 131008 (a trained VAE decoder is known to exceed the fp16 range); beyond that, and for single-pass
-    operands above 65504, values clip instead of turning into inf / NaN."""
+    and accurate for |x| <= 131008 (a trained VAE decoder is known to exceed the fp16 range); beyond that the pair clips at
+    +-131008, and single-pass operands clip at 65504, instead of turning into inf / NaN.
+
+    The 3-pass conv must equal the fp64 sum of the three terms it forms from the operand splits (gemm_ref.pass_product). Against
+    the fp64 conv of clip(x, +-131008) it is accurate to the pair's precision: 2^-22 below 65504, but above it lo = x - 65504 holds
+    only 11 bits (relative step <= 2^-12 of x) and the omitted lo * lo term is no longer negligible, so the bar there is 2 * 2^-12."""
     rng = np.random.default_rng(7)
     x = (rng.standard_normal((1, 128, 16, 16)) * scale / 4).astype(np.float32)  # |x| up to ~4.5 sigma = 1.1 * scale
     x[0, 5, 3, 3] = 1.2 * scale
     w = (rng.standard_normal((64, 128, 1, 1)) / np.sqrt(128)).astype(np.float32)
-    ref = F.conv2d(torch.from_numpy(x).double(), torch.from_numpy(w).double()).numpy()
+    ref = F.conv2d(torch.from_numpy(np.clip(x, -131008, 131008)).double(), torch.from_numpy(w).double()).numpy()
+    terms = G.pass_product(x[0].reshape(128, 256).T, w[:, :, 0, 0].T, 3).T.reshape(1, 64, 16, 16)
     out = ctx.test_conv2d(x, w, None, passes=3)
     assert np.isfinite(out).all()
-    e = rel(out, ref)
-    print(f"raw operand range, max |x| = {np.abs(x).max():.3g}: 3-pass rel L2 {e:.3e}")
-    assert e < 5e-5
+    e, et = rel(out, ref), rel(out, terms)
+    print(f"raw operand range, max |x| = {np.abs(x).max():.3g}: 3-pass rel L2 {e:.3e} (against the 3-pass terms {et:.3e})")
+    assert et < 5e-5
+    assert e < (5e-5 if scale <= 1.0e5 else 2 * 2.0 ** -12)
     out1 = ctx.test_conv2d(x, w, None, passes=1)
     assert np.isfinite(out1).all()  # single pass: clipped at 65504 above the fp16 range, never inf / NaN
     if scale <= 3.0e4:
         assert rel(out1, ref) < 1e-3
+
+
+@pytest.mark.parametrize("passes", [1, 2, 3])
+def test_gemm_fp16_pair_output_saturates(ctx, passes):
+    """An fp16 hi + lo output beyond the pair's range holds +-131008 exactly, never inf / NaN; inside it both halves equal the
+    split of the exact fp32 result. Integer operands, exact in fp16, so every pass count gives the same exact product."""
+    rng = np.random.default_rng(passes)
+    a = rng.integers(-8, 9, (200, 64)).astype(np.float32)
+    w = (rng.integers(-8, 9, (64, 320)) * 1024).astype(np.float32)  # |products| up to 2^16: results up to ~1e6, exact in fp32
+    ref = a.astype(np.float64) @ w.astype(np.float64)
+    big = np.abs(ref) > 131008
+    assert big.mean() > 0.2 and (~big).mean() > 0.2 and (np.abs(ref[~big]) > 65520).any()
+    hi, lo = ctx.test_gemm_ex(a, w, passes=passes, planes=True)
+    assert np.isfinite(hi).all() and np.isfinite(lo).all()
+    assert np.array_equal((hi + lo)[big], np.sign(ref[big]) * 131008)
+    ehi, elo = G.split_pair(ref.astype(np.float32))
+    assert np.array_equal(hi, ehi) and np.array_equal(lo, elo)
+
+
+@pytest.mark.parametrize("passes", [1, 2, 3])
+def test_gemm_nan_operand_stays_nan(ctx, passes):
+    """A NaN in row r of A makes output row r NaN at every pass count (the operand split keeps it NaN in both halves instead of
+    clipping it to a finite value); every other row is exact."""
+    rng = np.random.default_rng(10 + passes)
+    a = rng.integers(-4, 5, (200, 192)).astype(np.float32)
+    w = rng.integers(-4, 5, (192, 128)).astype(np.float32)
+    w[37] = 0.0  # NaN * 0 is NaN too
+    ref = a @ w
+    r = 131
+    a[r, 37] = np.nan
+    out = ctx.test_gemm_ex(a, w, passes=passes)
+    assert np.isnan(out[r]).all()
+    keep = np.arange(200) != r
+    assert np.array_equal(out[keep], ref[keep])
