@@ -4,15 +4,18 @@
 // (call sites: src/model/unet/mod.rs:716,726,729 ResBlock convs; :468,479 proj_in/out;
 //  :645-651 q/k/v/out; :580,553 GEGLU/ff; src/model/autoencoder/mod.rs:513-528, 567-606).
 //
-// One CTA = one 128 x BN output tile (x one K split). Warp roles:
+// gemm_tc_kernel: one CTA = one 128 x BN output tile (x one K split). Warp roles:
 //   warpgroup 0    : TMA producer (warp 0: cp.async.bulk.tensor 5-D activation boxes + 2-D weight boxes; warps 1-3 idle)
 //   warpgroups 1-2 : consumers. Each issues wgmma m64nBNk16 (fp16 x fp16 -> fp32 in registers) for 64 of the 128 rows, then
 //                    both write the accumulator to shared memory as a row-major fp32 image and run the epilogue from it
-//                    (bias / residual / GEGLU / statistics -> global)
+//                    (bias / residual / statistics -> global)
+// gemm_tc_persistent_kernel (LayerNorm-consuming and GEGLU epilogues): the same roles, at most one CTA per SM running a
+// sequence of tiles, the epilogue straight from the accumulator registers while the producer loads the next tile.
 // Multi-pass products (PASSES = 2, 3) add the low-order fp16 halves of the operands
 // (A_lo*B_hi, A_hi*B_lo) into the same accumulator for fp32-class accuracy.
 #include "gemm_tc.cuh"
 
+#include <algorithm>
 #include <cstring>
 
 namespace sdb {
@@ -39,15 +42,14 @@ struct AccLayout {
 };
 static constexpr int EW = 8;  // consumer / epilogue warps (two warpgroups)
 
+// QuickGELU x*sigmoid(1.702x), the CLIP MLP activation (act = 1)
+__device__ __forceinline__ float quick_gelu(float x) { return __fdividef(x, 1.0f + __expf(-1.702f * x)); }
 // Activation + fp32 / fp16(hi,lo) stores of 4 consecutive columns of one output row. Deliberately NOT inlined: the epilogue
 // runs once per CTA, so its cost is dominated by cold instruction fetch (ncu: stall_no_inst); one shared copy of this
 // body instead of one per unrolled row keeps the epilogue's code footprint small.
 __device__ __noinline__ void epilogue_store(float4 f, unsigned int o32, unsigned int o16, float* out_f32, __half* out_f16,
                                             __half* out_f16_lo, int act) {
-  if (act == 1) {
-    f.x = __fdividef(f.x, 1.0f + __expf(-1.702f * f.x)), f.y = __fdividef(f.y, 1.0f + __expf(-1.702f * f.y));
-    f.z = __fdividef(f.z, 1.0f + __expf(-1.702f * f.z)), f.w = __fdividef(f.w, 1.0f + __expf(-1.702f * f.w));
-  }
+  if (act == 1) f.x = quick_gelu(f.x), f.y = quick_gelu(f.y), f.z = quick_gelu(f.z), f.w = quick_gelu(f.w);
   if (out_f32) *reinterpret_cast<float4*>(out_f32 + o32) = f;
   if (out_f16) {
     const HalfPair2 s0 = split_f16x2(f.x, f.y), s1 = split_f16x2(f.z, f.w);
@@ -58,6 +60,25 @@ __device__ __noinline__ void epilogue_store(float4 f, unsigned int o32, unsigned
       *reinterpret_cast<uint2*>(out_f16_lo + o16) = *reinterpret_cast<uint2*>(l);
     }
   }
+}
+
+// 4 x 4 transpose of 32-bit values inside each quad of lanes (q = lane % 4): lane q ends with {x[q] of lane 0, ..., x[q] of
+// lane 3}. Two butterfly stages: lanes q and q ^ 1 swap the elements whose bit 0 differs from theirs (the 2 x 2 blocks
+// transpose), then lanes q and q ^ 2 swap on bit 1 (the blocks change places). The register epilogue uses it to turn 4 column
+// pairs per lane into 8 consecutive columns per lane.
+__device__ __forceinline__ uint4 quad_transpose(uint32_t (&x)[4], int q) {
+  const bool e = q & 1, f = q & 2;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const uint32_t v = __shfl_xor_sync(0xffffffffu, e ? x[2 * j] : x[2 * j + 1], 1);
+    if (e) x[2 * j] = v; else x[2 * j + 1] = v;
+  }
+#pragma unroll
+  for (int c = 0; c < 2; ++c) {
+    const uint32_t v = __shfl_xor_sync(0xffffffffu, f ? x[c] : x[2 + c], 2);
+    if (f) x[c] = v; else x[2 + c] = v;
+  }
+  return make_uint4(x[0], x[1], x[2], x[3]);
 }
 
 // Bucket reduction of the per-quarter column sums an epilogue left in shared memory (cs[q][col] = (sum, sumsq) of the 32 rows of
@@ -125,8 +146,8 @@ __host__ __device__ constexpr int region_bytes() {
 template <int BN, int PASSES, int STAGES, int EPI>
 __global__ void __launch_bounds__(128 + 32 * EW, 1)
 gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
-  constexpr bool kGN = EPI == EPI_GN, kLNS = EPI == EPI_LNS, kLNC = EPI == EPI_LNC || EPI == EPI_GEGLU_LNC;
-  constexpr bool kGEGLU = EPI == EPI_GEGLU || EPI == EPI_GEGLU_LNC;
+  static_assert(EPI == EPI_PLAIN || EPI == EPI_GN || EPI == EPI_LNS, "the register epilogues run in gemm_tc_persistent_kernel");
+  constexpr bool kGN = EPI == EPI_GN, kLNS = EPI == EPI_LNS;
   using L = StageLayout<BN, PASSES>;
   constexpr int EG = EW / 4;                                    // warps sharing one 32-row quarter of the tile
   constexpr int CSTEP = 32 * EG;                                // column stride between the chunks of one warp
@@ -305,24 +326,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     int mr8[8], ao[8];
     float4 bvs[NCHUNK], ad[8];
     const bool res_pair = p.res_hi != nullptr;  // the residual lives as an fp16 hi + lo pair (row stride ldc16)
-    const bool plain = p.split_k == 1 && !kGEGLU;
-    // EPI_LNC: mean / rstd of this lane's own accumulator row, from the partial row sums the producer of A left
-    float ln_mu = 0.f, ln_rs = 0.f;
-    float mu8[8], rs8[8];
-    float4 us[NCHUNK];
-    if constexpr (kLNC) {
-      if (m >= 0) {
-        const float2* sp = reinterpret_cast<const float2*>(p.ln_in) + (size_t)m * p.ln_in_slots;
-        float sm = 0.f, sq = 0.f;
-        for (int i = 0; i < p.ln_in_slots; ++i) {
-          const float2 v = sp[i];
-          sm += v.x, sq += v.y;
-        }
-        const float inv = 1.0f / (float)p.ln_C;
-        ln_mu = sm * inv;
-        ln_rs = rsqrtf(fmaxf(sq * inv - ln_mu * ln_mu, 0.f) + p.ln_eps);
-      }
-    }
+    const bool plain = p.split_k == 1;
     {
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -331,15 +335,6 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
         mr8[i] = mr;
         ao[i] = res_pair ? mr * p.ldc16 : mr * p.ldc;
         ad[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if constexpr (kLNC) mu8[i] = __shfl_sync(0xffffffffu, ln_mu, rr), rs8[i] = __shfl_sync(0xffffffffu, ln_rs, rr);
-      }
-      if constexpr (kLNC) {
-#pragma unroll
-        for (int j = 0; j < NCHUNK; ++j) {
-          const int col = col0 + half * 32 + j * CSTEP + cq;
-          us[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (half * 32 + j * CSTEP < BN && col < p.N) us[j] = *reinterpret_cast<const float4*>(p.ln_u + col);
-        }
       }
 #pragma unroll
       for (int j = 0; j < NCHUNK; ++j) {
@@ -349,7 +344,6 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       }
     }
     auto issue_addends = [&](int col) {
-      if constexpr (kLNC) return;  // a LayerNorm-consuming GEMM has no residual (run_gemm checks): no registers for them
       if (col >= p.N) return;
       if (res_pair) {
 #pragma unroll
@@ -393,7 +387,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       epilogue_store(f, (unsigned)(mr * p.ldc + col), (unsigned)(mr * p.ldc16 + col), p.out_f32, p.out_f16, p.out_f16_lo, p.act);
     };
 
-    if (!kGEGLU && p.split_k > 1) {
+    if (p.split_k > 1) {
       // raw partial sums -> workspace [split][M][N]
       const size_t Mtot = (size_t)p.nimg * p.OH * p.OW;
       float* wsbase = p.ws + (size_t)kz * Mtot * p.N;
@@ -516,40 +510,6 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
           tk[1] = 0u;
         }
       }
-    } else if (kGEGLU) {
-      // tile columns [0,BN/2) = x, [BN/2,BN) = gate; output columns blockIdx.y*BN/2 + [0,BN/2)
-      constexpr int HB = BN / 2;
-      const int ocol0 = blockIdx.y * HB;
-#pragma unroll 1
-      for (int c = half * 32; c < HB; c += CSTEP) {
-        const float4 bx = *reinterpret_cast<const float4*>(p.bias + col0 + c + cq);
-        const float4 bg = *reinterpret_cast<const float4*>(p.bias + col0 + HB + c + cq);
-        float4 ux = make_float4(0.f, 0.f, 0.f, 0.f), ug = ux;
-        if constexpr (kLNC) {
-          ux = *reinterpret_cast<const float4*>(p.ln_u + col0 + c + cq);
-          ug = *reinterpret_cast<const float4*>(p.ln_u + col0 + HB + c + cq);
-        }
-#pragma unroll 1
-        for (int i = 0; i < 8; ++i) {
-          const int rr = i * 4 + sub;
-          const int mr = __shfl_sync(0xffffffffu, m, rr);
-          float rmu = 0.f, rrs = 1.f;
-          if constexpr (kLNC) rmu = __shfl_sync(0xffffffffu, ln_mu, rr), rrs = __shfl_sync(0xffffffffu, ln_rs, rr);
-          if (mr >= 0) {
-            float4 tx = unstage(arow + c * 4, rr), tg = unstage(arow + (HB + c) * 4, rr);
-            if constexpr (kLNC) {
-              tx.x = rrs * (tx.x - rmu * ux.x), tx.y = rrs * (tx.y - rmu * ux.y), tx.z = rrs * (tx.z - rmu * ux.z), tx.w = rrs * (tx.w - rmu * ux.w);
-              tg.x = rrs * (tg.x - rmu * ug.x), tg.y = rrs * (tg.y - rmu * ug.y), tg.z = rrs * (tg.z - rmu * ug.z), tg.w = rrs * (tg.w - rmu * ug.w);
-            }
-            float4 y;
-            y.x = (tx.x + bx.x) * gelu_erf_fast(tg.x + bg.x);
-            y.y = (tx.y + bx.y) * gelu_erf_fast(tg.y + bg.y);
-            y.z = (tx.z + bx.z) * gelu_erf_fast(tg.z + bg.z);
-            y.w = (tx.w + bx.w) * gelu_erf_fast(tg.w + bg.w);
-            epilogue_store(y, 0u, (unsigned)(mr * p.ldc16 + ocol0 + c + cq), nullptr, p.out_f16, p.out_f16_lo, 0);
-          }
-        }
-      }
     } else {
       constexpr int NCH = NCHUNK;  // column chunks per warp (the warps of a lane quarter interleave them)
       if (!pre_issued) issue_addends(col0 + half * 32 + cq);
@@ -580,14 +540,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
                 const int k = b4 * 4 + i;
                 if (mr8[k] < 0) continue;
                 float4 f = t[i];
-                if constexpr (kLNC) {  // LayerNorm folded in: rstd * (acc - mean * u) ; beta^T W + bias comes in through bvs
-                  f.x = rs8[k] * (f.x - mu8[k] * us[j].x), f.y = rs8[k] * (f.y - mu8[k] * us[j].y);
-                  f.z = rs8[k] * (f.z - mu8[k] * us[j].z), f.w = rs8[k] * (f.w - mu8[k] * us[j].w);
-                }
-                if constexpr (kLNC)
-                  f.x += bvs[j].x, f.y += bvs[j].y, f.z += bvs[j].z, f.w += bvs[j].w;
-                else
-                  f.x += bvs[j].x + ad[k].x, f.y += bvs[j].y + ad[k].y, f.z += bvs[j].z + ad[k].z, f.w += bvs[j].w + ad[k].w;
+                f.x += bvs[j].x + ad[k].x, f.y += bvs[j].y + ad[k].y, f.z += bvs[j].z + ad[k].z, f.w += bvs[j].w + ad[k].w;
                 if constexpr (kLNS) {
                   lrs[k] += (f.x + f.y) + (f.z + f.w);
                   lrq[k] = fmaf(f.x, f.x, fmaf(f.y, f.y, fmaf(f.z, f.z, fmaf(f.w, f.w, lrq[k]))));
@@ -654,6 +607,381 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   if (dbg && threadIdx.x == 0) dbg[7] = clock64();
 }
 
+// The output tile a CTA works on: linear tile index t -> (m tile, n tile, z), m tile fastest, then n tile, then z (the K split,
+// or the output phase of the folded upsample conv). It is the order in which the hardware dispatched the 3-D grid of one CTA
+// per tile, so a persistent CTA taking tiles c, c + G, c + 2G, ... keeps the L2 reuse of the weight tiles that order gives.
+struct GemmTile {
+  int mt, nt, z;
+  int tw, th, w0, h0, n0, col0;
+  int up_a, up_b, kz, b_row0;
+  int it_begin, it_end;
+};
+template <int BN>
+__device__ __forceinline__ GemmTile gemm_tile_of(const GemmParams& p, int t, int m_tiles, int n_tiles) {
+  GemmTile T;
+  T.mt = t % m_tiles;
+  T.nt = (t / m_tiles) % n_tiles;
+  T.z = t / (m_tiles * n_tiles);
+  T.tw = T.mt % p.tiles_w;
+  T.th = (T.mt / p.tiles_w) % p.tiles_h;
+  T.w0 = T.tw * p.TW, T.h0 = T.th * p.TH, T.n0 = (T.mt / (p.tiles_w * p.tiles_h)) * p.TN;
+  T.col0 = T.nt * BN;
+  // z is the K split — or, for the folded nearest-2x upsample conv (p.up2, never split), the output phase (a, b): the four
+  // 2x2-tap phase convolutions of one layer run as ONE launch; phase shifts the taps, the weight rows and the output pixel
+  T.up_a = p.up2 ? (T.z >> 1) : 0, T.up_b = p.up2 ? (T.z & 1) : 0;
+  T.kz = p.up2 ? 0 : T.z;
+  T.b_row0 = T.col0 + (p.up2 ? T.z * p.N : 0);  // first weight row of this tile (phase-major packing)
+  const int total_iters = p.num_taps * p.kc + p.xkc;
+  const int per_split = (total_iters + p.split_k - 1) / p.split_k;
+  T.it_begin = T.kz * per_split;
+  T.it_end = min(total_iters, T.it_begin + per_split);
+  return T;
+}
+// output row index of accumulator row r of a tile (< 2^31 rows); -1 marks a row outside the tensor
+__device__ __forceinline__ int gemm_row_of(const GemmParams& p, const GemmTile& T, int r) {
+  const int pw = T.w0 + r % p.TW;
+  const int phh = T.h0 + (r / p.TW) % p.TH;
+  const int pn = T.n0 + r / (p.TW * p.TH);
+  return (pw < p.W && phh < p.H && pn < p.nimg) ? ((pn * p.OH + phh * p.os + p.oa + T.up_a) * p.OW + pw * p.os + p.ob + T.up_b) : -1;
+}
+
+// The instances whose epilogue runs from the accumulator registers — the LayerNorm-consuming and GEGLU projections, the
+// short-K multi-wave launches of the transformer blocks: they never write the accumulator image over the operand ring, so one
+// CTA runs a sequence of tiles (persistent grid) and the producer loads the next tile's operands while the consumers run the
+// epilogue of the current one. Their per-column addends (bias, LayerNorm column sums) are staged in shared memory once per
+// tile. The GroupNorm / LayerNorm-statistics epilogues and the split-K fold reduce across the rows or columns of the tile and
+// keep the shared-memory image (one tile per CTA). So do the plain instances: their per-row residual cannot be staged, and read
+// from global memory between the stores of a register epilogue it puts one L2 round trip per column pair on the critical path.
+template <int EPI>
+__host__ __device__ constexpr bool epi_from_registers() {
+  return EPI == EPI_LNC || EPI == EPI_GEGLU || EPI == EPI_GEGLU_LNC;
+}
+// bias and LayerNorm column sums of one tile for the register epilogue, after the ring's barriers
+template <int BN, int EPI>
+__host__ __device__ constexpr int epi_stage_bytes() {
+  return epi_from_registers<EPI>() ? 2 * BN * 4 : 0;
+}
+
+// The LayerNorm-consuming and GEGLU instances (epi_from_registers): the same producer / consumer roles and mainloop as
+// gemm_tc_kernel, run over a sequence of tiles per CTA, and the epilogue from the accumulator registers. gemm_tc_kernel keeps
+// its one-tile form: built from this tile loop, its instances measured 2 % slower in the mainloop (DESIGN.md §4).
+template <int BN, int PASSES, int STAGES, int EPI>
+__global__ void __launch_bounds__(128 + 32 * EW, 1)
+gemm_tc_persistent_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
+  static_assert(epi_from_registers<EPI>(), "the shared-memory epilogues run in gemm_tc_kernel");
+  constexpr bool kLNC = EPI == EPI_LNC || EPI == EPI_GEGLU_LNC;
+  constexpr bool kGEGLU = EPI == EPI_GEGLU || EPI == EPI_GEGLU_LNC;
+  using L = StageLayout<BN, PASSES>;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  // 1024-byte alignment is required by the 128B swizzle atoms
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + region_bytes<BN, PASSES, STAGES>());
+  uint64_t* empty_bar = full_bar + STAGES;
+  float* const stage_bias = reinterpret_cast<float*>(empty_bar + STAGES);  // this tile's [BN] bias, then [BN] column sums
+  float* const stage_u = stage_bias + BN;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  // ---- the tiles of this CTA: a 1-D grid of at most one CTA per SM, CTA c runs tiles c, c + G, c + 2G, ... (never split in K:
+  // run_gemm does not split a LayerNorm-consuming or GEGLU GEMM)
+  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
+  const int n_tiles = (p.N + BN - 1) / BN;
+  const int ntiles = m_tiles * n_tiles * (p.up2 ? 4 : 1);
+  const int t0 = blockIdx.x, tstep = gridDim.x;
+  long long* const dbg = (p.dbg && t0 == 0) ? p.dbg : nullptr;
+  if (dbg && threadIdx.x == 0) dbg[0] = clock64();
+  const int main_iters = p.num_taps * p.kc;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], EW);  // one arrival per consumer warp
+    }
+    fence_mbar_init();
+  }
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&maps.a[0][0]);
+    tma_prefetch_desc(&maps.b[0]);
+    if (p.kc0 < p.kc) tma_prefetch_desc(&maps.a[1][0]);
+  }
+  __syncthreads();
+  if (dbg && threadIdx.x == 0) dbg[1] = clock64();
+  // Programmatic dependent launch: everything above overlapped the previous kernel's tail. From here on each role waits for the
+  // previous kernel (griddepcontrol.wait) only where it first touches data that kernel may have written:
+  //   producer : WEIGHTS are immutable, so the weight tiles of the first STAGES k-chunks of the first tile are issued BEFORE the
+  //              wait; activation tiles after it
+  //   consumers: wait before the first read of the LayerNorm row statistics; all of this kernel's stores follow it
+  if (warp == 0) {
+    // ===================================================== TMA producer (one elected lane: see elect_one in common.cuh)
+    if (elect_one()) {
+      // ring slot and phase run on across the tiles of this CTA
+      int s = 0;
+      uint32_t ph = 0;
+#pragma unroll 1
+      for (int t = t0; t < ntiles; t += tstep) {
+        const GemmTile T = gemm_tile_of<BN>(p, t, m_tiles, n_tiles);
+        // iteration -> (activation source, channel chunk, tap shift) and the weight map / K coordinate that go with it
+        auto load_b = [&](int it, int s) {
+          const CUtensorMap* bm = it < main_iters ? maps.b : maps.bx;
+          const int bk = (it < main_iters ? it : it - main_iters) * BK;
+          uint8_t* sb = smem + s * L::BYTES + L::A_TILES * A_TILE_BYTES;
+          tma_load_2d(sb, &bm[0], &full_bar[s], bk, T.b_row0);
+          if (PASSES >= 3) tma_load_2d(sb + L::B_TILE_BYTES, &bm[1], &full_bar[s], bk, T.b_row0);
+        };
+        auto load_a = [&](int it, int s) {
+          int src, c0, cw, ch, cp;
+          if (it < main_iters) {
+            const int tap = it / p.kc;
+            const int cc = it - tap * p.kc;
+            src = cc >= p.kc0 ? 1 : 0;
+            c0 = (cc - (src ? p.kc0 : 0)) * BK;
+            cw = T.w0 + p.tap_dw[tap] + T.up_b, ch = T.h0 + p.tap_dh[tap] + T.up_a, cp = p.tap_ph[tap];
+          } else {
+            const int e = it - main_iters;
+            src = e >= p.xkc0 ? 3 : 2;
+            c0 = (e - (src == 3 ? p.xkc0 : 0)) * BK;
+            cw = T.w0, ch = T.h0, cp = 0;
+          }
+          uint8_t* st = smem + s * L::BYTES;
+          tma_load_5d(st, &maps.a[src][0], &full_bar[s], c0, cw, ch, cp, T.n0);
+          if (PASSES >= 2) tma_load_5d(st + A_TILE_BYTES, &maps.a[src][1], &full_bar[s], c0, cw, ch, cp, T.n0);
+        };
+        int it = T.it_begin;
+        if (t == t0) {
+          // ---- first tile, before the wait: weights only (the pipeline slots are all free: fresh barriers)
+          const int npre = min(STAGES, T.it_end - T.it_begin);
+          for (int i = 0; i < npre; ++i) {
+            mbar_expect_tx(&full_bar[i], L::BYTES);
+            load_b(it + i, i);
+          }
+          pdl_wait();
+          for (int i = 0; i < npre; ++i) load_a(it + i, i);
+          if (dbg) dbg[2] = clock64();
+          it += npre;
+          s = npre == STAGES ? 0 : npre;
+          ph = npre == STAGES ? 1 : 0;
+        }
+        // ---- steady state: a slot is refilled as soon as the consumers release it, also while they run an epilogue
+        for (; it < T.it_end; ++it) {
+          mbar_wait(&empty_bar[s], ph ^ 1);
+          mbar_expect_tx(&full_bar[s], L::BYTES);
+          load_a(it, s);
+          load_b(it, s);
+          if (++s == STAGES) {
+            s = 0;
+            ph ^= 1;
+          }
+        }
+      }
+    }
+  } else if (warp >= 4) {
+    // ===================================================== consumers: wgmma mainloop, then the epilogue
+    pdl_wait();  // the row statistics below come from the previous kernel; every store of this kernel follows
+    const int wg = (warp - 4) >> 2;  // rows [64 wg, 64 wg + 64) of the tile
+    int s = 0;
+    uint32_t ph = 0;
+#pragma unroll 1
+    for (int t = t0; t < ntiles; t += tstep) {
+      const GemmTile T = gemm_tile_of<BN>(p, t, m_tiles, n_tiles);
+      const bool first = t == t0;
+      const int col0 = T.col0;
+      // This thread's accumulator rows are ra = 64 wg + 16 (warp % 4) + lane / 4 and ra + 8. Their output rows, and for a
+      // LayerNorm-consuming GEMM their partial row statistics, are requested before the mainloop so that those loads travel while
+      // the products run.
+      const int ra = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      int mrow[2] = {-1, -1};
+      constexpr int LNPRE = 8;  // row-statistics slots loaded ahead of the mainloop (the rest after it)
+      float2 lnv[2][LNPRE];
+      // this tile's bias and LayerNorm column sums: one column per consumer thread, staged after the mainloop
+      const int te = threadIdx.x - 128;
+      float sbias = 0.f, su = 0.f;
+      if (te < BN && col0 + te < p.N) {
+        if (p.bias) sbias = p.bias[col0 + te];
+        if constexpr (kLNC) su = p.ln_u[col0 + te];
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mrow[h] = gemm_row_of(p, T, ra + 8 * h);
+        if constexpr (kLNC) {
+          const float2* sp = reinterpret_cast<const float2*>(p.ln_in) + (size_t)mrow[h] * p.ln_in_slots;
+#pragma unroll
+          for (int i = 0; i < LNPRE; ++i) lnv[h][i] = (mrow[h] >= 0 && i < p.ln_in_slots) ? sp[i] : make_float2(0.f, 0.f);
+        }
+      }
+      float acc[BN / 2];
+      {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        int prev = -1;
+        for (int it = T.it_begin; it < T.it_end; ++it) {
+          mbar_wait(&full_bar[s], ph);
+          if (dbg && threadIdx.x == 128 && first && it == T.it_begin) dbg[3] = clock64();
+          const uint32_t a_hi = smem_u32(smem + s * L::BYTES) + wg * (64 * 128);
+          const uint32_t a_lo = a_hi + A_TILE_BYTES;
+          const uint32_t b_hi = smem_u32(smem + s * L::BYTES) + L::A_TILES * A_TILE_BYTES;
+          const uint32_t b_lo = b_hi + L::B_TILE_BYTES;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) {
+            const uint32_t koff = k * 32;  // 16 fp16 = 32 bytes inside the 128B swizzle row
+            const uint64_t da = make_sdesc_sw128(a_hi + koff);
+            const uint64_t db = make_sdesc_sw128(b_hi + koff);
+            Wgmma<BN>::template ss<0>(acc, da, db, 1);
+            if (PASSES >= 2) Wgmma<BN>::template ss<0>(acc, make_sdesc_sw128(a_lo + koff), db, 1);
+            if (PASSES >= 3) Wgmma<BN>::template ss<0>(acc, da, make_sdesc_sw128(b_lo + koff), 1);
+          }
+          wgmma_commit();
+          // one group stays in flight: the products of the previous stage are complete, so its slot goes back to the producer
+          wgmma_wait<1>();
+          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+          prev = s;
+          if (++s == STAGES) {
+            s = 0;
+            ph ^= 1;
+          }
+        }
+        wgmma_wait<0>();
+        reg_fence(acc);
+        if (dbg && threadIdx.x == 128 && first) dbg[4] = clock64();
+        // the last stage goes back too: the producer fills the ring with the next tile's operands during this epilogue
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        asm volatile("bar.sync 1, %0;" ::"n"(EW * 32) : "memory");  // the previous tile's epilogue has read the staging
+        if (te < BN) stage_bias[te] = sbias, stage_u[te] = su;
+        asm volatile("bar.sync 1, %0;" ::"n"(EW * 32) : "memory");
+      }
+      {
+        // ---- epilogue from the accumulator registers. acc[4 jj + 2 h + e] is row ra + 8 h, tile column 8 jj + 2 (lane % 4) + e.
+        // Every element is the expression of the shared-memory epilogue it replaces, in the same order.
+        if (t + tstep >= ntiles) pdl_trigger();  // the last tile's epilogue starts: the next kernel may begin its prologue
+        if (dbg && threadIdx.x == 128 && first) dbg[5] = clock64();
+        const int cp = 2 * (lane & 3);
+        float ln_mu[2] = {0.f, 0.f}, ln_rs[2] = {0.f, 0.f};
+        if constexpr (kLNC) {
+          // EPI_LNC: mean / rstd of each row, from the partial row sums the producer of A left, added in slot order
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (mrow[h] >= 0) {
+              float sm = 0.f, sq = 0.f;
+#pragma unroll
+              for (int i = 0; i < LNPRE; ++i)
+                if (i < p.ln_in_slots) sm += lnv[h][i].x, sq += lnv[h][i].y;
+              const float2* sp = reinterpret_cast<const float2*>(p.ln_in) + (size_t)mrow[h] * p.ln_in_slots;
+              for (int i = LNPRE; i < p.ln_in_slots; ++i) {
+                const float2 v = sp[i];
+                sm += v.x, sq += v.y;
+              }
+              const float inv = 1.0f / (float)p.ln_C;
+              ln_mu[h] = sm * inv;
+              ln_rs[h] = rsqrtf(fmaxf(sq * inv - ln_mu[h] * ln_mu[h], 0.f) + p.ln_eps);
+            }
+          }
+        }
+        // Stores go out 32 columns at a time: the 4 lanes of a row exchange their column pairs (quad_transpose) so that each
+        // lane writes 8 consecutive fp16 columns with one 16-byte store, 64 contiguous bytes per row and warp instruction.
+        // Rows outside the tensor take part in the exchange and skip the store (the 4 lanes of a quad share their rows). A
+        // group's values are computed for both rows before any branch: run-time choices (activation, fp32 output) are taken
+        // once per group, so that the arithmetic of 8 column pairs interleaves.
+        const int q4 = lane & 3;
+        auto store_f16 = [&](uint32_t (&hi)[2][4], uint32_t (&lo)[2][4], int ocol) {
+          if (!p.out_f16) return;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const unsigned o16 = (unsigned)(mrow[h] * p.ldc16 + ocol + 8 * q4);
+            const uint4 vh = quad_transpose(hi[h], q4);
+            if (mrow[h] >= 0) *reinterpret_cast<uint4*>(p.out_f16 + o16) = vh;
+            if (p.out_f16_lo) {
+              const uint4 vl = quad_transpose(lo[h], q4);
+              if (mrow[h] >= 0) *reinterpret_cast<uint4*>(p.out_f16_lo + o16) = vl;
+            }
+          }
+        };
+        if constexpr (kGEGLU) {
+          // tile columns [0,BN/2) = x, [BN/2,BN) = gate: both halves of an output column are in this thread (jj and jj + BN/16)
+          constexpr int HB = BN / 2;
+          const int ocol0 = T.nt * HB;
+#pragma unroll
+          for (int g = 0; g < HB / 32; ++g) {
+            uint32_t hi[2][4], lo[2][4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const int jj = 4 * g + k, c = 8 * jj + cp;
+              const float2 bx = *reinterpret_cast<const float2*>(stage_bias + c);
+              const float2 bg = *reinterpret_cast<const float2*>(stage_bias + HB + c);
+              float2 ux = make_float2(0.f, 0.f), ug = ux;
+              if constexpr (kLNC) {
+                ux = *reinterpret_cast<const float2*>(stage_u + c);
+                ug = *reinterpret_cast<const float2*>(stage_u + HB + c);
+              }
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                float2 tx = make_float2(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1]);
+                float2 tg = make_float2(acc[4 * (jj + HB / 8) + 2 * h], acc[4 * (jj + HB / 8) + 2 * h + 1]);
+                if constexpr (kLNC) {
+                  const float rmu = ln_mu[h], rrs = ln_rs[h];
+                  tx.x = rrs * (tx.x - rmu * ux.x), tx.y = rrs * (tx.y - rmu * ux.y);
+                  tg.x = rrs * (tg.x - rmu * ug.x), tg.y = rrs * (tg.y - rmu * ug.y);
+                }
+                float2 y;
+                y.x = (tx.x + bx.x) * gelu_erf_fast(tg.x + bg.x);
+                y.y = (tx.y + bx.y) * gelu_erf_fast(tg.y + bg.y);
+                const HalfPair2 s2 = split_f16x2(y.x, y.y);
+                hi[h][k] = *reinterpret_cast<const uint32_t*>(&s2.hi), lo[h][k] = *reinterpret_cast<const uint32_t*>(&s2.lo);
+              }
+            }
+            store_f16(hi, lo, ocol0 + 32 * g);
+          }
+        } else {
+          // LayerNorm folded in: rstd * (acc - mean * u) ; beta^T W + bias comes in through the bias (no residual: run_gemm
+          // checks)
+#pragma unroll
+          for (int g = 0; g < BN / 32; ++g) {
+            if (col0 + 32 * g >= p.N) continue;  // N is a multiple of 32: a group is all in or all out
+            float2 f[2][4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const int c = 32 * g + 8 * k + cp;
+              const float2 bv = *reinterpret_cast<const float2*>(stage_bias + c);
+              const float2 us = *reinterpret_cast<const float2*>(stage_u + c);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                float2 v = make_float2(acc[4 * (4 * g + k) + 2 * h], acc[4 * (4 * g + k) + 2 * h + 1]);
+                v.x = ln_rs[h] * (v.x - ln_mu[h] * us.x), v.y = ln_rs[h] * (v.y - ln_mu[h] * us.y);
+                v.x += bv.x, v.y += bv.y;
+                f[h][k] = v;
+              }
+            }
+            if (p.act == 1) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int k = 0; k < 4; ++k) f[h][k].x = quick_gelu(f[h][k].x), f[h][k].y = quick_gelu(f[h][k].y);
+            }
+            if (p.out_f32) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                  if (mrow[h] >= 0) *reinterpret_cast<float2*>(p.out_f32 + (unsigned)(mrow[h] * p.ldc + col0 + 32 * g + 8 * k + cp)) = f[h][k];
+            }
+            uint32_t hi[2][4], lo[2][4];
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const HalfPair2 s2 = split_f16x2(f[h][k].x, f[h][k].y);
+                hi[h][k] = *reinterpret_cast<const uint32_t*>(&s2.hi), lo[h][k] = *reinterpret_cast<const uint32_t*>(&s2.lo);
+              }
+            store_f16(hi, lo, col0 + 32 * g);
+          }
+        }
+        if (dbg && threadIdx.x == 128 && first) dbg[6] = clock64();
+      }
+    }
+  }
+  __syncthreads();
+  if (dbg && threadIdx.x == 0) dbg[7] = clock64();
+}
+
 // ------------------------------------------------------------------ launcher
 // Opt-in maximum of dynamic shared memory per block on sm_90 (227 KB); the kernel adds 1 KB of alignment pad and two 8-byte
 // barriers per stage to the ring.
@@ -670,15 +998,26 @@ constexpr int pick_stages() {
 
 template <int BN, int PASSES, int STAGES, int EPI>
 static void launch_epi(const GemmMaps& maps, const GemmParams& p, cudaStream_t stream) {
-  constexpr int smem = region_bytes<BN, PASSES, STAGES>() + 2 * STAGES * 8 + 1024;
+  constexpr int smem = region_bytes<BN, PASSES, STAGES>() + 2 * STAGES * 8 + epi_stage_bytes<BN, EPI>() + 1024;
   static_assert(smem <= SMEM_OPTIN_MAX, "shared memory per block");
   static_assert(4 * BN * 8 <= AccLayout<BN>::GN_BYTES && 2 * (EW * 32) * 4 * 16 <= AccLayout<BN>::GN_BYTES,
                 "GroupNorm column sums must fit in the scratch after the accumulator image");
   static DeviceOnce once;
-  if (once.first())
-    SDB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, PASSES, STAGES, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid(p.tiles_n * p.tiles_h * p.tiles_w, (p.N + BN - 1) / BN, p.up2 ? 4 : p.split_k);
-  launch_k(gemm_tc_kernel<BN, PASSES, STAGES, EPI>, grid, dim3(128 + 32 * EW), (size_t)smem, stream, maps, p);
+  const bool first = once.first();
+  auto go = [&](void (*kernel)(const GemmMaps, const GemmParams), dim3 grid) {
+    if (first) SDB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    launch_k(kernel, grid, dim3(128 + 32 * EW), (size_t)smem, stream, maps, p);
+  };
+  const int m_tiles = p.tiles_n * p.tiles_h * p.tiles_w, n_tiles = (p.N + BN - 1) / BN;
+  if constexpr (epi_from_registers<EPI>()) {
+    // at most one CTA per SM, each running every gridDim.x-th tile
+    SDB_CHECK(p.split_k == 1 && p.ldc16 % 8 == 0 && reinterpret_cast<uintptr_t>(p.out_f16) % 16 == 0 &&
+                  reinterpret_cast<uintptr_t>(p.out_f16_lo) % 16 == 0,
+              "register epilogue: no K split, fp16 outputs written 8 columns (16 bytes) at a time");
+    go(gemm_tc_persistent_kernel<BN, PASSES, STAGES, EPI>, dim3(std::min(m_tiles * n_tiles * (p.up2 ? 4 : 1), g_num_sms)));
+  } else {
+    go(gemm_tc_kernel<BN, PASSES, STAGES, EPI>, dim3(m_tiles, n_tiles, p.up2 ? 4 : p.split_k));
+  }
 }
 // the statistics-producing epilogues exist for the tile widths their tensors use (run_gemm picks those widths for them)
 template <int BN, int PASSES, int STAGES>
