@@ -73,6 +73,26 @@ int sdb_load_dump_dir(sdb_ctx* ctx, const char* path);
 /* load_tensor::<B, D> (src/model/load.rs:30-47) for one file, no context needed: splits the leading `ndim` shape values
  * from the data. Returns the element count (data may be NULL to probe), or -1 (text via sdb_last_error(NULL)). */
 int64_t sdb_read_dump_tensor(const char* file, int ndim, int64_t* dims, float* data, int64_t capacity);
+/* SD-1.x single-file .safetensors checkpoints in the original LDM layout (DESIGN.md §7 f13): v1-4, v1-5, the inpainting and
+ * InstructPix2Pix releases and their fine-tunes. The key map is the one the reference's converter applies (load_state_dict into
+ * python/dump.py:565-570's StableDiffusion, then python/stablediffusion.py:8-14's savers): model.diffusion_model.* -> unet/...,
+ * first_stage_model.* -> autoencoder/..., cond_stage_model.transformer.text_model.* (or the older spelling without text_model.)
+ * -> clip/..., alphas_cumprod -> alpha_cumulative_products (absent: the SD-1 scaled-linear schedule). Linear weights are
+ * transposed to the registry's [in,out] (python/save.py:17-21), everything else is copied; F32, F16 and BF16 (mixed within a
+ * file) are widened exactly to fp32. Keys outside the model prefixes (model_ema.*, betas, ...), first_stage_model.loss.* and
+ * the CLIP position_ids are not read.
+ * A full checkpoint must hold every registry tensor; a VAE-only file (the standalone SD VAE releases: encoder.*, decoder.*,
+ * quant_conv.*, post_quant_conv.*) replaces exactly the autoencoder/... tensors, on any kind of context. The whole file (header,
+ * keys, shapes, dtypes, byte ranges, a conv_in width that fits the context) is validated before the first weight is written,
+ * so a rejected file leaves the context as it was. Afterwards, as after sdb_load_dump_dir: call sdb_finalize_weights; every
+ * loaded norm uses the default eps; LoRA adapters are kept and merged onto the new weights by that finalize. */
+int sdb_load_safetensors(sdb_ctx* ctx, const char* path);
+#define SDB_CKPT_FULL 0
+#define SDB_CKPT_VAE 1
+/* The validation of sdb_load_safetensors without a context or a device, reading no tensor data: kind = SDB_CKPT_FULL or
+ * SDB_CKPT_VAE, conv_in_width = 4, 8 or 9 (the context to create: sdb_create, sdb_create_pix2pix, sdb_create_inpaint), 0 for a
+ * VAE-only file. Either pointer may be NULL. Errors via sdb_last_error(NULL). */
+int sdb_probe_safetensors(const char* path, int* kind, int* conv_in_width);
 /* Fills every tensor with the deterministic synthetic stream documented in
  * stable_diffusion_burn_b200/synth.py (bit-identical to the numpy generator). */
 int sdb_init_synthetic(sdb_ctx* ctx, uint32_t seed);

@@ -45,6 +45,8 @@ extern "C" {
     fn sdb_last_error(ctx: *mut SdbCtx) -> *const c_char;
     fn sdb_set_tensor(ctx: *mut SdbCtx, name: *const c_char, host: *const f32, dims: *const i64, ndim: c_int) -> c_int;
     fn sdb_load_dump_dir(ctx: *mut SdbCtx, path: *const c_char) -> c_int;
+    fn sdb_load_safetensors(ctx: *mut SdbCtx, path: *const c_char) -> c_int;
+    fn sdb_probe_safetensors(path: *const c_char, kind: *mut c_int, conv_in_width: *mut c_int) -> c_int;
     fn sdb_finalize_weights(ctx: *mut SdbCtx) -> c_int;
     fn sdb_clip_forward(ctx: *mut SdbCtx, tokens: *const i32, n: c_int, l: c_int, out: *mut f32) -> c_int;
     fn sdb_encode_image(ctx: *mut SdbCtx, img: *const f32, n: c_int, h: c_int, w: c_int, latent: *mut f32) -> c_int;
@@ -115,6 +117,25 @@ pub struct StableDiffusion {
     ctx: *mut SdbCtx,
 }
 
+/// What an SD-1.x .safetensors file holds (include/sdb200.h: sdb_probe_safetensors).
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub enum Checkpoint {
+    /// every weight; the UNet's conv_in takes this many channels: 4 (`new`), 9 (`new_inpaint`) or 8 (`new_pix2pix`)
+    Full { conv_in_width: i32 },
+    /// the autoencoder's weights only (a standalone SD VAE release)
+    Vae,
+}
+
+/// Validates an SD-1.x single-file .safetensors checkpoint without a context or a device (DESIGN.md §7 f13).
+pub fn probe_safetensors(path: &str) -> Result<Checkpoint, SdbError> {
+    let cpath = CString::new(path).unwrap();
+    let (mut kind, mut width) = (0 as c_int, 0 as c_int);
+    if unsafe { sdb_probe_safetensors(cpath.as_ptr(), &mut kind, &mut width) } != 0 {
+        return Err(SdbError(unsafe { CStr::from_ptr(sdb_last_error(std::ptr::null_mut())) }.to_string_lossy().into()));
+    }
+    Ok(if kind == 0 { Checkpoint::Full { conv_in_width: width } } else { Checkpoint::Vae })
+}
+
 impl StableDiffusion {
     /// Replaces `StableDiffusionConfig::new().init(&device)` (src/model/stablediffusion/mod.rs:22-39).
     pub fn new(device: i32) -> Result<Self, SdbError> {
@@ -167,6 +188,13 @@ impl StableDiffusion {
     pub fn load_dump_dir(&self, path: &str) -> Result<(), SdbError> {
         let cpath = CString::new(path).unwrap();
         self.check(unsafe { sdb_load_dump_dir(self.ctx, cpath.as_ptr()) })
+    }
+
+    /// An SD-1.x single-file .safetensors checkpoint in the original LDM layout, or a VAE-only file (DESIGN.md §7 f13), in
+    /// place of converting it to a dump-dir tree; then `finalize_weights`. A rejected file leaves the weights as they were.
+    pub fn load_safetensors(&self, path: &str) -> Result<(), SdbError> {
+        let cpath = CString::new(path).unwrap();
+        self.check(unsafe { sdb_load_safetensors(self.ctx, cpath.as_ptr()) })
     }
 
     pub fn finalize_weights(&self) -> Result<(), SdbError> {

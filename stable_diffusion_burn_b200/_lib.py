@@ -61,6 +61,8 @@ SIGNATURES = [
     ("sdb_test_gemm_ex", C.c_int, [_ctx, _f32p, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, _f32p,
                                    C.c_int, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_read_dump_tensor", C.c_int64, [C.c_char_p, C.c_int, C.POINTER(C.c_int64), _f32p, C.c_int64]),
+    ("sdb_load_safetensors", C.c_int, [_ctx, C.c_char_p]),
+    ("sdb_probe_safetensors", C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("sdb_encode_image", C.c_int, [_ctx, _f32p, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_encode_image_dev", C.c_int, [_ctx, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     ("sdb_clip_forward", C.c_int, [_ctx, C.POINTER(C.c_int32), C.c_int, C.c_int, _f32p]),
@@ -153,6 +155,19 @@ def ptr(a: np.ndarray):
 
 class SdbError(RuntimeError):
     pass
+
+
+CKPT_FULL, CKPT_VAE = 0, 1  # include/sdb200.h: SDB_CKPT_FULL, SDB_CKPT_VAE
+
+
+def probe_safetensors(path):
+    """Validates an SD-1.x .safetensors checkpoint without a context or a GPU (include/sdb200.h: sdb_probe_safetensors) ->
+    (kind, conv_in_width): (CKPT_FULL, 4 / 8 / 9) or (CKPT_VAE, 0). Raises SdbError naming what is wrong."""
+    lib = load()
+    kind, width = C.c_int(), C.c_int()
+    if lib.sdb_probe_safetensors(os.fsencode(path), C.byref(kind), C.byref(width)) != 0:
+        raise SdbError(lib.sdb_last_error(None).decode())
+    return kind.value, width.value
 
 
 def _rows(a, what):
@@ -428,6 +443,11 @@ class Context:
 
     def load_dump_dir(self, path):
         self.check(self.lib.sdb_load_dump_dir(self.h, os.fsencode(path)))
+
+    def load_safetensors(self, path):
+        """An SD-1.x single-file checkpoint or a VAE-only file (include/sdb200.h: sdb_load_safetensors); finalize_weights
+        afterwards."""
+        self.check(self.lib.sdb_load_safetensors(self.h, os.fsencode(path)))
 
     def encode_image(self, img):
         a = f32(img)

@@ -204,6 +204,22 @@ int64_t sdb_read_dump_tensor(const char* file, int ndim, int64_t* dims, float* d
   }
 }
 
+int sdb_load_safetensors(sdb_ctx* ctx, const char* path) {
+  API_BEGIN(ctx)
+  model_load_safetensors(c, path);
+  API_END
+}
+
+int sdb_probe_safetensors(const char* path, int* kind, int* conv_in_width) {
+  try {
+    safetensors_probe(path, kind, conv_in_width);
+    return 0;
+  } catch (const std::exception& e) {
+    g_err = e.what();
+    return 1;
+  }
+}
+
 int sdb_init_synthetic(sdb_ctx* ctx, uint32_t seed) {
   API_BEGIN(ctx)
   c.norm_eps.clear();

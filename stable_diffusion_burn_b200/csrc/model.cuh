@@ -66,6 +66,9 @@ void model_clip_forward_host(Ctx& c, const int* tokens, int n, int L, float* out
 bool npy_read_f32(const std::string& file, std::vector<float>& out);
 long long dump_tensor_read(const std::string& file, int ndim, int64_t* dims, std::vector<float>& payload);
 void model_load_dump_dir(Ctx& c, const char* root);
+// SD-1.x single-file .safetensors checkpoints (safetensors.cu)
+void model_load_safetensors(Ctx& c, const char* path);
+void safetensors_probe(const char* path, int* kind, int* conv_in_width);
 void model_test_attention(Ctx& c, const float* q, const float* k, const float* v, int n, int Nq, int Nk, int C, int heads,
                           const int32_t* kvlen, int flags, float* out);
 // ResBlock / concat-GroupNorm test entries (sdb200.h: sdb_test_resblock, sdb_test_groupnorm_cat); trace = kTestTraceInts ints

@@ -17,7 +17,7 @@ import contextlib
 
 import numpy as np
 
-from ._lib import Context
+from ._lib import CKPT_FULL, Context, probe_safetensors
 
 
 class UNet:
@@ -90,6 +90,28 @@ class StableDiffusion:
     def load_dump_dir(self, path: str):
         """load_stable_diffusion(path, device) (src/model/stablediffusion/load.rs:16-33): the reference's dump-dir tree."""
         self.ctx.load_dump_dir(path)
+        self.ctx.finalize_weights()
+        return self
+
+    @classmethod
+    def from_checkpoint(cls, path, device: int = 0):
+        """A context of the kind an SD-1.x single-file .safetensors checkpoint needs (a 4-, 9- (inpaint=True) or 8-channel
+        (pix2pix=True) UNet, read from its conv_in), loaded from it and finalized. A VAE-only file raises ValueError: load it
+        into an existing model with load_checkpoint."""
+        kind, width = probe_safetensors(path)
+        if kind != CKPT_FULL:
+            raise ValueError(f"{path} holds only a VAE: load it with load_checkpoint into a model created from a full checkpoint")
+        sd = cls(device, inpaint=width == 9, pix2pix=width == 8)
+        try:
+            return sd.load_checkpoint(path)
+        except Exception:
+            sd.close()
+            raise
+
+    def load_checkpoint(self, path):
+        """An SD-1.x single-file .safetensors checkpoint (every weight and the schedule) or a VAE-only file (the autoencoder's
+        weights only) (DESIGN.md §7 f13), then finalize. A rejected file leaves the weights as they were."""
+        self.ctx.load_safetensors(path)
         self.ctx.finalize_weights()
         return self
 
