@@ -81,6 +81,15 @@ __device__ __forceinline__ uint4 quad_transpose(uint32_t (&x)[4], int q) {
   return make_uint4(x[0], x[1], x[2], x[3]);
 }
 
+// 4 consecutive columns of a residual kept as an fp16 hi + lo pair, as fp32 hi + lo
+__device__ __forceinline__ float4 res_pair4(const __half* hi, const __half* lo) {
+  const uint2 h = *reinterpret_cast<const uint2*>(hi);
+  const uint2 l = *reinterpret_cast<const uint2*>(lo);
+  const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(&h.x)), h1 = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
+  const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(&l.x)), l1 = __half22float2(*reinterpret_cast<const __half2*>(&l.y));
+  return make_float4(h0.x + l0.x, h0.y + l0.y, h1.x + l1.x, h1.y + l1.y);
+}
+
 // Bucket reduction of the per-quarter column sums an epilogue left in shared memory (cs[q][col] = (sum, sumsq) of the 32 rows of
 // lane quarter q), written as this tile's GroupNorm partials. `nq` quarters per image slice (4 = the whole tile is one image).
 // which images the 128 rows of this tile belong to: g_tn images per tile (1, 2 or 4), the first one, the tile's index inside it
@@ -348,13 +357,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       if (res_pair) {
 #pragma unroll
         for (int i = 0; i < 8; ++i)
-          if (mr8[i] >= 0) {
-            const uint2 h = *reinterpret_cast<const uint2*>(p.res_hi + (unsigned)(ao[i] + col));
-            const uint2 l = *reinterpret_cast<const uint2*>(p.res_lo + (unsigned)(ao[i] + col));
-            const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(&h.x)), h1 = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
-            const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(&l.x)), l1 = __half22float2(*reinterpret_cast<const __half2*>(&l.y));
-            ad[i] = make_float4(h0.x + l0.x, h0.y + l0.y, h1.x + l1.x, h1.y + l1.y);
-          }
+          if (mr8[i] >= 0) ad[i] = res_pair4(p.res_hi + (unsigned)(ao[i] + col), p.res_lo + (unsigned)(ao[i] + col));
         return;
       }
       if (p.residual == nullptr) return;
@@ -440,13 +443,7 @@ gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
             float4 bv = make_float4(0.f, 0.f, 0.f, 0.f), rs = bv;
             if (p.bias) bv = *reinterpret_cast<const float4*>(p.bias + col);
             if (p.residual) rs = *reinterpret_cast<const float4*>(p.residual + (size_t)mr * p.ldc + col);
-            if (p.res_hi) {
-              const uint2 h = *reinterpret_cast<const uint2*>(p.res_hi + (size_t)mr * p.ldc16 + col);
-              const uint2 l = *reinterpret_cast<const uint2*>(p.res_lo + (size_t)mr * p.ldc16 + col);
-              const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(&h.x)), h1 = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
-              const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(&l.x)), l1 = __half22float2(*reinterpret_cast<const __half2*>(&l.y));
-              rs = make_float4(h0.x + l0.x, h0.y + l0.y, h1.x + l1.x, h1.y + l1.y);
-            }
+            if (p.res_hi) rs = res_pair4(p.res_hi + (size_t)mr * p.ldc16 + col, p.res_lo + (size_t)mr * p.ldc16 + col);
             const float* wp = p.ws + (size_t)mr * p.N + col;
             const size_t zs = Mtot * p.N;
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);

@@ -501,9 +501,9 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
       static const bool dbg_on = getenv("SDB_GEMM_DBG") != nullptr;
       static long long* dbg_buf = nullptr;
       if (dbg_on) {
-        if (!dbg_buf) SDB_CUDA(cudaMallocManaged(&dbg_buf, 16 * sizeof(long long)));
+        if (!dbg_buf) SDB_CUDA(cudaMallocManaged(&dbg_buf, 8 * sizeof(long long)));
         SDB_CUDA(cudaStreamSynchronize(c.stream));
-        memset(dbg_buf, 0, 16 * sizeof(long long));
+        memset(dbg_buf, 0, 8 * sizeof(long long));
         p.dbg = dbg_buf;
       }
       const std::string label = c.dbg_label;
@@ -511,12 +511,11 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
         KernelScope ks(c, KC_GEMM, flops * phases_out, bytes * phases_out, flops * passes * phases_out);
         gemm_tc_launch(maps, p, BN, passes, c.stream);
       }
-      if (dbg_on) {  // bring-up aid: cycle stamps of CTA (0,0,0), printed relative to kernel entry
+      if (dbg_on) {  // bring-up aid: the 8 cycle stamps of the first CTA, printed relative to kernel entry (stamp 0)
         SDB_CUDA(cudaStreamSynchronize(c.stream));
-        fprintf(stderr, "gemm_dbg %s | cycles since entry: prologue %lld tma0 %lld landed %lld lastmma %lld accum %lld epi %lld exit %lld | chunk0: ld %lld stage %lld finish %lld (bias %lld loads0 %lld batch0 %lld)\n",
+        fprintf(stderr, "gemm_dbg %s | cycles since entry: prologue %lld tma0 %lld landed %lld lastmma %lld accum %lld epi %lld exit %lld | clock64 at entry %lld\n",
                 label.c_str(), dbg_buf[1] - dbg_buf[0], dbg_buf[2] - dbg_buf[0], dbg_buf[3] - dbg_buf[0],
-                dbg_buf[4] - dbg_buf[0], dbg_buf[5] - dbg_buf[0], dbg_buf[6] - dbg_buf[0], dbg_buf[7] - dbg_buf[0], dbg_buf[9] - dbg_buf[8], dbg_buf[10] - dbg_buf[9],
-                dbg_buf[11] - dbg_buf[10], dbg_buf[12] - dbg_buf[10], dbg_buf[13] - dbg_buf[12], dbg_buf[14] - dbg_buf[13]);
+                dbg_buf[4] - dbg_buf[0], dbg_buf[5] - dbg_buf[0], dbg_buf[6] - dbg_buf[0], dbg_buf[7] - dbg_buf[0], dbg_buf[0]);
       }
     }
     // (the split-K reduction happens inside the kernel: after a ticket rendezvous every split CTA folds its slice of the tile rows)

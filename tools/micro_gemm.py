@@ -1,5 +1,6 @@
-"""Fixed-cost probe of gemm_tc. With SDB_GEMM_DBG=1 every launch prints the clock64 stamps of CTA (0,0,0):
-prologue done / first TMA issued / first operands landed / last MMA issued / accumulator ready / epilogue done / exit."""
+"""Fixed-cost probe of gemm_tc. With SDB_GEMM_DBG=1 every launch prints the clock64 stamps of its first CTA, in cycles since
+entry: prologue done / first TMA issued / first operands landed / last MMA issued / accumulator ready / epilogue done / exit,
+then the raw clock64 counter value at entry."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
