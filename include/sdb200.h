@@ -311,12 +311,20 @@ int sdb_profile_get_issued(sdb_ctx* ctx, int cls, double* issued_flops);
 int64_t sdb_launch_count(sdb_ctx* ctx);
 
 /* ---- unit-test entry points for single kernels (host pointers) ------------------------------- */
-/* The GEMM test entries below (sdb_test_linear, sdb_test_gemm_ex, sdb_test_conv2d, sdb_test_ln_fold, sdb_test_conv_groupnorm)
- * take a trailing `trace`: NULL, or SDB_GEMM_TRACE_INTS ints that receive what each GEMM of the call launched, so a test can
- * assert which kernel instance it reached. [0] GEMMs, then 14 ints each from [1] (at most 4 GEMMs): the 13 of
- * sdb_test_clip_block (kind, N, BN, split-K, TN, TH, TW, extra-K channels, GroupNorm slots written, second-source channels,
- * passes, epilogue roles, activation), then the pipeline stages of the kernel instance. */
-#define SDB_GEMM_TRACE_INTS 64
+/* The test entries that take a trailing `trace` accept NULL, or SDB_TRACE_INTS ints that receive a record of every launch of
+ * the call whose choice a test asserts, in launch order: [0] the record count, then 16 ints per record from [1], a kind tag and
+ * its fields, zero-padded. A call whose records do not fit fails with an error naming the count; nothing is truncated. Kinds:
+ *   1 GEMM: kind (0 Linear, 1 1x1 conv, 2 3x3 conv, 3 stride 2, 4 folded nearest-2x, 5 stride 2 padded bottom/right), N, BN,
+ *     split-K, TN, TH, TW, extra-K channels, GroupNorm slots written, second-source channels, passes, epilogue roles (1
+ *     LayerNorm statistics, 2 LayerNorm-consuming, 4 GEGLU, 8 fp16-pair residual, 16 fp32 residual, 32 GroupNorm partials),
+ *     activation (1 QuickGELU), pipeline stages of the kernel instance
+ *   2 fused attention: dpad, Nq, Nk, split q / k (hi + lo), per-sample lengths, causal
+ *   3 GroupNorm staging: its path (1 fused statistics + apply, 2 apply from producer partials, 3 apply after the 64:1 pre-fold;
+ *     sums for the fused GroupNorm + small-Cout conv: 4 by the statistics kernel, 5 from producer partials, 6 after the pre-fold)
+ *   4 fused GroupNorm + small-Cout conv: rows per tile, channels per round, channel groups
+ *   5 autoencoder attention row softmax: values per thread
+ *   6 conditioned UNet conv_in: m, sample s reads the conditioning of sample s % m */
+#define SDB_TRACE_INTS 1024
 /* C[M,N] (fp32) = A[M,K] (fp32, rounded to the operand format) x B[K,N] (fp32 [in,out]) + bias.
  * Exercises the wgmma GEMM exactly as the Linear layers use it. */
 int sdb_test_linear(sdb_ctx* ctx, const float* a, const float* w, const float* bias, int M, int K, int N,
@@ -363,9 +371,8 @@ int sdb_test_attention(sdb_ctx* ctx, const float* q, const float* k, const float
  * bias (the model passes conv_in.bias + lin_embed(silu(emb))). flags: 1 / 2 = x0 / x1 are written by a producer that leaves
  * GroupNorm statistics (a 3-pass identity conv: the block then sees hi + lo of the input, 22 bits); otherwise an fp32 tensor
  * with an fp16 copy and no statistics. Outputs [n][cout][H][W]: out, out16 = its fp16 hi + lo copy (zero without the raw16
- * option), out_norm = SiLU(GroupNorm(out; norm2)) staged from the statistics conv2 left. trace (64 ints): [0] GroupNorm
- * stagings, [1..4] their path (1 fused, 2 apply from producer partials, 3 apply after the 64:1 pre-fold), [5] GEMMs, then 10 ints
- * per GEMM: kind, N, BN, split-K, TN, TH, TW, extra-K channels, GroupNorm slots written, second-source channels. */
+ * option), out_norm = SiLU(GroupNorm(out; norm2)) staged from the statistics conv2 left. trace: NULL or SDB_TRACE_INTS ints (see
+ * above). */
 int sdb_test_resblock(sdb_ctx* ctx, const float* x0, const float* x1, int n, int c0, int c1, int H, int W, int cout,
                       const float* norm1_g, const float* norm1_b, const float* conv1_w, const float* conv1_b, const float* norm2_g,
                       const float* norm2_b, const float* conv2_w, const float* conv2_b, const float* skip_w, const float* skip_b,
@@ -373,7 +380,7 @@ int sdb_test_resblock(sdb_ctx* ctx, const float* x0, const float* x1, int n, int
 /* GroupNorm(32 groups)(+SiLU) of cat([x0, x1]) (x1 NULL when c1 = 0) as an fp16 hi + lo operand, returned NCHW as hi + lo.
  * mode 0: statistics kernel over both sources + apply; 1: the fused statistics + apply kernel; 2: apply from the partials two
  * producers left (3-pass identity convs, which pass hi + lo of the inputs), with the 64:1 pre-fold above 128 slots per image.
- * trace as sdb_test_resblock. */
+ * trace: NULL or SDB_TRACE_INTS ints (see above). */
 int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n, int c0, int c1, int H, int W,
                            const float* gamma, const float* beta, int silu, int mode, float* y, int32_t* trace);
 /* One of the UNet's 16 SpatialTransformers (unet/mod.rs:461-481), index = its position in execution order (0..5 input blocks,
@@ -384,10 +391,7 @@ int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n
  * flags: 1 = the output carries an fp16 hi + lo copy (else out16 is zero). Outputs: out, out16 [n][C][H][W]; out_norm =
  * SiLU(GroupNorm(out; the block's own norm)) staged the way the next ResBlock stages its input; taps_y [4][n*H*W][C] = the residual
  * stream (hi + lo) after proj_in, attn1, attn2 and the MLP; taps_ln [3][n*H*W][2] = (sum, sum of squares) per token row that
- * norm1 / norm2 / norm3 read. trace (160 ints): [0] GroupNorm stagings, [1..4] their path (as sdb_test_resblock), [5] GEMMs, then
- * 12 ints per GEMM: kind, N, BN, split-K, TN, TH, TW, extra-K channels, GroupNorm slots written, second-source channels, passes,
- * epilogue roles (1 LayerNorm statistics, 2 LayerNorm-consuming, 4 GEGLU, 8 fp16-pair residual, 16 fp32 residual, 32 GroupNorm
- * partials); [126] attention launches, then 5 ints each from [127]: dpad, Nq, Nk, split q / k (hi + lo), per-sample lengths. */
+ * norm1 / norm2 / norm3 read. trace: NULL or SDB_TRACE_INTS ints (see above). */
 int sdb_test_spatial_transformer(sdb_ctx* ctx, int index, const float* x, int n, int c, int H, int W, const float* context,
                                  int lmax, const int32_t* lens, int flags, float* out, float* out16, float* out_norm, float* taps_y,
                                  float* taps_ln, int32_t* trace);
@@ -405,11 +409,8 @@ int sdb_test_spatial_transformer(sdb_ctx* ctx, int index, const float* x, int n,
  *   SDB_VAE_ENC_DOWN0..2  encoder/blocks/i/downsampler (c 128 / 256 / 512, H and W even) -> [n][c][H/2][W/2]; out_norm =
  *                      SiLU(GroupNorm(out; blocks/i+1/res1/norm1)) from the conv's partials
  * flags: 1 = x is staged with GroupNorm partials, as a ResnetBlock leaves it (a 3-pass identity conv: the stage sees hi + lo of x);
- * else the fp32 tensor without statistics. out16 / tap / out_norm may be NULL where a stage has none. trace (256 ints): [0]
- * GroupNorm stagings, [1..4] their path (1-3 as sdb_test_resblock; 4 sums by the statistics kernel, 5 sums from producer partials,
- * 6 after the 64:1 pre-fold), [5] GEMMs, 12 ints each from [6] (as sdb_test_spatial_transformer), [200] small-Cout conv launches,
- * [201..203] its rows per tile, channels per round and channel groups, [204] softmax launches, [205] their values per thread,
- * [206] m of SDB_VAE_UNET_IN's cond (0 without cond). */
+ * else the fp32 tensor without statistics. out16 / tap / out_norm may be NULL where a stage has none. trace: NULL or
+ * SDB_TRACE_INTS ints (see above). */
 enum {
   SDB_VAE_DEC_IN = 0,
   SDB_VAE_DEC_ATTN = 1,
@@ -431,8 +432,7 @@ int sdb_test_vae_stage(sdb_ctx* ctx, int stage, const float* x, const float* con
  * flags: 1 = the pad rows hold large finite junk instead of zeros. out [n][L][768] = the block output (index 12: the final
  * LayerNorm). taps (NULL, or unused for index 12) = 11 planes of [n][L][768] floats: LN1 (fp16 hi + lo), q, k (fp16), V (read
  * back from V^T, fp16), the attention output (hi + lo), x after the attention, LN2 (hi + lo), then QuickGELU(fc1) (hi + lo) as
- * [n][L][3072]. trace (80 ints): [0] GEMMs, 13 ints each from [1]: the 12 of sdb_test_spatial_transformer, then the epilogue
- * activation (1 QuickGELU); [70] attention launches, [71..76] dpad, Nq, Nk, split q / k, per-sample lengths, causal. */
+ * [n][L][3072]. trace: NULL or SDB_TRACE_INTS ints (see above). */
 int sdb_test_clip_block(sdb_ctx* ctx, int index, const float* x, int n, int L, int flags, float* out, float* taps,
                         int32_t* trace);
 /* The first `count` values of stochastic DDIM's noise z at timestep t (0 <= t < 1000) for noise_seed, as the fused sampler step

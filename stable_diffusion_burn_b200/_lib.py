@@ -595,26 +595,55 @@ class Context:
         return int(self.lib.sdb_launch_count(self.h))
 
     # ---- single-kernel test entries
-    # The GEMM entries take trace=True to also return what each of their GEMMs launched (include/sdb200.h: SDB_GEMM_TRACE_INTS):
-    # a list of dicts with the keys below, "epi" as the set of _EPI_ROLES names.
-    GEMM_TRACE_INTS = 64
+    # The traced entries fill SDB_TRACE_INTS ints with one 16-int record per launch (include/sdb200.h); _decode_trace turns them
+    # into the lists of the record kinds an entry launches, in launch order. The GEMM entries take trace=True to also return
+    # their "gemms" list.
+    TRACE_INTS = 1024
+    _TRACE_KINDS = {1: "gemms", 2: "attn", 3: "gn", 4: "conv", 5: "softmax", 6: "cond_mod"}
     _GEMM_TRACE_KEYS = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1", "passes", "epi", "act", "stages")
+    _ATTN_TRACE_KEYS = ("dpad", "Nq", "Nk", "qk3", "kvlen")
+    _EPI_ROLES = ("lns", "lnc", "geglu", "res16", "res32", "gn")
+    _GN_PATHS = {1: "fused", 2: "apply", 3: "apply+fold", 4: "sums:stats", 5: "sums:partials", 6: "sums:fold"}
 
     @staticmethod
-    def _trace_buf(trace):
+    def _trace_buf(trace=True):
         if not trace:
             return None, None
-        t = np.zeros(Context.GEMM_TRACE_INTS, np.int32)
+        t = np.zeros(Context.TRACE_INTS, np.int32)
         return t, t.ctypes.data_as(C.POINTER(C.c_int32))
 
     @classmethod
-    def _decode_gemm_trace(cls, t):
-        gemms = []
+    def _decode_trace(cls, t, kinds):
+        """-> {kind: entries} for the record kinds `kinds` of _TRACE_KINDS the entry launches (a record of another kind is an
+        error): "gemms": dicts of _GEMM_TRACE_KEYS with "epi" as the set of _EPI_ROLES names; "attn": dicts of _ATTN_TRACE_KEYS,
+        plus causal=1 on a causal launch; "gn": _GN_PATHS names; "conv": (rows per tile, channels per round, channel groups);
+        "softmax": values per thread; one entry per launch. "cond_mod": m of the one conditioned conv_in, 0 without one."""
+        tr = {k: 0 if k == "cond_mod" else [] for k in kinds}
         for i in range(int(t[0])):
-            g = dict(zip(cls._GEMM_TRACE_KEYS, (int(v) for v in t[1 + 14 * i:15 + 14 * i])))
-            g["epi"] = {r for b, r in enumerate(cls._EPI_ROLES) if g["epi"] >> b & 1}
-            gemms.append(g)
-        return gemms
+            kind, *f = (int(v) for v in t[1 + 16 * i:17 + 16 * i])
+            name = cls._TRACE_KINDS.get(kind)
+            if name not in tr:
+                raise ValueError(f"trace record {i}: kind {kind} is not one of {kinds}")
+            if name == "cond_mod":
+                if tr[name]:
+                    raise ValueError("trace: more than one conditioned conv_in")
+                tr[name] = f[0]
+                continue
+            if kind == 1:
+                rec = dict(zip(cls._GEMM_TRACE_KEYS, f))
+                rec["epi"] = {r for b, r in enumerate(cls._EPI_ROLES) if rec["epi"] >> b & 1}
+            elif kind == 2:
+                rec = dict(zip(cls._ATTN_TRACE_KEYS, f))
+                if f[5]:
+                    rec["causal"] = f[5]
+            elif kind == 3:
+                rec = cls._GN_PATHS[f[0]]
+            elif kind == 4:
+                rec = tuple(f[:3])
+            else:
+                rec = f[0]
+            tr[name].append(rec)
+        return tr
 
     def test_linear(self, a, w, bias=None, passes=1, trace=False):
         a = f32(a); w = f32(w)
@@ -624,7 +653,7 @@ class Context:
         t, tp = self._trace_buf(trace)
         self.check(self.lib.sdb_test_linear(self.h, ptr(a), ptr(w), ptr(b) if b is not None else None, M, K, N, passes, ptr(out),
                                             tp))
-        return (out, self._decode_gemm_trace(t)) if trace else out
+        return (out, self._decode_trace(t, ("gemms",))["gemms"]) if trace else out
 
     def test_gemm_ex(self, a, w, bias=None, residual=None, passes=1, geglu=False, from_f16=False, xa=None, xw=None,
                      planes=False, trace=False):
@@ -644,7 +673,7 @@ class Context:
         self.check(self.lib.sdb_test_gemm_ex(self.h, ptr(a), ptr(w), keep[0][1], keep[1][1], M, K, N, passes, flags, keep[2][1],
                                              keep[3][1], XK, ptr(out), tp))
         res = (out[0], out[1]) if planes else out
-        return (res, self._decode_gemm_trace(t)) if trace else res
+        return (res, self._decode_trace(t, ("gemms",))["gemms"]) if trace else res
 
     def test_conv2d(self, x, w, bias=None, stride=1, upsample=0, passes=1, trace=False):
         x = f32(x); w = f32(w)
@@ -657,7 +686,7 @@ class Context:
         t, tp = self._trace_buf(trace)
         self.check(self.lib.sdb_test_conv2d(self.h, ptr(x), ptr(w), ptr(b) if b is not None else None, n, cin, H, W, cout,
                                             k, stride, upsample, passes, ptr(y), tp))
-        return (y, self._decode_gemm_trace(t)) if trace else y
+        return (y, self._decode_trace(t, ("gemms",))["gemms"]) if trace else y
 
     def test_ln_fold(self, a, w0, b0, gamma, beta, w1, b1=None, a2=None, passes=3, geglu=False, trace=False):
         a, w0, b0, gamma, beta, w1 = (f32(v) for v in (a, w0, b0, gamma, beta, w1))
@@ -669,7 +698,7 @@ class Context:
         self.check(self.lib.sdb_test_ln_fold(self.h, ptr(a), ptr(a2) if a2 is not None else None, ptr(w0), ptr(b0), ptr(gamma),
                                              ptr(beta), ptr(w1), ptr(b1) if b1 is not None else None, M, K0, Cc, N, passes,
                                              1 if geglu else 0, ptr(out), tp))
-        return (out, self._decode_gemm_trace(t)) if trace else out
+        return (out, self._decode_trace(t, ("gemms",))["gemms"]) if trace else out
 
     def test_conv_groupnorm(self, x, w, bias, gamma, beta, passes=3, silu=False, stride=1, upsample=0, trace=False):
         x = f32(x); w = f32(w); bias = f32(bias); gamma = f32(gamma); beta = f32(beta)
@@ -682,22 +711,14 @@ class Context:
         t, tp = self._trace_buf(trace)
         self.check(self.lib.sdb_test_conv_groupnorm(self.h, ptr(x), ptr(w), ptr(bias), ptr(gamma), ptr(beta), n, cin, H, W, cout, k,
                                                     stride, upsample, passes, 1 if silu else 0, ptr(y), C.byref(slots), tp))
-        return (y, slots.value, self._decode_gemm_trace(t)) if trace else (y, slots.value)
-
-    @staticmethod
-    def _decode_trace(t):
-        """trace ints of sdb_test_resblock / sdb_test_groupnorm_cat -> {"gn": [...], "gemms": [...]}"""
-        paths = {1: "fused", 2: "apply", 3: "apply+fold"}
-        keys = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1")
-        gemms = [dict(zip(keys, (int(v) for v in t[6 + 10 * i:16 + 10 * i]))) for i in range(min(int(t[5]), 5))]
-        return {"gn": [paths.get(int(v), int(v)) for v in t[1:1 + min(int(t[0]), 4)]], "gemms": gemms}
+        return (y, slots.value, self._decode_trace(t, ("gemms",))["gemms"]) if trace else (y, slots.value)
 
     def test_resblock(self, x0, x1, norm1, conv1, norm2, conv2, skip=None, emb_bias=None, passes=1, x0_stats=True,
                       x1_stats=True):
         """One ResBlock (emb_bias given) or VAE ResnetBlock (emb_bias None) on cat([x0, x1]); norm* = (gamma, beta),
         conv* / skip = (weight OIHW, bias). -> (out, out16, out_norm, trace): the block output, its fp16 hi + lo copy,
-        SiLU(GroupNorm(out; norm2)) from the statistics conv2 left, and what ran ({"gn": paths, "gemms": launch choices,
-        "skip": "merged" | "separate" | "none"})."""
+        SiLU(GroupNorm(out; norm2)) from the statistics conv2 left, and what ran (_decode_trace, plus "skip": "merged" |
+        "separate" | "none")."""
         x0 = f32(x0)
         n, c0, H, W = x0.shape
         x1 = f32(x1) if x1 is not None else None
@@ -708,12 +729,11 @@ class Context:
         eb = f32(emb_bias) if emb_bias is not None else None
         p = lambda a: None if a is None else ptr(a)
         out, out16, outn = (np.empty((n, cout, H, W), np.float32) for _ in range(3))
-        trace = np.zeros(64, np.int32)
+        t, tp = self._trace_buf()
         flags = (1 if x0_stats else 0) | (2 if (x1 is not None and x1_stats) else 0)
         self.check(self.lib.sdb_test_resblock(self.h, ptr(x0), p(x1), n, c0, c1, H, W, cout, *(ptr(a) for a in keep), p(sk[0]),
-                                              p(sk[1]), p(eb), passes, flags, ptr(out), ptr(out16), ptr(outn),
-                                              trace.ctypes.data_as(C.POINTER(C.c_int32))))
-        tr = self._decode_trace(trace)
+                                              p(sk[1]), p(eb), passes, flags, ptr(out), ptr(out16), ptr(outn), tp))
+        tr = self._decode_trace(t, ("gn", "gemms"))
         g = tr["gemms"]
         tr["skip"] = "separate" if len(g) == 3 else ("merged" if g and g[-1]["xk"] > 0 else "none")
         return out, out16, outn, tr
@@ -727,18 +747,16 @@ class Context:
         c1 = 0 if x1 is None else x1.shape[1]
         g = f32(gamma); b = f32(beta)
         y = np.empty((n, c0 + c1, H, W), np.float32)
-        trace = np.zeros(64, np.int32)
+        t, tp = self._trace_buf()
         self.check(self.lib.sdb_test_groupnorm_cat(self.h, ptr(x0), None if x1 is None else ptr(x1), n, c0, c1, H, W, ptr(g), ptr(b),
-                                                   1 if silu else 0, int(mode), ptr(y), trace.ctypes.data_as(C.POINTER(C.c_int32))))
-        return y, self._decode_trace(trace)
-
-    _EPI_ROLES = ("lns", "lnc", "geglu", "res16", "res32", "gn")
+                                                   1 if silu else 0, int(mode), ptr(y), tp))
+        return y, self._decode_trace(t, ("gn", "gemms"))
 
     def test_spatial_transformer(self, index, x, context, lens, act16=True):
         """The UNet's SpatialTransformer number `index` (execution order, 0..15) on its finalized weights. x [n, C, H, W];
         context [n, Lmax, 768] with per-sample lengths lens [n]. -> dict: out, out16 (its fp16 hi + lo copy, zero unless act16),
         out_norm = SiLU(GroupNorm(out; the block's norm)), y [4, n*H*W, C] (the residual stream after proj_in, attn1, attn2, MLP),
-        ln [3, n*H*W, 2] (the row sums norm1..3 read), trace ({"gn": paths, "gemms": [...], "attn": [...]})."""
+        ln [3, n*H*W, 2] (the row sums norm1..3 read), trace (_decode_trace)."""
         x = f32(x); context = f32(context)
         n, c, H, W = x.shape
         lens = np.ascontiguousarray(lens, dtype=np.int32)
@@ -746,28 +764,16 @@ class Context:
         out, out16, outn = (np.empty((n, c, H, W), np.float32) for _ in range(3))
         y = np.empty((4, n * H * W, c), np.float32)
         ln = np.empty((3, n * H * W, 2), np.float32)
-        t = np.zeros(160, np.int32)
-        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
+        t, tp = self._trace_buf()
         self.check(self.lib.sdb_test_spatial_transformer(self.h, int(index), ptr(x), n, c, H, W, ptr(context), context.shape[1],
-                                                         i32(lens), 1 if act16 else 0, ptr(out), ptr(out16), ptr(outn), ptr(y),
-                                                         ptr(ln), i32(t)))
-        paths = {1: "fused", 2: "apply", 3: "apply+fold"}
-        keys = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1", "passes")
-        gemms = []
-        for i in range(min(int(t[5]), 10)):
-            g = dict(zip(keys, (int(v) for v in t[6 + 12 * i:17 + 12 * i])))
-            g["epi"] = {r for b, r in enumerate(self._EPI_ROLES) if int(t[17 + 12 * i]) >> b & 1}
-            gemms.append(g)
-        attn = [dict(zip(("dpad", "Nq", "Nk", "qk3", "kvlen"), (int(v) for v in t[127 + 5 * i:132 + 5 * i])))
-                for i in range(min(int(t[126]), 4))]
-        tr = {"gn": [paths.get(int(v), int(v)) for v in t[1:1 + min(int(t[0]), 4)]], "gemms": gemms, "attn": attn}
-        return dict(out=out, out16=out16, out_norm=outn, y=y, ln=ln, trace=tr)
+                                                         lens.ctypes.data_as(C.POINTER(C.c_int32)), 1 if act16 else 0, ptr(out),
+                                                         ptr(out16), ptr(outn), ptr(y), ptr(ln), tp))
+        return dict(out=out, out16=out16, out_norm=outn, y=y, ln=ln, trace=self._decode_trace(t, ("gn", "gemms", "attn")))
 
     # sdb_test_vae_stage stages (include/sdb200.h: SDB_VAE_*): name -> (stage, input channels, output channels)
     VAE_STAGES = {"dec_in": (0, 4, 512), "dec_attn": (1, 512, 512), "enc_attn": (2, 512, 512), "dec_out": (3, 128, 3),
                   "unet_out": (4, 320, 4), "enc_out": (5, 512, 8), "enc_in": (6, 4, 128), "unet_in": (7, 4, 320),
                   "enc_down0": (8, 128, 128), "enc_down1": (9, 256, 256), "enc_down2": (10, 512, 512)}
-    _GN_PATHS = {1: "fused", 2: "apply", 3: "apply+fold", 4: "sums:stats", 5: "sums:partials", 6: "sums:fold"}
 
     def test_vae_stage(self, stage, x, cond=None, scale=1.0, stats=True, quant=None):
         """One autoencoder stage (or the UNet's conv_in / out conv) on the finalized weights, by name of VAE_STAGES. x
@@ -775,8 +781,7 @@ class Context:
         the strided quant slice's scale; stats: x carries producer GroupNorm partials; quant ("enc_out" only): None for the plain
         quant slice, or an [n, 5, H, W] array the strided + scaled slice writes channels 1-4 of (the rest is kept).
         -> dict: out [n, cout, Ho, Wo]; out16 (its fp16 hi + lo copy, "unet_in"); tap (the attention output before proj_out, or
-        the quant slice's output); out_norm (the next ResnetBlock's norm1 operand); trace ({"gn", "gemms", "conv", "softmax",
-        "cond_mod"})."""
+        the quant slice's output); out_norm (the next ResnetBlock's norm1 operand); trace (_decode_trace)."""
         sid, cin, cout = self.VAE_STAGES[stage]
         x = f32(x)
         n, c, H, W = x.shape
@@ -792,47 +797,30 @@ class Context:
             tap = np.zeros((n, 4, H, W), np.float32) if quant is None else f32(quant).copy()
             assert quant is None or tap.shape == (n, 5, H, W)
         cnd = f32(cond) if cond is not None else None
-        t = np.zeros(256, np.int32)
+        t, tp = self._trace_buf()
         p = lambda a: None if a is None else ptr(a)
         flags = (1 if stats else 0) | (2 if quant is not None else 0)
         self.check(self.lib.sdb_test_vae_stage(self.h, sid, ptr(x), p(cnd), n, c, H, W, float(scale), flags, ptr(out), p(out16),
-                                               p(tap), p(out_norm), t.ctypes.data_as(C.POINTER(C.c_int32))))
-        keys = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1", "passes")
-        gemms = []
-        for i in range(min(int(t[5]), 16)):
-            g = dict(zip(keys, (int(v) for v in t[6 + 12 * i:17 + 12 * i])))
-            g["epi"] = {r for b, r in enumerate(self._EPI_ROLES) if int(t[17 + 12 * i]) >> b & 1}
-            gemms.append(g)
-        tr = {"gn": [self._GN_PATHS.get(int(v), int(v)) for v in t[1:1 + min(int(t[0]), 4)]], "gemms": gemms,
-              "conv": [tuple(int(v) for v in t[201:204])] * int(t[200]), "softmax": [int(t[205])] * int(t[204]),
-              "cond_mod": int(t[206])}
-        return dict(out=out, out16=out16, tap=tap, out_norm=out_norm, trace=tr)
+                                               p(tap), p(out_norm), tp))
+        return dict(out=out, out16=out16, tap=tap, out_norm=out_norm,
+                    trace=self._decode_trace(t, ("gn", "gemms", "conv", "softmax", "cond_mod")))
 
     CLIP_TAPS = ("ln1", "q", "k", "v", "o", "x_attn", "ln2", "h")
 
     def test_clip_block(self, index, x, junk=False, taps=True):
         """CLIP block `index` (0..11), or the final LayerNorm (12), on the finalized weights. x [n, L, 768] is the residual
         stream entering it; junk: the pad rows of the row pitch hold large finite values instead of zeros. -> dict: out
-        [n, L, 768]; the taps of CLIP_TAPS ([n, L, 768], h [n, L, 3072]) unless taps is False or index is 12; trace ({"gemms":
-        [...], "attn": [...]})."""
+        [n, L, 768]; the taps of CLIP_TAPS ([n, L, 768], h [n, L, 3072]) unless taps is False or index is 12; trace
+        (_decode_trace)."""
         x = f32(x)
         n, L, D = x.shape
         assert D == 768
         out = np.empty((n, L, 768), np.float32)
         tp = np.zeros((11, n, L, 768), np.float32) if taps and index < 12 else None
-        t = np.zeros(80, np.int32)
-        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
+        t, trp = self._trace_buf()
         self.check(self.lib.sdb_test_clip_block(self.h, int(index), ptr(x), n, L, 1 if junk else 0, ptr(out),
-                                                None if tp is None else ptr(tp), i32(t)))
-        keys = ("kind", "N", "BN", "split", "TN", "TH", "TW", "xk", "gn_slots", "a1", "passes")
-        gemms = []
-        for i in range(min(int(t[0]), 5)):
-            g = dict(zip(keys, (int(v) for v in t[1 + 13 * i:12 + 13 * i])))
-            g["epi"] = {r for b, r in enumerate(self._EPI_ROLES) if int(t[12 + 13 * i]) >> b & 1}
-            g["act"] = int(t[13 + 13 * i])
-            gemms.append(g)
-        attn = [dict(zip(("dpad", "Nq", "Nk", "qk3", "kvlen", "causal"), (int(v) for v in t[71:77])))] * min(int(t[70]), 1)
-        res = dict(out=out, trace={"gemms": gemms, "attn": attn})
+                                                None if tp is None else ptr(tp), trp))
+        res = dict(out=out, trace=self._decode_trace(t, ("gemms", "attn")))
         if tp is not None:
             res.update({k: tp[i] for i, k in enumerate(self.CLIP_TAPS[:7])})
             res["h"] = tp[7:].reshape(n, L, 3072)

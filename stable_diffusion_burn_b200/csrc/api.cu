@@ -632,43 +632,15 @@ int64_t sdb_launch_count(sdb_ctx* ctx) { return ctx ? ctx->c.launches : -1; }
 // ------------------------------------------------------------------------------ single-kernel test entries
 // (host pointers; each call stages through the context's work arena)
 
-// The GEMM launch record of one test call (trace = NULL or SDB_GEMM_TRACE_INTS ints, include/sdb200.h): [0] GEMMs, then per GEMM
-// the 13 ints of Ctx::GemmRecord and the stage count of the kernel instance run_gemm chose.
-struct GemmTraceScope {
-  static constexpr int kPer = 14, kMax = (SDB_GEMM_TRACE_INTS - 1) / kPer;
-  Ctx& c;
-  int32_t* out;
-  GemmTraceScope(Ctx& c, int32_t* out) : c(c), out(out) {
-    c.gemm_trace.clear();
-    c.trace_on = out != nullptr;
-  }
-  ~GemmTraceScope() { c.trace_on = false; }
-  void write() const {
-    if (!out) return;
-    SDB_CHECK((int)c.gemm_trace.size() <= kMax, "GEMM trace: too many GEMMs for the trace");
-    std::fill(out, out + SDB_GEMM_TRACE_INTS, 0);
-    out[0] = (int)c.gemm_trace.size();
-    for (size_t i = 0; i < c.gemm_trace.size(); ++i) {
-      const Ctx::GemmRecord& r = c.gemm_trace[i];
-      const int v[kPer] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels, r.passes, r.epi,
-                           r.act, gemm_tc_stages(r.BN, r.passes)};
-      std::copy(v, v + kPer, out + 1 + kPer * i);
-    }
-  }
-};
-
 int sdb_test_linear(sdb_ctx* ctx, const float* a, const float* w, const float* bias, int M, int K, int N, int passes,
                     float* out, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  GemmTraceScope ts(c, trace);
-  float* d_a = c.work.get<float>((size_t)M * K);
-  float* d_w = c.work.get<float>((size_t)K * N);
-  float* d_b = bias ? c.work.get<float>(N) : nullptr;
+  TraceScope ts(c, trace);
+  float* d_a = upload(c, a, (size_t)M * K);
+  float* d_w = upload(c, w, (size_t)K * N);
+  float* d_b = upload(c, bias, N);
   float* d_c = c.work.get<float>((size_t)M * N);
-  SDB_CUDA(cudaMemcpyAsync(d_a, a, sizeof(float) * M * K, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_w, w, sizeof(float) * K * N, cudaMemcpyHostToDevice, c.stream));
-  if (bias) SDB_CUDA(cudaMemcpyAsync(d_b, bias, sizeof(float) * N, cudaMemcpyHostToDevice, c.stream));
   ActOp A;
   A.p.hi = c.work.get<__half>((size_t)M * K);
   A.p.lo = c.work.get<__half>((size_t)M * K);
@@ -693,20 +665,15 @@ int sdb_test_gemm_ex(sdb_ctx* ctx, const float* a, const float* w, const float* 
                      int passes, int flags, const float* xa, const float* xw, int XK, float* out, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  GemmTraceScope ts(c, trace);
+  TraceScope ts(c, trace);
   const bool geglu = flags & 1, from_f16 = flags & 4, planes = flags & 8;
   SDB_CHECK(!planes || from_f16, "gemm_ex test: the separate fp16 planes (flag 8) need the fp16 outputs (flag 4)");
   SDB_CHECK(!geglu || (N % 128 == 0 && !residual && !xa), "GEGLU test: N (= 2 * hidden) must be a multiple of 128, no residual / extra K");
   const int Nout = geglu ? N / 2 : N;
-  auto up = [&](const float* h, size_t cnt) {
-    float* d = c.work.get<float>(cnt);
-    SDB_CUDA(cudaMemcpyAsync(d, h, sizeof(float) * cnt, cudaMemcpyHostToDevice, c.stream));
-    return d;
-  };
-  float* d_a = up(a, (size_t)M * K);
-  float* d_w = up(w, (size_t)K * N);
-  float* d_b = bias ? up(bias, N) : nullptr;
-  float* d_r = residual ? up(residual, (size_t)M * N) : nullptr;
+  float* d_a = upload(c, a, (size_t)M * K);
+  float* d_w = upload(c, w, (size_t)K * N);
+  float* d_b = upload(c, bias, N);
+  float* d_r = upload(c, residual, (size_t)M * N);
   float* d_c = c.work.get<float>((size_t)M * Nout);
   ActOp A;
   A.p = Half2Ptr{c.work.get<__half>((size_t)M * K), c.work.get<__half>((size_t)M * K)};
@@ -726,8 +693,8 @@ int sdb_test_gemm_ex(sdb_ctx* ctx, const float* a, const float* w, const float* 
   ExtraK xk;
   if (xa) {
     SDB_CHECK(xw && XK % 64 == 0, "extra-K test operands");
-    float* d_xa = up(xa, (size_t)M * XK);
-    float* d_xw = up(xw, (size_t)XK * N);
+    float* d_xa = upload(c, xa, (size_t)M * XK);
+    float* d_xw = upload(c, xw, (size_t)XK * N);
     xk.x0.p = Half2Ptr{c.work.get<__half>((size_t)M * XK), c.work.get<__half>((size_t)M * XK)};
     xk.x0.W = M, xk.x0.C = XK;
     convert_f16_launch(d_xa, (long long)M * XK, xk.x0.p, c.stream);
@@ -743,14 +710,7 @@ int sdb_test_gemm_ex(sdb_ctx* ctx, const float* a, const float* w, const float* 
   ep.bias = d_bp, ep.residual = d_r, ep.geglu = geglu ? 1 : 0;
   run_gemm(c, G_LINEAR, A, nullptr, Wp, passes, ep, xa ? &xk : nullptr);
   if (geglu || from_f16) {
-    std::vector<__half> hi((size_t)M * Nout), lo((size_t)M * Nout);
-    SDB_CUDA(cudaMemcpyAsync(hi.data(), o16.hi, hi.size() * 2, cudaMemcpyDeviceToHost, c.stream));
-    SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, lo.size() * 2, cudaMemcpyDeviceToHost, c.stream));
-    SDB_CUDA(cudaStreamSynchronize(c.stream));
-    if (planes)
-      for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]), out[hi.size() + i] = __half2float(lo[i]);
-    else
-      for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
+    fetch_pair(c, o16, (size_t)M * Nout, out, planes);
   } else {
     SDB_CUDA(cudaMemcpyAsync(out, d_c, sizeof(float) * M * Nout, cudaMemcpyDeviceToHost, c.stream));
     SDB_CUDA(cudaStreamSynchronize(c.stream));
@@ -763,21 +723,18 @@ int sdb_test_conv2d(sdb_ctx* ctx, const float* x, const float* w, const float* b
                     int cout, int ksize, int stride, int upsample, int passes, float* y, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  GemmTraceScope ts(c, trace);
+  TraceScope ts(c, trace);
   SDB_CHECK(ksize == 1 || ksize == 3, "ksize");
   SDB_CHECK(stride == 1 || (stride == 2 && ksize == 3 && !upsample), "stride");
   const int Hin = H, Win = W;
   const int Ho = upsample ? 2 * H : (stride == 2 ? H / 2 : H), Wo = upsample ? 2 * W : (stride == 2 ? W / 2 : W);
   const size_t xin = (size_t)n * cin * Hin * Win, yout = (size_t)n * cout * Ho * Wo;
-  float* d_x = c.work.get<float>(xin);
+  float* d_x = upload(c, x, xin);
   float* d_xh = c.work.get<float>(xin);
-  float* d_w = c.work.get<float>((size_t)cout * cin * ksize * ksize);
-  float* d_b = bias ? c.work.get<float>(cout) : nullptr;
+  float* d_w = upload(c, w, (size_t)cout * cin * ksize * ksize);
+  float* d_b = upload(c, bias, cout);
   float* d_yh = c.work.get<float>(yout);
   float* d_y = c.work.get<float>(yout);
-  SDB_CUDA(cudaMemcpyAsync(d_x, x, sizeof(float) * xin, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_w, w, sizeof(float) * cout * cin * ksize * ksize, cudaMemcpyHostToDevice, c.stream));
-  if (bias) SDB_CUDA(cudaMemcpyAsync(d_b, bias, sizeof(float) * cout, cudaMemcpyHostToDevice, c.stream));
   nchw_to_nhwc_launch(d_x, n, cin, Hin, Win, d_xh, c.stream);
   ActOp A;
   A.n = n, A.C = cin;
@@ -827,16 +784,11 @@ int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float*
                      float* out, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  GemmTraceScope ts(c, trace);
+  TraceScope ts(c, trace);
   SDB_CHECK(C % 160 == 0 && K0 % 64 == 0 && (!geglu || (N % 128 == 0 && b1)), "ln_fold test shapes");
-  auto up = [&](const float* h, size_t cnt) {
-    float* d = c.work.get<float>(cnt);
-    SDB_CUDA(cudaMemcpyAsync(d, h, sizeof(float) * cnt, cudaMemcpyHostToDevice, c.stream));
-    return d;
-  };
   auto h2 = [&](size_t cnt) { return Half2Ptr{c.work.get<__half>(cnt), c.work.get<__half>(cnt)}; };
-  float *d_w0 = up(w0, (size_t)K0 * C), *d_b0 = up(b0, C), *d_g = up(gamma, C), *d_be = up(beta, C), *d_w1 = up(w1, (size_t)C * N);
-  float* d_b1 = b1 ? up(b1, N) : nullptr;
+  float *d_w0 = upload(c, w0, (size_t)K0 * C), *d_b0 = upload(c, b0, C), *d_g = upload(c, gamma, C), *d_be = upload(c, beta, C),
+        *d_w1 = upload(c, w1, (size_t)C * N), *d_b1 = upload(c, b1, N);
   WeightOp W0;
   W0.p = h2((size_t)C * K0), W0.N = C, W0.K = K0;
   pack_linear_launch(d_w0, K0, C, W0.p, 0, c.stream);
@@ -861,7 +813,7 @@ int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float*
   const int ls = ln_slots(C);
   float* st = c.work.get<float>((size_t)M * ls * 2);
   for (int pass = 0; pass < (a2 ? 2 : 1); ++pass) {
-    float* d_a = up(pass ? a2 : a, (size_t)M * K0);
+    float* d_a = upload(c, pass ? a2 : a, (size_t)M * K0);
     ActOp A;
     A.p = h2((size_t)M * K0), A.W = M, A.C = K0;
     convert_f16_launch(d_a, (long long)M * K0, A.p, c.stream);
@@ -880,11 +832,7 @@ int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float*
     ep.ln_in = st, ep.ln_in_slots = ls, ep.ln_C = C, ep.ln_eps = 1e-5f, ep.ln_u_hi = u_hi, ep.ln_u_full = u_full, ep.bias = v;
     run_gemm(c, G_LINEAR, Y, nullptr, W1, passes, ep);
   }
-  std::vector<__half> hi((size_t)M * Nout), lo((size_t)M * Nout);
-  SDB_CUDA(cudaMemcpyAsync(hi.data(), o16.hi, hi.size() * 2, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, lo.size() * 2, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-  for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
+  fetch_pair(c, o16, (size_t)M * Nout, out);
   ts.write();
   API_END
 }
@@ -894,26 +842,19 @@ int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const 
                             float* y, int* used_epilogue_stats, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  GemmTraceScope ts(c, trace);
+  TraceScope ts(c, trace);
   SDB_CHECK(ksize == 1 || ksize == 3, "ksize");
   SDB_CHECK((stride == 1 && (upsample == 0 || (upsample == 1 && ksize == 3))) || (stride == 2 && ksize == 3 && !upsample),
             "stride / upsample");
   const int Ho = upsample ? 2 * H : (stride == 2 ? H / 2 : H), Wo = upsample ? 2 * W : (stride == 2 ? W / 2 : W);
   const size_t xin = (size_t)n * cin * H * W, yout = (size_t)n * cout * Ho * Wo;
-  auto up = [&](const float* h, size_t cnt) {
-    float* d = c.work.get<float>(cnt);
-    SDB_CUDA(cudaMemcpyAsync(d, h, sizeof(float) * cnt, cudaMemcpyHostToDevice, c.stream));
-    return d;
-  };
-  float* d_x = up(x, xin);
-  float* d_w = up(w, (size_t)cout * cin * ksize * ksize);
-  float* d_b = bias ? up(bias, cout) : nullptr;
-  float* d_g = up(gamma, cout);
-  float* d_be = up(beta, cout);
+  float* d_x = upload(c, x, xin);
+  float* d_w = upload(c, w, (size_t)cout * cin * ksize * ksize);
+  float* d_b = upload(c, bias, cout);
+  float* d_g = upload(c, gamma, cout);
+  float* d_be = upload(c, beta, cout);
   float* d_xh = c.work.get<float>(xin);
   float* d_conv = c.work.get<float>(yout);
-  float* d_yh = c.work.get<float>(yout);
-  float* d_y = c.work.get<float>(yout);
   nchw_to_nhwc_launch(d_x, n, cin, H, W, d_xh, c.stream);
   // operand, packing and GEMM kind as the model's downsample (stride 2) and upsample convs use them (see sdb_test_conv2d)
   ActOp A;
@@ -944,16 +885,7 @@ int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const 
   GnSrc s0, s1;
   s0.x = d_conv, s0.C = cout, s0.part = gn.buf, s0.cap = gn.cap, s0.slots = gn.slots;
   gn_apply_launch(s0, s1, gn.bucket, n, Ho, Wo, silu, d_g, d_be, 1e-5f, o16, c.stream);
-  std::vector<__half> hi(yout), lo(yout);
-  SDB_CUDA(cudaMemcpyAsync(hi.data(), o16.hi, yout * 2, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, yout * 2, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-  std::vector<float> nhwc(yout);
-  for (size_t i = 0; i < yout; ++i) nhwc[i] = __half2float(hi[i]) + __half2float(lo[i]);
-  SDB_CUDA(cudaMemcpyAsync(d_yh, nhwc.data(), yout * 4, cudaMemcpyHostToDevice, c.stream));
-  nhwc_to_nchw_launch(d_yh, n, cout, Ho, Wo, d_y, c.stream);
-  SDB_CUDA(cudaMemcpyAsync(y, d_y, sizeof(float) * yout, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  fetch_half2(c, o16, n, cout, Ho, Wo, y);
   ts.write();
   API_END
 }
@@ -963,18 +895,15 @@ int sdb_test_groupnorm(sdb_ctx* ctx, const float* x, const float* gamma, const f
   API_BEGIN(ctx)
   c.work.reset();
   const size_t cnt = (size_t)n * ch * H * W;
-  float* d_x = c.work.get<float>(cnt);
+  float* d_x = upload(c, x, cnt);
   float* d_xh = c.work.get<float>(cnt);
   float* d_yh = c.work.get<float>(cnt);
   float* d_y = c.work.get<float>(cnt);
-  float* d_g = c.work.get<float>(ch);
-  float* d_b = c.work.get<float>(ch);
+  float* d_g = upload(c, gamma, ch);
+  float* d_b = upload(c, beta, ch);
   double* d_s = c.work.get<double>((size_t)n * 64);
   unsigned int* d_t = c.work.get<unsigned int>(n);
   float* d_p = c.work.get<float>(gn_stats_partial_floats(n, H * W));
-  SDB_CUDA(cudaMemcpyAsync(d_x, x, sizeof(float) * cnt, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_g, gamma, sizeof(float) * ch, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_b, beta, sizeof(float) * ch, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaMemsetAsync(d_t, 0, sizeof(unsigned int) * n, c.stream));
   nchw_to_nhwc_launch(d_x, n, ch, H, W, d_xh, c.stream);
   gn_stats_launch(d_xh, ch, nullptr, 0, n, H * W, d_s, d_p, d_t, c.stream);
@@ -989,13 +918,10 @@ int sdb_test_layernorm(sdb_ctx* ctx, const float* x, const float* gamma, const f
   API_BEGIN(ctx)
   c.work.reset();
   const size_t cnt = (size_t)rows * ch;
-  float* d_x = c.work.get<float>(cnt);
+  float* d_x = upload(c, x, cnt);
   float* d_y = c.work.get<float>(cnt);
-  float* d_g = c.work.get<float>(ch);
-  float* d_b = c.work.get<float>(ch);
-  SDB_CUDA(cudaMemcpyAsync(d_x, x, sizeof(float) * cnt, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_g, gamma, sizeof(float) * ch, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_b, beta, sizeof(float) * ch, cudaMemcpyHostToDevice, c.stream));
+  float* d_g = upload(c, gamma, ch);
+  float* d_b = upload(c, beta, ch);
   layernorm_launch(d_x, rows, ch, d_g, d_b, 1e-5f, Half2Ptr{}, d_y, c.stream);
   SDB_CUDA(cudaMemcpyAsync(y, d_y, sizeof(float) * cnt, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));

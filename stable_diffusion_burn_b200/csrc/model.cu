@@ -633,7 +633,7 @@ struct Fwd {
       const int nbk = x.C / x.gn.bucket;
       const float* part = x.gn.buf;
       int cap = x.gn.cap, slots = x.gn.slots;
-      if (c.trace_on) c.gn_trace.push_back(slots > 128 ? GN_PATH_SUMS_FOLD : GN_PATH_SUMS_PARTIALS);
+      if (c.trace_on) c.trace.push_back({TRACE_GN, {slots > 128 ? GN_PATH_SUMS_FOLD : GN_PATH_SUMS_PARTIALS}});
       if (slots > 128) {
         const int s2 = gn_fold_slots(slots);
         float* folded = c.work.get<float>((size_t)nb * s2 * nbk * 2);
@@ -645,7 +645,7 @@ struct Fwd {
       gn_sums_from_partials_launch(part, cap, slots, nbk, x.C, x.gn.bucket, nb, sums, c.stream);
       return sums;
     }
-    if (c.trace_on) c.gn_trace.push_back(GN_PATH_SUMS_STATS);
+    if (c.trace_on) c.trace.push_back({TRACE_GN, {GN_PATH_SUMS_STATS}});
     float* part = c.work.get<float>(gn_stats_partial_floats(nb, HW));
     KernelScope ks(c, KC_GN_STATS, 0, (double)nb * HW * x.C * 4.0);
     gn_stats_launch(x.p, x.C, nullptr, 0, nb, HW, sums, part, tk, c.stream);
@@ -699,7 +699,8 @@ struct Fwd {
       };
       src(x0, s0);
       if (x1) src(*x1, s1);
-      if (c.trace_on) c.gn_trace.push_back(x0.gn.slots > 128 || (x1 && x1->gn.slots > 128) ? GN_PATH_APPLY_FOLD : GN_PATH_APPLY);
+      if (c.trace_on)
+        c.trace.push_back({TRACE_GN, {x0.gn.slots > 128 || (x1 && x1->gn.slots > 128) ? GN_PATH_APPLY_FOLD : GN_PATH_APPLY}});
       KernelScope ks(c, KC_PREP, 0, (double)nb * HW * C * (4.0 + 2.0 + (lo ? 2.0 : 0.0)));
       gn_apply_launch(s0, s1, x0.gn.bucket, nb, x0.H, x0.W, silu ? 1 : 0, nw.gamma, nw.beta, nw.eps, a.p, c.stream);
       return a;
@@ -708,7 +709,7 @@ struct Fwd {
     unsigned int* tk = gn_tickets + (size_t)gn_slot * nb * 2;
     gn_slot++;
     float* part = c.work.get<float>(gn_fused_partial_floats(nb, HW));
-    if (c.trace_on) c.gn_trace.push_back(GN_PATH_FUSED);
+    if (c.trace_on) c.trace.push_back({TRACE_GN, {GN_PATH_FUSED}});
     KernelScope ks(c, KC_PREP, 0, (double)nb * HW * C * (8.0 + 2.0 + (lo ? 2.0 : 0.0)));
     gn_fused_launch(x0.p, x0.C, x1 ? x1->p : nullptr, x1 ? x1->C : 0, nb, x0.H, x0.W, silu ? 1 : 0, nw.gamma, nw.beta, nw.eps,
                     a.p, part, tk, c.stream);
@@ -981,12 +982,14 @@ static void unet_cond_io(const Ctx& c, int nb, const float* d_x, const float* d_
 static void unet_conv_in(Fwd& f, const UNetBlockW& b, const UNetIO& io, const Act& o) {
   Ctx& c = f.c;
   KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * io.H * io.W * 9.0 * b.cin * b.cout);
-  if (b.cin != 4)
+  if (b.cin != 4) {
     conv3x3_cin_cond_launch(b.cin, io.x, io.x_stride, io.cond, io.cond_stride, io.cond_mod, f.nb, io.H, io.W, mptr(c, b.conv.wi),
                             b.conv.bias, b.cout, o.p, o.raw16, c.stream);
-  else
+    if (c.trace_on) c.trace.push_back({TRACE_COND, {io.cond_mod}});
+  } else {
     conv3x3_cin4_launch(io.x, f.nb, io.H, io.W, mptr(c, b.conv.wi), b.conv.bias, b.cout, nullptr, nullptr, 1.f, o.p, o.raw16,
                         c.stream);
+  }
 }
 
 // GroupNorm + SiLU + 3x3 conv to cout <= 8 channels, fused, fp32 on CUDA cores, NCHW result y [nb,cout,H,W]: the UNet's out
@@ -998,7 +1001,7 @@ static void norm_conv_out(Fwd& f, const Act& x, const NormW& norm, const ConvW& 
   KernelScope ks(c, KC_SMALLCONV, 2.0 * f.nb * x.H * x.W * 9.0 * x.C * cout);
   const SmallCoutVariant v = conv3x3_small_cout_launch(x.p, f.nb, x.H, x.W, x.C, sums, norm.gamma, norm.beta, norm.eps,
                                                        conv.w_small, conv.bias, cout, y, c.stream);
-  if (c.trace_on) c.conv_trace.insert(c.conv_trace.end(), {v.th, v.ck, v.ks});
+  if (c.trace_on) c.trace.push_back({TRACE_CONV, {v.th, v.ck, v.ks}});
 }
 
 static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
@@ -1175,7 +1178,7 @@ static void run_vae_attention(Fwd& f, VaeAttnW& a, const Act& x, Act& out, Half2
     {
       KernelScope ks(c, KC_ELEMENTWISE, 0, (double)HW * HW * 6.0);
       const int per = softmax_rows_launch(S, HW, HW, scale, p16, c.stream);
-      if (c.trace_on) c.softmax_trace.push_back(per);
+      if (c.trace_on) c.trace.push_back({TRACE_SOFTMAX, {per}});
     }
     WeightOp vs;
     vs.p.hi = vT.hi + (size_t)s * HW, vs.p.lo = vT.lo ? vT.lo + (size_t)s * HW : nullptr;
@@ -2143,6 +2146,41 @@ void model_clip_forward_host(Ctx& c, const int* tokens, int n, int L, float* out
   SDB_CUDA(cudaStreamSynchronize(c.stream));
 }
 
+// ================================================================================ test-entry launch records and staging
+void TraceScope::write() const {
+  if (!out) return;
+  static_assert(sizeof(TraceRecord) == 16 * sizeof(int32_t), "sdb200.h documents 16-int records");
+  constexpr size_t kMax = (SDB_TRACE_INTS - 1) / 16;
+  SDB_CHECK(c.trace.size() <= kMax, "launch trace: " + std::to_string(c.trace.size()) + " records do not fit SDB_TRACE_INTS (" +
+                                        std::to_string(kMax) + " records)");
+  std::fill(out, out + SDB_TRACE_INTS, 0);
+  out[0] = (int)c.trace.size();
+  std::memcpy(out + 1, c.trace.data(), c.trace.size() * sizeof(TraceRecord));
+}
+
+void fetch_pair(Ctx& c, Half2Ptr p, size_t count, float* out, bool planes) {
+  std::vector<__half> hi(p.hi ? count : 0), lo(p.lo ? count : 0);
+  if (p.hi) SDB_CUDA(cudaMemcpyAsync(hi.data(), p.hi, count * 2, cudaMemcpyDeviceToHost, c.stream));
+  if (p.lo) SDB_CUDA(cudaMemcpyAsync(lo.data(), p.lo, count * 2, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  for (size_t i = 0; i < count; ++i) {
+    const float h = p.hi ? __half2float(hi[i]) : 0.f, l = p.lo ? __half2float(lo[i]) : 0.f;
+    if (planes)
+      out[i] = h, out[count + i] = l;
+    else
+      out[i] = h + l;
+  }
+}
+
+void fetch_half2(Ctx& c, Half2Ptr p, int n, int C, int H, int W, float* out) {
+  const size_t hw = (size_t)H * W;
+  std::vector<float> v((size_t)n * hw * C);
+  fetch_pair(c, p, v.size(), v.data());
+  for (int s = 0; s < n; ++s)
+    for (size_t i = 0; i < hw; ++i)
+      for (int ch = 0; ch < C; ++ch) out[((size_t)s * C + ch) * hw + i] = v[((size_t)s * hw + i) * C + ch];
+}
+
 // ================================================================================ attention unit-test entry
 // V transposed (flags & 2): stages q / k / V^T exactly as model_clip_forward_dev does
 static void test_attention_vt(Ctx& c, const float* q, const float* k, const float* v, int n, int L, int C, int heads,
@@ -2160,34 +2198,23 @@ static void test_attention_vt(Ctx& c, const float* q, const float* k, const floa
         hqk[row * 2 * C + C + j] = __float2half(k[src]);
         hvT[(size_t)j * Mp + row] = __float2half(v[src]);
       }
-  __half* dqk = c.work.get<__half>(hqk.size());
-  __half* dvT = c.work.get<__half>(hvT.size());
+  const __half* dqk = upload(c, hqk.data(), hqk.size());
   Half2Ptr o16;
   o16.hi = c.work.get<__half>((size_t)Mr * C);
   o16.lo = c.work.get<__half>((size_t)Mr * C);
-  int* dlen = lens ? c.work.get<int>(n) : nullptr;
-  SDB_CUDA(cudaMemcpyAsync(dqk, hqk.data(), hqk.size() * 2, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(dvT, hvT.data(), hvT.size() * 2, cudaMemcpyHostToDevice, c.stream));
-  if (lens) SDB_CUDA(cudaMemcpyAsync(dlen, lens, n * 4, cudaMemcpyHostToDevice, c.stream));
   AttnOp at;
   at.q = dqk, at.ldq = 2 * C, at.q_col0 = 0, at.q_rows = Lp;
   at.k = dqk, at.ldk = 2 * C, at.k_col0 = C, at.k_rows = Lp;
-  at.vT = dvT, at.ldv = Mp;
+  at.vT = upload(c, hvT.data(), hvT.size()), at.ldv = Mp;
   at.nb = n, at.heads = heads, at.d = d, at.dpad = d, at.Nq = L, at.Nk = L;
-  at.kvlen = dlen;
+  at.kvlen = upload(c, lens, n);
   at.causal = causal ? 1 : 0;
   at.out = o16, at.ldo = C;
   run_attention(c, at);
-  std::vector<__half> hi((size_t)Mr * C), lo((size_t)Mr * C);
-  SDB_CUDA(cudaMemcpyAsync(hi.data(), o16.hi, hi.size() * 2, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, lo.size() * 2, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  std::vector<float> o((size_t)Mr * C);
+  fetch_pair(c, o16, o.size(), o.data());
   for (int s = 0; s < n; ++s)
-    for (int i = 0; i < L; ++i)
-      for (int j = 0; j < C; ++j) {
-        const size_t src = ((size_t)s * Lp + i) * C + j;
-        out[((size_t)s * L + i) * C + j] = __half2float(hi[src]) + __half2float(lo[src]);
-      }
+    for (int i = 0; i < L; ++i) std::copy_n(&o[((size_t)s * Lp + i) * C], C, out + ((size_t)s * L + i) * C);
 }
 
 void model_test_attention(Ctx& c, const float* q, const float* k, const float* v, int n, int Nq, int Nk, int C, int heads,
@@ -2226,55 +2253,25 @@ void model_test_attention(Ctx& c, const float* q, const float* k, const float* v
           split(k[((size_t)s * Nk + i) * C + h * d + j], hkv[((size_t)s * Nkp + i) * 2 * hd + h * dpad + j], hkv_lo[((size_t)s * Nkp + i) * 2 * hd + h * dpad + j]);
           hkv[((size_t)s * Nkp + i) * 2 * hd + hd + h * dpad + j] = __float2half(v[((size_t)s * Nk + i) * C + h * d + j]);
         }
-  __half* dq = c.work.get<__half>(hq.size());
-  __half* dkv = c.work.get<__half>(hkv.size());
-  __half* dq_lo = c.work.get<__half>(hq.size());
-  __half* dkv_lo = c.work.get<__half>(hkv.size());
-  SDB_CUDA(cudaMemcpyAsync(dq_lo, hq_lo.data(), hq.size() * 2, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(dkv_lo, hkv_lo.data(), hkv.size() * 2, cudaMemcpyHostToDevice, c.stream));
+  const __half* dkv = upload(c, hkv.data(), hkv.size());
   Half2Ptr o16;
   o16.hi = c.work.get<__half>((size_t)n * Nq * C);
   o16.lo = c.work.get<__half>((size_t)n * Nq * C);
-  int* dlen = c.work.get<int>(n);  // always set: the key matrix is padded to Nkp rows per sample
-  SDB_CUDA(cudaMemcpyAsync(dq, hq.data(), hq.size() * 2, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(dkv, hkv.data(), hkv.size() * 2, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(dlen, lens.data(), n * 4, cudaMemcpyHostToDevice, c.stream));
   AttnOp at;
-  at.q = dq, at.ldq = hd, at.q_rows = Nq;
+  at.q = upload(c, hq.data(), hq.size()), at.ldq = hd, at.q_rows = Nq;
   at.k = dkv, at.ldk = 2 * hd, at.k_rows = Nkp;
   at.vT = dkv, at.ldv = 2 * hd, at.v_mn = 1, at.v_col0 = hd;
-  at.q_lo = dq_lo, at.k_lo = dkv_lo;  // used by the head dims that have the split-product kernel (40, 80) unless attn_split = 0
+  // used by the head dims that have the split-product kernel (40, 80) unless attn_split = 0
+  at.q_lo = upload(c, hq_lo.data(), hq_lo.size()), at.k_lo = upload(c, hkv_lo.data(), hkv_lo.size());
   at.nb = n, at.heads = heads, at.d = d, at.dpad = dpad, at.Nq = Nq, at.Nk = Nkp;
-  at.kvlen = dlen;
+  at.kvlen = upload(c, lens.data(), n);  // always set: the key matrix is padded to Nkp rows per sample
   at.causal = flags & 1;
   at.out = o16, at.ldo = C;
   run_attention(c, at);
-  std::vector<__half> hi((size_t)n * Nq * C), lo((size_t)n * Nq * C);
-  SDB_CUDA(cudaMemcpyAsync(hi.data(), o16.hi, hi.size() * 2, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(lo.data(), o16.lo, lo.size() * 2, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-  for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
+  fetch_pair(c, o16, (size_t)n * Nq * C, out);
 }
 
 // ================================================================================ ResBlock / GroupNorm unit-test entries
-namespace {
-struct TraceScope {  // records the GEMM choices and GroupNorm paths of everything queued while it lives
-  Ctx& c;
-  explicit TraceScope(Ctx& c_) : c(c_) {
-    c.gemm_trace.clear(), c.attn_trace.clear(), c.gn_trace.clear(), c.conv_trace.clear(), c.softmax_trace.clear();
-    c.trace_on = true;
-  }
-  ~TraceScope() { c.trace_on = false; }
-};
-}  // namespace
-
-static float* upload(Ctx& c, const float* h, size_t count) {
-  if (!h) return nullptr;
-  float* d = c.work.get<float>(count);
-  SDB_CUDA(cudaMemcpyAsync(d, h, count * 4, cudaMemcpyHostToDevice, c.stream));
-  return d;
-}
-
 static ConvW test_conv_weights(Ctx& c, Fwd& f, const float* w, const float* b, int cin, int cout, int k) {
   SDB_CHECK(cin % 64 == 0 && cout % 32 == 0, "test conv: channels must be multiples of 64 (in) and 32 (out)");
   ConvW cw;
@@ -2327,32 +2324,6 @@ static Act stage_activation(Fwd& f, const float* h, int C, int H, int W, bool st
   return a;
 }
 
-// NHWC fp16 hi + lo (or nothing: zeros) -> NCHW fp32 on the host
-static void fetch_half2(Ctx& c, Half2Ptr p, int n, int C, int H, int W, float* out) {
-  const size_t cnt = (size_t)n * C * H * W;
-  std::vector<__half> hi(cnt), lo(cnt);
-  if (p.hi) SDB_CUDA(cudaMemcpyAsync(hi.data(), p.hi, cnt * 2, cudaMemcpyDeviceToHost, c.stream));
-  if (p.lo) SDB_CUDA(cudaMemcpyAsync(lo.data(), p.lo, cnt * 2, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-  for (int s = 0; s < n; ++s)
-    for (int i = 0; i < H * W; ++i)
-      for (int ch = 0; ch < C; ++ch) {
-        const size_t src = ((size_t)s * H * W + i) * C + ch;
-        out[((size_t)s * C + ch) * H * W + i] = (p.hi ? __half2float(hi[src]) : 0.f) + (p.lo ? __half2float(lo[src]) : 0.f);
-      }
-}
-
-static void write_trace(const Ctx& c, int32_t* trace) {
-  std::fill(trace, trace + kTestTraceInts, 0);
-  trace[0] = (int)c.gn_trace.size();
-  for (size_t i = 0; i < c.gn_trace.size() && i < 4; ++i) trace[1 + i] = c.gn_trace[i];
-  trace[5] = (int)c.gemm_trace.size();
-  for (size_t i = 0; i < c.gemm_trace.size() && i < 5; ++i) {
-    const Ctx::GemmRecord& r = c.gemm_trace[i];
-    const int v[10] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels};
-    std::copy(v, v + 10, trace + 6 + 10 * i);
-  }
-}
 
 void model_test_resblock(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, int Cout,
                          const float* n1g, const float* n1b, const float* w1, const float* b1, const float* n2g, const float* n2b,
@@ -2382,10 +2353,10 @@ void model_test_resblock(Ctx& c, const float* x0, const float* x1, int n, int C0
   Act o = f.act16(H, W, Cout);
   ActOp g;
   {
-    TraceScope ts(c);
+    TraceScope ts(c, trace);
     run_resblock(f, nw1, cw1, nw2, cw2, wsk ? &sk : nullptr, bias_merged, passes, a0, x1 ? &a1 : nullptr, d_emb, o);
     g = f.gn_operand(o, nullptr, nw2, true, true);  // a consumer of the output: reads the partials conv_out left
-    write_trace(c, trace);
+    ts.write();
   }
   float* d = c.work.get<float>(o.count());
   nhwc_to_nchw_launch(o.p, n, Cout, H, W, d, c.stream);
@@ -2406,7 +2377,7 @@ void model_test_groupnorm_cat(Ctx& c, const float* x0, const float* x1, int n, i
   const Act a0 = stage_activation(f, x0, C0, H, W, mode == 2);
   Act a1;
   if (x1) a1 = stage_activation(f, x1, C1, H, W, mode == 2);
-  TraceScope ts(c);
+  TraceScope ts(c, trace);
   ActOp g;
   if (mode == 0) {
     double* sums = c.work.get<double>((size_t)n * 64);
@@ -2418,7 +2389,7 @@ void model_test_groupnorm_cat(Ctx& c, const float* x0, const float* x1, int n, i
   } else {
     g = f.gn_operand(a0, x1 ? &a1 : nullptr, nw, silu != 0, true);
   }
-  write_trace(c, trace);
+  ts.write();
   fetch_half2(c, g.p, n, C, H, W, y);
 }
 
@@ -2441,11 +2412,10 @@ void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, in
   // context [n][Lpad][768], zero padded, per-sample lengths: as model_unet_forward_dev / the sampling entries stage it
   const int Lpad = round_up(Lmax, 32);
   float* ctxp = c.work.get<float>((size_t)n * Lpad * 768);
-  int* d_len = c.work.get<int>(n);
   SDB_CUDA(cudaMemsetAsync(ctxp, 0, (size_t)n * Lpad * 768 * 4, c.stream));
   SDB_CUDA(cudaMemcpy2DAsync(ctxp, (size_t)Lpad * 768 * 4, context, (size_t)Lmax * 768 * 4, (size_t)Lmax * 768 * 4, n,
                              cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_len, lens, 4 * n, cudaMemcpyHostToDevice, c.stream));
+  int* d_len = upload(c, lens, n);
   CtxState cs;
   prepare_context(f, ctxp, Lpad, d_len, cs);
   const Act a = stage_activation(f, x, C, H, W, true);
@@ -2455,24 +2425,10 @@ void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, in
   for (float*& l : taps.ln) l = c.work.get<float>((size_t)Mt * ls * 2);
   ActOp g;
   {
-    TraceScope ts(c);
+    TraceScope ts(c, trace);
     run_spatial_transformer(f, st, cs, cs.kv[index], a, o, &taps);
     g = f.gn_operand(o, nullptr, st.norm, true, true);  // a consumer of the output, as the next ResBlock's norm_in stages it
-    std::fill(trace, trace + kStTraceInts, 0);
-    trace[0] = (int)c.gn_trace.size();
-    for (size_t i = 0; i < c.gn_trace.size() && i < 4; ++i) trace[1 + i] = c.gn_trace[i];
-    trace[5] = (int)c.gemm_trace.size();
-    for (size_t i = 0; i < c.gemm_trace.size() && i < 10; ++i) {
-      const Ctx::GemmRecord& r = c.gemm_trace[i];
-      const int v[12] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels, r.passes, r.epi};
-      std::copy(v, v + 12, trace + 6 + 12 * i);
-    }
-    trace[126] = (int)c.attn_trace.size();
-    for (size_t i = 0; i < c.attn_trace.size() && i < 4; ++i) {
-      const Ctx::AttnRecord& r = c.attn_trace[i];
-      const int v[5] = {r.dpad, r.Nq, r.Nk, r.qk3, r.kvlen};
-      std::copy(v, v + 5, trace + 127 + 5 * i);
-    }
+    ts.write();
   }
   float* d = c.work.get<float>(o.count());
   nhwc_to_nchw_launch(o.p, n, C, H, W, d, c.stream);
@@ -2480,14 +2436,7 @@ void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, in
   fetch_half2(c, o.raw16, n, C, H, W, out16);
   fetch_half2(c, g.p, n, C, H, W, out_norm);
   // taps: y as [Mt][C] hi + lo, the statistics folded over their slots in index order (as the consuming epilogue adds them)
-  const size_t cnt = (size_t)Mt * C;
-  std::vector<__half> hi(cnt), lo(cnt);
-  for (int i = 0; i < 4; ++i) {
-    SDB_CUDA(cudaMemcpyAsync(hi.data(), taps.y[i].hi, cnt * 2, cudaMemcpyDeviceToHost, c.stream));
-    SDB_CUDA(cudaMemcpyAsync(lo.data(), taps.y[i].lo, cnt * 2, cudaMemcpyDeviceToHost, c.stream));
-    SDB_CUDA(cudaStreamSynchronize(c.stream));
-    for (size_t e = 0; e < cnt; ++e) taps_y[i * cnt + e] = __half2float(hi[e]) + __half2float(lo[e]);
-  }
+  for (int i = 0; i < 4; ++i) fetch_pair(c, taps.y[i], (size_t)Mt * C, taps_y + i * Mt * C);
   std::vector<float> sl((size_t)Mt * ls * 2);
   for (int i = 0; i < 3; ++i) {
     SDB_CUDA(cudaMemcpyAsync(sl.data(), taps.ln[i], sl.size() * 4, cudaMemcpyDeviceToHost, c.stream));
@@ -2514,7 +2463,7 @@ void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, 
   Model& m = M(c);
   EncoderW& e = m.enc;
   SDB_CHECK(stage >= SDB_VAE_DEC_IN && stage <= SDB_VAE_ENC_DOWN2, "test_vae_stage: stage is one of SDB_VAE_*");
-  SDB_CHECK(n >= 1 && H >= 1 && W >= 1 && x && out && trace, "test_vae_stage: arguments");
+  SDB_CHECK(n >= 1 && H >= 1 && W >= 1 && x && out, "test_vae_stage: arguments");
   SDB_CHECK((flags & ~3) == 0 && (!(flags & 2) || stage == SDB_VAE_ENC_OUT),
             "test_vae_stage: flags are 1 (x with producer GroupNorm partials) | 2 (SDB_VAE_ENC_OUT: strided, scaled quant slice)");
   const bool attn = stage == SDB_VAE_DEC_ATTN || stage == SDB_VAE_ENC_ATTN;
@@ -2553,10 +2502,8 @@ void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, 
   float* q = nullptr;
   const size_t qcount = (size_t)n * ((flags & 2) ? 5 : 4) * HW;
   ActOp g;
-  int cond_mod = 0;
-  std::fill(trace, trace + kVaeTraceInts, 0);
   {
-    TraceScope ts(c);
+    TraceScope ts(c, trace);
     switch (stage) {
       case SDB_VAE_DEC_IN:
         vae_dec_conv_in(f, d_x, scale, o);
@@ -2591,7 +2538,6 @@ void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, 
       case SDB_VAE_UNET_IN: {
         UNetIO io{d_x, nullptr, nullptr, H, W};
         unet_cond_io(c, n, d_x, d_cond, io);
-        cond_mod = io.cond ? io.cond_mod : 0;
         unet_conv_in(f, m.in_blocks[0], io, o);
         break;
       }
@@ -2600,19 +2546,7 @@ void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, 
         g = f.gn_operand(o, nullptr, e.blocks[di + 1].res[0].norm1, true, true);  // the next block's first ResnetBlock
         break;
     }
-    trace[0] = (int)c.gn_trace.size();
-    for (size_t i = 0; i < c.gn_trace.size() && i < 4; ++i) trace[1 + i] = c.gn_trace[i];
-    trace[5] = (int)c.gemm_trace.size();
-    for (size_t i = 0; i < c.gemm_trace.size() && i < 16; ++i) {
-      const Ctx::GemmRecord& r = c.gemm_trace[i];
-      const int v[12] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels, r.passes, r.epi};
-      std::copy(v, v + 12, trace + 6 + 12 * i);
-    }
-    trace[200] = (int)c.conv_trace.size() / 3;
-    std::copy(c.conv_trace.begin(), c.conv_trace.begin() + std::min<size_t>(c.conv_trace.size(), 3), trace + 201);
-    trace[204] = (int)c.softmax_trace.size();
-    if (!c.softmax_trace.empty()) trace[205] = c.softmax_trace.back();
-    trace[206] = cond_mod;
+    ts.write();
   }
   if (y) {
     SDB_CUDA(cudaMemcpyAsync(out, y, (size_t)n * cout * HW * 4, cudaMemcpyDeviceToHost, c.stream));
@@ -2631,7 +2565,7 @@ void model_test_clip_block(Ctx& c, int index, const float* x, int n, int L, int 
   Model& m = M(c);
   const int nblk = (int)m.clip.blocks.size();
   SDB_CHECK(index >= 0 && index <= nblk, "test_clip_block: index is a block 0..11, or 12 for the final LayerNorm");
-  SDB_CHECK(n >= 1 && L >= 1 && L <= 77 && x && out && trace, "test_clip_block: arguments (1 <= L <= 77)");
+  SDB_CHECK(n >= 1 && L >= 1 && L <= 77 && x && out, "test_clip_block: arguments (1 <= L <= 77)");
   SDB_CHECK((flags & ~1) == 0, "test_clip_block: flags are 1 (pad rows hold large finite junk instead of zeros)");
   const int D = 768;
   Fwd f(c, n);
@@ -2659,26 +2593,13 @@ void model_test_clip_block(Ctx& c, int index, const float* x, int n, int L, int 
     tp.x_attn = c.work.get<float>((size_t)Mr * D);
   }
   float* y = index < nblk ? b.x : c.work.get<float>((size_t)Mr * D);
-  std::fill(trace, trace + kClipTraceInts, 0);
   {
-    TraceScope ts(c);
+    TraceScope ts(c, trace);
     if (index < nblk)
       run_clip_block(f, m.clip.blocks[index], b, tp.qk ? &tp : nullptr);
     else
       clip_layernorm(c, b, m.clip.ln_final, Half2Ptr{}, y);
-    trace[0] = (int)c.gemm_trace.size();
-    for (size_t i = 0; i < c.gemm_trace.size() && i < 5; ++i) {
-      const Ctx::GemmRecord& r = c.gemm_trace[i];
-      const int v[13] = {r.kind, r.N, r.BN, r.split, r.TN, r.TH, r.TW, r.xk_channels, r.gn_slots, r.a1_channels, r.passes, r.epi,
-                         r.act};
-      std::copy(v, v + 13, trace + 1 + 13 * i);
-    }
-    trace[70] = (int)c.attn_trace.size();
-    if (!c.attn_trace.empty()) {
-      const Ctx::AttnRecord& r = c.attn_trace[0];
-      const int v[6] = {r.dpad, r.Nq, r.Nk, r.qk3, r.kvlen, r.causal};
-      std::copy(v, v + 6, trace + 71);
-    }
+    ts.write();
   }
   // real rows only, [n][L][width]
   auto real_rows = [&](const std::vector<float>& src, int width, int col0, int pitch, float* dst) {
@@ -2693,30 +2614,26 @@ void model_test_clip_block(Ctx& c, int index, const float* x, int n, int L, int 
     SDB_CUDA(cudaStreamSynchronize(c.stream));
     return h;
   };
-  auto fetch16 = [&](const __half* hi, const __half* lo, size_t count) {
-    std::vector<__half> h(count), l(lo ? count : 0);
-    SDB_CUDA(cudaMemcpyAsync(h.data(), hi, count * 2, cudaMemcpyDeviceToHost, c.stream));
-    if (lo) SDB_CUDA(cudaMemcpyAsync(l.data(), lo, count * 2, cudaMemcpyDeviceToHost, c.stream));
-    SDB_CUDA(cudaStreamSynchronize(c.stream));
+  auto fetch16 = [&](Half2Ptr p, size_t count) {
     std::vector<float> v(count);
-    for (size_t i = 0; i < count; ++i) v[i] = __half2float(h[i]) + (lo ? __half2float(l[i]) : 0.f);
+    fetch_pair(c, p, count, v.data());
     return v;
   };
   real_rows(fetch32(y, (size_t)Mr * D), D, 0, D, out);
   if (!tp.qk) return;
   const size_t tc = (size_t)n * L * D;  // one [n][L][768] tap
-  real_rows(fetch16(tp.ln1.hi, tp.ln1.lo, (size_t)Mr * D), D, 0, D, taps);
-  const std::vector<float> qk = fetch16(tp.qk, nullptr, (size_t)Mr * 2 * D);
+  real_rows(fetch16(tp.ln1, (size_t)Mr * D), D, 0, D, taps);
+  const std::vector<float> qk = fetch16({tp.qk, nullptr}, (size_t)Mr * 2 * D);
   real_rows(qk, D, 0, 2 * D, taps + tc);
   real_rows(qk, D, D, 2 * D, taps + 2 * tc);
-  const std::vector<float> vT = fetch16(tp.vT, nullptr, (size_t)D * b.Mp);
+  const std::vector<float> vT = fetch16({tp.vT, nullptr}, (size_t)D * b.Mp);
   for (int s = 0; s < n; ++s)
     for (int l = 0; l < L; ++l)
       for (int j = 0; j < D; ++j) taps[3 * tc + ((size_t)s * L + l) * D + j] = vT[(size_t)j * b.Mp + (size_t)s * Lp + l];
-  real_rows(fetch16(tp.o.hi, tp.o.lo, (size_t)Mr * D), D, 0, D, taps + 4 * tc);
+  real_rows(fetch16(tp.o, (size_t)Mr * D), D, 0, D, taps + 4 * tc);
   real_rows(fetch32(tp.x_attn, (size_t)Mr * D), D, 0, D, taps + 5 * tc);
-  real_rows(fetch16(tp.ln2.hi, tp.ln2.lo, (size_t)Mr * D), D, 0, D, taps + 6 * tc);
-  real_rows(fetch16(tp.h.hi, tp.h.lo, (size_t)Mr * 4 * D), 4 * D, 0, 4 * D, taps + 7 * tc);
+  real_rows(fetch16(tp.ln2, (size_t)Mr * D), D, 0, D, taps + 6 * tc);
+  real_rows(fetch16(tp.h, (size_t)Mr * 4 * D), 4 * D, 0, 4 * D, taps + 7 * tc);
 }
 
 }  // namespace sdb

@@ -69,27 +69,47 @@ void model_load_dump_dir(Ctx& c, const char* root);
 // SD-1.x single-file .safetensors checkpoints (safetensors.cu)
 void model_load_safetensors(Ctx& c, const char* path);
 void safetensors_probe(const char* path, int* kind, int* conv_in_width);
+
+// ---- test entries (host pointers; each call stages through the context's work arena)
+// Records every traced launch while it lives, when `out` (SDB_TRACE_INTS ints, sdb200.h) is not null; write() fills `out` and
+// fails the call if the records do not fit.
+struct TraceScope {
+  Ctx& c;
+  int32_t* out;
+  TraceScope(Ctx& c, int32_t* out) : c(c), out(out) {
+    c.trace.clear();
+    c.trace_on = out != nullptr;
+  }
+  ~TraceScope() { c.trace_on = false; }
+  void write() const;
+};
+// `count` host values copied to a new work-arena buffer on the context's stream (null host: null)
+template <class T>
+T* upload(Ctx& c, const T* host, size_t count) {
+  if (!host) return nullptr;
+  T* d = c.work.get<T>(count);
+  SDB_CUDA(cudaMemcpyAsync(d, host, count * sizeof(T), cudaMemcpyHostToDevice, c.stream));
+  return d;
+}
+// `count` fp16 hi + lo pairs read back as fp32 (a null half reads as 0): out[i] = hi[i] + lo[i], or with planes hi to
+// out[0, count) and lo to out[count, 2 count)
+void fetch_pair(Ctx& c, Half2Ptr p, size_t count, float* out, bool planes = false);
+// fetch_pair of an NHWC [n][H][W][C] tensor, written NCHW
+void fetch_half2(Ctx& c, Half2Ptr p, int n, int C, int H, int W, float* out);
+
 void model_test_attention(Ctx& c, const float* q, const float* k, const float* v, int n, int Nq, int Nk, int C, int heads,
                           const int32_t* kvlen, int flags, float* out);
-// ResBlock / concat-GroupNorm test entries (sdb200.h: sdb_test_resblock, sdb_test_groupnorm_cat); trace = kTestTraceInts ints
-constexpr int kTestTraceInts = 64;
 void model_test_resblock(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, int Cout,
                          const float* n1g, const float* n1b, const float* w1, const float* b1, const float* n2g, const float* n2b,
                          const float* w2, const float* b2, const float* wsk, const float* bsk, const float* emb_bias, int passes,
                          int flags, float* out, float* out16, float* outn, int32_t* trace);
 void model_test_groupnorm_cat(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, const float* gamma,
                               const float* beta, int silu, int mode, float* y, int32_t* trace);
-// SpatialTransformer test entry (sdb200.h: sdb_test_spatial_transformer); trace = kStTraceInts ints
-constexpr int kStTraceInts = 160;
 void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, int C, int H, int W, const float* context, int Lmax,
                                     const int32_t* lens, int flags, float* out, float* out16, float* out_norm, float* taps_y,
                                     float* taps_ln, int32_t* trace);
-// autoencoder stage test entry (sdb200.h: sdb_test_vae_stage); trace = kVaeTraceInts ints
-constexpr int kVaeTraceInts = 256;
 void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, int n, int C, int H, int W, float scale, int flags,
                           float* out, float* out16, float* tap, float* out_norm, int32_t* trace);
-// CLIP block test entry (sdb200.h: sdb_test_clip_block); trace = kClipTraceInts ints
-constexpr int kClipTraceInts = 80;
 void model_test_clip_block(Ctx& c, int index, const float* x, int n, int L, int flags, float* out, float* taps, int32_t* trace);
 
 }  // namespace sdb

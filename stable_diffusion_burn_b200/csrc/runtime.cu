@@ -219,7 +219,7 @@ void run_attention(Ctx& c, const AttnOp& a) {
     memset(dbg_buf, 0, 256 * sizeof(long long));
     p.dbg = dbg_buf;
   }
-  if (c.trace_on) c.attn_trace.push_back({a.dpad, a.Nq, a.Nk, p.qk3, a.kvlen ? 1 : 0, a.causal});
+  if (c.trace_on) c.trace.push_back({TRACE_ATTN, {a.dpad, a.Nq, a.Nk, p.qk3, a.kvlen ? 1 : 0, a.causal}});
   {
     KernelScope ks(c, KC_ATTN, flops, 0);
     attention_launch(am, p, c.stream);
@@ -403,7 +403,8 @@ void run_gemm(Ctx& c, int kind, const ActOp& a0in, const ActOp* a1in, const Weig
   if (c.trace_on) {
     const int epi = (ep.ln_out ? EPI_ROLE_LNS : 0) | (ep.ln_in ? EPI_ROLE_LNC : 0) | (ep.geglu ? EPI_ROLE_GEGLU : 0) |
                     (ep.residual16.hi ? EPI_ROLE_RES16 : 0) | (ep.residual ? EPI_ROLE_RES32 : 0) | (gn ? EPI_ROLE_GN : 0);
-    c.gemm_trace.push_back({kind_in, w.N, BN, split, p.TN, p.TH, p.TW, p.xkc * 64, gn ? gn->slots : 0, a1in ? a1.C : 0, passes, epi, ep.act});
+    c.trace.push_back({TRACE_GEMM, {kind_in, w.N, BN, split, p.TN, p.TH, p.TW, p.xkc * 64, gn ? gn->slots : 0, a1in ? a1.C : 0, passes,
+                                    epi, ep.act, gemm_tc_stages(BN, passes)}});
   }
   p.gn_part = gn ? gn->buf : nullptr;
   p.gn_cap = gn ? gn->cap : 0, p.gn_bucket = gn ? gn->bucket : 1;

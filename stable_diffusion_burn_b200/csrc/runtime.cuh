@@ -47,9 +47,17 @@ enum GnPath : int {
   GN_PATH_SUMS_PARTIALS = 5,
   GN_PATH_SUMS_FOLD = 6
 };
-// epilogue roles of a recorded GEMM (Ctx::GemmRecord::epi): LayerNorm statistics out, LayerNorm-consuming correction, GEGLU,
-// fp16-pair residual, fp32 residual, GroupNorm partials out
+// epilogue roles of a recorded GEMM (TraceRecord of TRACE_GEMM): LayerNorm statistics out, LayerNorm-consuming correction,
+// GEGLU, fp16-pair residual, fp32 residual, GroupNorm partials out
 enum EpiRole : int { EPI_ROLE_LNS = 1, EPI_ROLE_LNC = 2, EPI_ROLE_GEGLU = 4, EPI_ROLE_RES16 = 8, EPI_ROLE_RES32 = 16, EPI_ROLE_GN = 32 };
+
+// One launch record of a test entry (include/sdb200.h: SDB_TRACE_INTS, where each kind's fields are listed), so a test can assert
+// it reached the path it is meant to cover: a kind tag, then fixed-width fields, zero-padded.
+enum TraceKind : int { TRACE_GEMM = 1, TRACE_ATTN = 2, TRACE_GN = 3, TRACE_CONV = 4, TRACE_SOFTMAX = 5, TRACE_COND = 6 };
+struct TraceRecord {
+  int kind;
+  int f[15];
+};
 
 enum KernelClass : int {
   KC_GEMM = 0,
@@ -188,21 +196,9 @@ struct Ctx {
   // SDB_DEBUG_SYNC=1: synchronise after every launch and report the failing op (bring-up aid)
   bool debug_sync = false;
   std::string dbg_label;
-  // launch record for the test entries (sdb_test_resblock, sdb_test_spatial_transformer): what run_gemm chose per GEMM, what
-  // run_attention launched and which GroupNorm path Fwd::gn_operand took, so a test can assert it reached the path it is meant
-  // to cover. epi: EPI_ROLE_* bits of the epilogue (gn only when the statistics were really written); act: Epilogue::act
-  struct GemmRecord {
-    int kind, N, BN, split, TN, TH, TW, xk_channels, gn_slots, a1_channels, passes, epi, act;
-  };
-  struct AttnRecord {
-    int dpad, Nq, Nk, qk3, kvlen, causal;
-  };
+  // the launch records of a test entry, in launch order (TraceScope, model.cuh)
   bool trace_on = false;
-  std::vector<GemmRecord> gemm_trace;
-  std::vector<AttnRecord> attn_trace;
-  std::vector<int> gn_trace;  // GN_PATH_*
-  std::vector<int> conv_trace;     // fused GroupNorm + small-Cout convs: TH, CK, KS of each launch (sdb_test_vae_stage)
-  std::vector<int> softmax_trace;  // VAE attention row softmax: PER of each launch
+  std::vector<TraceRecord> trace;
 
   float* master_ptr(const std::string& name);
   const TensorInfo& info(const std::string& name);

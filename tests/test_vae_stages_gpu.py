@@ -176,6 +176,7 @@ class Precision:
 # name: H, W, n, the query-row stride of the reference
 ATTN_CASES = {
     "hw64_n3": (8, 8, 3, 1),       # two images per proj_out tile, the last tile half masked
+    "hw64_n7": (8, 8, 7, 1),       # 18 GEMMs and 7 softmax launches in one call, each with its own trace record
     "16x16_n4": (16, 16, 4, 1),    # a full decode chunk: samples 1-3 of the per-sample loop
     "12x16": (12, 16, 2, 1),       # HW = 192: 1.5 proj_out tiles per image, which leaves no partials (the consumer's GroupNorm
                                    # runs fused); H*W must be a multiple of 64 (P is the P.V product's 64-channel operand)
@@ -185,7 +186,7 @@ ATTN_CASES = {
 }
 
 
-def expect_attn_trace(tr, h, w, n, passes, stats):
+def expect_attention_trace(tr, h, w, n, passes, stats):
     hw = h * w
     g = tr["gemms"]
     assert len(g) == 3 + 2 * n + 1, len(g)
@@ -223,7 +224,7 @@ def attn_check(ctx, P, stage, case, passes, variant="default", r=0.0, x=None, ke
     o = res["tap"].reshape(n, 512, hw)[:, :, rows]
     e_add, e_o, e_max = rel(out - xs, ref - xs), rel(o, ref_o), relmax(out, ref)
     per_sample = [rel(out[s] - xs[s], ref[s] - xs[s]) for s in range(n)]
-    slots = expect_attn_trace(res["trace"], h, w, n, passes, True)
+    slots = expect_attention_trace(res["trace"], h, w, n, passes, True)
     en = rel(res["out_norm"], ref_gn_silu(P, ATTN_NEXT[stage], res["out"]))
     print(f"vae {stage} {case} [{variant}] P={passes} softmax PER {res['trace']['softmax'][0]} proj_out slots {slots} "
           f"gn {res['trace']['gn']} median max P {pmax:.3f} P<2^-24 {under:.2f}: added rel L2 {e_add:.3e} "
@@ -290,6 +291,15 @@ def test_vae_attention_large_v_bias(ctx, vae, stage):
     sign = np.where(np.random.default_rng(3).random(512) < 0.5, -1.0, 1.0)
     up = {f"{name}/v/bias": (10.0 * vrms * sign).astype(np.float32)}
     _with_tensors(ctx, vae, up, lambda P2: attn_check(ctx, P2, stage, "hw64_n3", 3, "v bias x10", x=x, key="vbias"))
+
+
+def test_vae_attention_trace_overflow(ctx, vae):
+    """dec_attn at 8x8 with n = 30 records 96 launches (64 GEMMs, 30 softmaxes, 2 GroupNorm stagings), more than SDB_TRACE_INTS
+    holds: the call fails with the record count and the capacity instead of truncating, and the next call on the context runs"""
+    x = activation("dec_attn/overflow", 30, 512, 8, 8)
+    with pytest.raises(RuntimeError, match=r"96 records do not fit SDB_TRACE_INTS \(63 records\)"):
+        ctx.test_vae_stage("dec_attn", x, stats=True)
+    attn_check(ctx, vae, "dec_attn", "hw64_n3", 3)
 
 
 # ------------------------------------------------------------------------------------------------ small-Cout conv
