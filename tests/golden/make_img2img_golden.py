@@ -1,5 +1,6 @@
-"""Writes tests/golden/img2img_b2.npz (and no other fixture) from the img2img oracle (tests/img2img_oracle.py) on the synthetic
-weights (seed 0): n = 2, 256x256 px (32x32 latent), L = 7, Lu = 2, cfg 5.0, 4 steps at strength 0.5 (k = 2: t = 499, 249).
+"""Writes tests/golden/img2img_b2.npz (and no other fixture) from the img2img oracle (tests/sampler_oracle.py:
+sampler_img2img_latent, DDIM) on the synthetic weights (seed 0): n = 2, 256x256 px (32x32 latent), L = 7, Lu = 2, cfg 5.0,
+4 steps at strength 0.5 (k = 2: t = 499, 249).
 Stores the inputs (images, masks, noise), z0, the latent mask w, the final latent and the u8 output at a stride of 2.
 Run from the repo root:  python tests/golden/make_img2img_golden.py
 """
@@ -16,6 +17,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import sd_oracle as O  # noqa: E402
 from stable_diffusion_burn_b200 import synth  # noqa: E402
 import img2img_oracle as IO  # noqa: E402
+import sampler_oracle as SO  # noqa: E402
 
 OUT = os.path.dirname(os.path.abspath(__file__))
 
@@ -31,7 +33,8 @@ def main():
     taps = {}
     t1 = time.time()
     with torch.no_grad():
-        lat = IO.img2img_latent(P, ctx, unc, cfg["scale"], cfg["n_steps"], image, cfg["strength"], noise, mask_u8=mask, taps=taps)
+        lat = SO.sampler_img2img_latent(P, ctx, unc, cfg["scale"], cfg["n_steps"], image, cfg["strength"], noise, mask_u8=mask,
+                                        taps=taps)
         u8 = O.to_u8(O.latent_to_image_f32(P, lat))
     print("img2img", time.time() - t1, flush=True)
     np.savez_compressed(os.path.join(OUT, "img2img_b2.npz"), image=image, mask=mask, noise=noise, z0=taps["z0"], w=taps["w"],

@@ -2,20 +2,17 @@
 
 An inpainting checkpoint's UNet reads cat(x_t, latent mask, masked-image latent) (the order of diffusers' inpainting pipeline and
 of the original LDM LatentInpaintDiffusion). The reference has no such model; the functions below follow the semantics the CUDA
-path implements, on top of tests/img2img_oracle.py (conversion, strength rule, z0), tests/sampler_oracle.py (the samplers' step
-arithmetic) and oracle/sd_oracle.py (encode_image, forward_diffuser, whose UNet takes whatever conv_in holds). Elementwise rules
+path implements, on top of tests/img2img_oracle.py (conversion), tests/sampler_oracle.py (strength rule, z0, start latent, the
+step loop) and oracle/sd_oracle.py (encode_image, forward_diffuser, whose UNet takes whatever conv_in holds). Elementwise rules
 are evaluated in numpy float32, one rounding per operation. The fixture tests/golden/inpaint_b2.npz is written by
 tests/golden/make_inpaint_golden.py from img2img_inputs() and INPAINT_CASES.
 """
 from __future__ import annotations
 
-import math
-
 import numpy as np
 import torch
 
-from oracle.sd_oracle import ddim_timesteps, encode_image, forward_diffuser
-from stable_diffusion_burn_b200 import synth
+from oracle.sd_oracle import encode_image, forward_diffuser
 
 import img2img_oracle as IO
 import sampler_oracle as SO
@@ -39,8 +36,7 @@ def masked_image(image_u8, mask_u8):
 
 def inpaint_cond(P, image_u8, mask_u8):
     """The UNet's extra input channels [n,5,H,W]: the latent mask, then z_m = fl(encode_image(x_m) * 0.18215)."""
-    z_m = np.multiply(encode_image(P, torch.from_numpy(masked_image(image_u8, mask_u8))).to(torch.float32).numpy(),
-                      np.float32(0.18215))
+    z_m = SO.scaled_latent(encode_image(P, torch.from_numpy(masked_image(image_u8, mask_u8))))
     return np.concatenate([latent_mask(mask_u8)[:, None], z_m], 1)
 
 
@@ -52,37 +48,16 @@ def inpaint_latent(P, context, uncond, scale, n_steps, image_u8, strength, noise
     if mask_u8 is None:
         raise ValueError("inpainting with a 9-channel UNet needs a mask")
     SO.check_sampler(kind, eta)
-    alphas = P("alpha_cumulative_products").to(torch.float32)
-    first, ts = IO.img2img_start(strength, n_steps)
-    _, step = ddim_timesteps(n_steps)
-    z0 = np.multiply(encode_image(P, torch.from_numpy(IO.image_u8_to_float(image_u8))).to(torch.float32).numpy(),
-                     np.float32(0.18215))
+    first, ts = SO.img2img_start(strength, n_steps)
+    z0 = SO.scaled_latent(encode_image(P, torch.from_numpy(IO.image_u8_to_float(image_u8))))
     cond = inpaint_cond(P, image_u8, mask_u8)
     if taps is not None:
         taps["z0"], taps["m_lat"], taps["z_m"] = z0, cond[:, 0], cond[:, 1:]
-    eps = np.asarray(noise, np.float32)
-    a0 = float(alphas[ts[first]])
-    latent = torch.from_numpy(np.add(np.multiply(np.float32(math.sqrt(a0)), z0),
-                                     np.multiply(np.float32(math.sqrt(1.0 - a0)), eps))).to(P.dtype)
+    a0 = float(P("alpha_cumulative_products").to(torch.float32)[ts[first]])
+    start = SO.start_latent(a0, z0, np.asarray(noise, np.float32))
     cond_t = torch.from_numpy(cond).to(P.dtype)
-    x0_prev, h_prev = None, None
-    for t in ts[first:]:
-        a_t = float(alphas[t])
-        a_prev = float(alphas[t - step]) if t >= step else 1.0
-        pred = forward_diffuser(P, torch.cat([latent, cond_t], 1), t, context, uncond, scale)
-        predx0 = (latent - pred * math.sqrt(1.0 - a_t)) / math.sqrt(a_t)
-        if kind == SO.DDIM and eta == 0.0:
-            latent = predx0 * math.sqrt(a_prev) + pred * math.sqrt(1.0 - a_prev)
-        elif kind == SO.DDIM:
-            s, dir_ = SO.ddim_coefs(a_t, a_prev, eta)
-            z = synth.step_noise(noise_seed, t, tuple(latent.shape))
-            latent = torch.from_numpy(SO.ddim_eta_update(predx0.numpy(), pred.numpy(), a_prev, s, dir_, z))
-        else:
-            cx, cd, c2, h = SO.dpmpp_coefs(a_t, a_prev, h_prev)
-            x0 = predx0.numpy()
-            latent = torch.from_numpy(SO.dpmpp_update(latent.numpy(), x0, x0_prev, cx, cd, c2))
-            x0_prev, h_prev = x0, h
-    return latent
+    guide = lambda x, t: forward_diffuser(P, torch.cat([x, cond_t], 1), t, context, uncond, scale)
+    return SO.guided_latent(P, n_steps, start, guide, kind, eta, noise_seed, first)
 
 
 def zero_extension(conv_in4):

@@ -5,9 +5,9 @@ InstructPix2Pix (Brooks et al. 2023) conditions an SD-1.x UNet on the input imag
 posterior mode of the image, unscaled. Each step evaluates the UNet three times and combines the results with a text and an
 image scale, as the original edit_cli.py and diffusers' StableDiffusionInstructPix2PixPipeline do. The reference has no such
 model; the functions below follow the semantics the CUDA path implements, on top of tests/img2img_oracle.py (the image
-conversion), tests/sampler_oracle.py (the samplers' step arithmetic) and oracle/sd_oracle.py (encode_image and unet_forward,
-whose conv_in takes whatever width P holds). The fixture tests/golden/pix2pix_b2.npz is written by
-tests/golden/make_pix2pix_golden.py from PIX2PIX_CASES.
+conversion), tests/sampler_oracle.py (the step loop) and oracle/sd_oracle.py (encode_image and unet_forward, whose conv_in
+takes whatever width P holds). The fixture tests/golden/pix2pix_b2.npz is written by tests/golden/make_pix2pix_golden.py from
+PIX2PIX_CASES.
 """
 from __future__ import annotations
 
@@ -16,8 +16,7 @@ import math
 import numpy as np
 import torch
 
-from oracle.sd_oracle import ddim_timesteps, encode_image, unet_forward
-from stable_diffusion_burn_b200 import synth
+from oracle.sd_oracle import encode_image, unet_forward
 
 import img2img_oracle as IO
 import sampler_oracle as SO
@@ -38,34 +37,6 @@ def check_scales(text_scale, image_scale):
 def three_way(e_u, e_i, e_t, text_scale, image_scale):
     """pred = e_U + s_T (e_T - e_I) + s_I (e_I - e_U), left to right, one rounding per operation in the tensors' dtype."""
     return (e_u + (e_t - e_i) * text_scale) + (e_i - e_u) * image_scale
-
-
-def guided_latent(P, n_steps, latent0, guide, kind=SO.DDIM, eta=0.0, noise_seed=0):
-    """The full DDIM schedule from t = 999 under any sampler, pred = guide(latent, t) at each step -> the final latent
-    (torch). The updates are those of sampler_oracle.sampler_latent."""
-    SO.check_sampler(kind, eta)
-    alphas = P("alpha_cumulative_products").to(torch.float32)
-    ts, step = ddim_timesteps(n_steps)
-    latent = torch.as_tensor(np.asarray(latent0)).to(P.dtype)
-    x0_prev, h_prev = None, None
-    for t in ts:
-        a_t = float(alphas[t])
-        a_prev = float(alphas[t - step]) if t >= step else 1.0
-        pred = guide(latent, t)
-        predx0 = (latent - pred * math.sqrt(1.0 - a_t)) / math.sqrt(a_t)
-        if kind == SO.DDIM and eta == 0.0:
-            latent = predx0 * math.sqrt(a_prev) + pred * math.sqrt(1.0 - a_prev)
-        elif kind == SO.DDIM:
-            s, dir_ = SO.ddim_coefs(a_t, a_prev, eta)
-            z = synth.step_noise(noise_seed, t, tuple(latent.shape))
-            latent = torch.from_numpy(SO.ddim_eta_update(predx0.numpy(), pred.numpy(), a_prev, s, dir_, z))
-        else:
-            cx, cd, c2, h = SO.dpmpp_coefs(a_t, a_prev, h_prev)
-            x0 = predx0.numpy()
-            latent = torch.from_numpy(SO.dpmpp_update(latent.numpy(), x0, x0_prev, cx, cd, c2))
-            x0_prev, h_prev = x0, h
-        latent = latent.to(P.dtype)
-    return latent
 
 
 def pix2pix_latent(P, ctx, unc, text_scale, image_scale, n_steps, image_u8, latent0, kind=SO.DDIM, eta=0.0, noise_seed=0,
@@ -89,7 +60,7 @@ def pix2pix_latent(P, ctx, unc, text_scale, image_scale, n_steps, image_u8, late
         e_u = unet_forward(P, torch.cat([x, zero], 1), t, u_ctx)
         return three_way(e_u, e_i, e_t, text_scale, image_scale)
 
-    return guided_latent(P, n_steps, latent0, guide, kind, eta, noise_seed)
+    return SO.guided_latent(P, n_steps, latent0, guide, kind, eta, noise_seed)
 
 
 def zero_extension(conv_in4):

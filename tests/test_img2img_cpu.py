@@ -11,6 +11,7 @@ from oracle import sd_oracle as O
 from stable_diffusion_burn_b200 import synth
 
 import img2img_oracle as IO
+import sampler_oracle as SO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "img2img_b2.npz")
@@ -30,19 +31,19 @@ def rel(a, b):
     (1, 1.0, [999]),
 ])
 def test_strength_to_schedule(n_steps, strength, ts_run):
-    first, ts = IO.img2img_start(strength, n_steps)
+    first, ts = SO.img2img_start(strength, n_steps)
     assert ts[first:] == ts_run
 
 
 @pytest.mark.parametrize("n_steps", [1, 4, 20, 50])
 def test_strength_below_one_step_rejected(n_steps):
     N = len(O.ddim_timesteps(n_steps)[0])
-    IO.img2img_start(1.0 / N, n_steps)  # the smallest valid strength runs one step
+    SO.img2img_start(1.0 / N, n_steps)  # the smallest valid strength runs one step
     with pytest.raises(ValueError, match=f"1/{N}"):
-        IO.img2img_start(np.nextafter(1.0 / N, 0.0), n_steps)
+        SO.img2img_start(np.nextafter(1.0 / N, 0.0), n_steps)
     for bad in (0.0, -0.5, 1.5, float("nan"), float("inf")):
         with pytest.raises(ValueError):
-            IO.img2img_start(bad, n_steps)
+            SO.img2img_start(bad, n_steps)
 
 
 def test_image_u8_to_float_formula():
@@ -85,16 +86,15 @@ def small():
 
 def _run(s, n_steps, strength, mask=None, taps=None):
     with torch.no_grad():
-        return IO.img2img_latent(s["P"], s["ctx"], s["unc"], 5.0, n_steps, s["img"], strength, s["noise"], mask_u8=mask,
-                                taps=taps).numpy()
+        return SO.sampler_img2img_latent(s["P"], s["ctx"], s["unc"], 5.0, n_steps, s["img"], strength, s["noise"],
+                                         mask_u8=mask, taps=taps).numpy()
 
 
 def test_strength_one_is_txt2img_from_the_noised_image(small):
     taps = {}
     got = _run(small, 2, 1.0, taps=taps)
     a0 = float(small["P"]("alpha_cumulative_products")[999])
-    sa, sb = np.float32(np.sqrt(a0)), np.float32(np.sqrt(1.0 - a0))
-    init = sa * taps["z0"] + sb * small["noise"]
+    init = SO.start_latent(a0, taps["z0"], small["noise"])
     with torch.no_grad():
         want = O.sample_latent(small["P"], small["ctx"], small["unc"], 5.0, 2, torch.from_numpy(init)).numpy()
     assert np.array_equal(got, want)
@@ -124,7 +124,7 @@ def test_fixture_inputs_and_z0_w():
     with torch.no_grad():
         z = O.encode_image(P, torch.from_numpy(IO.image_u8_to_float(image))).numpy()
     # torch's CPU convolutions may pick other algorithms on another machine: the encoder bar of tests/test_vae_encoder.py
-    assert rel(g["z0"], np.multiply(z, np.float32(0.18215))) < 1e-5
+    assert rel(g["z0"], SO.scaled_latent(z)) < 1e-5
 
 
 def test_fixture_rederived(small):
@@ -132,8 +132,9 @@ def test_fixture_rederived(small):
     g = np.load(GOLD)
     P = small["P"]
     with torch.no_grad():
-        lat = IO.img2img_latent(P, torch.from_numpy(synth.make_context(2, 7, seed=3)), small["unc"], IO.IMG2IMG["scale"],
-                               IO.IMG2IMG["n_steps"], g["image"], IO.IMG2IMG["strength"], g["noise"], mask_u8=g["mask"])
+        lat = SO.sampler_img2img_latent(P, torch.from_numpy(synth.make_context(2, 7, seed=3)), small["unc"],
+                                        IO.IMG2IMG["scale"], IO.IMG2IMG["n_steps"], g["image"], IO.IMG2IMG["strength"],
+                                        g["noise"], mask_u8=g["mask"])
         u8 = O.to_u8(O.latent_to_image_f32(P, lat))
     assert rel(lat.numpy(), g["latent"]) < 1e-4
     d = np.abs(u8[:, ::2, ::2, :].astype(np.int16) - g["u8"].astype(np.int16))

@@ -11,6 +11,7 @@ import torch
 from stable_diffusion_burn_b200 import _lib, synth
 
 import img2img_oracle as IO
+import sampler_oracle as SO
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "img2img_b2.npz")
@@ -58,7 +59,7 @@ def test_golden(case):
 
 def test_conversion_and_final_paste_bit_exact(sd, case):
     x = IO.image_u8_to_float(case["image"])  # numpy float32, the same n (= the same encoder chunking)
-    want = np.multiply(sd.encode_image(x), np.float32(0.18215))
+    want = SO.scaled_latent(sd.encode_image(x))
     assert np.array_equal(case["z0"], want)
     w = IO.mask_to_latent(case["mask"])
     keep = np.broadcast_to((w == 0)[:, None], case["lat"].shape)
@@ -75,8 +76,7 @@ def test_all_255_mask_is_no_mask(case):
 def test_strength_one_is_txt2img(sd, case):
     got = case["run"](strength=1.0, latent=True, rgb=False)
     abar = float(sd.get_tensor("alpha_cumulative_products", (1000,))[999])
-    sa, sb = np.float32(np.sqrt(abar)), np.float32(np.sqrt(1.0 - abar))
-    init = np.add(np.multiply(sa, case["z0"]), np.multiply(sb, case["noise"]))
+    init = SO.start_latent(abar, case["z0"], case["noise"])
     want = sd.sample_latent(case["ctx"], case["unc"], SCALE, STEPS, init_latent=init)
     assert np.array_equal(got, want)
 

@@ -103,42 +103,23 @@ def test_golden(sd9, case):
         assert e < 2e-3 and frac >= 0.998 and dmax <= 4, name
 
 
-def _fma(a, b, c):
-    """fl32(a b + c) with one rounding (the product of two float32 values is exact in float64)."""
-    return (np.asarray(a, np.float64) * np.asarray(b, np.float64) + np.asarray(c, np.float64)).astype(np.float32)
-
-
 def _host_loop(sd, case, name, strength):
     """sdb_img2img on a 9-channel context restated on the host: z0 and z_m from sdb_encode_image, the latent mask and the start
     latent in numpy, each step's two UNet outputs from sdb_forward_diffuser on [n,9,H,W] = x | m_lat | z_m, and the update with
     the fused step's contractions (tests/test_sampler_gpu.py: _host_loop)."""
     kind, eta = SAMPLERS[name]
-    f = np.float32
-    z0 = np.multiply(sd.encode_image(IO.image_u8_to_float(case["image"])), f(0.18215))
-    z_m = np.multiply(sd.encode_image(NO.masked_image(case["image"], case["mask"])), f(0.18215))
+    z0 = SO.scaled_latent(sd.encode_image(IO.image_u8_to_float(case["image"])))
+    z_m = SO.scaled_latent(sd.encode_image(NO.masked_image(case["image"], case["mask"])))
     cond = np.concatenate([NO.latent_mask(case["mask"])[:, None], z_m], 1)
     alphas = sd.get_tensor("alpha_cumulative_products", (1000,))
-    first, ts = IO.img2img_start(strength, STEPS)
-    step = 1000 // STEPS
-    a0 = float(alphas[ts[first]])
-    x = np.add(np.multiply(f(math.sqrt(a0)), z0), np.multiply(f(math.sqrt(1.0 - a0)), case["noise"]))
-    x0_prev, h_prev = None, None
-    for t in ts[first:]:
-        a_t = float(alphas[t]); a_prev = float(alphas[t - step]) if t >= step else 1.0
+    first, ts = SO.img2img_start(strength, STEPS)
+
+    def guide(x, t):
         _, u, c = sd.forward_diffuser(np.concatenate([x, cond], 1), t, case["ctx"], case["unc"], SCALE)
-        pred = _fma(np.subtract(c, u), f(SCALE), u)
-        x0 = np.divide(_fma(-pred, f(math.sqrt(1.0 - a_t)), x), f(math.sqrt(a_t)))
-        if kind == SO.DDIM and eta == 0.0:
-            x = _fma(pred, f(math.sqrt(1.0 - a_prev)), np.multiply(x0, f(math.sqrt(a_prev))))
-        elif kind == SO.DDIM:
-            s, d = SO.ddim_coefs(a_t, a_prev, eta)
-            z = sd.test_step_noise(NSEED, t, x.size).reshape(x.shape)
-            x = SO.ddim_eta_update(x0, pred, a_prev, s, d, z)
-        else:
-            cx, cd, c2, h = SO.dpmpp_coefs(a_t, a_prev, h_prev)
-            x = SO.dpmpp_update(x, x0, x0_prev, cx, cd, c2)
-            x0_prev, h_prev = x0, h
-    return x
+        return SO.fma(np.subtract(c, u), np.float32(SCALE), u)
+
+    return SO.step_loop(SO.start_latent(float(alphas[ts[first]]), z0, case["noise"]), guide, alphas, STEPS, SO.KERNEL, kind, eta,
+                        lambda t, shape: sd.test_step_noise(NSEED, t, math.prod(shape)).reshape(shape), first)
 
 
 @pytest.mark.parametrize("name", list(SAMPLERS))

@@ -62,7 +62,7 @@ def test_image_latent_is_unscaled():
         c_i = PO.image_latent(P, img).numpy()
         enc = O.encode_image(P, torch.from_numpy(IO.image_u8_to_float(img))).numpy()
     assert np.array_equal(c_i, enc)
-    assert rel(np.multiply(enc, np.float32(0.18215)), c_i) > 0.5
+    assert rel(SO.scaled_latent(enc), c_i) > 0.5
 
 
 @pytest.fixture(scope="module")
@@ -101,7 +101,7 @@ def test_image_scale_one_is_cfg_on_the_image(f64, kind):
         got = PO.pix2pix_latent(P, f64["ctx"], f64["unc"], 5.0, 1.0, 2, f64["img"], f64["latent0"], kind=kind).numpy()
         c_i = PO.image_latent(P, f64["img"])
         guide = lambda x, t: O.forward_diffuser(P, torch.cat([x, c_i], 1), t, f64["ctx"], f64["unc"], 5.0)
-        want = PO.guided_latent(P, 2, f64["latent0"], guide, kind=kind).numpy()
+        want = SO.guided_latent(P, 2, f64["latent0"], guide, kind=kind).numpy()
     print(f"image scale 1, kind {kind}: rel {rel(got, want):.3e}")
     assert rel(got, want) < 1e-12
 

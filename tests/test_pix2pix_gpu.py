@@ -110,11 +110,6 @@ def test_golden(sd8, case):
         assert e < 2e-3 and frac >= 0.998 and dmax <= 4, name
 
 
-def _fma(a, b, c):
-    """fl32(a b + c) with one rounding (the product of two float32 values is exact in float64)."""
-    return (np.asarray(a, np.float64) * np.asarray(b, np.float64) + np.asarray(c, np.float64)).astype(np.float32)
-
-
 def _host_loop(sd, case, name, unc, c_i=None):
     """sdb_edit_image restated on the host: c_I from sdb_encode_image (unscaled), each step's three UNet outputs from ONE
     sdb_unet_forward at batch 3n on [3n,8,H,W] = (x | 0), (x | c_I), (x | c_I) under (negative, negative, prompt) — the call's
@@ -125,29 +120,16 @@ def _host_loop(sd, case, name, unc, c_i=None):
         c_i = sd.encode_image(IO.image_u8_to_float(case["image"]))
     n = c_i.shape[0]
     ctx3 = np.concatenate([np.repeat(unc[None], 2 * n, 0), case["ctx"]], 0)
-    alphas = sd.get_tensor("alpha_cumulative_products", (1000,))
-    ts, step = list(range(999, -1, -(1000 // STEPS))), 1000 // STEPS
-    x = case["latent0"].copy()
-    x0_prev, h_prev = None, None
-    for t in ts:
-        a_t = float(alphas[t]); a_prev = float(alphas[t - step]) if t >= step else 1.0
+
+    def guide(x, t):
         x3 = np.concatenate([np.concatenate([x, np.zeros_like(c_i)], 1), np.concatenate([x, c_i], 1),
                              np.concatenate([x, c_i], 1)], 0)
         e = sd.unet_forward(x3, t, ctx3)
         u, i, tx = e[:n], e[n:2 * n], e[2 * n:]
-        pred = np.add(np.add(u, np.multiply(f(TS), np.subtract(tx, i))), np.multiply(f(IS), np.subtract(i, u)))
-        x0 = np.divide(_fma(-pred, f(math.sqrt(1.0 - a_t)), x), f(math.sqrt(a_t)))
-        if kind == SO.DDIM and eta == 0.0:
-            x = _fma(pred, f(math.sqrt(1.0 - a_prev)), np.multiply(x0, f(math.sqrt(a_prev))))
-        elif kind == SO.DDIM:
-            s, d = SO.ddim_coefs(a_t, a_prev, eta)
-            z = sd.test_step_noise(NSEED, t, x.size).reshape(x.shape)
-            x = SO.ddim_eta_update(x0, pred, a_prev, s, d, z)
-        else:
-            cx, cd, c2, h = SO.dpmpp_coefs(a_t, a_prev, h_prev)
-            x = SO.dpmpp_update(x, x0, x0_prev, cx, cd, c2)
-            x0_prev, h_prev = x0, h
-    return x
+        return np.add(np.add(u, np.multiply(f(TS), np.subtract(tx, i))), np.multiply(f(IS), np.subtract(i, u)))
+
+    return SO.step_loop(case["latent0"], guide, sd.get_tensor("alpha_cumulative_products", (1000,)), STEPS, SO.KERNEL, kind, eta,
+                        lambda t, shape: sd.test_step_noise(NSEED, t, math.prod(shape)).reshape(shape))
 
 
 @pytest.mark.parametrize("name", list(SAMPLERS))
@@ -167,7 +149,7 @@ def test_image_latent_is_unscaled(sd8, case):
     print(f"c_I rel to the fixture's {rel(c_i, case['g']['c_I']):.3e}")
     assert rel(c_i, case["g"]["c_I"]) < 1e-3
     assert np.array_equal(got, _host_loop(sd8, case, "ddim", unc7, c_i))
-    scaled = _host_loop(sd8, case, "ddim", unc7, np.multiply(c_i, np.float32(0.18215)))
+    scaled = _host_loop(sd8, case, "ddim", unc7, SO.scaled_latent(c_i))
     print(f"pix2pix: result with a scaled image latent differs by rel L2 {rel(scaled, got):.3e}")
     assert rel(scaled, got) > 1e-3
 

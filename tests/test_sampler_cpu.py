@@ -11,7 +11,6 @@ import torch
 from oracle import sd_oracle as O
 from stable_diffusion_burn_b200 import synth
 
-import img2img_oracle as IO
 import sampler_oracle as SO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -133,7 +132,7 @@ def test_fixture_inputs():
     assert np.array_equal(g["noise"], synth.make_latent(2, 32, 32, seed=41))
     for k in ("dpmpp", "eta", "inpaint"):
         assert g[f"{k}_latent"].shape == (2, 4, 32, 32) and g[f"{k}_u8"].shape == (2, 128, 128, 3)
-    first, ts = IO.img2img_start(SO.SAMPLER_CASES["strength"], SO.SAMPLER_CASES["n_steps"])
+    first, ts = SO.img2img_start(SO.SAMPLER_CASES["strength"], SO.SAMPLER_CASES["n_steps"])
     assert ts[first:] == [749, 499, 249]
 
 

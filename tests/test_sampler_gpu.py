@@ -77,37 +77,18 @@ def test_golden(sd, case):
         assert e < 2e-3 and frac >= 0.998 and dmax <= 4, name
 
 
-def _fma(a, b, c):
-    """fl32(a b + c) with one rounding (the product of two float32 values is exact in float64)."""
-    return (np.asarray(a, np.float64) * np.asarray(b, np.float64) + np.asarray(c, np.float64)).astype(np.float32)
-
-
 def _host_loop(sd, case, kind, eta):
     """sample_latent restated on the host around sdb_forward_diffuser: the two UNet outputs of each step from the library, the
-    guidance combine and x0 as the fused step's SASS computes them (pred = fma(c - u, scale, u), x0 = fma(-pred, sqrt(1 - a_t), x)
-    / sqrt(a_t), the eta = 0 update fma(pred, sqrt(1 - a'), fl(x0 sqrt(a')))), the new updates from the oracle (numpy float32,
-    no contraction, as the kernel's __f*_rn). So only the sampler arithmetic is compared."""
-    alphas = sd.get_tensor("alpha_cumulative_products", (1000,))
-    ts, step = list(range(999, -1, -(1000 // STEPS))), 1000 // STEPS
-    f = np.float32
-    x = case["noise"].copy()
-    x0_prev, h_prev = None, None
-    for t in ts:
-        a_t = float(alphas[t]); a_prev = float(alphas[t - step]) if t >= step else 1.0
+    guidance combine as the fused step's SASS computes it (pred = fma(c - u, scale, u)), then the oracle's step_loop with its
+    KERNEL arithmetic (x0 = fma(-pred, sqrt(1 - a_t), x) / sqrt(a_t), the eta = 0 update fma(pred, sqrt(1 - a'),
+    fl(x0 sqrt(a')))), the new updates from the oracle (numpy float32, no contraction, as the kernel's __f*_rn) and eta's noise
+    from sdb_test_step_noise. So only the sampler arithmetic is compared."""
+    def guide(x, t):
         _, u, c = sd.forward_diffuser(x, t, case["ctx"], case["unc"], SCALE)
-        pred = _fma(np.subtract(c, u), f(SCALE), u)
-        x0 = np.divide(_fma(-pred, f(math.sqrt(1.0 - a_t)), x), f(math.sqrt(a_t)))
-        if kind == SO.DDIM and eta == 0.0:
-            x = _fma(pred, f(math.sqrt(1.0 - a_prev)), np.multiply(x0, f(math.sqrt(a_prev))))
-        elif kind == SO.DDIM:
-            s, d = SO.ddim_coefs(a_t, a_prev, eta)
-            z = sd.test_step_noise(NSEED, t, x.size).reshape(x.shape)
-            x = SO.ddim_eta_update(x0, pred, a_prev, s, d, z)
-        else:
-            cx, cd, c2, h = SO.dpmpp_coefs(a_t, a_prev, h_prev)
-            x = SO.dpmpp_update(x, x0, x0_prev, cx, cd, c2)
-            x0_prev, h_prev = x0, h
-    return x
+        return SO.fma(np.subtract(c, u), np.float32(SCALE), u)
+
+    return SO.step_loop(case["noise"], guide, sd.get_tensor("alpha_cumulative_products", (1000,)), STEPS, SO.KERNEL, kind, eta,
+                        lambda t, shape: sd.test_step_noise(NSEED, t, math.prod(shape)).reshape(shape))
 
 
 @pytest.mark.parametrize("name", list(SAMPLERS))
@@ -134,8 +115,7 @@ def test_img2img_identities(sd, case, name):
     """strength 1 = txt2img from the same start latent; an all-255 mask = no mask; for every sampler."""
     abar = float(sd.get_tensor("alpha_cumulative_products", (1000,))[999])
     from img2img_oracle import image_u8_to_float
-    z0 = np.multiply(sd.encode_image(image_u8_to_float(case["image"])), np.float32(0.18215))
-    init = np.add(np.multiply(np.float32(math.sqrt(abar)), z0), np.multiply(np.float32(math.sqrt(1.0 - abar)), case["noise"]))
+    init = SO.start_latent(abar, SO.scaled_latent(sd.encode_image(image_u8_to_float(case["image"]))), case["noise"])
     got = case["i2i"](name, strength=1.0)
     with sampler(sd, *SAMPLERS[name]):
         want = sd.sample_latent(case["ctx"], case["unc"], SCALE, STEPS, init_latent=init)
