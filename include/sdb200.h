@@ -325,18 +325,18 @@ int64_t sdb_launch_count(sdb_ctx* ctx);
  *   5 autoencoder attention row softmax: values per thread
  *   6 conditioned UNet conv_in: m, sample s reads the conditioning of sample s % m */
 #define SDB_TRACE_INTS 1024
-/* C[M,N] (fp32) = A[M,K] (fp32, rounded to the operand format) x B[K,N] (fp32 [in,out]) + bias.
- * Exercises the wgmma GEMM exactly as the Linear layers use it. */
-int sdb_test_linear(sdb_ctx* ctx, const float* a, const float* w, const float* bias, int M, int K, int N,
-                    int passes, float* c, int32_t* trace);
-/* The GEMM's other epilogues and K-loop forms, each reachable in isolation: out = A[M,K] x W[K,N] (+ bias) (+ residual[M,N])
- * (+ XA[M,XK] x XW[XK,N], the "extra K" operands the ResBlock skip conv rides on). flags: 1 = GEGLU (W = [K][x | gate], out
- * [M, N/2] = (x + b_x) * gelu_erf(gate + b_g), unet/mod.rs:578-592); 4 = read the result back from the fp16 hi + lo outputs;
+/* The GEMM as the Linear layers use it, and its other epilogues and K-loop forms, each reachable in isolation: out = A[M,K]
+ * (fp32, rounded to the operand format) x W[K,N] (fp32 [in,out]) (+ bias) (+ residual[M,N]) (+ XA[M,XK] x XW[XK,N], the
+ * "extra K" operands the ResBlock skip conv rides on). flags: 0 = the plain Linear product, fp32 out; 1 = GEGLU (W = [K][x |
+ * gate], out [M, N/2] = (x + b_x) * gelu_erf(gate + b_g), unet/mod.rs:578-592); 4 = read the result back from the fp16 hi + lo
+ * outputs;
  * 8 (with 4) = return the two fp16 planes separately: out = [2][M][N (or N/2)], hi then lo, each value converted to float.
  * Split-K is chosen by the library's own policy (small M x N grid, long K). */
 int sdb_test_gemm_ex(sdb_ctx* ctx, const float* a, const float* w, const float* bias, const float* residual, int M, int K,
                      int N, int passes, int flags, const float* xa, const float* xw, int XK, float* out, int32_t* trace);
-/* conv2d NCHW fp32 in/out through the implicit-GEMM path (3x3 pad 1 stride 1|2, or 1x1). */
+/* conv2d NCHW fp32 in/out through the implicit-GEMM path as the model runs it (its operand staging, weight packing and GEMM
+ * kinds): 1x1, 3x3 pad 1, 3x3 stride 2 (ksize 3: the UNet downsample), or upsample = 1 (ksize 3): nearest 2x upsample folded
+ * into the weights. cin a multiple of 64, cout of 32; any other stride / upsample combination is an error. */
 int sdb_test_conv2d(sdb_ctx* ctx, const float* x, const float* w, const float* bias, int n, int cin, int H,
                     int W, int cout, int ksize, int stride, int upsample, int passes, float* y, int32_t* trace);
 /* The LayerNorm-free TransformerBlock chain in isolation (unet/mod.rs:521-527): y = a w0 + b0 (+ a2 w0 + b0 accumulated in place
@@ -346,16 +346,14 @@ int sdb_test_conv2d(sdb_ctx* ctx, const float* x, const float* w, const float* b
 int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float* w0, const float* b0, const float* gamma,
                      const float* beta, const float* w1, const float* b1, int M, int K0, int C, int N, int passes, int geglu,
                      float* out, int32_t* trace);
-/* conv (3x3 pad 1 or 1x1) whose epilogue also leaves the GroupNorm statistics of its output, followed by the apply-only
- * GroupNorm(+SiLU) that consumes them (the ResBlock's conv_in -> norm_out -> SiLU chain, unet/mod.rs:716-725). stride 2 (3x3)
- * is the UNet downsample conv, upsample = 1 (3x3) the folded nearest-2x + conv of the upsample blocks. NCHW fp32 in/out;
- * *slots = partial-statistics slots per image the GEMM wrote (> 0). */
+/* The conv of sdb_test_conv2d whose epilogue also leaves the GroupNorm statistics of its output, in the partial buffer the
+ * model gives an activation of that width, followed by the apply-only GroupNorm(+SiLU) that consumes them (the ResBlock's
+ * conv_in -> norm_out -> SiLU chain, unet/mod.rs:716-725). NCHW fp32 in/out; *slots = partial-statistics slots per image the
+ * GEMM wrote. With the gn_epilogue option at 0 the model leaves no statistics, and the call fails with "the GEMM did not
+ * produce GroupNorm statistics for this shape" (*slots = 0). */
 int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const float* bias, const float* gamma,
                             const float* beta, int n, int cin, int H, int W, int cout, int ksize, int stride, int upsample,
                             int passes, int silu, float* y, int* slots, int32_t* trace);
-/* GroupNorm(32 groups)+optional SiLU, NCHW fp32 in/out. */
-int sdb_test_groupnorm(sdb_ctx* ctx, const float* x, const float* gamma, const float* beta, int n, int c,
-                       int H, int W, int silu, float* y);
 /* LayerNorm over the last dim, [rows, c]. */
 int sdb_test_layernorm(sdb_ctx* ctx, const float* x, const float* gamma, const float* beta, int rows, int c,
                        float* y);
@@ -378,8 +376,8 @@ int sdb_test_resblock(sdb_ctx* ctx, const float* x0, const float* x1, int n, int
                       const float* norm2_b, const float* conv2_w, const float* conv2_b, const float* skip_w, const float* skip_b,
                       const float* emb_bias, int passes, int flags, float* out, float* out16, float* out_norm, int32_t* trace);
 /* GroupNorm(32 groups)(+SiLU) of cat([x0, x1]) (x1 NULL when c1 = 0) as an fp16 hi + lo operand, returned NCHW as hi + lo.
- * mode 0: statistics kernel over both sources + apply; 1: the fused statistics + apply kernel; 2: apply from the partials two
- * producers left (3-pass identity convs, which pass hi + lo of the inputs), with the 64:1 pre-fold above 128 slots per image.
+ * mode 1: the fused statistics + apply kernel; 2: apply from the partials the producers left (3-pass identity convs, which
+ * pass hi + lo of the inputs), with the 64:1 pre-fold above 128 slots per image. Any other mode is an error.
  * trace: NULL or SDB_TRACE_INTS ints (see above). */
 int sdb_test_groupnorm_cat(sdb_ctx* ctx, const float* x0, const float* x1, int n, int c0, int c1, int H, int W,
                            const float* gamma, const float* beta, int silu, int mode, float* y, int32_t* trace);

@@ -100,7 +100,6 @@ SIGNATURES = [
                                   C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     ("sdb_profile_get_issued", C.c_int, [_ctx, C.c_int, C.POINTER(C.c_double)]),
     ("sdb_launch_count", C.c_int64, [_ctx]),
-    ("sdb_test_linear", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_conv2d", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                   C.c_int, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_ln_fold", C.c_int, [_ctx, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -120,7 +119,6 @@ SIGNATURES = [
                                      _f32p, _f32p, _f32p, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_clip_block", C.c_int, [_ctx, C.c_int, _f32p, C.c_int, C.c_int, C.c_int, _f32p, _f32p, C.POINTER(C.c_int32)]),
     ("sdb_test_step_noise", C.c_int, [_ctx, C.c_uint64, C.c_int, C.c_int64, _f32p]),
-    ("sdb_test_groupnorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_test_layernorm", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, _f32p]),
     ("sdb_test_attention", C.c_int, [_ctx, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.POINTER(C.c_int32), C.c_int, _f32p]),
@@ -646,14 +644,8 @@ class Context:
         return tr
 
     def test_linear(self, a, w, bias=None, passes=1, trace=False):
-        a = f32(a); w = f32(w)
-        M, K = a.shape; N = w.shape[1]
-        out = np.empty((M, N), np.float32)
-        b = f32(bias) if bias is not None else None
-        t, tp = self._trace_buf(trace)
-        self.check(self.lib.sdb_test_linear(self.h, ptr(a), ptr(w), ptr(b) if b is not None else None, M, K, N, passes, ptr(out),
-                                            tp))
-        return (out, self._decode_trace(t, ("gemms",))["gemms"]) if trace else out
+        """The plain Linear product a w (+ bias), fp32 out: test_gemm_ex without its other epilogues and K-loop forms."""
+        return self.test_gemm_ex(a, w, bias, passes=passes, trace=trace)
 
     def test_gemm_ex(self, a, w, bias=None, residual=None, passes=1, geglu=False, from_f16=False, xa=None, xw=None,
                      planes=False, trace=False):
@@ -738,9 +730,9 @@ class Context:
         tr["skip"] = "separate" if len(g) == 3 else ("merged" if g and g[-1]["xk"] > 0 else "none")
         return out, out16, outn, tr
 
-    def test_groupnorm_cat(self, x0, x1, gamma, beta, silu=False, mode=0):
-        """GroupNorm(+SiLU) of cat([x0, x1]) as the fp16 hi + lo operand. mode 0: statistics kernel + apply, 1: fused kernel,
-        2: apply from identity-producer partials (inputs pass as hi + lo). -> (y NCHW, trace)"""
+    def test_groupnorm_cat(self, x0, x1, gamma, beta, silu=False, mode=1):
+        """GroupNorm(+SiLU) of cat([x0, x1]) as the fp16 hi + lo operand. mode 1: fused kernel, 2: apply from identity-producer
+        partials (inputs pass as hi + lo). -> (y NCHW, trace)"""
         x0 = f32(x0)
         n, c0, H, W = x0.shape
         x1 = f32(x1) if x1 is not None else None
@@ -825,13 +817,6 @@ class Context:
             res.update({k: tp[i] for i, k in enumerate(self.CLIP_TAPS[:7])})
             res["h"] = tp[7:].reshape(n, L, 3072)
         return res
-
-    def test_groupnorm(self, x, gamma, beta, silu=False):
-        x = f32(x); n, c, H, W = x.shape
-        y = np.empty_like(x)
-        g = f32(gamma); b = f32(beta)
-        self.check(self.lib.sdb_test_groupnorm(self.h, ptr(x), ptr(g), ptr(b), n, c, H, W, 1 if silu else 0, ptr(y)))
-        return y
 
     def test_step_noise(self, noise_seed, t, count):
         """stochastic DDIM's noise z at timestep t: the first `count` values (numpy mirror: synth.step_noise)."""

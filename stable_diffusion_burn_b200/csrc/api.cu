@@ -632,90 +632,11 @@ int64_t sdb_launch_count(sdb_ctx* ctx) { return ctx ? ctx->c.launches : -1; }
 // ------------------------------------------------------------------------------ single-kernel test entries
 // (host pointers; each call stages through the context's work arena)
 
-int sdb_test_linear(sdb_ctx* ctx, const float* a, const float* w, const float* bias, int M, int K, int N, int passes,
-                    float* out, int32_t* trace) {
-  API_BEGIN(ctx)
-  c.work.reset();
-  TraceScope ts(c, trace);
-  float* d_a = upload(c, a, (size_t)M * K);
-  float* d_w = upload(c, w, (size_t)K * N);
-  float* d_b = upload(c, bias, N);
-  float* d_c = c.work.get<float>((size_t)M * N);
-  ActOp A;
-  A.p.hi = c.work.get<__half>((size_t)M * K);
-  A.p.lo = c.work.get<__half>((size_t)M * K);
-  A.W = M, A.C = K;
-  WeightOp Wp;
-  Wp.p.hi = c.work.get<__half>((size_t)N * K);
-  Wp.p.lo = c.work.get<__half>((size_t)N * K);
-  Wp.N = N, Wp.K = K;
-  convert_f16_launch(d_a, (long long)M * K, A.p, c.stream);
-  pack_linear_launch(d_w, K, N, Wp.p, 0, c.stream);
-  Epilogue ep;
-  ep.out_f32 = d_c;
-  ep.bias = d_b;
-  run_gemm(c, G_LINEAR, A, nullptr, Wp, passes, ep);
-  SDB_CUDA(cudaMemcpyAsync(out, d_c, sizeof(float) * M * N, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-  ts.write();
-  API_END
-}
-
 int sdb_test_gemm_ex(sdb_ctx* ctx, const float* a, const float* w, const float* bias, const float* residual, int M, int K, int N,
                      int passes, int flags, const float* xa, const float* xw, int XK, float* out, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  TraceScope ts(c, trace);
-  const bool geglu = flags & 1, from_f16 = flags & 4, planes = flags & 8;
-  SDB_CHECK(!planes || from_f16, "gemm_ex test: the separate fp16 planes (flag 8) need the fp16 outputs (flag 4)");
-  SDB_CHECK(!geglu || (N % 128 == 0 && !residual && !xa), "GEGLU test: N (= 2 * hidden) must be a multiple of 128, no residual / extra K");
-  const int Nout = geglu ? N / 2 : N;
-  float* d_a = upload(c, a, (size_t)M * K);
-  float* d_w = upload(c, w, (size_t)K * N);
-  float* d_b = upload(c, bias, N);
-  float* d_r = upload(c, residual, (size_t)M * N);
-  float* d_c = c.work.get<float>((size_t)M * Nout);
-  ActOp A;
-  A.p = Half2Ptr{c.work.get<__half>((size_t)M * K), c.work.get<__half>((size_t)M * K)};
-  A.W = M, A.C = K;
-  convert_f16_launch(d_a, (long long)M * K, A.p, c.stream);
-  WeightOp Wp;
-  Wp.p = Half2Ptr{c.work.get<__half>((size_t)N * K), c.work.get<__half>((size_t)N * K)};
-  Wp.N = N, Wp.K = K;
-  float* d_bp = d_b;
-  if (geglu) {
-    SDB_CHECK(bias, "GEGLU test needs a bias");
-    d_bp = c.work.get<float>(N);
-    pack_geglu_launch(d_w, d_b, K, N / 2, 64, Wp.p, d_bp, c.stream);
-  } else {
-    pack_linear_launch(d_w, K, N, Wp.p, 0, c.stream);
-  }
-  ExtraK xk;
-  if (xa) {
-    SDB_CHECK(xw && XK % 64 == 0, "extra-K test operands");
-    float* d_xa = upload(c, xa, (size_t)M * XK);
-    float* d_xw = upload(c, xw, (size_t)XK * N);
-    xk.x0.p = Half2Ptr{c.work.get<__half>((size_t)M * XK), c.work.get<__half>((size_t)M * XK)};
-    xk.x0.W = M, xk.x0.C = XK;
-    convert_f16_launch(d_xa, (long long)M * XK, xk.x0.p, c.stream);
-    xk.w.p = Half2Ptr{c.work.get<__half>((size_t)N * XK), c.work.get<__half>((size_t)N * XK)};
-    xk.w.N = N, xk.w.K = XK;
-    pack_linear_launch(d_xw, XK, N, xk.w.p, 0, c.stream);
-  }
-  Epilogue ep;
-  Half2Ptr o16;
-  if (geglu || from_f16) o16 = Half2Ptr{c.work.get<__half>((size_t)M * Nout), c.work.get<__half>((size_t)M * Nout)};
-  ep.out_f32 = geglu ? nullptr : d_c;
-  ep.out_f16 = o16;
-  ep.bias = d_bp, ep.residual = d_r, ep.geglu = geglu ? 1 : 0;
-  run_gemm(c, G_LINEAR, A, nullptr, Wp, passes, ep, xa ? &xk : nullptr);
-  if (geglu || from_f16) {
-    fetch_pair(c, o16, (size_t)M * Nout, out, planes);
-  } else {
-    SDB_CUDA(cudaMemcpyAsync(out, d_c, sizeof(float) * M * Nout, cudaMemcpyDeviceToHost, c.stream));
-    SDB_CUDA(cudaStreamSynchronize(c.stream));
-  }
-  ts.write();
+  model_test_gemm_ex(c, a, w, bias, residual, M, K, N, passes, flags, xa, xw, XK, out, trace);
   API_END
 }
 
@@ -723,59 +644,7 @@ int sdb_test_conv2d(sdb_ctx* ctx, const float* x, const float* w, const float* b
                     int cout, int ksize, int stride, int upsample, int passes, float* y, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  TraceScope ts(c, trace);
-  SDB_CHECK(ksize == 1 || ksize == 3, "ksize");
-  SDB_CHECK(stride == 1 || (stride == 2 && ksize == 3 && !upsample), "stride");
-  const int Hin = H, Win = W;
-  const int Ho = upsample ? 2 * H : (stride == 2 ? H / 2 : H), Wo = upsample ? 2 * W : (stride == 2 ? W / 2 : W);
-  const size_t xin = (size_t)n * cin * Hin * Win, yout = (size_t)n * cout * Ho * Wo;
-  float* d_x = upload(c, x, xin);
-  float* d_xh = c.work.get<float>(xin);
-  float* d_w = upload(c, w, (size_t)cout * cin * ksize * ksize);
-  float* d_b = upload(c, bias, cout);
-  float* d_yh = c.work.get<float>(yout);
-  float* d_y = c.work.get<float>(yout);
-  nchw_to_nhwc_launch(d_x, n, cin, Hin, Win, d_xh, c.stream);
-  ActOp A;
-  A.n = n, A.C = cin;
-  WeightOp Wp;
-  Wp.N = cout;
-  int kind, mode = 0;
-  if (ksize == 1) {
-    kind = G_CONV1, A.H = Hin, A.W = Win;
-    Wp.K = cin;
-  } else if (stride == 2) {
-    kind = G_CONV3_S2, mode = PREP_PHASE2, A.P = 4, A.H = Hin / 2, A.W = Win / 2;
-    Wp.K = 9 * cin;
-  } else if (upsample == 1) {
-    kind = G_CONV3_UP2, A.H = Hin, A.W = Win;
-    Wp.K = 4 * cin;
-  } else if (upsample == 2) {
-    kind = G_CONV3, mode = PREP_UP2, A.H = 2 * Hin, A.W = 2 * Win;
-    Wp.K = 9 * cin;
-  } else {
-    kind = G_CONV3, A.H = Hin, A.W = Win;
-    Wp.K = 9 * cin;
-  }
-  const size_t a_elems = (size_t)n * A.P * A.H * A.W * cin;
-  A.p.hi = c.work.get<__half>(a_elems);
-  A.p.lo = c.work.get<__half>(a_elems);
-  const size_t w_elems = (size_t)cout * Wp.K * (kind == G_CONV3_UP2 ? 4 : 1);
-  Wp.p.hi = c.work.get<__half>(w_elems);
-  Wp.p.lo = c.work.get<__half>(w_elems);
-  prep_operand_launch(d_xh, cin, nullptr, 0, n, Hin, Win, mode, nullptr, nullptr, nullptr, 0.f, A.p, c.stream);
-  if (kind == G_CONV3_UP2)
-    pack_conv_up2_launch(d_w, cout, cin, Wp.p, c.stream);
-  else
-    pack_conv_launch(d_w, cout, cin, ksize, Wp.p, c.stream);
-  Epilogue ep;
-  ep.out_f32 = d_yh;
-  ep.bias = d_b;
-  run_gemm(c, kind, A, nullptr, Wp, passes, ep);
-  nhwc_to_nchw_launch(d_yh, n, cout, Ho, Wo, d_y, c.stream);
-  SDB_CUDA(cudaMemcpyAsync(y, d_y, sizeof(float) * yout, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-  ts.write();
+  model_test_conv2d(c, x, w, bias, n, cin, H, W, cout, ksize, stride, upsample, passes, y, trace);
   API_END
 }
 
@@ -784,56 +653,7 @@ int sdb_test_ln_fold(sdb_ctx* ctx, const float* a, const float* a2, const float*
                      float* out, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  TraceScope ts(c, trace);
-  SDB_CHECK(C % 160 == 0 && K0 % 64 == 0 && (!geglu || (N % 128 == 0 && b1)), "ln_fold test shapes");
-  auto h2 = [&](size_t cnt) { return Half2Ptr{c.work.get<__half>(cnt), c.work.get<__half>(cnt)}; };
-  float *d_w0 = upload(c, w0, (size_t)K0 * C), *d_b0 = upload(c, b0, C), *d_g = upload(c, gamma, C), *d_be = upload(c, beta, C),
-        *d_w1 = upload(c, w1, (size_t)C * N), *d_b1 = upload(c, b1, N);
-  WeightOp W0;
-  W0.p = h2((size_t)C * K0), W0.N = C, W0.K = K0;
-  pack_linear_launch(d_w0, K0, C, W0.p, 0, c.stream);
-  // consumer weights with gamma folded in, u / v vectors (the same recipe as pack_st)
-  WeightOp W1;
-  W1.p = h2((size_t)N * C), W1.N = N, W1.K = C;
-  Half2Ptr scratch = h2((size_t)N * C);
-  float *u_hi = c.work.get<float>(N), *u_full = c.work.get<float>(N), *v = c.work.get<float>(N), *bp = c.work.get<float>(N);
-  if (geglu) {
-    pack_geglu_launch(d_w1, d_b1, C, N / 2, 64, W1.p, bp, c.stream, d_g);
-    pack_geglu_launch(d_w1, d_b1, C, N / 2, 64, scratch, nullptr, c.stream, d_be);
-  } else {
-    pack_linear_launch(d_w1, C, N, W1.p, 0, c.stream, 0, 0, d_g);
-    pack_linear_launch(d_w1, C, N, scratch, 0, c.stream, 0, 0, d_be);
-  }
-  rowsum_f16_launch(W1.p, N, C, u_hi, u_full, c.stream);
-  rowsum_f16_launch(scratch, N, C, nullptr, v, c.stream);
-  if (geglu) add_vec_launch(v, bp, N, v, c.stream);
-  else if (d_b1) add_vec_launch(v, d_b1, N, v, c.stream);
-  // producer(s): y = a w0 + b0 (+ a2 w0 + b0 accumulated in place onto the fp16 pair), leaving row statistics
-  Half2Ptr y16 = h2((size_t)M * C);
-  const int ls = ln_slots(C);
-  float* st = c.work.get<float>((size_t)M * ls * 2);
-  for (int pass = 0; pass < (a2 ? 2 : 1); ++pass) {
-    float* d_a = upload(c, pass ? a2 : a, (size_t)M * K0);
-    ActOp A;
-    A.p = h2((size_t)M * K0), A.W = M, A.C = K0;
-    convert_f16_launch(d_a, (long long)M * K0, A.p, c.stream);
-    Epilogue ep;
-    ep.out_f16 = y16, ep.bias = d_b0, ep.ln_out = st;
-    if (pass) ep.residual16 = y16;
-    run_gemm(c, G_LINEAR, A, nullptr, W0, 3, ep);
-  }
-  const int Nout = geglu ? N / 2 : N;
-  Half2Ptr o16 = h2((size_t)M * Nout);
-  {
-    ActOp Y;
-    Y.p = y16, Y.W = M, Y.C = C;
-    Epilogue ep;
-    ep.out_f16 = o16, ep.geglu = geglu ? 1 : 0;
-    ep.ln_in = st, ep.ln_in_slots = ls, ep.ln_C = C, ep.ln_eps = 1e-5f, ep.ln_u_hi = u_hi, ep.ln_u_full = u_full, ep.bias = v;
-    run_gemm(c, G_LINEAR, Y, nullptr, W1, passes, ep);
-  }
-  fetch_pair(c, o16, (size_t)M * Nout, out);
-  ts.write();
+  model_test_ln_fold(c, a, a2, w0, b0, gamma, beta, w1, b1, M, K0, C, N, passes, geglu, out, trace);
   API_END
 }
 
@@ -842,75 +662,8 @@ int sdb_test_conv_groupnorm(sdb_ctx* ctx, const float* x, const float* w, const 
                             float* y, int* used_epilogue_stats, int32_t* trace) {
   API_BEGIN(ctx)
   c.work.reset();
-  TraceScope ts(c, trace);
-  SDB_CHECK(ksize == 1 || ksize == 3, "ksize");
-  SDB_CHECK((stride == 1 && (upsample == 0 || (upsample == 1 && ksize == 3))) || (stride == 2 && ksize == 3 && !upsample),
-            "stride / upsample");
-  const int Ho = upsample ? 2 * H : (stride == 2 ? H / 2 : H), Wo = upsample ? 2 * W : (stride == 2 ? W / 2 : W);
-  const size_t xin = (size_t)n * cin * H * W, yout = (size_t)n * cout * Ho * Wo;
-  float* d_x = upload(c, x, xin);
-  float* d_w = upload(c, w, (size_t)cout * cin * ksize * ksize);
-  float* d_b = upload(c, bias, cout);
-  float* d_g = upload(c, gamma, cout);
-  float* d_be = upload(c, beta, cout);
-  float* d_xh = c.work.get<float>(xin);
-  float* d_conv = c.work.get<float>(yout);
-  nchw_to_nhwc_launch(d_x, n, cin, H, W, d_xh, c.stream);
-  // operand, packing and GEMM kind as the model's downsample (stride 2) and upsample convs use them (see sdb_test_conv2d)
-  ActOp A;
-  A.n = n, A.C = cin, A.H = H, A.W = W;
-  int kind = ksize == 1 ? G_CONV1 : G_CONV3, mode = 0;
-  if (stride == 2) kind = G_CONV3_S2, mode = PREP_PHASE2, A.P = 4, A.H = H / 2, A.W = W / 2;
-  if (upsample) kind = G_CONV3_UP2;
-  A.p = Half2Ptr{c.work.get<__half>(xin), c.work.get<__half>(xin)};
-  prep_operand_launch(d_xh, cin, nullptr, 0, n, H, W, mode, nullptr, nullptr, nullptr, 0.f, A.p, c.stream);
-  WeightOp Wp;
-  Wp.N = cout, Wp.K = (upsample ? 4 : ksize * ksize) * cin;
-  const size_t w_elems = (size_t)cout * Wp.K * (upsample ? 4 : 1);
-  Wp.p = Half2Ptr{c.work.get<__half>(w_elems), c.work.get<__half>(w_elems)};
-  if (upsample)
-    pack_conv_up2_launch(d_w, cout, cin, Wp.p, c.stream);
-  else
-    pack_conv_launch(d_w, cout, cin, ksize, Wp.p, c.stream);
-  GnPart gn;
-  gn.bucket = cout % 320 == 0 ? 10 : cout / 32;
-  gn.cap = std::max(3 * ((Ho * Wo + 127) / 128), 160);
-  gn.buf = c.work.get<float>((size_t)n * gn.cap * (cout / gn.bucket) * 2);
-  Epilogue ep;
-  ep.out_f32 = d_conv, ep.bias = d_b, ep.gn = &gn;
-  run_gemm(c, kind, A, nullptr, Wp, passes, ep);
-  if (used_epilogue_stats) *used_epilogue_stats = gn.slots;
-  SDB_CHECK(gn.slots > 0, "the GEMM did not produce GroupNorm statistics for this shape");
-  Half2Ptr o16{c.work.get<__half>(yout), c.work.get<__half>(yout)};
-  GnSrc s0, s1;
-  s0.x = d_conv, s0.C = cout, s0.part = gn.buf, s0.cap = gn.cap, s0.slots = gn.slots;
-  gn_apply_launch(s0, s1, gn.bucket, n, Ho, Wo, silu, d_g, d_be, 1e-5f, o16, c.stream);
-  fetch_half2(c, o16, n, cout, Ho, Wo, y);
-  ts.write();
-  API_END
-}
-
-int sdb_test_groupnorm(sdb_ctx* ctx, const float* x, const float* gamma, const float* beta, int n, int ch, int H, int W,
-                       int silu, float* y) {
-  API_BEGIN(ctx)
-  c.work.reset();
-  const size_t cnt = (size_t)n * ch * H * W;
-  float* d_x = upload(c, x, cnt);
-  float* d_xh = c.work.get<float>(cnt);
-  float* d_yh = c.work.get<float>(cnt);
-  float* d_y = c.work.get<float>(cnt);
-  float* d_g = upload(c, gamma, ch);
-  float* d_b = upload(c, beta, ch);
-  double* d_s = c.work.get<double>((size_t)n * 64);
-  unsigned int* d_t = c.work.get<unsigned int>(n);
-  float* d_p = c.work.get<float>(gn_stats_partial_floats(n, H * W));
-  SDB_CUDA(cudaMemsetAsync(d_t, 0, sizeof(unsigned int) * n, c.stream));
-  nchw_to_nhwc_launch(d_x, n, ch, H, W, d_xh, c.stream);
-  gn_stats_launch(d_xh, ch, nullptr, 0, n, H * W, d_s, d_p, d_t, c.stream);
-  gn_apply_f32_launch(d_xh, ch, n, H * W, silu, d_s, d_g, d_b, 1e-5f, d_yh, c.stream);
-  nhwc_to_nchw_launch(d_yh, n, ch, H, W, d_y, c.stream);
-  SDB_CUDA(cudaMemcpyAsync(y, d_y, sizeof(float) * cnt, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
+  model_test_conv_groupnorm(c, x, w, bias, gamma, beta, n, cin, H, W, cout, ksize, stride, upsample, passes, silu, y,
+                            used_epilogue_stats, trace);
   API_END
 }
 

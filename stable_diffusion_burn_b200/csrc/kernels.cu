@@ -1,5 +1,5 @@
 // kernels.cu — HBM-bound kernels around the tensor-core GEMMs: GroupNorm statistics, operand staging
-// (GroupNorm-apply + SiLU + fp16 hi/lo split, upsample / stride-2 phase layouts), LayerNorm, the
+// (GroupNorm-apply + SiLU + fp16 hi/lo split, stride-2 phase layout), LayerNorm, the
 // small CUDA-core convolutions (Cin = 4, Cout <= 4), sampler elementwise ops, weight packing.
 // All activations are NHWC; loads/stores are 8- or 16-byte vectors, coalesced along channels.
 #include "kernels.cuh"
@@ -30,15 +30,14 @@ __device__ __forceinline__ void split_store1(float f, __half* hi, __half* lo, si
 // ============================================================ GroupNorm statistics
 // Deterministic two-level reduction (no floating-point atomics): every CTA reduces its pixel chunk per group in a
 // fixed order and writes a partial; the last CTA of an image (ticket counter) folds the partials in chunk order.
-__global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__ x0, int C0,
-                                                       const float* __restrict__ x1, int C1, int HW, int pix_per_cta,
+__global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__ x, int C, int HW, int pix_per_cta,
                                                        double* __restrict__ sums, float* __restrict__ partials,
                                                        unsigned int* __restrict__ tickets) {
   pdl_enter();
   __shared__ float s_pair[2][1280];  // per channel-pair (sum, sumsq), C <= 2560
   __shared__ bool s_last;
   const int n = blockIdx.y;
-  const int C = C0 + C1, gs = C / 32;
+  const int gs = C / 32;
   const int p0 = blockIdx.x * pix_per_cta;
   const int p1 = min(HW, p0 + pix_per_cta);
   // thread -> (channel pair, pixel lane): narrow tensors (C/2 < 256) spread the spare threads over pixels
@@ -47,29 +46,20 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
   const int nslot = npair >= 256 ? npair : npair * pg;    // (pixel lane, pair) partials, <= 1280
   for (int slot = threadIdx.x; slot < nslot; slot += blockDim.x) {
     const int cp = slot % npair, pl = slot / npair;
-    const int c = cp * 2;
-    const float* ptr;
-    int stride;
-    if (c < C0) {
-      ptr = x0 + (size_t)n * HW * C0 + c;
-      stride = C0;
-    } else {
-      ptr = x1 + (size_t)n * HW * C1 + (c - C0);
-      stride = C1;
-    }
+    const float* ptr = x + (size_t)n * HW * C + cp * 2;
     float s = 0.f, q = 0.f;
     int p = p0 + pl;
     for (; p + 3 * pg < p1; p += 4 * pg) {
-      float2 v0 = *reinterpret_cast<const float2*>(ptr + (size_t)p * stride);
-      float2 v1 = *reinterpret_cast<const float2*>(ptr + (size_t)(p + pg) * stride);
-      float2 v2 = *reinterpret_cast<const float2*>(ptr + (size_t)(p + 2 * pg) * stride);
-      float2 v3 = *reinterpret_cast<const float2*>(ptr + (size_t)(p + 3 * pg) * stride);
+      float2 v0 = *reinterpret_cast<const float2*>(ptr + (size_t)p * C);
+      float2 v1 = *reinterpret_cast<const float2*>(ptr + (size_t)(p + pg) * C);
+      float2 v2 = *reinterpret_cast<const float2*>(ptr + (size_t)(p + 2 * pg) * C);
+      float2 v3 = *reinterpret_cast<const float2*>(ptr + (size_t)(p + 3 * pg) * C);
       s += (v0.x + v0.y) + (v1.x + v1.y) + (v2.x + v2.y) + (v3.x + v3.y);
       q += (v0.x * v0.x + v0.y * v0.y) + (v1.x * v1.x + v1.y * v1.y) + (v2.x * v2.x + v2.y * v2.y) +
            (v3.x * v3.x + v3.y * v3.y);
     }
     for (; p < p1; p += pg) {
-      float2 v = *reinterpret_cast<const float2*>(ptr + (size_t)p * stride);
+      float2 v = *reinterpret_cast<const float2*>(ptr + (size_t)p * C);
       s += v.x + v.y;
       q += v.x * v.x + v.y * v.y;
     }
@@ -104,13 +94,13 @@ size_t gn_stats_partial_floats(int n, int HW) {
   return (size_t)n * ceil_div(HW, pix) * 64;
 }
 
-void gn_stats_launch(const float* x0, int C0, const float* x1, int C1, int n, int HW, double* sums, float* partials,
-                     unsigned int* tickets, cudaStream_t st) {
-  SDB_CHECK((C0 + C1) % 64 == 0 && C0 % 2 == 0 && C0 + C1 <= 2560, "GroupNorm channels");
+void gn_stats_launch(const float* x, int C, int n, int HW, double* sums, float* partials, unsigned int* tickets,
+                     cudaStream_t st) {
+  SDB_CHECK(C % 64 == 0 && C <= 2560, "GroupNorm channels");
   int pix = (int)((((long long)HW * n) + 591) / 592);
   if (pix < 16) pix = 16;
   dim3 grid(ceil_div(HW, pix), n);
-  launch_k(gn_stats_kernel, grid, dim3(256), 0, st, x0, C0, x1, C1, HW, pix, sums, partials, tickets);
+  launch_k(gn_stats_kernel, grid, dim3(256), 0, st, x, C, HW, pix, sums, partials, tickets);
   SDB_CUDA(cudaGetLastError());
 }
 
@@ -130,21 +120,10 @@ __device__ __forceinline__ void gn_affine(const double* sums, int n, int c, int 
 // ============================================================ operand staging
 __global__ void __launch_bounds__(256)
 prep_operand_kernel(const float* __restrict__ x0, int C0, const float* __restrict__ x1, int C1, int H, int W,
-                    int pix_per_cta, int mode, const double* __restrict__ sums, const float* __restrict__ gamma,
-                    const float* __restrict__ beta, float eps, __half* __restrict__ out_hi,
-                    __half* __restrict__ out_lo) {
+                    int pix_per_cta, int phase2, __half* __restrict__ out_hi, __half* __restrict__ out_lo) {
   pdl_enter();
-  extern __shared__ float s_aff[];  // scale[C], shift[C]
   const int n = blockIdx.y;
   const int C = C0 + C1, HW = H * W;
-  float* s_scale = s_aff;
-  float* s_shift = s_aff + C;
-  if (mode & PREP_NORM) {
-    const int gs = C / 32;
-    const double inv_cnt = 1.0 / ((double)gs * HW);
-    for (int c = threadIdx.x; c < C; c += blockDim.x) gn_affine(sums, n, c, gs, inv_cnt, eps, gamma, beta, s_scale[c], s_shift[c]);
-    __syncthreads();
-  }
   const int p0 = blockIdx.x * pix_per_cta;
   const int p1 = min(HW, p0 + pix_per_cta);
   const int c8n = C / 8;
@@ -156,23 +135,8 @@ prep_operand_kernel(const float* __restrict__ x0, int C0, const float* __restric
     float4 a = *reinterpret_cast<const float4*>(src);
     float4 b = *reinterpret_cast<const float4*>(src + 4);
     float f[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    if (mode & PREP_NORM) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] = f[j] * s_scale[c + j] + s_shift[c + j];
-    }
-    if (mode & PREP_SILU) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] = silu_f(f[j]);
-    }
     const int h = p / W, w = p % W;
-    if (mode & PREP_UP2) {
-      const size_t base = (((size_t)n * 2 * H + 2 * h) * 2 * W + 2 * w) * C + c;
-      const size_t rowstride = (size_t)2 * W * C;
-      split_store8(f, out_hi + base, out_lo ? out_lo + base : nullptr);
-      split_store8(f, out_hi + base + C, out_lo ? out_lo + base + C : nullptr);
-      split_store8(f, out_hi + base + rowstride, out_lo ? out_lo + base + rowstride : nullptr);
-      split_store8(f, out_hi + base + rowstride + C, out_lo ? out_lo + base + rowstride + C : nullptr);
-    } else if (mode & PREP_PHASE2) {
+    if (phase2) {
       const int ph = (h & 1) * 2 + (w & 1);
       const size_t o = ((((size_t)n * 4 + ph) * (H / 2) + (h >> 1)) * (W / 2) + (w >> 1)) * C + c;
       split_store8(f, out_hi + o, out_lo ? out_lo + o : nullptr);
@@ -183,16 +147,14 @@ prep_operand_kernel(const float* __restrict__ x0, int C0, const float* __restric
   }
 }
 
-void prep_operand_launch(const float* x0, int C0, const float* x1, int C1, int n, int H, int W, int mode,
-                         const double* sums, const float* gamma, const float* beta, float eps, Half2Ptr out,
+void prep_operand_launch(const float* x0, int C0, const float* x1, int C1, int n, int H, int W, bool phase2, Half2Ptr out,
                          cudaStream_t st) {
   const int C = C0 + C1, HW = H * W;
   SDB_CHECK(C % 8 == 0 && C0 % 8 == 0, "operand channels must be multiples of 8");
   int pix = (int)((((long long)HW * n) + 1183) / 1184);
   if (pix < 8) pix = 8;
   dim3 grid(ceil_div(HW, pix), n);
-  const size_t smem = (mode & PREP_NORM) ? (size_t)2 * C * sizeof(float) : 0;
-  launch_k(prep_operand_kernel, grid, dim3(256), smem, st, x0, C0, x1, C1, H, W, pix, mode, sums, gamma, beta, eps, out.hi, out.lo);
+  launch_k(prep_operand_kernel, grid, dim3(256), 0, st, x0, C0, x1, C1, H, W, pix, phase2 ? 1 : 0, out.hi, out.lo);
   SDB_CUDA(cudaGetLastError());
 }
 
@@ -528,28 +490,6 @@ void gn_fused_launch(const float* x0, int C0, const float* x1, int C1, int n, in
   SDB_CHECK((long long)grid.x * grid.y <= 592, "fused GroupNorm grid must stay co-resident");
   launch_k(gn_fused_kernel, grid, dim3(256), (size_t)2 * C * sizeof(float), st, x0, C0, x1, C1, H, W, pix, silu, gamma, beta, eps, out.hi,
            out.lo, partials, tickets);
-  SDB_CUDA(cudaGetLastError());
-}
-
-__global__ void __launch_bounds__(256)
-gn_apply_f32_kernel(const float* __restrict__ x, int C, int HW, int silu, const double* __restrict__ sums,
-                    const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float* __restrict__ y) {
-  const int n = blockIdx.y;
-  const int gs = C / 32;
-  const double inv_cnt = 1.0 / ((double)gs * HW);
-  const size_t total = (size_t)HW * C;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = int(i % C);
-    float sc, sh;
-    gn_affine(sums, n, c, gs, inv_cnt, eps, gamma, beta, sc, sh);
-    float v = x[(size_t)n * total + i] * sc + sh;
-    y[(size_t)n * total + i] = silu ? silu_f(v) : v;
-  }
-}
-void gn_apply_f32_launch(const float* x, int C, int n, int HW, int silu, const double* sums, const float* gamma,
-                         const float* beta, float eps, float* y, cudaStream_t st) {
-  dim3 grid(ceil_div((long long)HW * C, 256 * 8), n);
-  gn_apply_f32_kernel<<<grid, 256, 0, st>>>(x, C, HW, silu, sums, gamma, beta, eps, y);
   SDB_CUDA(cudaGetLastError());
 }
 

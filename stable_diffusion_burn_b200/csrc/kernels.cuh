@@ -11,12 +11,11 @@ struct Half2Ptr {
   __half* lo = nullptr;
 };
 
-// ---- GroupNorm (reference src/model/groupnorm/mod.rs:53-82), NHWC fp32, optional 2-source concat
-// sums: [n][32][2] doubles (sum, sum of squares). Deterministic: per-CTA partials (scratch `partials`,
+// ---- GroupNorm (reference src/model/groupnorm/mod.rs:53-82), NHWC fp32
+// sums: [n][32][2] doubles (sum, sum of squares) of one tensor. Deterministic: per-CTA partials (scratch `partials`,
 // gn_stats_partial_floats(n,HW) floats) folded in fixed order by the last CTA; `tickets` [n] must be zero.
 size_t gn_stats_partial_floats(int n, int HW);
-void gn_stats_launch(const float* x0, int C0, const float* x1, int C1, int n, int HW, double* sums, float* partials,
-                     unsigned int* tickets, cudaStream_t st);
+void gn_stats_launch(const float* x, int C, int n, int HW, double* sums, float* partials, unsigned int* tickets, cudaStream_t st);
 // One-launch GroupNorm(+SiLU) -> fp16 hi(/lo) operand: statistics and apply fused through an in-kernel grid wait.
 // tickets: [n] zeroed counters; partials: gn_fused_partial_floats(n,HW) floats of scratch.
 size_t gn_fused_partial_floats(int n, int HW);
@@ -38,17 +37,10 @@ void gn_sums_from_partials_launch(const float* part, int cap, int slots, int nbk
                                   cudaStream_t st);
 void gn_apply_launch(const GnSrc& s0, const GnSrc& s1, int bucket, int n, int H, int W, int silu, const float* gamma,
                      const float* beta, float eps, Half2Ptr out, cudaStream_t st);
-// mode bits
-enum : int { PREP_NORM = 1, PREP_SILU = 2, PREP_UP2 = 4, PREP_PHASE2 = 8 };
-// Stages a conv/GEMM A operand: y = [silu]([groupnorm](cat(x0,x1))) -> fp16 hi(/lo).
-//   PREP_UP2    : nearest 2x upsample while writing (output [n][2H][2W][C])
-//   PREP_PHASE2 : split into 4 stride-2 phase planes (output [n][4][H/2][W/2][C])
-void prep_operand_launch(const float* x0, int C0, const float* x1, int C1, int n, int H, int W, int mode,
-                         const double* sums, const float* gamma, const float* beta, float eps, Half2Ptr out,
+// Stages a conv/GEMM A operand without normalisation: cat(x0, x1) -> fp16 hi(/lo), [n][H][W][C], or with phase2 split into the
+// four stride-2 phase planes [n][4][H/2][W/2][C] (the stride-2 conv input)
+void prep_operand_launch(const float* x0, int C0, const float* x1, int C1, int n, int H, int W, bool phase2, Half2Ptr out,
                          cudaStream_t st);
-// fp32 output variant of GroupNorm(+SiLU) used by the unit-test entry and by the small-N convs
-void gn_apply_f32_launch(const float* x, int C, int n, int HW, int silu, const double* sums, const float* gamma,
-                         const float* beta, float eps, float* y, cudaStream_t st);
 
 // ---- LayerNorm (burn nn::LayerNorm; call sites unet/mod.rs:523-525): rows x C fp32 -> fp16 hi(/lo) or fp32
 void layernorm_launch(const float* x, int rows, int C, const float* gamma, const float* beta, float eps,

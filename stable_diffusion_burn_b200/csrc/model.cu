@@ -52,24 +52,30 @@ static float* wsrc(Ctx& c, int idx) {
   return mptr(c, idx);
 }
 
-static void pack_conv(Ctx& c, ConvW& w, bool up2 = false) {
-  w.bias = mptr(c, w.bi);
-  if (w.cin % 64 != 0 || w.cout % 32 != 0) {  // CUDA-core convs
+// An OIHW conv weight `src` packed into `a` for the kernel that runs the conv: the implicit GEMM ([Cout][k*k*Cin], or with up2 the
+// nearest-2x upsample folded in, [4][Cout][4*Cin]) when Cin is a multiple of 64 and Cout of 32; otherwise a CUDA-core conv, which
+// reads fp32 [Cout][9][Cin] for a 3x3 conv with Cout <= 8 and the master weights for the rest
+static void pack_conv_weight(Ctx& c, ConvW& w, const float* src, Arena& a, bool up2) {
+  if (w.cin % 64 != 0 || w.cout % 32 != 0) {
     if (w.cout <= 8 && w.k == 3 && w.cin % 4 == 0) {
-      w.w_small = c.packed.get<float>((size_t)w.cout * 9 * w.cin);
-      pack_small_cout_launch(wsrc(c, w.wi), w.cout, w.cin, w.w_small, c.stream);
+      w.w_small = a.get<float>((size_t)w.cout * 9 * w.cin);
+      pack_small_cout_launch(src, w.cout, w.cin, w.w_small, c.stream);
     }
     return;
   }
   if (up2) {
-    w.packed.p = alloc_half2(c.packed, (size_t)16 * w.cout * w.cin);
+    w.packed.p = alloc_half2(a, (size_t)16 * w.cout * w.cin);
     w.packed.N = w.cout, w.packed.K = 4 * w.cin;
-    pack_conv_up2_launch(wsrc(c, w.wi), w.cout, w.cin, w.packed.p, c.stream);
+    pack_conv_up2_launch(src, w.cout, w.cin, w.packed.p, c.stream);
   } else {
-    w.packed.p = alloc_half2(c.packed, (size_t)w.cout * w.k * w.k * w.cin);
+    w.packed.p = alloc_half2(a, (size_t)w.cout * w.k * w.k * w.cin);
     w.packed.N = w.cout, w.packed.K = w.k * w.k * w.cin;
-    pack_conv_launch(wsrc(c, w.wi), w.cout, w.cin, w.k, w.packed.p, c.stream);
+    pack_conv_launch(src, w.cout, w.cin, w.k, w.packed.p, c.stream);
   }
+}
+static void pack_conv(Ctx& c, ConvW& w, bool up2 = false) {
+  w.bias = mptr(c, w.bi);
+  pack_conv_weight(c, w, wsrc(c, w.wi), c.packed, up2);
 }
 static void pack_lin(Ctx& c, LinW& w) {
   w.bias = mptr(c, w.bi);
@@ -102,43 +108,44 @@ static void pack_resblock(Ctx& c, ResBlockW& r, int passes) {
   }
   r.lin_embed.bias = mptr(c, r.lin_embed.bi);
 }
+// The LayerNorms of the TransformerBlock (unet/mod.rs:523-525) have no launch: gamma is folded into the weights of the GEMM that
+// consumes the normalised tensor (W' = diag(gamma) W), u = row sums of the packed W' (the exact fp16 values the tensor cores
+// multiply), v = beta^T W; the GEMM reads the raw tensor and applies rstd * (acc - mean * u) + v + bias. pack(dst, scale) packs the
+// consumer's [N][K] weights with input feature i multiplied by scale[i]: w.p with gamma, then `scratch` (N * K pairs at least) with
+// beta, whose hi + lo hold 22 bits of beta * W. u_hi, u_full and v ([N] each) come from arena `a`; the caller adds its bias to v.
+static void ln_fold(Ctx& c, Arena& a, Half2Ptr scratch, WeightOp& w, float*& u_hi, float*& u_full, float*& v,
+                    const std::function<void(Half2Ptr, const float*)>& pack, const NormW& ln) {
+  pack(w.p, ln.gamma);
+  u_hi = a.get<float>(w.N), u_full = a.get<float>(w.N), v = a.get<float>(w.N);
+  rowsum_f16_launch(w.p, w.N, w.K, u_hi, u_full, c.stream);
+  SDB_CUDA(cudaMemsetAsync(scratch.hi, 0, (size_t)w.N * w.K * 2, c.stream));  // head-pad rows stay zero
+  SDB_CUDA(cudaMemsetAsync(scratch.lo, 0, (size_t)w.N * w.K * 2, c.stream));
+  pack(scratch, ln.beta);
+  rowsum_f16_launch(scratch, w.N, w.K, nullptr, v, c.stream);
+}
 static void pack_st(Ctx& c, SpatialTransformerW& s, int passes) {
   s.passes = passes;
   pack_norm(c, s.norm), pack_norm(c, s.ln1), pack_norm(c, s.ln2), pack_norm(c, s.ln3);
   pack_conv(c, s.proj_in), pack_conv(c, s.proj_out);
   const int hd = s.heads * s.dpad;
-  // The three LayerNorms of the TransformerBlock (unet/mod.rs:523-525) have no launch: gamma is folded into the weights of the
-  // GEMM that consumes the normalised tensor (W' = diag(gamma) W), u = column sums of the packed W' (the exact fp16 values the
-  // tensor cores multiply), v = beta^T W (+ bias); the GEMM reads the raw tensor and applies rstd * (acc - mean * u) + v.
-  // The v vectors come from a scratch packing with beta in place of gamma (hi + lo = 22 bits of beta * W).
   Half2Ptr scratch = alloc_half2(c.work, (size_t)8 * s.c * s.c);
-  auto fold = [&](WeightOp& w, float*& u_hi, float*& u_full, float*& v, const std::function<void(Half2Ptr, const float*)>& pack,
-                  const NormW& ln) {
-    pack(w.p, ln.gamma);
-    u_hi = c.packed.get<float>(w.N), u_full = c.packed.get<float>(w.N), v = c.packed.get<float>(w.N);
-    rowsum_f16_launch(w.p, w.N, w.K, u_hi, u_full, c.stream);
-    SDB_CUDA(cudaMemsetAsync(scratch.hi, 0, (size_t)w.N * w.K * 2, c.stream));  // head-pad rows stay zero
-    SDB_CUDA(cudaMemsetAsync(scratch.lo, 0, (size_t)w.N * w.K * 2, c.stream));
-    pack(scratch, ln.beta);
-    rowsum_f16_launch(scratch, w.N, w.K, nullptr, v, c.stream);
-  };
   s.w_qkv1.p = alloc_half2(c.packed, (size_t)3 * hd * s.c), s.w_qkv1.N = 3 * hd, s.w_qkv1.K = s.c;
-  fold(s.w_qkv1, s.u_qkv_hi, s.u_qkv_full, s.v_qkv, [&](Half2Ptr dst, const float* sc) {
+  ln_fold(c, c.packed, scratch, s.w_qkv1, s.u_qkv_hi, s.u_qkv_full, s.v_qkv, [&](Half2Ptr dst, const float* sc) {
     pack_heads(c, s.attn1.query, s.heads, s.d, s.dpad, dst, 0, sc);
     pack_heads(c, s.attn1.key, s.heads, s.d, s.dpad, dst, hd, sc);
     pack_heads(c, s.attn1.value, s.heads, s.d, s.dpad, dst, 2 * hd, sc);
   }, s.ln1);
   pack_lin(c, s.attn1.out), s.w_o1 = s.attn1.out.packed;
   s.w_q2.p = alloc_half2(c.packed, (size_t)hd * s.c), s.w_q2.N = hd, s.w_q2.K = s.c;
-  fold(s.w_q2, s.u_q2_hi, s.u_q2_full, s.v_q2,
-       [&](Half2Ptr dst, const float* sc) { pack_heads(c, s.attn2.query, s.heads, s.d, s.dpad, dst, 0, sc); }, s.ln2);
+  ln_fold(c, c.packed, scratch, s.w_q2, s.u_q2_hi, s.u_q2_full, s.v_q2,
+          [&](Half2Ptr dst, const float* sc) { pack_heads(c, s.attn2.query, s.heads, s.d, s.dpad, dst, 0, sc); }, s.ln2);
   s.w_kv2.p = alloc_half2(c.packed, (size_t)2 * hd * 768), s.w_kv2.N = 2 * hd, s.w_kv2.K = 768;
   pack_heads(c, s.attn2.key, s.heads, s.d, s.dpad, s.w_kv2.p, 0);
   pack_heads(c, s.attn2.value, s.heads, s.d, s.dpad, s.w_kv2.p, hd);
   pack_lin(c, s.attn2.out), s.w_o2 = s.attn2.out.packed;
   s.w_geglu.p = alloc_half2(c.packed, (size_t)8 * s.c * s.c), s.w_geglu.N = 8 * s.c, s.w_geglu.K = s.c;
   s.geglu_bias = c.packed.get<float>((size_t)8 * s.c);
-  fold(s.w_geglu, s.u_geglu_hi, s.u_geglu_full, s.v_geglu, [&](Half2Ptr dst, const float* sc) {
+  ln_fold(c, c.packed, scratch, s.w_geglu, s.u_geglu_hi, s.u_geglu_full, s.v_geglu, [&](Half2Ptr dst, const float* sc) {
     pack_geglu_launch(wsrc(c, s.geglu.wi), mptr(c, s.geglu.bi), s.c, 4 * s.c, 64, dst, dst.hi == s.w_geglu.p.hi ? s.geglu_bias : nullptr,
                       c.stream, sc);
   }, s.ln3);
@@ -630,26 +637,31 @@ struct Fwd {
     gn_slot++;
     const int HW = x.H * x.W;
     if (x.gn.slots > 0) {
+      if (c.trace_on) c.trace.push_back({TRACE_GN, {x.gn.slots > 128 ? GN_PATH_SUMS_FOLD : GN_PATH_SUMS_PARTIALS}});
+      const GnSrc s = partials(x);
       const int nbk = x.C / x.gn.bucket;
-      const float* part = x.gn.buf;
-      int cap = x.gn.cap, slots = x.gn.slots;
-      if (c.trace_on) c.trace.push_back({TRACE_GN, {slots > 128 ? GN_PATH_SUMS_FOLD : GN_PATH_SUMS_PARTIALS}});
-      if (slots > 128) {
-        const int s2 = gn_fold_slots(slots);
-        float* folded = c.work.get<float>((size_t)nb * s2 * nbk * 2);
-        KernelScope ks(c, KC_GN_STATS, 0, (double)nb * slots * nbk * 8.0);
-        gn_fold_launch(part, cap, slots, nbk, nb, folded, c.stream);
-        part = folded, cap = s2, slots = s2;
-      }
-      KernelScope ks(c, KC_GN_STATS, 0, (double)nb * slots * nbk * 8.0);
-      gn_sums_from_partials_launch(part, cap, slots, nbk, x.C, x.gn.bucket, nb, sums, c.stream);
+      KernelScope ks(c, KC_GN_STATS, 0, (double)nb * s.slots * nbk * 8.0);
+      gn_sums_from_partials_launch(s.part, s.cap, s.slots, nbk, x.C, x.gn.bucket, nb, sums, c.stream);
       return sums;
     }
     if (c.trace_on) c.trace.push_back({TRACE_GN, {GN_PATH_SUMS_STATS}});
     float* part = c.work.get<float>(gn_stats_partial_floats(nb, HW));
     KernelScope ks(c, KC_GN_STATS, 0, (double)nb * HW * x.C * 4.0);
-    gn_stats_launch(x.p, x.C, nullptr, 0, nb, HW, sums, part, tk, c.stream);
+    gn_stats_launch(x.p, x.C, nb, HW, sums, part, tk, c.stream);
     return sums;
+  }
+  // x with its producer's partials, pre-folded 64:1 above 128 slots: keeps the fold each consumer CTA repeats short
+  GnSrc partials(const Act& x) {
+    GnSrc s;
+    s.x = x.p, s.C = x.C, s.part = x.gn.buf, s.cap = x.gn.cap, s.slots = x.gn.slots;
+    if (x.gn.slots > 128) {
+      const int nbk = x.C / x.gn.bucket, s2 = gn_fold_slots(x.gn.slots);
+      float* folded = c.work.get<float>((size_t)nb * s2 * nbk * 2);
+      KernelScope ks(c, KC_GN_STATS, 0, (double)nb * x.gn.slots * nbk * 8.0);
+      gn_fold_launch(x.gn.buf, x.gn.cap, x.gn.slots, nbk, nb, folded, c.stream);
+      s.part = folded, s.cap = s2, s.slots = s2;
+    }
+    return s;
   }
   Act act16(int H, int W, int C) {
     Act a = act(H, W, C);
@@ -686,19 +698,7 @@ struct Fwd {
     a.p = half2((size_t)nb * x0.H * x0.W * C, lo);
     const int HW = x0.H * x0.W;
     if (x0.gn.slots > 0 && (!x1 || (x1->gn.slots > 0 && x1->gn.bucket == x0.gn.bucket)) && (C / 32) % x0.gn.bucket == 0) {
-      GnSrc s0, s1;
-      auto src = [&](const Act& x, GnSrc& s) {
-        s.x = x.p, s.C = x.C, s.part = x.gn.buf, s.cap = x.gn.cap, s.slots = x.gn.slots;
-        if (x.gn.slots > 128) {  // large image: shorten the per-CTA fold with a first pass over groups of 64 slots
-          const int nbk = x.C / x.gn.bucket, s2 = gn_fold_slots(x.gn.slots);
-          float* folded = c.work.get<float>((size_t)nb * s2 * nbk * 2);
-          KernelScope ks(c, KC_GN_STATS, 0, (double)nb * x.gn.slots * nbk * 8.0);
-          gn_fold_launch(x.gn.buf, x.gn.cap, x.gn.slots, nbk, nb, folded, c.stream);
-          s.part = folded, s.cap = s2, s.slots = s2;
-        }
-      };
-      src(x0, s0);
-      if (x1) src(*x1, s1);
+      const GnSrc s0 = partials(x0), s1 = x1 ? partials(*x1) : GnSrc{};
       if (c.trace_on)
         c.trace.push_back({TRACE_GN, {x0.gn.slots > 128 || (x1 && x1->gn.slots > 128) ? GN_PATH_APPLY_FOLD : GN_PATH_APPLY}});
       KernelScope ks(c, KC_PREP, 0, (double)nb * HW * C * (4.0 + 2.0 + (lo ? 2.0 : 0.0)));
@@ -715,19 +715,18 @@ struct Fwd {
                     a.p, part, tk, c.stream);
     return a;
   }
-  // raw (un-normalised) fp16 staging; mode 0, PREP_PHASE2 (stride-2 conv input)
-  ActOp raw_operand(const Act& x0, const Act* x1, int mode, bool lo) {
+  // raw (un-normalised) fp16 staging; phase2: the four stride-2 phase planes a stride-2 conv reads
+  ActOp raw_operand(const Act& x0, const Act* x1, bool phase2, bool lo) {
     const int C = x0.C + (x1 ? x1->C : 0);
     ActOp a;
     a.n = nb, a.C = C;
-    if (mode & PREP_PHASE2)
+    if (phase2)
       a.P = 4, a.H = x0.H / 2, a.W = x0.W / 2;
     else
       a.H = x0.H, a.W = x0.W;
     a.p = half2((size_t)nb * x0.H * x0.W * C, lo);
     KernelScope ks(c, KC_PREP, 0, (double)x0.n * x0.H * x0.W * C * (4.0 + 2.0 + (lo ? 2.0 : 0.0)));
-    prep_operand_launch(x0.p, x0.C, x1 ? x1->p : nullptr, x1 ? x1->C : 0, nb, x0.H, x0.W, mode, nullptr, nullptr, nullptr,
-                        0.f, a.p, c.stream);
+    prep_operand_launch(x0.p, x0.C, x1 ? x1->p : nullptr, x1 ? x1->C : 0, nb, x0.H, x0.W, phase2, a.p, c.stream);
     return a;
   }
   ActOp rows_operand(Half2Ptr p, long long rows, int C) {
@@ -751,7 +750,7 @@ static void run_resblock(Fwd& f, const NormW& n1, const ConvW& c1, const NormW& 
       raw = f.raw16_operand(x0);
       if (x1) raw1 = f.raw16_operand(*x1);
     } else {
-      raw = f.raw_operand(x0, x1, 0, lo);
+      raw = f.raw_operand(x0, x1, false, lo);
     }
   }
   Act h = f.act(x0.H, x0.W, c1.cout);
@@ -1048,7 +1047,7 @@ static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
         o = f.act16(H / 2, W / 2, b.cout);
         const size_t mk = c.work.off;
         const bool lo = b.conv.passes >= 2 || c.opt_precision >= 2;
-        ActOp a = f.raw_operand(x0, nullptr, PREP_PHASE2, lo);
+        ActOp a = f.raw_operand(x0, nullptr, true, lo);
         Epilogue ep;
         ep.out_f32 = o.p, ep.out_f16 = o.raw16, ep.bias = b.conv.bias, ep.gn = &o.gn;
         run_gemm(c, G_CONV3_S2, a, nullptr, b.conv.packed, b.conv.passes, ep);
@@ -1081,7 +1080,7 @@ static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
         }
         // unet/mod.rs:390-398: nearest 2x + conv3x3, folded into four 2x2-tap phase convolutions
         const bool lo = b.conv.passes >= 2 || c.opt_precision >= 2;
-        ActOp a = u.raw16.hi ? f.raw16_operand(u) : f.raw_operand(u, nullptr, 0, lo);
+        ActOp a = u.raw16.hi ? f.raw16_operand(u) : f.raw_operand(u, nullptr, false, lo);
         Epilogue ep;
         ep.out_f32 = o.p, ep.out_f16 = o.raw16, ep.bias = b.conv.bias, ep.gn = &o.gn;
         run_gemm(c, G_CONV3_UP2, a, nullptr, b.conv.packed, b.conv.passes, ep);
@@ -1236,7 +1235,7 @@ static void vae_decode(Fwd& f, const float* d_latent, int H, int W, float pre_sc
       Act o = f.act16(2 * H, 2 * W, db.up.cout);  // read raw by the next block's nin_shortcut
       const size_t mk = c.work.off;
       const bool lo = db.up.passes >= 2 || c.opt_precision >= 2;
-      ActOp a = x.raw16.hi ? f.raw16_operand(x) : f.raw_operand(x, nullptr, 0, lo);
+      ActOp a = x.raw16.hi ? f.raw16_operand(x) : f.raw_operand(x, nullptr, false, lo);
       Epilogue ep;
       ep.out_f32 = o.p, ep.out_f16 = o.raw16, ep.bias = db.up.bias, ep.gn = &o.gn;
       run_gemm(c, G_CONV3_UP2, a, nullptr, db.up.packed, db.up.passes, ep);
@@ -1268,7 +1267,7 @@ static void vae_enc_down(Fwd& f, const ConvW& down, const Act& x, Act& o) {
   Ctx& c = f.c;
   SDB_CHECK(x.H % 2 == 0 && x.W % 2 == 0, "encode_image: image height and width must be multiples of 8");
   const size_t mk = c.work.off;
-  ActOp a = f.raw_operand(x, nullptr, PREP_PHASE2, true);
+  ActOp a = f.raw_operand(x, nullptr, true, true);
   Epilogue ep;
   ep.out_f32 = o.p, ep.bias = down.bias, ep.gn = &o.gn;
   run_gemm(c, G_CONV3_S2_PAD01, a, nullptr, down.packed, down.passes, ep);
@@ -2181,6 +2180,14 @@ void fetch_half2(Ctx& c, Half2Ptr p, int n, int C, int H, int W, float* out) {
       for (int ch = 0; ch < C; ++ch) out[((size_t)s * C + ch) * hw + i] = v[((size_t)s * hw + i) * C + ch];
 }
 
+// NCHW host output of an NHWC fp32 activation
+static void fetch_act(Ctx& c, const Act& a, float* out) {
+  float* d = c.work.get<float>(a.count());
+  nhwc_to_nchw_launch(a.p, a.n, a.C, a.H, a.W, d, c.stream);
+  SDB_CUDA(cudaMemcpyAsync(out, d, a.count() * 4, cudaMemcpyDeviceToHost, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));
+}
+
 // ================================================================================ attention unit-test entry
 // V transposed (flags & 2): stages q / k / V^T exactly as model_clip_forward_dev does
 static void test_attention_vt(Ctx& c, const float* q, const float* k, const float* v, int n, int L, int C, int heads,
@@ -2271,18 +2278,175 @@ void model_test_attention(Ctx& c, const float* q, const float* k, const float* v
   fetch_pair(c, o16, (size_t)n * Nq * C, out);
 }
 
-// ================================================================================ ResBlock / GroupNorm unit-test entries
-static ConvW test_conv_weights(Ctx& c, Fwd& f, const float* w, const float* b, int cin, int cout, int k) {
+// ================================================================================ GEMM, conv and LayerNorm-fold test entries
+void model_test_gemm_ex(Ctx& c, const float* a, const float* w, const float* bias, const float* residual, int M, int K, int N,
+                        int passes, int flags, const float* xa, const float* xw, int XK, float* out, int32_t* trace) {
+  TraceScope ts(c, trace);
+  const bool geglu = flags & 1, from_f16 = flags & 4, planes = flags & 8;
+  SDB_CHECK(!planes || from_f16, "gemm_ex test: the separate fp16 planes (flag 8) need the fp16 outputs (flag 4)");
+  SDB_CHECK(!geglu || (N % 128 == 0 && !residual && !xa), "GEGLU test: N (= 2 * hidden) must be a multiple of 128, no residual / extra K");
+  const int Nout = geglu ? N / 2 : N;
+  float* d_a = upload(c, a, (size_t)M * K);
+  float* d_w = upload(c, w, (size_t)K * N);
+  float* d_b = upload(c, bias, N);
+  float* d_r = upload(c, residual, (size_t)M * N);
+  float* d_c = c.work.get<float>((size_t)M * Nout);
+  ActOp A;
+  A.p = alloc_half2(c.work, (size_t)M * K);
+  A.W = M, A.C = K;
+  convert_f16_launch(d_a, (long long)M * K, A.p, c.stream);
+  WeightOp Wp;
+  Wp.p = alloc_half2(c.work, (size_t)N * K);
+  Wp.N = N, Wp.K = K;
+  float* d_bp = d_b;
+  if (geglu) {
+    SDB_CHECK(bias, "GEGLU test needs a bias");
+    d_bp = c.work.get<float>(N);
+    pack_geglu_launch(d_w, d_b, K, N / 2, 64, Wp.p, d_bp, c.stream);
+  } else {
+    pack_linear_launch(d_w, K, N, Wp.p, 0, c.stream);
+  }
+  ExtraK xk;
+  if (xa) {
+    SDB_CHECK(xw && XK % 64 == 0, "extra-K test operands");
+    float* d_xa = upload(c, xa, (size_t)M * XK);
+    float* d_xw = upload(c, xw, (size_t)XK * N);
+    xk.x0.p = alloc_half2(c.work, (size_t)M * XK);
+    xk.x0.W = M, xk.x0.C = XK;
+    convert_f16_launch(d_xa, (long long)M * XK, xk.x0.p, c.stream);
+    xk.w.p = alloc_half2(c.work, (size_t)N * XK);
+    xk.w.N = N, xk.w.K = XK;
+    pack_linear_launch(d_xw, XK, N, xk.w.p, 0, c.stream);
+  }
+  Epilogue ep;
+  Half2Ptr o16;
+  if (geglu || from_f16) o16 = alloc_half2(c.work, (size_t)M * Nout);
+  ep.out_f32 = geglu ? nullptr : d_c;
+  ep.out_f16 = o16;
+  ep.bias = d_bp, ep.residual = d_r, ep.geglu = geglu ? 1 : 0;
+  run_gemm(c, G_LINEAR, A, nullptr, Wp, passes, ep, xa ? &xk : nullptr);
+  if (geglu || from_f16) {
+    fetch_pair(c, o16, (size_t)M * Nout, out, planes);
+  } else {
+    SDB_CUDA(cudaMemcpyAsync(out, d_c, sizeof(float) * M * Nout, cudaMemcpyDeviceToHost, c.stream));
+    SDB_CUDA(cudaStreamSynchronize(c.stream));
+  }
+  ts.write();
+}
+
+// A test conv's OIHW weights (device) packed into the work arena by the model's packer; only the implicit-GEMM layouts
+static ConvW test_conv_weights(Ctx& c, const float* w, float* b, int cin, int cout, int k, bool up2 = false) {
   SDB_CHECK(cin % 64 == 0 && cout % 32 == 0, "test conv: channels must be multiples of 64 (in) and 32 (out)");
   ConvW cw;
   cw.cin = cin, cw.cout = cout, cw.k = k;
-  cw.packed.p = f.half2((size_t)cout * k * k * cin, true);
-  cw.packed.N = cout, cw.packed.K = k * k * cin;
-  pack_conv_launch(upload(c, w, (size_t)cout * cin * k * k), cout, cin, k, cw.packed.p, c.stream);
-  cw.bias = upload(c, b, cout);
+  pack_conv_weight(c, cw, w, c.work, up2);
+  cw.bias = b;
   return cw;
 }
 
+// A conv on a host NCHW tensor the way the model runs its GEMM convs: the input staged by Fwd::raw_operand, the weights by
+// pack_conv_weight, the output an activation from Fwd::act. 1x1 (G_CONV1), 3x3 pad 1 (G_CONV3), 3x3 stride 2 on the four phase
+// planes (G_CONV3_S2, the UNet downsample), 3x3 after a nearest-2x upsample folded into the weights (G_CONV3_UP2). gn: the epilogue
+// also writes the output's GroupNorm partials into the buffer Fwd::act gave it (none with the gn_epilogue option off)
+static Act test_conv(Fwd& f, const float* x, const float* w, const float* bias, int cin, int H, int W, int cout, int k, int stride,
+                     int upsample, int passes, bool gn) {
+  Ctx& c = f.c;
+  SDB_CHECK(k == 1 || k == 3, "ksize");
+  SDB_CHECK((stride == 1 && (upsample == 0 || (upsample == 1 && k == 3))) || (stride == 2 && k == 3 && !upsample),
+            "stride / upsample");
+  Act xh;
+  xh.n = f.nb, xh.H = H, xh.W = W, xh.C = cin;
+  xh.p = c.work.get<float>(xh.count());
+  nchw_to_nhwc_launch(upload(c, x, xh.count()), f.nb, cin, H, W, xh.p, c.stream);
+  const ActOp a = f.raw_operand(xh, nullptr, stride == 2, true);
+  const ConvW cw = test_conv_weights(c, upload(c, w, (size_t)cout * cin * k * k), upload(c, bias, cout), cin, cout, k, upsample);
+  const int kind = k == 1 ? G_CONV1 : stride == 2 ? G_CONV3_S2 : upsample ? G_CONV3_UP2 : G_CONV3;
+  Act o = f.act(upsample ? 2 * H : H / stride, upsample ? 2 * W : W / stride, cout);
+  Epilogue ep;
+  ep.out_f32 = o.p, ep.bias = cw.bias;
+  if (gn) ep.gn = &o.gn;
+  run_gemm(c, kind, a, nullptr, cw.packed, passes, ep);
+  return o;
+}
+
+void model_test_conv2d(Ctx& c, const float* x, const float* w, const float* bias, int n, int cin, int H, int W, int cout, int k,
+                       int stride, int upsample, int passes, float* y, int32_t* trace) {
+  Fwd f(c, n);
+  TraceScope ts(c, trace);
+  fetch_act(c, test_conv(f, x, w, bias, cin, H, W, cout, k, stride, upsample, passes, false), y);
+  ts.write();
+}
+
+void model_test_conv_groupnorm(Ctx& c, const float* x, const float* w, const float* bias, const float* gamma, const float* beta,
+                               int n, int cin, int H, int W, int cout, int k, int stride, int upsample, int passes, int silu,
+                               float* y, int* slots, int32_t* trace) {
+  Fwd f(c, n);
+  TraceScope ts(c, trace);
+  const Act o = test_conv(f, x, w, bias, cin, H, W, cout, k, stride, upsample, passes, true);
+  if (slots) *slots = o.gn.slots;
+  SDB_CHECK(o.gn.slots > 0, "the GEMM did not produce GroupNorm statistics for this shape");
+  Half2Ptr o16 = alloc_half2(c.work, o.count());
+  GnSrc s0, s1;
+  s0.x = o.p, s0.C = cout, s0.part = o.gn.buf, s0.cap = o.gn.cap, s0.slots = o.gn.slots;
+  gn_apply_launch(s0, s1, o.gn.bucket, n, o.H, o.W, silu, upload(c, gamma, cout), upload(c, beta, cout), 1e-5f, o16, c.stream);
+  fetch_half2(c, o16, n, cout, o.H, o.W, y);
+  ts.write();
+}
+
+void model_test_ln_fold(Ctx& c, const float* a, const float* a2, const float* w0, const float* b0, const float* gamma,
+                        const float* beta, const float* w1, const float* b1, int M, int K0, int C, int N, int passes, int geglu,
+                        float* out, int32_t* trace) {
+  TraceScope ts(c, trace);
+  SDB_CHECK(C % 160 == 0 && K0 % 64 == 0 && (!geglu || (N % 128 == 0 && b1)), "ln_fold test shapes");
+  float *d_w0 = upload(c, w0, (size_t)K0 * C), *d_b0 = upload(c, b0, C), *d_w1 = upload(c, w1, (size_t)C * N),
+        *d_b1 = upload(c, b1, N);
+  NormW ln;
+  ln.c = C, ln.gamma = upload(c, gamma, C), ln.beta = upload(c, beta, C);
+  WeightOp W0;
+  W0.p = alloc_half2(c.work, (size_t)C * K0), W0.N = C, W0.K = K0;
+  pack_linear_launch(d_w0, K0, C, W0.p, 0, c.stream);
+  // the consumer's weights with the LayerNorm folded in, as pack_st folds it
+  WeightOp W1;
+  W1.p = alloc_half2(c.work, (size_t)N * C), W1.N = N, W1.K = C;
+  float* bp = geglu ? c.work.get<float>(N) : nullptr;
+  float *u_hi, *u_full, *v;
+  ln_fold(c, c.work, alloc_half2(c.work, (size_t)N * C), W1, u_hi, u_full, v, [&](Half2Ptr dst, const float* sc) {
+    if (geglu)
+      pack_geglu_launch(d_w1, d_b1, C, N / 2, 64, dst, dst.hi == W1.p.hi ? bp : nullptr, c.stream, sc);
+    else
+      pack_linear_launch(d_w1, C, N, dst, 0, c.stream, 0, 0, sc);
+  }, ln);
+  if (geglu) add_vec_launch(v, bp, N, v, c.stream);
+  else if (d_b1) add_vec_launch(v, d_b1, N, v, c.stream);
+  // producer(s): y = a w0 + b0 (+ a2 w0 + b0 accumulated in place onto the fp16 pair), leaving row statistics
+  Half2Ptr y16 = alloc_half2(c.work, (size_t)M * C);
+  const int ls = ln_slots(C);
+  float* st = c.work.get<float>((size_t)M * ls * 2);
+  for (int pass = 0; pass < (a2 ? 2 : 1); ++pass) {
+    float* d_a = upload(c, pass ? a2 : a, (size_t)M * K0);
+    ActOp A;
+    A.p = alloc_half2(c.work, (size_t)M * K0), A.W = M, A.C = K0;
+    convert_f16_launch(d_a, (long long)M * K0, A.p, c.stream);
+    Epilogue ep;
+    ep.out_f16 = y16, ep.bias = d_b0, ep.ln_out = st;
+    if (pass) ep.residual16 = y16;
+    run_gemm(c, G_LINEAR, A, nullptr, W0, 3, ep);
+  }
+  const int Nout = geglu ? N / 2 : N;
+  Half2Ptr o16 = alloc_half2(c.work, (size_t)M * Nout);
+  {
+    ActOp Y;
+    Y.p = y16, Y.W = M, Y.C = C;
+    Epilogue ep;
+    ep.out_f16 = o16, ep.geglu = geglu ? 1 : 0;
+    ep.ln_in = st, ep.ln_in_slots = ls, ep.ln_C = C, ep.ln_eps = 1e-5f, ep.ln_u_hi = u_hi, ep.ln_u_full = u_full, ep.bias = v;
+    run_gemm(c, G_LINEAR, Y, nullptr, W1, passes, ep);
+  }
+  fetch_pair(c, o16, (size_t)M * Nout, out);
+  ts.write();
+}
+
+// ================================================================================ ResBlock / GroupNorm unit-test entries
 // An NCHW host tensor staged as a model activation. stats = true: written by a 3-pass identity 3x3 conv with the epilogue a
 // ResBlock output gets (fp32, fp16 hi/lo copy, GroupNorm partials); the 3-pass product returns hi + lo of the input (22 bits,
 // exact in fp32). stats = false: the fp32 tensor and its fp16 copy without statistics, as the UNet's conv_in leaves it.
@@ -2306,16 +2470,14 @@ static Act stage_activation(Fwd& f, const float* h, int C, int H, int W, bool st
   SDB_CUDA(cudaMemsetAsync(id, 0, (size_t)C * C * 9 * 4, c.stream));
   const std::vector<float> ones(C, 1.f);
   SDB_CUDA(cudaMemcpy2DAsync(id + 4, (size_t)(C + 1) * 9 * 4, ones.data(), 4, 4, C, cudaMemcpyHostToDevice, c.stream));
-  WeightOp wid;
-  wid.p = f.half2((size_t)C * C * 9, true), wid.N = C, wid.K = 9 * C;
-  pack_conv_launch(id, C, C, 3, wid.p, c.stream);
+  const ConvW wid = test_conv_weights(c, id, nullptr, C, C, 3);
   Epilogue ep;
   ep.out_f32 = a.p, ep.out_f16 = a.raw16, ep.gn = &a.gn;
   // 3 passes whatever the precision option forces on the block under test: the staging must hand on hi + lo of the input
   const int prec = c.opt_precision;
   c.opt_precision = 0;
   try {
-    run_gemm(c, G_CONV3, A, nullptr, wid, 3, ep);
+    run_gemm(c, G_CONV3, A, nullptr, wid.packed, 3, ep);
   } catch (...) {
     c.opt_precision = prec;
     throw;
@@ -2338,11 +2500,12 @@ void model_test_resblock(Ctx& c, const float* x0, const float* x1, int n, int C0
   NormW nw1, nw2;
   nw1.c = Cin, nw1.gamma = upload(c, n1g, Cin), nw1.beta = upload(c, n1b, Cin);
   nw2.c = Cout, nw2.gamma = upload(c, n2g, Cout), nw2.beta = upload(c, n2b, Cout);
-  const ConvW cw1 = test_conv_weights(c, f, w1, b1, Cin, Cout, 3), cw2 = test_conv_weights(c, f, w2, b2, Cout, Cout, 3);
+  const ConvW cw1 = test_conv_weights(c, upload(c, w1, (size_t)Cout * Cin * 9), upload(c, b1, Cout), Cin, Cout, 3);
+  const ConvW cw2 = test_conv_weights(c, upload(c, w2, (size_t)Cout * Cout * 9), upload(c, b2, Cout), Cout, Cout, 3);
   ConvW sk;
   float* bias_merged = nullptr;
   if (wsk) {  // packed as pack_resblock / pack_resnet do
-    sk = test_conv_weights(c, f, wsk, bsk, Cin, Cout, 1);
+    sk = test_conv_weights(c, upload(c, wsk, (size_t)Cout * Cin), upload(c, bsk, Cout), Cin, Cout, 1);
     bias_merged = c.work.get<float>(Cout);
     add_vec_launch(cw2.bias, sk.bias, Cout, bias_merged, c.stream);
   }
@@ -2368,27 +2531,17 @@ void model_test_resblock(Ctx& c, const float* x0, const float* x1, int n, int C0
 void model_test_groupnorm_cat(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, const float* gamma,
                               const float* beta, int silu, int mode, float* y, int32_t* trace) {
   SDB_CHECK(n >= 1 && H >= 1 && W >= 1 && C0 > 0 && C1 >= 0 && (C1 > 0) == (x1 != nullptr), "test_groupnorm_cat: shapes");
-  SDB_CHECK(mode >= 0 && mode <= 2, "test_groupnorm_cat: mode is 0 (statistics kernel + apply), 1 (fused), 2 (producer partials)");
+  SDB_CHECK(mode == 1 || mode == 2, "test_groupnorm_cat: mode is 1 (fused statistics + apply) or 2 (apply from producer partials)");
   const int C = C0 + C1;
   Fwd f(c, n);
-  f.init_sums(2);
+  f.init_sums(1);
   NormW nw;
   nw.c = C, nw.gamma = upload(c, gamma, C), nw.beta = upload(c, beta, C);
   const Act a0 = stage_activation(f, x0, C0, H, W, mode == 2);
   Act a1;
   if (x1) a1 = stage_activation(f, x1, C1, H, W, mode == 2);
   TraceScope ts(c, trace);
-  ActOp g;
-  if (mode == 0) {
-    double* sums = c.work.get<double>((size_t)n * 64);
-    float* part = c.work.get<float>(gn_stats_partial_floats(n, H * W));
-    gn_stats_launch(a0.p, C0, x1 ? a1.p : nullptr, C1, n, H * W, sums, part, f.gn_tickets, c.stream);
-    g.p = f.half2((size_t)n * H * W * C, true);
-    prep_operand_launch(a0.p, C0, x1 ? a1.p : nullptr, C1, n, H, W, PREP_NORM | (silu ? PREP_SILU : 0), sums, nw.gamma, nw.beta,
-                        nw.eps, g.p, c.stream);
-  } else {
-    g = f.gn_operand(a0, x1 ? &a1 : nullptr, nw, silu != 0, true);
-  }
+  const ActOp g = f.gn_operand(a0, x1 ? &a1 : nullptr, nw, silu != 0, true);
   ts.write();
   fetch_half2(c, g.p, n, C, H, W, y);
 }
@@ -2450,13 +2603,6 @@ void model_test_spatial_transformer(Ctx& c, int index, const float* x, int n, in
 }
 
 // ================================================================================ autoencoder stage test entry
-// NCHW host output of an NHWC fp32 activation
-static void fetch_act(Ctx& c, const Act& a, float* out) {
-  float* d = c.work.get<float>(a.count());
-  nhwc_to_nchw_launch(a.p, a.n, a.C, a.H, a.W, d, c.stream);
-  SDB_CUDA(cudaMemcpyAsync(out, d, a.count() * 4, cudaMemcpyDeviceToHost, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));
-}
 
 void model_test_vae_stage(Ctx& c, int stage, const float* x, const float* cond, int n, int Cx, int H, int W, float scale, int flags,
                           float* out, float* out16, float* tap, float* out_norm, int32_t* trace) {

@@ -97,6 +97,16 @@ void fetch_pair(Ctx& c, Half2Ptr p, size_t count, float* out, bool planes = fals
 // fetch_pair of an NHWC [n][H][W][C] tensor, written NCHW
 void fetch_half2(Ctx& c, Half2Ptr p, int n, int C, int H, int W, float* out);
 
+void model_test_gemm_ex(Ctx& c, const float* a, const float* w, const float* bias, const float* residual, int M, int K, int N,
+                        int passes, int flags, const float* xa, const float* xw, int XK, float* out, int32_t* trace);
+void model_test_conv2d(Ctx& c, const float* x, const float* w, const float* bias, int n, int cin, int H, int W, int cout, int k,
+                       int stride, int upsample, int passes, float* y, int32_t* trace);
+void model_test_conv_groupnorm(Ctx& c, const float* x, const float* w, const float* bias, const float* gamma, const float* beta,
+                               int n, int cin, int H, int W, int cout, int k, int stride, int upsample, int passes, int silu,
+                               float* y, int* slots, int32_t* trace);
+void model_test_ln_fold(Ctx& c, const float* a, const float* a2, const float* w0, const float* b0, const float* gamma,
+                        const float* beta, const float* w1, const float* b1, int M, int K0, int C, int N, int passes, int geglu,
+                        float* out, int32_t* trace);
 void model_test_attention(Ctx& c, const float* q, const float* k, const float* v, int n, int Nq, int Nk, int C, int heads,
                           const int32_t* kvlen, int flags, float* out);
 void model_test_resblock(Ctx& c, const float* x0, const float* x1, int n, int C0, int C1, int H, int W, int Cout,

@@ -54,7 +54,6 @@ CONV_CASES = [
     (1, 128, 64, 64, 64, 3, 2, 0),
     (2, 64, 8, 8, 64, 3, 1, 1),
     (1, 64, 16, 16, 128, 3, 1, 1),
-    (1, 64, 16, 16, 128, 3, 1, 2),
     (2, 128, 16, 16, 64, 1, 1, 0),
     (1, 64, 256, 256, 64, 3, 1, 0),
 ]
@@ -71,18 +70,6 @@ def test_conv2d(ctx, n, cin, H, W, cout, k, stride, up, passes):
     out = ctx.test_conv2d(x, w, b, stride=stride, upsample=up, passes=passes)
     assert out.shape == ref.shape
     assert rel(out, ref) < TOL[passes]
-
-
-@pytest.mark.parametrize("n,c,H,W", [(2, 320, 16, 16), (1, 64, 8, 8), (2, 960, 8, 8), (1, 128, 64, 64), (1, 1920, 4, 4)])
-@pytest.mark.parametrize("silu", [False, True])
-def test_groupnorm(ctx, n, c, H, W, silu):
-    x = rnd((n, c, H, W), 21) * 3 + 0.7
-    g = 1 + 0.1 * rnd((c,), 22); b = 0.1 * rnd((c,), 23)
-    ref = F.group_norm(torch.from_numpy(x).double(), 32, torch.from_numpy(g).double(), torch.from_numpy(b).double(), 1e-5)
-    if silu:
-        ref = F.silu(ref)
-    out = ctx.test_groupnorm(x, g, b, silu)
-    assert rel(out, ref.numpy()) < 5e-6
 
 
 # n, cin, H, W, cout, ksize: plain tiles (one image per tile), two / four images per tile (8x8, 8x4), split-K (small grid, long
