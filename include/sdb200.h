@@ -116,6 +116,10 @@ int sdb_finalize_weights(sdb_ctx* ctx);
  * context [n,L,768] -> out [n,4,H,W]. */
 int sdb_unet_forward(sdb_ctx* ctx, const float* x, int32_t timestep, const float* context,
                      int n, int H, int W, int L, float* out);
+/* sdb_unet_forward at a real timestep t (DESIGN.md §7 f15), for callers that drive their own sampler on a grid of fractional
+ * timesteps: t finite and in [0, 999], rounded once to f32 for the sinusoidal embedding. At an integer t the output equals
+ * sdb_unet_forward's bit for bit. */
+int sdb_unet_forward_at(sdb_ctx* ctx, const float* x, double t, const float* context, int n, int H, int W, int L, float* out);
 /* Autoencoder::decode_latent (src/model/autoencoder/mod.rs:68-71): latent [n,4,H,W] -> img [n,3,8H,8W]. */
 int sdb_decode_latent(sdb_ctx* ctx, const float* latent, int n, int H, int W, float* img);
 /* StableDiffusion::sample_latent (src/model/stablediffusion/mod.rs:102-160), DDIM eta=0 (the default sampler; see
@@ -210,6 +214,21 @@ int sdb_edit_image_dev(sdb_ctx* ctx, const uint8_t* d_image, const float* d_cont
 #define SDB_SAMPLER_DDIM 0
 #define SDB_SAMPLER_DPMPP_2M 1
 int sdb_set_sampler(sdb_ctx* ctx, int kind, double eta, uint64_t noise_seed);
+/* The grid the sampler walks (DESIGN.md §7 f15), context state read by exactly the entries that read sdb_set_sampler. N = n_steps.
+ * SDB_SCHEDULE_DDIM (the default): the reference's timesteps (0..1000).rev().step_by(1000/n_steps), abar = alpha_cumulative_products[t].
+ * SDB_SCHEDULE_KARRAS: the sigma grid of Karras et al. 2022 (rho = 7; k-diffusion's get_sigmas_karras) between sigma_max =
+ *   sigma_999 and sigma_min = sigma_0 of the table sigma_j = sqrt((1 - abar_j) / abar_j): sigma_i = (sigma_max^(1/7) + i/(N-1)
+ *   (sigma_min^(1/7) - sigma_max^(1/7)))^7, i < N, then sigma_N = 0. Step i evaluates the UNet at the real timestep
+ *   t_i = sigma_to_t(sigma_i) (k-diffusion's: linear in log sigma between table neighbours, rounded once to f32) and runs the
+ *   sampler's update from abar_i = 1/(1 + sigma_i^2) to abar_{i+1} (1 after the last step). In k-diffusion's terms: DDIM eta = 0
+ *   is sample_euler, DDIM eta is sample_euler_ancestral(eta), DPM-Solver++(2M) is sample_dpmpp_2m. The latent is the library's
+ *   x = sqrt(abar) x0 + sqrt(1 - abar) eps throughout: the start latent is used as is (diffusers' init_noise_sigma
+ *   convention). img2img runs the last floor(strength * N) steps; eta noise is keyed by the step's index i in the grid instead of
+ *   the timestep value. Every call checks that alpha_cumulative_products is finite, in (0, 1) and strictly decreasing.
+ * An unknown kind is an error and leaves the setting unchanged. No cached graph is invalidated. */
+#define SDB_SCHEDULE_DDIM 0
+#define SDB_SCHEDULE_KARRAS 1
+int sdb_set_schedule(sdb_ctx* ctx, int kind);
 
 /* ---- LoRA adapters (DESIGN.md §7 f8) ------------------------------------------------------------------------------------- */
 /* An adapter (id >= 0) is a set of terms; a term targets one registry weight with down [r][fan-in] (fan-in = in for a Linear,

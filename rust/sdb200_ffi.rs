@@ -80,6 +80,9 @@ extern "C" {
                           d_init_latent: *const c_void, h: c_int, w: c_int, d_latent_out: *mut c_void, d_rgb_out: *mut c_void,
                           stream: *mut c_void) -> c_int;
     fn sdb_set_sampler(ctx: *mut SdbCtx, kind: c_int, eta: f64, noise_seed: u64) -> c_int;
+    fn sdb_set_schedule(ctx: *mut SdbCtx, kind: c_int) -> c_int;
+    fn sdb_unet_forward_at(ctx: *mut SdbCtx, x: *const f32, t: f64, context: *const f32, n: c_int, h: c_int, w: c_int, l: c_int,
+                           out: *mut f32) -> c_int;
     fn sdb_tensor_count(ctx: *mut SdbCtx) -> c_int;
     fn sdb_tensor_info(ctx: *mut SdbCtx, index: c_int, name: *mut *const c_char, dims: *mut i64, ndim: *mut c_int) -> c_int;
     fn sdb_lora_add(ctx: *mut SdbCtx, adapter: c_int, tensor: *const c_char, rank: c_int, down: *const f32, up: *const f32,
@@ -105,12 +108,22 @@ pub struct SdbError(pub String);
 
 const SDB_SAMPLER_DDIM: c_int = 0;
 const SDB_SAMPLER_DPMPP_2M: c_int = 1;
+const SDB_SCHEDULE_DDIM: c_int = 0;
+const SDB_SCHEDULE_KARRAS: c_int = 1;
 
 /// The sampler of the sampling calls (include/sdb200.h: sdb_set_sampler).
 #[derive(Clone, Copy, Debug)]
 pub enum Sampler {
     Ddim { eta: f64 },
     DpmPp2M,
+}
+
+/// The grid the sampler walks (include/sdb200.h: sdb_set_schedule): the reference's timesteps, or the sigma grid of Karras et
+/// al. 2022 (rho = 7) at fractional timesteps.
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub enum Schedule {
+    Ddim,
+    Karras,
 }
 
 pub struct StableDiffusion {
@@ -220,6 +233,15 @@ impl StableDiffusion {
         let mut out = vec![0f32; n * 4 * h * w];
         self.check(unsafe {
             sdb_unet_forward(self.ctx, x.as_ptr(), timestep, context.as_ptr(), n as c_int, h as c_int, w as c_int, l as c_int, out.as_mut_ptr())
+        })?;
+        Ok(out)
+    }
+
+    /// `unet_forward` at a real timestep t in [0, 999] (an extension, DESIGN.md §7 f15): at an integer t the same bits.
+    pub fn unet_forward_at(&self, x: &[f32], [n, h, w]: [usize; 3], t: f64, context: &[f32], l: usize) -> Result<Vec<f32>, SdbError> {
+        let mut out = vec![0f32; n * 4 * h * w];
+        self.check(unsafe {
+            sdb_unet_forward_at(self.ctx, x.as_ptr(), t, context.as_ptr(), n as c_int, h as c_int, w as c_int, l as c_int, out.as_mut_ptr())
         })?;
         Ok(out)
     }
@@ -343,6 +365,17 @@ impl StableDiffusion {
             Sampler::DpmPp2M => (SDB_SAMPLER_DPMPP_2M, 0.0),
         };
         self.check(unsafe { sdb_set_sampler(self.ctx, kind, eta, noise_seed) })
+    }
+
+    /// The grid `set_sampler`'s sampler walks until changed (an extension, DESIGN.md §7 f15): `Schedule::Ddim` (the reference's,
+    /// the default) or `Schedule::Karras`. Euler Karras = `Ddim { eta: 0 }`, Euler a Karras = `Ddim { eta: 1 }`, DPM++ 2M Karras =
+    /// `DpmPp2M`, each with `Schedule::Karras`.
+    pub fn set_schedule(&self, schedule: Schedule) -> Result<(), SdbError> {
+        let kind = match schedule {
+            Schedule::Ddim => SDB_SCHEDULE_DDIM,
+            Schedule::Karras => SDB_SCHEDULE_KARRAS,
+        };
+        self.check(unsafe { sdb_set_schedule(self.ctx, kind) })
     }
 
     /// One term of LoRA adapter `adapter` (an extension, DESIGN.md §7 f8) on registry weight `tensor`: `down` = rank x fan-in

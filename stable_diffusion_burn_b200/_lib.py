@@ -81,6 +81,8 @@ SIGNATURES = [
     ("sdb_edit_image_dev", C.c_int, [_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_double,
                                      C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("sdb_set_sampler", C.c_int, [_ctx, C.c_int, C.c_double, C.c_uint64]),
+    ("sdb_set_schedule", C.c_int, [_ctx, C.c_int]),
+    ("sdb_unet_forward_at", C.c_int, [_ctx, _f32p, C.c_double, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, _f32p]),
     ("sdb_lora_add", C.c_int, [_ctx, C.c_int, C.c_char_p, C.c_int, _f32p, _f32p, C.c_double]),
     ("sdb_lora_scale", C.c_int, [_ctx, C.c_int, C.c_double]),
     ("sdb_lora_remove", C.c_int, [_ctx, C.c_int]),
@@ -365,6 +367,17 @@ class Context:
             kind = self.SAMPLERS[kind]
         self.check(self.lib.sdb_set_sampler(self.h, int(kind), float(eta), int(noise_seed)))
 
+    SCHEDULES = {"ddim": 0, "karras": 1}  # SDB_SCHEDULE_DDIM, SDB_SCHEDULE_KARRAS
+
+    def set_schedule(self, kind=0):
+        """The grid every sampling entry walks until changed (include/sdb200.h: sdb_set_schedule; DESIGN.md §7 f15). kind: 0 /
+        "ddim" (the reference's integer timesteps) or 1 / "karras" (the sigma grid of Karras et al. 2022, rho = 7)."""
+        if isinstance(kind, str):
+            if kind not in self.SCHEDULES:
+                raise ValueError(f"unknown schedule {kind!r}: one of {', '.join(self.SCHEDULES)}")
+            kind = self.SCHEDULES[kind]
+        self.check(self.lib.sdb_set_schedule(self.h, int(kind)))
+
     # ---- LoRA adapters (include/sdb200.h: sdb_lora_*; DESIGN.md §7 f8)
     def lora_add(self, adapter, tensor, down, up, alpha):
         """One term of adapter `adapter`: registry weight `tensor`, down [r, fan-in] (a conv's [r, in, k, k] is flattened), up
@@ -416,6 +429,16 @@ class Context:
         L = context.shape[1]
         out = np.empty((n, 4, H, W), np.float32)
         self.check(self.lib.sdb_unet_forward(self.h, ptr(x), int(t), ptr(context), n, H, W, L, ptr(out)))
+        return out
+
+    def unet_forward_at(self, x, t, context):
+        """unet_forward at a real timestep t (finite, in [0, 999], rounded once to float32); at an integer t the same bits."""
+        x = f32(x); context = f32(context)
+        n, ch, H, W = x.shape
+        if ch != self.unet_in_channels():
+            raise ValueError(f"x has {ch} channels; this context's UNet takes {self.unet_in_channels()}")
+        out = np.empty((n, 4, H, W), np.float32)
+        self.check(self.lib.sdb_unet_forward_at(self.h, ptr(x), float(t), ptr(context), n, H, W, context.shape[1], ptr(out)))
         return out
 
     def forward_diffuser(self, latent, t, context, uncond, scale):

@@ -316,6 +316,13 @@ int sdb_unet_forward(sdb_ctx* ctx, const float* x, int32_t timestep, const float
   API_END
 }
 
+int sdb_unet_forward_at(sdb_ctx* ctx, const float* x, double t, const float* context, int n, int H, int W, int L, float* out) {
+  API_BEGIN(ctx)
+  need_final(c);
+  model_unet_forward_at_host(c, x, t, context, n, H, W, L, out);
+  API_END
+}
+
 int sdb_unet_forward_dev(sdb_ctx* ctx, const float* d_x, int32_t timestep, const float* d_context, int n, int H, int W,
                          int L, float* d_out, void* stream) {
   API_BEGIN(ctx)
@@ -536,6 +543,16 @@ int sdb_set_sampler(sdb_ctx* ctx, int kind, double eta, uint64_t noise_seed) {
   snprintf(msg, sizeof(msg), "sampler: DPM-Solver++(2M) is deterministic; eta %.17g must be 0", eta);
   SDB_CHECK(kind != SDB_SAMPLER_DPMPP_2M || eta == 0.0, msg);
   c.sampler_kind = kind, c.sampler_eta = eta, c.sampler_noise_seed = noise_seed;
+  API_END
+}
+
+// ------------------------------------------------------------------------------ schedule (DESIGN.md §7 f15)
+int sdb_set_schedule(sdb_ctx* ctx, int kind) {
+  API_BEGIN(ctx)
+  char msg[160];
+  snprintf(msg, sizeof(msg), "schedule: unknown kind %d (SDB_SCHEDULE_DDIM = 0, SDB_SCHEDULE_KARRAS = 1)", kind);
+  SDB_CHECK(kind == SDB_SCHEDULE_DDIM || kind == SDB_SCHEDULE_KARRAS, msg);
+  c.sampler_schedule = kind;
   API_END
 }
 

@@ -939,15 +939,17 @@ void quant_conv_slice_scaled_launch(const float* x, const float* w, const float*
 
 // ============================================================ time embedding + GEMV
 // y[N] = act(x[K] W[K][N] + b); a block owns 32 outputs, 8 k-slices reduced through smem.
-// t_dev != null: x is the sinusoidal timestep embedding (reference unet/mod.rs:24-29), K must be 320.
+// t_dev != null: x is the sinusoidal timestep embedding (reference unet/mod.rs:24-29), K must be 320. T: the timestep's type, int
+// (the schedule's timesteps) or float (a real t, DESIGN §7 f15); at an integer t both give the same (float)t and the same rows.
+template <class T>
 __global__ void __launch_bounds__(256)
-gemv_kernel(const float* __restrict__ x, const int* __restrict__ t_dev, const float* __restrict__ W,
+gemv_kernel(const float* __restrict__ x, const T* __restrict__ t_dev, const float* __restrict__ W,
             const float* __restrict__ b, int K, int N, int silu, float* __restrict__ y) {
   pdl_enter();
   __shared__ float s_part[8][32];
   __shared__ float s_x[1280];
   if (t_dev) {
-    const int t = *t_dev;
+    const T t = *t_dev;
     for (int i = threadIdx.x; i < 160; i += blockDim.x) {
       // freqs = exp(arange(half) * (-ln(10000)/half)); args = t*freqs; [cos | sin]
       const float f = expf((float)i * (float)(-9.210340371976184 / 160.0));
@@ -975,25 +977,36 @@ gemv_kernel(const float* __restrict__ x, const int* __restrict__ t_dev, const fl
 }
 void gemv_launch(const float* x, const float* W, const float* b, int K, int N, float* y, cudaStream_t st) {
   SDB_CHECK(K <= 1280, "gemv K");
-  launch_k(gemv_kernel, dim3(ceil_div(N, 32)), dim3(256), 0, st, x, (const int*)nullptr, W, b, K, N, 0, y);
+  launch_k(gemv_kernel<int>, dim3(ceil_div(N, 32)), dim3(256), 0, st, x, (const int*)nullptr, W, b, K, N, 0, y);
   SDB_CUDA(cudaGetLastError());
 }
 // emb_silu = silu(lin2(silu(lin1(timestep_embedding(t)))))  — two multi-CTA GEMVs
+template <class T>
+static void time_embed_go(const T* t, const float* w1, const float* b1, const float* w2, const float* b2, float* hidden,
+                          float* emb_silu, cudaStream_t st) {
+  launch_k(gemv_kernel<T>, dim3(40), dim3(256), 0, st, (const float*)nullptr, t, w1, b1, 320, 1280, 1, hidden);
+  launch_k(gemv_kernel<int>, dim3(40), dim3(256), 0, st, (const float*)hidden, (const int*)nullptr, w2, b2, 1280, 1280, 1,
+           emb_silu);
+  SDB_CUDA(cudaGetLastError());
+}
 void time_embed_launch(const int* t, const float* w1, const float* b1, const float* w2, const float* b2, float* hidden,
                        float* emb_silu, cudaStream_t st) {
-  launch_k(gemv_kernel, dim3(40), dim3(256), 0, st, (const float*)nullptr, t, w1, b1, 320, 1280, 1, hidden);
-  launch_k(gemv_kernel, dim3(40), dim3(256), 0, st, (const float*)hidden, (const int*)nullptr, w2, b2, 1280, 1280, 1, emb_silu);
-  SDB_CUDA(cudaGetLastError());
+  time_embed_go(t, w1, b1, w2, b2, hidden, emb_silu, st);
+}
+void time_embed_launch(const float* t, const float* w1, const float* b1, const float* w2, const float* b2, float* hidden,
+                       float* emb_silu, cudaStream_t st) {
+  time_embed_go(t, w1, b1, w2, b2, hidden, emb_silu, st);
 }
 
 // Time embedding for ALL timesteps of a sampling schedule in one pass (the rows depend on t alone: sample_latent computes them once
 // per call instead of once per step; the weights of the 22 lin_embed layers, 103 MB of fp32, stream once per R rows instead of
 // once per step). Same arithmetic, in the same order, as gemv_kernel: the rows are bit-identical to the per-step path.
 //   y[row][N] = act(x[row][K] W[K][N] + b),  row = blockIdx.y * R + r
-// t_embed != null: x is the sinusoidal embedding of t_embed[row] (K = 320). t_rowmap != null: output row index = t_rowmap[row].
-template <int R>
+// t_embed != null: x is the sinusoidal embedding of t_embed[row] (K = 320; T as gemv_kernel's). t_rowmap != null: output row
+// index = t_rowmap[row].
+template <int R, class T>
 __global__ void __launch_bounds__(256)
-gemv_rows_kernel(const float* __restrict__ x, const int* __restrict__ t_embed, const int* __restrict__ t_rowmap, int rows,
+gemv_rows_kernel(const float* __restrict__ x, const T* __restrict__ t_embed, const int* __restrict__ t_rowmap, int rows,
                  const float* __restrict__ W, const float* __restrict__ b, int K, int N, int silu, float* __restrict__ y,
                  long long y_stride) {
   pdl_enter();
@@ -1002,7 +1015,7 @@ gemv_rows_kernel(const float* __restrict__ x, const int* __restrict__ t_embed, c
   const int r0 = blockIdx.y * R, nr = min(R, rows - r0);
   for (int r = 0; r < nr; ++r) {
     if (t_embed) {
-      const int t = t_embed[r0 + r];
+      const T t = t_embed[r0 + r];
       for (int i = threadIdx.x; i < 160; i += blockDim.x) {
         const float f = expf((float)i * (float)(-9.210340371976184 / 160.0));
         const float a = (float)t * f;
@@ -1039,19 +1052,31 @@ gemv_rows_kernel(const float* __restrict__ x, const int* __restrict__ t_embed, c
     }
   }
 }
-// rows of emb_all are indexed by the TIMESTEP VALUE (emb_all[t][N]): the in-graph selection needs no step counter
+// Row j of the call's timesteps t_embed[j] goes to emb_all row row_of[j] (emb_all[row_of[j]][N]): the in-graph selection needs no
+// step counter. The DDIM grid's rows are its timestep values (t_embed = row_of); the Karras grid's real t of step j goes to row j.
+template <class T>
+static void time_embed_rows_go(const T* t_embed, const int* row_of, int rows, const float* w1, const float* b1, const float* w2,
+                               const float* b2, const float* w_all, const float* b_all, int n_all, float* hidden, float* emb_silu,
+                               float* emb_all, cudaStream_t st) {
+  constexpr int R = 5;
+  const dim3 gy(40, ceil_div(rows, R));
+  launch_k(gemv_rows_kernel<R, T>, gy, dim3(256), 0, st, (const float*)nullptr, t_embed, (const int*)nullptr, rows, w1, b1, 320,
+           1280, 1, hidden, (long long)1280);
+  launch_k(gemv_rows_kernel<R, int>, gy, dim3(256), 0, st, (const float*)hidden, (const int*)nullptr, (const int*)nullptr, rows, w2,
+           b2, 1280, 1280, 1, emb_silu, (long long)1280);
+  launch_k(gemv_rows_kernel<R, int>, dim3(ceil_div(n_all, 32), ceil_div(rows, R)), dim3(256), 0, st, (const float*)emb_silu,
+           (const int*)nullptr, row_of, rows, w_all, b_all, 1280, n_all, 0, emb_all, (long long)n_all);
+  SDB_CUDA(cudaGetLastError());
+}
 void time_embed_rows_launch(const int* t_dev, int rows, const float* w1, const float* b1, const float* w2, const float* b2,
                             const float* w_all, const float* b_all, int n_all, float* hidden, float* emb_silu, float* emb_all,
                             cudaStream_t st) {
-  constexpr int R = 5;
-  const dim3 gy(40, ceil_div(rows, R));
-  launch_k(gemv_rows_kernel<R>, gy, dim3(256), 0, st, (const float*)nullptr, t_dev, (const int*)nullptr, rows, w1, b1, 320, 1280, 1,
-           hidden, (long long)1280);
-  launch_k(gemv_rows_kernel<R>, gy, dim3(256), 0, st, (const float*)hidden, (const int*)nullptr, (const int*)nullptr, rows, w2, b2,
-           1280, 1280, 1, emb_silu, (long long)1280);
-  launch_k(gemv_rows_kernel<R>, dim3(ceil_div(n_all, 32), ceil_div(rows, R)), dim3(256), 0, st, (const float*)emb_silu,
-           (const int*)nullptr, t_dev, rows, w_all, b_all, 1280, n_all, 0, emb_all, (long long)n_all);
-  SDB_CUDA(cudaGetLastError());
+  time_embed_rows_go(t_dev, t_dev, rows, w1, b1, w2, b2, w_all, b_all, n_all, hidden, emb_silu, emb_all, st);
+}
+void time_embed_rows_launch(const float* t_dev, const int* row_of, int rows, const float* w1, const float* b1, const float* w2,
+                            const float* b2, const float* w_all, const float* b_all, int n_all, float* hidden, float* emb_silu,
+                            float* emb_all, cudaStream_t st) {
+  time_embed_rows_go(t_dev, row_of, rows, w1, b1, w2, b2, w_all, b_all, n_all, hidden, emb_silu, emb_all, st);
 }
 // out[N] = emb_all[*t_dev][N]: the one launch of the UNet step graph that replaces the three GEMVs
 __global__ void __launch_bounds__(256)

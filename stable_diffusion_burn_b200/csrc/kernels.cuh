@@ -77,10 +77,18 @@ SmallCoutVariant conv3x3_small_cout_launch(const float* x, int n, int H, int W, 
 // emb = lin2(silu(lin1([cos|sin](t*f)))) ; then for every ResBlock r: e_r = lin_embed_r(silu(emb))
 void time_embed_launch(const int* t_dev, const float* w1, const float* b1, const float* w2, const float* b2, float* hidden,
                        float* emb_silu, cudaStream_t st);
+// the same at a real timestep (DESIGN §7 f15): at an integer t, the int overload's rows bit for bit
+void time_embed_launch(const float* t_dev, const float* w1, const float* b1, const float* w2, const float* b2, float* hidden,
+                       float* emb_silu, cudaStream_t st);
 // the same for `rows` timesteps at once (t_dev[rows]); emb_all[t][n_all] is indexed by the timestep value. Bit-identical rows.
 void time_embed_rows_launch(const int* t_dev, int rows, const float* w1, const float* b1, const float* w2, const float* b2,
                             const float* w_all, const float* b_all, int n_all, float* hidden, float* emb_silu, float* emb_all,
                             cudaStream_t st);
+// real timesteps t_dev[rows] (the Karras grid): the rows of t_dev[j] go to emb_all[row_of[j]], bit-identical to time_embed_launch
+// at t_dev[j]
+void time_embed_rows_launch(const float* t_dev, const int* row_of, int rows, const float* w1, const float* b1, const float* w2,
+                            const float* b2, const float* w_all, const float* b_all, int n_all, float* hidden, float* emb_silu,
+                            float* emb_all, cudaStream_t st);
 void emb_select_launch(const float* emb_all, const int* t_dev, int N, float* out, cudaStream_t st);
 // y[N] = x[K] @ W[K][N] + b  (tiny GEMV, W fp32 [in,out])
 void gemv_launch(const float* x, const float* W, const float* b, int K, int N, float* y, cudaStream_t st);
@@ -105,7 +113,7 @@ struct SamplerStep {   // per-step scalars, computed on the host in double and p
   // keyed by step_noise_keys(noise_seeds[s], t) instead of (k0, k1). Any kind, STEP_DDIM included, may run per sample.
   const float* scales = nullptr;         // device [n]
   const uint64_t* noise_seeds = nullptr;  // device [n]
-  int t = 0;                             // timestep value of the step
+  int t = 0;  // the step's noise key (step_noise_keys): the timestep value (DDIM grid) or the index in the Karras grid
 };
 // One launch per step. groups = 2: eu / ec [count] the unconditional / prompt predictions, the update goes to both halves of
 // lat [2][count]. groups = 3 (InstructPix2Pix): eu = eps [3][count] holds e_U | e_I | e_T (ec unused),

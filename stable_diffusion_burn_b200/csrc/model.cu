@@ -20,6 +20,7 @@
 namespace sdb {
 
 static Model& M(Ctx& c) { return *reinterpret_cast<Model*>(c.model); }
+static const Model& M(const Ctx& c) { return *reinterpret_cast<const Model*>(c.model); }
 static int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
 // tensor-core passes per product as a function of the UNet resolution level (0 = full latent resolution).
@@ -955,6 +956,7 @@ struct UNetIO {
   float* out;          // [nb,4,H,W] NCHW
   int H, W;
   const float* emb_all = nullptr;  // [1000][emb_total] rows precomputed per timestep value (sample_latent), or null
+  const float* tf_dev = nullptr;   // device real timestep (DESIGN §7 f15): the per-step embedding reads it instead of t_dev
   // 9- / 8-channel conv_in (DESIGN §7 f9, f10): input channels 4.. of sample i at cond + (i % cond_mod) * cond_stride
   long long x_stride = 0;
   const float* cond = nullptr;
@@ -1020,8 +1022,12 @@ static void unet_forward(Fwd& f, const UNetIO& io, const CtxState& cs) {
   } else {
     {
       KernelScope ks(c, KC_ELEMENTWISE);
-      time_embed_launch(io.t_dev, mptr(c, m.lin1_time.wi), m.lin1_time.bias, mptr(c, m.lin2_time.wi), m.lin2_time.bias,
-                        emb_hidden, emb_silu, c.stream);
+      if (io.tf_dev)
+        time_embed_launch(io.tf_dev, mptr(c, m.lin1_time.wi), m.lin1_time.bias, mptr(c, m.lin2_time.wi), m.lin2_time.bias,
+                          emb_hidden, emb_silu, c.stream);
+      else
+        time_embed_launch(io.t_dev, mptr(c, m.lin1_time.wi), m.lin1_time.bias, mptr(c, m.lin2_time.wi), m.lin2_time.bias,
+                          emb_hidden, emb_silu, c.stream);
     }
     {
       KernelScope ks(c, KC_ELEMENTWISE, 2.0 * 1280 * m.emb_total, 4.0 * 1280 * m.emb_total);
@@ -1349,9 +1355,10 @@ struct StreamJoin {  // run on c.stream ordered after / before the caller's stre
 }  // namespace
 
 // UNet pass over nb samples with per-sample context lengths. d_ctx_padded [nb][Lpad][768]. d_x / d_cond: see unet_cond_io.
+// d_tf: a real timestep the time embedding reads instead of d_t (emb_all null).
 static void unet_pass(Ctx& c, int nb, const float* d_x, const int* d_t, const float* d_ctx_padded, int Lpad, int* d_kvlen,
                       int H, int W, float* d_out, const CtxState* shared_cs, const float* emb_all = nullptr,
-                      const float* d_cond = nullptr) {
+                      const float* d_cond = nullptr, const float* d_tf = nullptr) {
   Fwd f(c, nb);
   const size_t mark = c.work.off;
   CtxState local;
@@ -1361,14 +1368,21 @@ static void unet_pass(Ctx& c, int nb, const float* d_x, const int* d_t, const fl
     cs = &local;
   }
   UNetIO io{d_x, d_t, d_out, H, W};
-  io.emb_all = emb_all;
+  io.emb_all = emb_all, io.tf_dev = d_tf;
   unet_cond_io(c, nb, d_x, d_cond, io);
   unet_forward(f, io, *cs);
   c.work.off = mark;
 }
 
-void model_unet_forward_dev(Ctx& c, const float* d_x, int t, const float* d_context, int n, int H, int W, int L,
-                            float* d_out, cudaStream_t caller) {
+// The timestep of a single UNet pass: the integer t of sdb_unet_forward, or the real t of sdb_unet_forward_at, rounded once to f32
+struct PassTime {
+  int t = 0;
+  bool real = false;
+  float tf = 0.f;
+};
+
+static void unet_forward_dev(Ctx& c, const float* d_x, PassTime pt, const float* d_context, int n, int H, int W, int L,
+                             float* d_out, cudaStream_t caller) {
   SDB_CHECK(n >= 1 && H % 8 == 0 && W % 8 == 0 && L >= 1, "unet_forward arguments");
   // the deepest level has (H/8)*(W/8) tokens per sample; TMA tile origins inside the V^T matrix are
   // per-sample column offsets and must stay 16-byte aligned
@@ -1383,22 +1397,49 @@ void model_unet_forward_dev(Ctx& c, const float* d_x, int t, const float* d_cont
   SDB_CUDA(cudaMemsetAsync(ctxp, 0, (size_t)n * Lpad * 768 * 4, c.stream));
   SDB_CUDA(cudaMemcpy2DAsync(ctxp, (size_t)Lpad * 768 * 4, d_context, (size_t)L * 768 * 4, (size_t)L * 768 * 4, n,
                              cudaMemcpyDeviceToDevice, c.stream));
-  SDB_CUDA(cudaMemcpyAsync(d_t, &t, 4, cudaMemcpyHostToDevice, c.stream));
+  if (pt.real)
+    SDB_CUDA(cudaMemcpyAsync(d_t, &pt.tf, 4, cudaMemcpyHostToDevice, c.stream));
+  else
+    SDB_CUDA(cudaMemcpyAsync(d_t, &pt.t, 4, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaMemcpyAsync(d_len, lens.data(), 4 * n, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));  // host staging buffers (t, lens) must outlive the copies
-  unet_pass(c, n, d_x, d_t, ctxp, Lpad, d_len, H, W, d_out, nullptr);
+  unet_pass(c, n, d_x, d_t, ctxp, Lpad, d_len, H, W, d_out, nullptr, nullptr, nullptr, pt.real ? (const float*)d_t : nullptr);
 }
 
-void model_unet_forward_host(Ctx& c, const float* x, int t, const float* context, int n, int H, int W, int L, float* out) {
+void model_unet_forward_dev(Ctx& c, const float* d_x, int t, const float* d_context, int n, int H, int W, int L,
+                            float* d_out, cudaStream_t caller) {
+  PassTime pt;
+  pt.t = t;
+  unet_forward_dev(c, d_x, pt, d_context, n, H, W, L, d_out, caller);
+}
+
+static void unet_forward_host(Ctx& c, const float* x, PassTime pt, const float* context, int n, int H, int W, int L, float* out) {
   const size_t xe = (size_t)n * 4 * H * W, ie = (size_t)n * c.unet_cin * H * W, ce = (size_t)n * L * 768;
   float* d_x = (float*)c.io(0, ie * 4);
   float* d_c = (float*)c.io(1, ce * 4);
   float* d_o = (float*)c.io(2, xe * 4);
   SDB_CUDA(cudaMemcpyAsync(d_x, x, ie * 4, cudaMemcpyHostToDevice, c.stream));
   SDB_CUDA(cudaMemcpyAsync(d_c, context, ce * 4, cudaMemcpyHostToDevice, c.stream));
-  model_unet_forward_dev(c, d_x, t, d_c, n, H, W, L, d_o, c.stream);
+  unet_forward_dev(c, d_x, pt, d_c, n, H, W, L, d_o, c.stream);
   SDB_CUDA(cudaMemcpyAsync(out, d_o, xe * 4, cudaMemcpyDeviceToHost, c.stream));
   SDB_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+void model_unet_forward_host(Ctx& c, const float* x, int t, const float* context, int n, int H, int W, int L, float* out) {
+  PassTime pt;
+  pt.t = t;
+  unet_forward_host(c, x, pt, context, n, H, W, L, out);
+}
+
+// sdb_unet_forward at a real timestep (DESIGN §7 f15): t finite in [0, 999], rounded once to f32; the time embedding takes the
+// float path, which at an integer t gives sdb_unet_forward's rows, hence its output, bit for bit
+void model_unet_forward_at_host(Ctx& c, const float* x, double t, const float* context, int n, int H, int W, int L, float* out) {
+  char msg[160];
+  snprintf(msg, sizeof(msg), "unet_forward_at: t = %.17g must be finite and in [0, 999]", t);
+  SDB_CHECK(std::isfinite(t) && t >= 0.0 && t <= 999.0, msg);
+  PassTime pt;
+  pt.real = true, pt.tf = (float)t;
+  unet_forward_host(c, x, pt, context, n, H, W, L, out);
 }
 
 // The autoencoder's mid attention (run_vae_attention) takes the latent's H * W positions as one row of S and of P: the row
@@ -1509,10 +1550,76 @@ static std::vector<int> ddim_timesteps(int n_steps) {
   return ts;
 }
 
+// The Karras et al. 2022 sigma grid (DESIGN §7 f15; k-diffusion's get_sigmas_karras at rho = 7 and sigma_to_t). The sigma table
+// sigma_j = sqrt((1 - abar_j) / abar_j), abar read as f32 and widened, needs every abar_j finite, in (0, 1) and strictly
+// decreasing in j: checked on every call, since a load can replace the schedule.
+static double karras_sigma(const std::vector<float>& alphas, int j) {
+  const double a = (double)alphas[j];
+  return std::sqrt((1.0 - a) / a);
+}
+
+static std::vector<double> karras_log_sigmas(const std::vector<float>& alphas) {
+  std::vector<double> ls(alphas.size());
+  for (size_t j = 0; j < alphas.size(); ++j) {
+    const double a = (double)alphas[j];
+    char msg[240];
+    snprintf(msg, sizeof(msg),
+             "Karras schedule: alpha_cumulative_products[%d] = %.9g: every value must be finite, in (0, 1) and below the one "
+             "before it",
+             (int)j, a);
+    SDB_CHECK(std::isfinite(a) && a > 0.0 && a < 1.0 && (j == 0 || a < (double)alphas[j - 1]), msg);
+    ls[j] = std::log(karras_sigma(alphas, (int)j));
+  }
+  return ls;
+}
+
+// k-diffusion's sigma_to_t: linear in log sigma between the table neighbours; the low index is the largest j with
+// log sigma_j <= log sigma, clamped to [0, 998], and w is clamped to [0, 1]
+static double karras_sigma_to_t(const std::vector<double>& ls, double sigma) {
+  const double l = std::log(sigma);
+  int lo = 0;
+  for (int j = 0; j < (int)ls.size(); ++j)
+    if (ls[j] <= l) lo = j;
+  lo = std::min(lo, (int)ls.size() - 2);
+  const double w = std::min(1.0, std::max(0.0, (ls[lo] - l) / (ls[lo] - ls[lo + 1])));
+  return (1.0 - w) * lo + w * (lo + 1);
+}
+
+// The steps a sampling call walks (DESIGN §7 f6, f15): step i runs at abar[i] toward abar[i + 1]; abar[N] = 1.
+//   DDIM grid (the reference's): ts[i] = 999 - i (1000 / n_steps), abar[i] = alphas[ts[i]] widened from f32.
+//   Karras grid: sigma_i = (sigma_max^(1/7) + i / (N - 1) (sigma_min^(1/7) - sigma_max^(1/7)))^7 with sigma_max = sigma_999 and
+//   sigma_min = sigma_0 (the ends exactly; N = 1: sigma_max alone), abar[i] = 1 / (1 + sigma_i^2), tf[i] = sigma_to_t(sigma_i)
+//   rounded once to f32.
+struct Grid {
+  std::vector<int> ts;       // DDIM grid: the timestep values
+  std::vector<float> tf;     // Karras grid: the real timesteps (empty on the DDIM grid)
+  std::vector<double> abar;  // [N + 1]
+  int n() const { return (int)abar.size() - 1; }
+  bool karras() const { return !tf.empty(); }
+};
+
+static Grid sample_grid(const Ctx& c, const std::vector<float>& alphas, int n_steps) {
+  Grid g;
+  if (c.sampler_schedule == SDB_SCHEDULE_KARRAS) {
+    const std::vector<double> ls = karras_log_sigmas(alphas);
+    const double smax = karras_sigma(alphas, 999), smin = karras_sigma(alphas, 0);
+    const double rmax = std::pow(smax, 1.0 / 7.0), rmin = std::pow(smin, 1.0 / 7.0);
+    for (int i = 0; i < n_steps; ++i) {
+      double sig = i == 0 ? smax : (i == n_steps - 1 ? smin : std::pow(rmax + (double)i / (n_steps - 1) * (rmin - rmax), 7.0));
+      g.tf.push_back((float)karras_sigma_to_t(ls, sig));
+      g.abar.push_back(1.0 / (1.0 + sig * sig));
+    }
+  } else {
+    g.ts = ddim_timesteps(n_steps);
+    for (int t : g.ts) g.abar.push_back((double)alphas[t]);  // read as f32, widened (stablediffusion/mod.rs:124-140)
+  }
+  g.abar.push_back(1.0);
+  return g;
+}
+
 // The schedule index img2img starts from (DESIGN §7 f5): k = floor(strength * N) of the N timesteps run, the last k of them.
-static int img2img_first(double strength, int n_steps) {
+static int img2img_first(double strength, int N) {
   SDB_CHECK(std::isfinite(strength) && strength > 0.0 && strength <= 1.0, "img2img: strength must be finite and in (0, 1]");
-  const int N = (int)ddim_timesteps(n_steps).size();
   const int k = (int)std::floor(strength * (double)N);
   char msg[160];
   snprintf(msg, sizeof(msg), "img2img: strength %.17g runs none of the %d timesteps; the smallest valid strength is 1/%d = %.17g",
@@ -1586,7 +1693,9 @@ static int check_request(const Ctx& c, const SampleRequest& r, bool host) {
     snprintf(msg, sizeof(msg), "edit_image: image_scale = %.17g is not finite", r.image_scale);
     SDB_CHECK(std::isfinite(r.image_scale), msg);
   }
-  return img2img ? img2img_first(r.strength, r.n_steps) : 0;
+  // the active schedule's grid: N, and on the Karras grid the check of the schedule tensor
+  const int N = sample_grid(c, M(c).alphas_host, r.n_steps).n();
+  return img2img ? img2img_first(r.strength, N) : 0;
 }
 
 namespace {
@@ -1650,13 +1759,11 @@ static void encode_images(Ctx& c, const uint8_t* d_image, const float* d_enc_in,
   }
 }
 
-// The fused step's per-step scalars for timestep t (DESIGN §7 f6): computed in double, rounded once to f32. h_prev: DPM++'s h of
-// the previous step this call ran; has_prev: the step has one (second order).
-static void step_scalars(const Ctx& c, const std::vector<float>& alphas, int kind, int t, int step, bool has_prev, double& h_prev,
+// The fused step's per-step scalars for a step from abar a_t to a_prev (DESIGN §7 f6, f15): computed in double, rounded once to
+// f32. last: the final step (a_prev = 1); key: the step's noise key (Grid). h_prev: DPM++'s h of the previous step this call ran;
+// has_prev: the step has one (second order).
+static void step_scalars(const Ctx& c, int kind, double a_t, double a_prev, bool last, int key, bool has_prev, double& h_prev,
                          CfgStepArgs& a) {
-  // alphas are read as f32 and widened to f64 (stablediffusion/mod.rs:124-140)
-  const double a_t = (double)alphas[t];
-  const double a_prev = (t >= step) ? (double)alphas[t - step] : 1.0;
   double dir = std::sqrt(1.0 - a_prev);
   SamplerStep& s = a.s;
   if (kind != STEP_DDIM) {
@@ -1665,8 +1772,8 @@ static void step_scalars(const Ctx& c, const std::vector<float>& alphas, int kin
       const double sig = c.sampler_eta * std::sqrt((1.0 - a_prev) / (1.0 - a_t)) * std::sqrt(1.0 - a_t / a_prev);
       dir = std::sqrt(std::max(0.0, 1.0 - a_prev - sig * sig));
       s.s = (float)sig;
-      step_noise_keys(c.sampler_noise_seed, t, &s.k0, &s.k1);
-    } else if (t < step) {  // DPM++ final step: sigma' = 0, h = inf: first order, x' = x0
+      step_noise_keys(c.sampler_noise_seed, key, &s.k0, &s.k1);
+    } else if (last) {  // DPM++ final step: sigma' = 0, h = inf: first order, x' = x0
       s.cx = 0.f, s.cd = 1.f;
     } else {  // DPM-Solver++(2M) (Lu et al. 2022), data prediction, lambda = ln(alpha / sigma)
       const double lam = std::log(std::sqrt(a_t) / std::sqrt(1.0 - a_t));
@@ -1681,7 +1788,7 @@ static void step_scalars(const Ctx& c, const std::vector<float>& alphas, int kin
       h_prev = h;
     }
   }
-  s.t = t;
+  s.t = key;
   a.sqrt_1m_at = (float)std::sqrt(1.0 - a_t), a.sqrt_at = (float)std::sqrt(a_t), a.sqrt_aprev = (float)std::sqrt(a_prev);
   a.dir_coef = (float)dir;
 }
@@ -1723,7 +1830,7 @@ static Model::GraphEntry step_graph(Ctx& c, Model::GraphEntry want, int* d_tcur,
 // (forward_diffuser :162-192) run as ONE batch-(groups n) UNet pass: weights stream from HBM once. Two groups: unconditional |
 // prompt. Three (an edit): negative without the image, negative with it, prompt with it, and k.cond holds each group's image
 // channels. Runs on c.stream; the caller joins the streams.
-static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const StepCond& k, int H, int W, float* d_latent_out,
+static void sample_loop(Ctx& c, const Batch& b, const Grid& grid, int first, const StepCond& k, int H, int W, float* d_latent_out,
                         uint8_t* d_rgb) {
   Model& m = M(c);
   c.work.reset();
@@ -1756,25 +1863,44 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const St
     for (int g = 0; g < groups; ++g)
       SDB_CUDA(cudaMemcpyAsync(xb + g * le, k.start, le * 4, cudaMemcpyDeviceToDevice, c.stream));
   }
-  const int step = 1000 / n_steps;
-  std::vector<int> ts = ddim_timesteps(n_steps);
-  ts.erase(ts.begin(), ts.begin() + first);  // img2img runs the last k timesteps only
-  SDB_CUDA(cudaMemcpyAsync(d_t, ts.data(), ts.size() * 4, cudaMemcpyHostToDevice, c.stream));
-  SDB_CUDA(cudaStreamSynchronize(c.stream));  // host staging buffers (ts, lens) must outlive the copies
+  // img2img runs the last k steps only. d_t holds, per step the call runs, the word the step graph reads at d_tcur: the timestep
+  // value on the DDIM grid; on the Karras grid (DESIGN §7 f15) the grid index i, which is the step's emb_all row, or with
+  // emb_hoist off the f32 bits of its real timestep, which the per-step embedding reads
+  const int N = grid.n(), rows = N - first;
+  const bool karras = grid.karras(), real_t = karras && !c.opt_emb_hoist;
+  std::vector<int> words(rows);
+  for (int i = first; i < N; ++i) {
+    int& w = words[i - first];
+    if (!karras)
+      w = grid.ts[i];
+    else if (real_t)
+      memcpy(&w, &grid.tf[i], 4);
+    else
+      w = i;
+  }
+  SDB_CUDA(cudaMemcpyAsync(d_t, words.data(), rows * 4, cudaMemcpyHostToDevice, c.stream));
+  // the Karras grid's real timesteps, for the hoisted embedding rows (an io slot: the work arena's layout is the DDIM grid's)
+  float* d_tf = karras && c.opt_emb_hoist ? (float*)c.io(kIoSchedule, 1000 * 4) : nullptr;
+  if (d_tf) SDB_CUDA(cudaMemcpyAsync(d_tf, grid.tf.data() + first, rows * 4, cudaMemcpyHostToDevice, c.stream));
+  SDB_CUDA(cudaStreamSynchronize(c.stream));  // host staging buffers (words, tf, lens) must outlive the copies
 
   // time-embedding rows of every timestep of the schedule, once per call (unet/mod.rs:19-30, 115-118, 718-722 depend on t alone).
-  // Fixed-size table indexed by the timestep value: the addresses of everything allocated after it do not depend on n_steps,
-  // which the cached step graphs rely on.
+  // Fixed-size table indexed by the timestep value (DDIM grid) or the grid index (Karras grid): the addresses of everything
+  // allocated after it do not depend on n_steps or on the grid, which the cached step graphs rely on.
   float* emb_all = nullptr;
   if (c.opt_emb_hoist) {
     emb_all = c.work.get<float>((size_t)1000 * m.emb_total);
     const size_t mk = c.work.off;
-    float* hid = c.work.get<float>(ts.size() * 1280);
-    float* sil = c.work.get<float>(ts.size() * 1280);
+    float* hid = c.work.get<float>((size_t)rows * 1280);
+    float* sil = c.work.get<float>((size_t)rows * 1280);
     {
-      KernelScope ks(c, KC_ELEMENTWISE, 2.0 * 1280 * m.emb_total * ts.size(), 4.0 * 1280 * m.emb_total * ((ts.size() + 4) / 5));
-      time_embed_rows_launch(d_t, (int)ts.size(), mptr(c, m.lin1_time.wi), m.lin1_time.bias, mptr(c, m.lin2_time.wi),
-                             m.lin2_time.bias, m.emb_w_all, m.emb_b_all, m.emb_total, hid, sil, emb_all, c.stream);
+      KernelScope ks(c, KC_ELEMENTWISE, 2.0 * 1280 * m.emb_total * rows, 4.0 * 1280 * m.emb_total * ((rows + 4) / 5));
+      if (d_tf)
+        time_embed_rows_launch(d_tf, d_t, rows, mptr(c, m.lin1_time.wi), m.lin1_time.bias, mptr(c, m.lin2_time.wi),
+                               m.lin2_time.bias, m.emb_w_all, m.emb_b_all, m.emb_total, hid, sil, emb_all, c.stream);
+      else
+        time_embed_rows_launch(d_t, rows, mptr(c, m.lin1_time.wi), m.lin1_time.bias, mptr(c, m.lin2_time.wi),
+                               m.lin2_time.bias, m.emb_w_all, m.emb_b_all, m.emb_total, hid, sil, emb_all, c.stream);
     }
     c.launches += 2;  // three launches under one scope
     c.work.off = mk;  // stream order: the temporaries are dead before anything else is written there
@@ -1785,11 +1911,15 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const St
   prepare_context(f, ctxp, Lpad, d_len, cs);  // context K/V: once per image, not once per step
 
   int* d_tcur = c.work.get<int>(1);
-  auto pass = [&] { unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all, k.cond); };
-  // one CUDA graph of the UNet step per (nb,H,W,Lpad); replayed with a different timestep slot each step
+  auto pass = [&] {
+    unet_pass(c, nb, xb, d_tcur, nullptr, Lpad, d_len, H, W, eps, &cs, emb_all, k.cond, real_t ? (const float*)d_tcur : nullptr);
+  };
+  // one CUDA graph of the UNet step per (nb,H,W,Lpad); replayed with a different timestep slot each step. The hoisted embedding
+  // reads an emb_all row on either grid, so a Karras call replays the DDIM graph of its shape; the per-step embedding of a real
+  // timestep is another graph (bit 2 of the key), so neither kind of graph replays the other
   Model::GraphEntry graph;
   graph.key = ((long long)nb << 48) ^ ((long long)H << 36) ^ ((long long)W << 24) ^ ((long long)Lpad << 8) ^
-              (long long)(c.opt_precision & 3);
+              (long long)(c.opt_precision & 3) ^ (real_t ? 4ll : 0ll);
   graph.xb = xb, graph.eps = eps, graph.kv = cs.kv[0].kv, graph.work_mark = c.work.off, graph.cond = k.cond;
   if (c.opt_graphs && !c.profiling) graph = step_graph(c, graph, d_tcur, d_t, pass);
   // the sampler (DESIGN §7 f6): DDIM with eta = 0 is sample_latent's own step
@@ -1803,7 +1933,7 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const St
   call.s.hist = dpm ? (float*)c.io(kIoSamplerHist, le * 4) : nullptr;
   call.s.scales = b.d_scale, call.s.noise_seeds = b.d_noise_seed;  // per-sample step (batch entries) when set
   double h_prev = 0.0;  // DPM++: h of the previous step this call ran (none before the first)
-  for (size_t i = 0; i < ts.size(); ++i) {
+  for (int i = 0; i < rows; ++i) {
     SDB_CUDA(cudaMemcpyAsync(d_tcur, d_t + i, 4, cudaMemcpyDeviceToDevice, c.stream));
     if (graph.exec) {
       SDB_CUDA(cudaGraphLaunch(graph.exec, c.stream));
@@ -1814,7 +1944,8 @@ static void sample_loop(Ctx& c, const Batch& b, int n_steps, int first, const St
     }
     KernelScope ks(c, KC_ELEMENTWISE);
     CfgStepArgs a = call;
-    step_scalars(c, m.alphas_host, a.kind, ts[i], step, i > 0, h_prev, a);
+    const int gi = first + i;  // the step's index in the grid: Karras noise is keyed by it, DDIM noise by the timestep value
+    step_scalars(c, a.kind, grid.abar[gi], grid.abar[gi + 1], gi + 1 == N, karras ? gi : grid.ts[gi], i > 0, h_prev, a);
     cfg_step_launch(a, c.stream);
   }
   c.work.off = graph.work_mark;
@@ -1881,9 +2012,10 @@ static void sample_run(Ctx& c, const SampleRequest& r, int first) {
     randn_seeds_launch(d, n, 4ll * H * W, tab.seed, c.stream);
     start = d;
   }
+  const Grid grid = sample_grid(c, m.alphas_host, r.n_steps);
   StepCond k;
   if (r.kind == SAMPLE_IMG2IMG) {
-    const double abar = (double)m.alphas_host[ddim_timesteps(r.n_steps)[first]];  // read as f32, widened (mod.rs:124-140)
+    const double abar = grid.abar[first];
     k.sa = (float)std::sqrt(abar), k.sb = (float)std::sqrt(1.0 - abar);
     const bool inpaint = c.unet_cin == 9;
     k.eps = start, k.mask = inpaint ? nullptr : r.mask;
@@ -1911,7 +2043,7 @@ static void sample_run(Ctx& c, const SampleRequest& r, int first) {
   } else {
     k.start = start;
   }
-  sample_loop(c, b, r.n_steps, first, k, H, W, r.latent_out, r.rgb);
+  sample_loop(c, b, grid, first, k, H, W, r.latent_out, r.rgb);
 }
 
 void model_sample_dev(Ctx& c, const SampleRequest& r, cudaStream_t caller) {

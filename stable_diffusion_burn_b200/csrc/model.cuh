@@ -22,6 +22,7 @@ bool model_lora_pending(Ctx& c);
 void model_get_merged_tensor(Ctx& c, const char* tensor, float* host, int64_t count);
 
 void model_unet_forward_host(Ctx& c, const float* x, int t, const float* context, int n, int H, int W, int L, float* out);
+void model_unet_forward_at_host(Ctx& c, const float* x, double t, const float* context, int n, int H, int W, int L, float* out);
 void model_unet_forward_dev(Ctx& c, const float* d_x, int t, const float* d_context, int n, int H, int W, int L,
                             float* d_out, cudaStream_t caller);
 void model_decode_host(Ctx& c, const float* latent, int n, int H, int W, float* img);

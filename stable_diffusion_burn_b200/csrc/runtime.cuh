@@ -139,6 +139,7 @@ constexpr int kIoLatentOut = 3;
 constexpr int kIoRgb = 4;
 constexpr int kIoImage = 5;      // u8 [n,8H,8W,3]
 constexpr int kIoMask = 6;       // u8 [n,8H,8W]
+constexpr int kIoSchedule = 7;   // the Karras grid's real timesteps [<= 1000] f32 (DESIGN §7 f15)
 constexpr int kIoImg2ImgZ0 = 8;  // encoded image latent z0 [n,4,H,W]
 constexpr int kIoImg2ImgW = 9;   // latent mask w [n,H,W]
 constexpr int kIoSamplerHist = 10;  // DPM-Solver++(2M): x0 of the previous step [n,4,H,W]
@@ -172,6 +173,8 @@ struct Ctx {
   int sampler_kind = 0;
   double sampler_eta = 0.0;
   uint64_t sampler_noise_seed = 0;
+  // the grid those entries walk (sdb_set_schedule, DESIGN §7 f15): SDB_SCHEDULE_DDIM or SDB_SCHEDULE_KARRAS
+  int sampler_schedule = 0;
   // input channels of the UNet's conv_in: 4 (sdb_create), 9 (sdb_create_inpaint: latent | mask | masked-image latent) or 8
   // (sdb_create_pix2pix: latent | image latent)
   int unet_cin = 4;
@@ -183,8 +186,8 @@ struct Ctx {
   double cls_issued[KC_COUNT] = {0};  // tensor-core FLOPs actually issued (x passes for split-fp16 products)
   int64_t cls_launches[KC_COUNT] = {0};
   // grow-only device staging for the host-buffer entry points (no cudaMalloc/cudaFree per call: each is a device-wide sync).
-  // Slots 0..6: host-entry staging; kIoImg2Img*, kIoSamplerHist, kIoBatchTab, kIoUNetCond: buffers the sampling entries
-  // keep outside the work arena.
+  // Slots 0..6: host-entry staging; kIoSchedule, kIoImg2Img*, kIoSamplerHist, kIoBatchTab, kIoUNetCond: buffers the sampling
+  // entries keep outside the work arena.
   struct IoBuf {
     void* p = nullptr;
     size_t cap = 0;

@@ -156,74 +156,78 @@ class StableDiffusion:
 
     # ---- hot path
     # sampler / eta / noise_seed (an extension, DESIGN.md §7 f6): "ddim" (eta in [0, 1]; eta = 0 is the reference's sampler) or
-    # "dpmpp_2m" (DPM-Solver++(2M), eta = 0). They hold for the one call; the context's default sampler is restored after it.
+    # "dpmpp_2m" (DPM-Solver++(2M), eta = 0). schedule (f15): "ddim" (the reference's timesteps) or "karras" (the sigma grid of
+    # Karras et al. 2022). They hold for the one call; the context's default sampler and schedule are restored after it.
     @contextlib.contextmanager
-    def _sampler(self, sampler, eta, noise_seed):
+    def _sampler(self, sampler, eta, noise_seed, schedule="ddim"):
         self.ctx.set_sampler(sampler, eta, noise_seed)
         try:
+            self.ctx.set_schedule(schedule)
             yield
         finally:
             self.ctx.set_sampler(0, 0.0, 0)
+            self.ctx.set_schedule(0)
 
     def sample_image(self, context, unconditional_context, unconditional_guidance_scale: float, n_steps: int,
                      init_latent=None, seed: int = 0, height: int = 512, width: int = 512, sampler: str = "ddim",
-                     eta: float = 0.0, noise_seed: int = 0):
+                     eta: float = 0.0, noise_seed: int = 0, schedule: str = "ddim"):
         """-> list of n flat uint8 arrays of H*W*3 (HWC RGB), like the reference's Vec<Vec<u8>>."""
-        with self._sampler(sampler, eta, noise_seed):
+        with self._sampler(sampler, eta, noise_seed, schedule):
             rgb = self.ctx.sample_image(context, unconditional_context, unconditional_guidance_scale, n_steps,
                                         init_latent=init_latent, seed=seed, H=height // 8, W=width // 8)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
 
     def sample_latent(self, context, unconditional_context, unconditional_guidance_scale: float, n_steps: int,
                       init_latent=None, seed: int = 0, height: int = 512, width: int = 512, sampler: str = "ddim",
-                      eta: float = 0.0, noise_seed: int = 0) -> np.ndarray:
-        with self._sampler(sampler, eta, noise_seed):
+                      eta: float = 0.0, noise_seed: int = 0, schedule: str = "ddim") -> np.ndarray:
+        with self._sampler(sampler, eta, noise_seed, schedule):
             return self.ctx.sample_latent(context, unconditional_context, unconditional_guidance_scale, n_steps,
                                           init_latent=init_latent, seed=seed, H=height // 8, W=width // 8)
 
     def img2img(self, image, context, unconditional_context, unconditional_guidance_scale: float, n_steps: int,
                 strength: float, mask=None, noise=None, seed: int = 0, sampler: str = "ddim", eta: float = 0.0,
-                noise_seed: int = 0):
+                noise_seed: int = 0, schedule: str = "ddim"):
         """Image-to-image / masked inpainting (an extension: the reference has none; DESIGN.md §7 f5). image u8
         [n, height, width, 3] HWC RGB, the format sample_image returns; mask u8 [n, height, width] (255 = regenerate,
         0 = keep) or None; strength in (0, 1]. With inpaint=True the mask is required, binary (>= 128 regenerates), and
         conditions the UNet, which sees the masked image, instead of a blend after each step. -> list of n flat uint8 arrays of
         height*width*3, like sample_image."""
-        with self._sampler(sampler, eta, noise_seed):
+        with self._sampler(sampler, eta, noise_seed, schedule):
             rgb = self.ctx.img2img(image, context, unconditional_context, unconditional_guidance_scale, n_steps, strength,
                                    mask=mask, noise=noise, seed=seed)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
 
     def edit_image(self, image, context, unconditional_context, guidance_scale: float = 7.5, image_guidance_scale: float = 1.5,
                    n_steps: int = 100, init_latent=None, seed: int = 0, sampler: str = "ddim", eta: float = 0.0,
-                   noise_seed: int = 0):
+                   noise_seed: int = 0, schedule: str = "ddim"):
         """InstructPix2Pix editing (pix2pix=True; DESIGN.md §7 f10): image u8 [n, height, width, 3] HWC RGB, the format
         sample_image returns; context [n, L, 768] the instructions; unconditional_context [Lu, 768]. Every step runs the UNet on
         (no image, negative), (image, negative) and (image, instruction) and combines them with guidance_scale (text) and
         image_guidance_scale, the defaults of the original pipeline. -> list of n flat uint8 arrays of height*width*3, like
         sample_image."""
-        with self._sampler(sampler, eta, noise_seed):
+        with self._sampler(sampler, eta, noise_seed, schedule):
             rgb = self.ctx.edit_image(image, context, unconditional_context, guidance_scale, image_guidance_scale, n_steps,
                                       init_latent=init_latent, seed=seed)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
 
     # ---- batches of different requests (an extension, DESIGN.md §7 f7): one UNet pass per step for all of them
     def sample_batch(self, contexts, unconditional_contexts, guidance_scales, n_steps: int, seeds, height: int = 512,
-                     width: int = 512, sampler: str = "ddim", eta: float = 0.0, noise_seeds=None):
+                     width: int = 512, sampler: str = "ddim", eta: float = 0.0, noise_seeds=None, schedule: str = "ddim"):
         """contexts: list of n [1, L_i, 768] (what `context` returns; lengths may differ); unconditional_contexts: one [Lu, 768]
         shared by every request or a list of n; guidance_scales: one number or a list of n; seeds: list of n (request i gets the
         image sample_image gives for seeds[i] alone, to rounding); noise_seeds: list of n keying eta > 0 noise per request, or None.
         -> list of n flat uint8 arrays of height*width*3, like sample_image."""
-        with self._sampler(sampler, eta, 0):
+        with self._sampler(sampler, eta, 0, schedule):
             rgb = self.ctx.sample_batch(contexts, unconditional_contexts, guidance_scales, n_steps, seeds=seeds,
                                         noise_seeds=noise_seeds, H=height // 8, W=width // 8)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
 
     def img2img_batch(self, images, contexts, unconditional_contexts, guidance_scales, n_steps: int, strength: float,
-                      masks=None, seeds=None, noise=None, sampler: str = "ddim", eta: float = 0.0, noise_seeds=None):
+                      masks=None, seeds=None, noise=None, sampler: str = "ddim", eta: float = 0.0, noise_seeds=None,
+                      schedule: str = "ddim"):
         """img2img over a batch of different requests: images u8 [n, height, width, 3]; masks u8 [n, height, width] or None;
         the other arguments as sample_batch. -> list of n flat uint8 arrays of height*width*3."""
-        with self._sampler(sampler, eta, 0):
+        with self._sampler(sampler, eta, 0, schedule):
             rgb = self.ctx.img2img_batch(images, contexts, unconditional_contexts, guidance_scales, n_steps, strength, mask=masks,
                                          noise=noise, seeds=seeds, noise_seeds=noise_seeds)
         return [rgb[i].reshape(-1) for i in range(rgb.shape[0])]
